@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- throughput of the quorum-tally + Reed-Solomon accept path on B200.
+"""bench.py -- throughput of the quorum-tally + Reed-Solomon accept path on H100.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload cfg3|cfg2|cfg3b|cfg4|cfg5]
 
@@ -13,6 +13,7 @@ encode + distribute + coverage tally) and "cfg5" (Raft scan), each with its own 
   value      RS shard GB/s = (d+p)*L bytes per codeword * codewords / time   (whole job, all ranks)
   e2e        same metric through the host-buffer C-ABI call (pinned host memory, H2D + D2H inside)
   roofline   algorithmic bytes per launch / CUDA-event kernel time vs MEASURED_PEAKS.json hbm_gbs
+             (falls back to the H100 SXM data-sheet 3.35 TB/s; copy_gbs_this_box is the copy bandwidth measured live)
   cpu_baseline / --impl reference: the CPU oracle port of the reference path on this box's cores
 
 N > 1 (one process per GPU): groups shard across ranks; replica r of a group led from rank h is simulated on rank
@@ -48,7 +49,11 @@ D, P, DATA_LEN = 3, 2, 4096
 R, THRESH_RSPAXOS, THRESH_MULTIPAXOS = 5, 4, 3
 G_PER_GPU = 1 << 20
 METRIC = "RS shard GB/s on the fused RSPaxos accept step (RS(3,2) encode + quorum tally); consensus slots committed/s in slots_committed_per_s"
-NVLINK_REF_GBS = 770.0      # measured peer copy per direction, B200_PROFILING.md
+NVLINK_REF_GBS = 450.0      # H100 SXM data sheet: NVLink 4 at 900 GB/s both directions together (not a measured figure)
+# Crossword's mixed 256 B..64 KB codewords need ~71 GiB at 2^20 (payload arena + parity planes + five replica logs),
+# too close to an 80 GB H100's capacity; 2^19 need ~36 GiB.
+CFG4_GROUPS = 1 << 19
+DUMP_GROUPS, DUMP_PARITY_GROUPS, DUMP_SEED = 1 << 16, 2048, 0xD0D0
 
 
 def parse_args():
@@ -72,7 +77,13 @@ def parse_args():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-sub", action="store_true", help="skip the cfg2/cfg3b/cfg4/cfg5 sub-benches")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="cfg3/cfg2 on one GPU: after the timed steps, write what the last step returned as DIR/<name>.npy "
+                         "(commit words and commit_bar of a fixed seeded sample of groups, parity planes of a smaller one)")
+    args = ap.parse_args()
+    if args.dump_outputs and (args.workload not in ("cfg3", "cfg2") or args.gpus != 1 or args.impl != "ours"):
+        ap.error("--dump-outputs covers the cfg3 and cfg2 main lines of --impl ours on one GPU")
+    return args
 
 
 def measured_peaks():
@@ -80,7 +91,7 @@ def measured_peaks():
     if f.exists():
         j = json.loads(f.read_text())
         return float(j["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (measured copy bandwidth)"
-    return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+    return 3350.0, "fallback: H100 SXM data-sheet HBM3 bandwidth 3.35 TB/s (not measured)"
 
 
 def copy_bandwidth_here(torch, dev):
@@ -102,28 +113,17 @@ def copy_bandwidth_here(torch, dev):
         return None
 
 
-def profile_traffic(key: str):
-    """dram bytes per launch from the committed ncu --set full captures (profiles/traffic.json), or None."""
-    f = ROOT / "profiles" / "traffic.json"
-    if f.exists():
-        try:
-            return json.loads(f.read_text()).get(key)
-        except Exception:
-            return None
-    return None
-
-
-def roofline_obj(alg_bytes, ms, peak, peak_src, kernel, traffic_key, **extra):
+def roofline_obj(alg_bytes, ms, peak, peak_src, kernel, **extra):
     ach = alg_bytes / (ms * 1e-3) / 1e9
     d = {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-         "traffic": profile_traffic(traffic_key), "kernel": kernel, "kernel_ms": ms,
+         "kernel": kernel, "kernel_ms": ms,
          "algorithmic_bytes_per_launch": int(alg_bytes), "peak_source": peak_src + " (burst figure; kernel timed alone)"}
     d.update(extra)
     return d
 
 
 class ClockSampler:
-    """Samples nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """Samples nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -229,7 +229,7 @@ def cpu_arm(steps: int, warmup: int, n_cw: int, workload: str):
     from oracle import pyoracle as oracle
     cpus = sorted(FULL_AFFINITY) if FULL_AFFINITY else list(range(os.cpu_count() or 1))
     threads = physical_cores(cpus)
-    if os.environ.get("SS_CPU_THREADS"):                 # tuning knobs (profiles/r02_cpu_arm_sweep.txt)
+    if os.environ.get("SS_CPU_THREADS"):                 # tuning knobs
         threads = int(os.environ["SS_CPU_THREADS"])
     mode = (1 if oracle.have_avx2() else 0) | (0 if os.environ.get("SS_CPU_SCHED") == "dynamic" else oracle.MODE_STATIC)
     L = oracle.cw_shard_len(DATA_LEN, D)
@@ -298,7 +298,7 @@ WORKLOAD_TEXT = {
     "cfg3": "cfg3: RSPaxos (3,5) fused RS(3,2) encode + quorum tally (4 of 5), 2^20 groups x 4096 B request batch + 64-slot ack window per GPU",
     "cfg2": "cfg2: MultiPaxos 5-replica quorum tally (3 of 5), 2^20 groups x 64 slots per GPU",
     "cfg3b": "cfg3b: reconstruct_data, 2^20 codewords, 50% intact / 25% one data shard / 25% two shards missing",
-    "cfg4": "cfg4: Crossword n=5 d=3 T=5 f=2, 2^20 codewords, data_len uniform over {256..65536}, spr uniform {1,2,3}",
+    "cfg4": "cfg4: Crossword n=5 d=3 T=5 f=2, 2^19 codewords, data_len uniform over {256..65536}, spr uniform {1,2,3}",
     "cfg5": "cfg5: Raft 7-replica match-index commit scan, 2^22 groups, 64-slot term window",
 }
 
@@ -313,7 +313,31 @@ def config_dict(args, world):
             "sharding": f"groups x{world} (independent shards)" + ("" if world == 1 else
                         f" + shard planes delivered to the simulated peers' GPUs over NVLink (exchange = {args.exchange}); followers' ack planes "
                         "stored back by a follower kernel; ordering by step flags in device memory (no host sync or NCCL per step)"),
-            "l2": "inputs (4 GiB payload + 2.9 GB parity per GPU) exceed the 126 MB L2; no flush needed"}
+            "l2": "inputs (4 GiB payload + 2.9 GB parity per GPU) exceed the H100's 50 MB L2; no flush needed"}
+
+
+def dump_outputs(out_dir: Path, n: int, parity, committed, bar):
+    """Writes what the last timed step returned to its caller, for comparing two builds output for output: the commit
+    words (split into 32-bit halves, exact in float64) and commit_bar of a fixed seeded sample of groups, and the parity
+    planes of DUMP_PARITY_GROUPS groups spread over that sample (all of them would be gigabytes)."""
+    out_dir.mkdir(parents=True, exist_ok=True)
+    rng = np.random.default_rng(DUMP_SEED)
+    idx = np.sort(rng.choice(n, size=min(n, DUMP_GROUPS), replace=False))
+    arrays = {"group_index": idx.astype(np.float64)}
+    if committed is not None:
+        cw = committed.cpu().numpy().view(np.uint64)[idx]
+        arrays["committed_lo"] = (cw & np.uint64(0xFFFFFFFF)).astype(np.float64)
+        arrays["committed_hi"] = (cw >> np.uint64(32)).astype(np.float64)
+        arrays["commit_bar"] = bar.cpu().numpy().view(np.uint32)[idx].astype(np.float64)
+    if parity is not None:
+        import torch
+        pidx = idx[::max(1, len(idx) // DUMP_PARITY_GROUPS)][:DUMP_PARITY_GROUPS]
+        arrays["parity_index"] = pidx.astype(np.float64)
+        arrays["parity"] = parity[:, torch.from_numpy(pidx.astype(np.int64)).to(parity.device)].cpu().numpy().astype(np.float32)
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= 64 << 20, f"dump of {total} bytes exceeds 64 MiB"
+    for name, a in arrays.items():
+        np.save(out_dir / f"{name}.npy", a)
 
 
 def _time_steps(torch, fn, steps, warmup):
@@ -455,9 +479,8 @@ def run_ours(args):
         torch.cuda.synchronize()
 
     # The clock sampler is started BEFORE the warm-up: forking nvidia-smi takes rank 0's host thread tens of ms, and at N > 1
-    # the other ranks' first timed steps would wait that long for rank 0's first launch (profiles/r02_timeline_n8_*_serial*:
-    # one 70-100 ms interval at the start of the timed region on every rank but 0 -- the "5 ms/step outside the kernel" of
-    # round 1's N = 8 run).
+    # the other ranks' first timed steps would wait that long for rank 0's first launch (one long interval at the start of
+    # the timed region on every rank but 0, visible with --timeline).
     sampler = ClockSampler(local) if rank == 0 else None
     for _ in range(max(3, args.warmup)):
         step()
@@ -483,6 +506,9 @@ def run_ours(args):
     clocks = sampler.stop() if sampler else None
     status = ctx.device_status()
     assert status == 0, f"device status {status}: a step-flag wait timed out"
+    if args.dump_outputs:
+        dump_outputs(Path(args.dump_outputs), n, None if args.workload == "cfg2" else parity,
+                     None if args.no_tally else committed, None if args.no_tally else bar)
     # kernel-only duration (CUDA events around the launches), measured in a second pass so the events do not perturb
     # the whole-step timing above
     k_evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.steps)]
@@ -557,10 +583,9 @@ def run_ours(args):
         alg = alg_rs + (0 if args.no_tally else alg_tally)
         value = alg_rs * n * world / (ms_per_step * 1e-3) / 1e9
         unit = "GB/s"
-    tkey = (args.workload if R == 5 else f"{args.workload}_r{R}") + ("_5planes" if (world > 1 and args.workload == "cfg3") else "")
     # N > 1: the step also writes the d data-shard planes (every replica's log is a separate buffer), SURVEY 8d "state which"
     alg_kernel = alg + (D * L if (world > 1 and args.workload == "cfg3") else 0)
-    roofline = roofline_obj(alg_kernel * n, kernel_ms, peak, peak_src, timed_kernel, tkey)
+    roofline = roofline_obj(alg_kernel * n, kernel_ms, peak, peak_src, timed_kernel)
     if world > 1 and args.workload == "cfg3":
         roofline["note"] = ("kernel = the encode + tally launch alone; in exchange mode ce it writes all five planes to local HBM "
                             "(algorithmic bytes include the three data-shard planes), in mode p2p its stores cross NVLink")
@@ -586,8 +611,8 @@ def run_ours(args):
                             "nvlink_gbs_per_step": nv_bytes / (ms_per_step * 1e-3) / 1e9,
                             "nvlink_gbs_in_kernel": nv_bytes / (kernel_ms * 1e-3) / 1e9 if args.exchange == "p2p" else None,
                             "frac_of_slower_bound": max(nv_ms, hbm_ms) / ms_per_step,
-                            "note": "target time = slower of HBM bytes / measured copy bandwidth and NVLink bytes / 770 GB/s "
-                                    "(measured peer-copy reference, B200_PROFILING.md)"}
+                            "note": "target time = slower of HBM bytes / measured copy bandwidth and NVLink bytes / 450 GB/s "
+                                    "(H100 SXM data-sheet NVLink bandwidth per direction, not measured)"}
     if rank == 0:
         here = copy_bandwidth_here(torch, dev)
         if here:
@@ -599,7 +624,7 @@ def run_ours(args):
     if not args.no_e2e:
         e2e = bench_e2e(env, data, n)
 
-    # free the cfg3 state before the sub-benches (cfg4 needs ~70 GB)
+    # free the cfg3 state before the sub-benches (cfg4 needs ~36 GiB)
     if rep is not None:
         if world > 1:
             dist.barrier()
@@ -673,7 +698,7 @@ def bench_cfg2(env, n):
     b.record()
     torch.cuda.synchronize()
     ms_plain = a.elapsed_time(b) / iters
-    # The launch is ~10 us of work: back-to-back launches from the host leave a gap of a few us between kernels.  A
+    # The launch is only microseconds of work: back-to-back launches from the host leave a gap of a few us between kernels.  A
     # CUDA graph of the four rotated launches removes most of it (the engine's tick would be captured the same way).
     ms = ms_plain
     graphed = False
@@ -708,8 +733,8 @@ def bench_cfg2(env, n):
     return {"workload": WORKLOAD_TEXT["cfg2"] + ", 4 rotated plane sets (208 MB > L2)",
             "slots_committed_per_s": n * 64 / (ms * 1e-3), "ms_per_step": ms, "ms_per_step_plain_launches": ms_plain,
             "cuda_graph": graphed, "timing": graph_note,
-            "roofline": roofline_obj(alg, ms, peak, env["peak_src"], "tally_planes_x2_kernel", "cfg2",
-                                     note="52 B/group; 8.4 us of traffic per launch at the copy bandwidth, 10.7 us kernel under ncu; the rest is launch gap")}
+            "roofline": roofline_obj(alg, ms, peak, env["peak_src"], "tally_planes_x2_kernel",
+                                     note="52 B/group; short launches, so the gap between them weighs on the figure")}
 
 
 def bench_e2e(env, data_dev, n):
@@ -793,7 +818,7 @@ def bench_cfg5(env, steps, warmup):
     return {"metric": "Raft groups scanned/s (7 replicas, 64-slot window)", "value": G * world / (ms * 1e-3), "unit": "groups/s",
             "dtype": "u32", "groups": G, "workload": WORKLOAD_TEXT["cfg5"], "ms_per_step": ms, "n_gpus": world,
             "parity_check": "first 2^16 groups (the tile the batch repeats) bit-exact vs oracle",
-            "roofline": roofline_obj(alg, ms, peak, env["peak_src"], "raft_scan_kernel", "cfg5",
+            "roofline": roofline_obj(alg, ms, peak, env["peak_src"], "raft_scan_kernel",
                                      note="charged 296 B/group (SURVEY 8d); the probe path reads fewer term words"),
             "gpu_launches": int(launches)}
 
@@ -832,7 +857,7 @@ def bench_cfg3b(env, steps, warmup):
             "value": alg / (ms * 1e-3) / 1e9, "unit": "GB/s", "groups": n, "workload": WORKLOAD_TEXT["cfg3b"], "ms_per_step": ms,
             "codewords_per_s": n / (ms * 1e-3), "roundtrip_bit_exact": bool(ok),
             "parity_check": "every regenerated data shard of every codeword == the original (encode -> erase -> reconstruct)",
-            "roofline": roofline_obj(alg, ms, peak, env["peak_src"], kernel, "cfg3b"), "gpu_launches": int(launches)}
+            "roofline": roofline_obj(alg, ms, peak, env["peak_src"], kernel), "gpu_launches": int(launches)}
 
 
 def bench_cfg4(env, steps, warmup):
@@ -842,7 +867,7 @@ def bench_cfg4(env, steps, warmup):
     from oracle import pyoracle as oracle
     from summerset_b200 import sharding, workloads as wl
     from summerset_b200.api import crossword_brr_assignment, cw_slot_pitch
-    n = args.groups
+    n = min(args.groups, CFG4_GROUPS)
     lens, spr = wl.cfg4_lengths(n, seed_extra=0)      # same sizes on every rank (payload bytes differ by rank)
     lay = wl.ragged_layout(lens, D)
     gen = torch.Generator(device=dev); gen.manual_seed(wl.SEED_BASE + 4 + rank)
@@ -920,9 +945,9 @@ def bench_cfg4(env, steps, warmup):
                           "hbm_GBps_per_rank": alg_dist / (ms * 1e-3) / 1e9,
                           "nvlink_bytes_per_rank": nv_bytes, "nvlink_bound_ms": nv_ms, "hbm_bound_ms": hbm_ms,
                           "frac_of_slower_bound": max(nv_ms, hbm_ms) / ms,
-                          "roofline": roofline_obj(alg_dist, ms_dist, peak, env["peak_src"], dist_kernel, "cfg4_distribute") if ms_dist else None},
+                          "roofline": roofline_obj(alg_dist, ms_dist, peak, env["peak_src"], dist_kernel) if ms_dist else None},
            "slots_committed_per_s": n * world / (ms * 1e-3), "encode_only_ms": ms_enc, "parity_check": note,
-           "roofline": roofline_obj(alg, ms_enc, peak, env["peak_src"], enc_kernel, "cfg4"), "gpu_launches": int(launches)}
+           "roofline": roofline_obj(alg, ms_enc, peak, env["peak_src"], enc_kernel), "gpu_launches": int(launches)}
     if world > 1:
         dist.barrier()
         for q in peer_log:

@@ -10,7 +10,7 @@
  * instances commit -- what the Rust shim's run() loop does once per event-loop turn.
  *
  * build: gcc -O2 examples/c_abi_demo.c -Iinclude -Lsummerset_b200 -lsummerset_b200 -Wl,-rpath,$PWD/summerset_b200 -o c_abi_demo
- * Without an sm_100 GPU it prints the library's refusal (there is no CPU fallback) and exits 3.
+ * Without an sm_90 GPU it prints the library's refusal (there is no CPU fallback) and exits 3.
  */
 #include <stdint.h>
 #include <stdio.h>

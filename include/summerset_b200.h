@@ -1,7 +1,7 @@
 /*
  * summerset_b200.h -- C ABI of libsummerset_b200.so
  *
- * The B200 (sm_100a) implementation of Summerset's quorum-tally + Reed-Solomon hot path.
+ * The H100 (sm_90a) implementation of Summerset's quorum-tally + Reed-Solomon hot path.
  * Plain C: pointers and sizes only, no torch / C++ types.  This is the boundary a Rust
  * `extern "C"` block (INTEGRATION.md) binds; the GenericReplica / SmrProtocol surface
  * (src/server/replica.rs:15-42, src/protocols/mod.rs:118-215) is untouched by it.
@@ -22,7 +22,7 @@
  *   - `_dev` entry points take DEVICE pointers and are asynchronous on the context's stream;
  *     the others take HOST pointers, copy in/out and return when the result is in host memory.
  *   - No CPU fallback: every compute entry point fails with SS_ERR_NO_DEVICE / SS_ERR_CUDA when
- *     no sm_100 device is usable.
+ *     no sm_90 device is usable.
  */
 #ifndef SUMMERSET_B200_H
 #define SUMMERSET_B200_H
@@ -57,7 +57,7 @@ enum {
     SS_ERR_INVALID_ARG = -20,
     SS_ERR_UNSUPPORTED = -21,
     SS_ERR_OUT_OF_MEMORY = -22,
-    SS_ERR_NO_DEVICE = -30,   /* no CUDA device / not sm_100: there is NO CPU fallback */
+    SS_ERR_NO_DEVICE = -30,   /* no CUDA device / not sm_90: there is NO CPU fallback */
     SS_ERR_CUDA = -31
 };
 
@@ -361,8 +361,8 @@ int ss_follower_ack_dev(ss_ctx *ctx, const uint64_t *ack_src, uint64_t *const *a
  * the coder's (d, T-d) code and writes, for every codeword g, the spr[g] shards the balanced round-robin assignment gives
  * replica r -- shards {(r*dj + k) mod T : k < spr[g]}, dj = T / n_replicas (crossword/mod.rs:866-888) -- into
  * replica_logs[r] at rep_off[g] + k*SS_CW_SLOT_PITCH(L_g), k = 0..spr-1 (bytes past L_g zero; the pitch is L_g rounded up
- * to 32 bytes so that every slot of a log built from 32-byte aligned offsets starts on a DRAM sector: with a 16-byte
- * pitch the same kernel is 7 % slower, profiles/r02_distribute_variants.txt).  replica_logs is a HOST array
+ * to 32 bytes so that every slot of a log built from 32-byte aligned offsets starts on a DRAM sector, which a 16-byte
+ * pitch does not give).  replica_logs is a HOST array
  * of n_replicas device pointers, local or peer (ss_ipc_open): the kernel's stores are the shard transfer.  Per codeword
  * (n-1)*spr*L_g bytes cross to other replicas, as in the reference.  Any code with d <= 8 and T a multiple of
  * n_replicas <= 16 (crossword/mod.rs:805-830); n = 5 with RS(3,2) runs the hand-specialised kernel. */
@@ -546,7 +546,7 @@ int ss_engine_raft_ingest(ss_engine *engine, const uint32_t *rec_group, const ui
                           const uint32_t *rec_end_slot, uint64_t n_records);
 
 /* ---- tuning / introspection (bench + tests) ------------------------------------------------ */
-/* Tuning knob for experiments (profiles/r01_row_kernel_sweep.txt); 0 = the measured-best defaults.
+/* Tuning knob for experiments; 0 = the defaults.
  *   bits 0-3  kernel choice / register budget: 1 = flat one-column-per-thread RS(3,2) kernel instead of the row kernel,
  *             5 = bit-plane generic kernels instead of the Horner ones, 8 = global-table Horner reconstruct instead of the
  *             shared-memory small-code kernel; 3 / 6 / 7 = 32 / 64 / 56-register builds of the row kernel (default 40)

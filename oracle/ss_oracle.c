@@ -2,7 +2,7 @@
  * ss_oracle.c -- CPU ORACLE (test infrastructure; see ss_oracle.h for scope and pinning status).
  *
  * Restates, in plain C, the algorithms on the reference's quorum-tally + Reed-Solomon path.
- * Every function cites the reference file:line (relative to /root/reference) it follows.
+ * Every function cites the reference file:line (relative to the reference tree's root) it follows.
  * Build: `make -C oracle` (gcc -O3 -fopenmp; SIMD paths use per-function target attributes and
  * a runtime CPU check, so the .so stays runnable on a host without AVX2).
  */

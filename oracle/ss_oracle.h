@@ -6,7 +6,7 @@
  * (summerset_b200/csrc, libsummerset_b200.so) never links, imports or calls it.
  *
  * It is a plain-C restatement of the reference's Rust path (josehu07/summerset @ 1daf80aa;
- * paths relative to /root/reference):
+ * paths relative to the reference tree's root):
  *   src/utils/rscoding.rs            RSCodeword geometry / encode / reconstruct / verify
  *   src/utils/bitmap.rs              Bitmap (replica-id / shard-id bitset)
  *   src/protocols/multipaxos/messages.rs:370-443   MultiPaxos accept-reply tally

@@ -1,4 +1,4 @@
-"""Builds libsummerset_b200.so (the C-ABI library) in-tree with nvcc for sm_100a.
+"""Builds libsummerset_b200.so (the C-ABI library) in-tree with nvcc for sm_90a (H100).
 
 Usage: python -m summerset_b200.build [--force] [--verbose]
 The .so is git-ignored but travels to the GPU box with the gpurun snapshot.
@@ -21,7 +21,7 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 CCBIN = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
 FLAGS = [
     "-O3", "-std=c++17", "-lineinfo",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-Xcompiler", "-fPIC",
     "-ccbin", CCBIN,
     "--expt-relaxed-constexpr",
@@ -74,7 +74,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
             sys.stderr.write(f"[build] {s}\n{out}\n")
     if failed:
         raise RuntimeError("nvcc compilation failed")
-    link = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-ccbin", CCBIN,
+    link = [NVCC, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-ccbin", CCBIN,
             "-Xcompiler", "-fPIC", "-o", str(OUT), *objs, "-ldl"]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:

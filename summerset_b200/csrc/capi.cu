@@ -293,7 +293,7 @@ const char *ss_strerror(int code) {
         case SS_ERR_INVALID_ARG: return "invalid argument";
         case SS_ERR_UNSUPPORTED: return "unsupported configuration";
         case SS_ERR_OUT_OF_MEMORY: return "out of device memory";
-        case SS_ERR_NO_DEVICE: return "no usable sm_100 CUDA device (no CPU fallback)";
+        case SS_ERR_NO_DEVICE: return "no usable sm_90 CUDA device (no CPU fallback)";
         case SS_ERR_CUDA: return "CUDA error";
         default: return "unknown error";
     }
@@ -313,8 +313,8 @@ static int ctx_create_common(int device, void *stream, bool borrow, ss_ctx **out
     if (device < 0 || device >= count) return set_error(SS_ERR_INVALID_ARG, "device %d out of range [0,%d)", device, count);
     cudaDeviceProp prop;
     SS_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10)
-        return set_error(SS_ERR_NO_DEVICE, "device %d is sm_%d%d; kernels are built for sm_100a only", device, prop.major,
+    if (prop.major != 9 || prop.minor != 0)
+        return set_error(SS_ERR_NO_DEVICE, "device %d is sm_%d%d; kernels are built for sm_90a only", device, prop.major,
                          prop.minor);
     SS_CUDA(cudaSetDevice(device));
     ss_ctx *ctx = new (std::nothrow) ss_ctx();
@@ -855,7 +855,7 @@ static int encode_uniform_host(ss_rs_coder *c, const uint8_t *data, uint64_t dat
     const bool tally = planes != nullptr;
     const uint64_t L = (uint64_t(data_len) + d - 1) / d, ds = (L + 15) & ~uint64_t(15);
     if (data_stride < data_len || shard_stride < L) return set_error(SS_ERR_INVALID_ARG, "stride shorter than element");
-    // chunk: 16 MiB of payload measured best (profiles/r01_pcie_probe.txt); SS_E2E_CHUNK_MB overrides, for tuning
+    // chunk: 16 MiB of payload by default; SS_E2E_CHUNK_MB overrides, for tuning
     uint64_t chunk_mb = 16;
     if (const char *e = getenv("SS_E2E_CHUNK_MB")) { const long v = atol(e); if (v >= 1 && v <= 4096) chunk_mb = static_cast<uint64_t>(v); }
     uint64_t C = (chunk_mb << 20) / data_stride;

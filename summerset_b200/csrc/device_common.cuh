@@ -1,4 +1,4 @@
-// device_common.cuh -- device-side helpers shared by the kernel files (sm_100a).
+// device_common.cuh -- device-side helpers shared by the kernel files (sm_90a).
 #pragma once
 #ifndef __CUDACC_RTC__
 #include <cuda_runtime.h>

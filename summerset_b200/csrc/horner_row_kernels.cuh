@@ -48,8 +48,8 @@ struct EncRowGen {
 };
 
 // multiply four packed field elements by x: shift on the FMA pipe, prmt sign mask + two lop3 on the ALU pipe.
-// (A flavour that took the reduction term from a high multiply -- 1 ALU + 3 FMA-pipe instructions -- measured the
-// same on B200 and was dropped: profiles/r01_cluster_codes_sweep.txt, variant 4096.)
+// (A flavour that took the reduction term from a high multiply -- 1 ALU + 3 FMA-pipe instructions -- was no faster and
+// was dropped.)
 __device__ __forceinline__ uint32_t xtime_word(uint32_t x) { return ((x * 2u) & 0xfefefefeu) ^ (msb_mask(x) & 0x1d1d1d1du); }
 
 // the d source vectors of column k of one codeword, funnelled to shard alignment and masked to the payload

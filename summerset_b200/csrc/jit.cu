@@ -90,7 +90,7 @@ int jit_compile(int d, int p, const uint8_t *rows, int which, std::vector<char> 
         coefs += tmp;
     }
     const std::string def_d = "-DSS_JIT_D=" + std::to_string(d), def_p = "-DSS_JIT_P=" + std::to_string(p), def_c = "-DSS_JIT_COEFS=" + coefs;
-    const char *opts[] = {"--gpu-architecture=sm_100a", "-std=c++17", def_d.c_str(), def_p.c_str(), def_c.c_str()};
+    const char *opts[] = {"--gpu-architecture=sm_90a", "-std=c++17", def_d.c_str(), def_p.c_str(), def_c.c_str()};
     nvrtcProgram prog = nullptr;
     nvrtcResult r = rt.CreateProgram(&prog, kJitSource, "summerset_b200_jit.cu", 0, nullptr, nullptr);
     if (r != NVRTC_SUCCESS) { log = std::string("nvrtcCreateProgram: ") + rt.GetErrorString(r); return SS_ERR_UNSUPPORTED; }
@@ -154,7 +154,7 @@ int jit_ensure(ss_rs_coder *c, int which) {
     c->jit_kernel[which] = k;
     c->jit_library[which] = lib;
     c->jit_state[which] = 1;
-    c->jit_message = "specialised by NVRTC (" + name + ", " + std::to_string(cubin.size()) + " bytes of sm_100a code)";
+    c->jit_message = "specialised by NVRTC (" + name + ", " + std::to_string(cubin.size()) + " bytes of sm_90a code)";
     return SS_OK;
 }
 

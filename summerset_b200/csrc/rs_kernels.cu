@@ -1,4 +1,4 @@
-// rs_kernels.cu -- Reed-Solomon GF(2^8) shard encode / reconstruct kernels for sm_100a.
+// rs_kernels.cu -- Reed-Solomon GF(2^8) shard encode / reconstruct kernels for sm_90a.
 //
 // What they replace (reference, josehu07/summerset @ 1daf80aa):
 //   RSCodeword::from_data split + compute_parity  src/utils/rscoding.rs:165-243,447-486
@@ -1092,9 +1092,8 @@ __device__ __forceinline__ void cw_column(const CwDistribute &P, const uint8_t *
 //   B  the SHORT codewords of the run, pooled into one column sequence dealt 32 lanes at a time, each lane looking up
 //      which codeword its column is in (lane j of the warp holds the geometry of codeword j of the run).
 // Why the pooling: walked alone, a payload of 256 B costs a full pass of ~400 warp instructions for 6 useful lanes; a batch
-// of such payloads runs 3.3x faster pooled (0.30 ms vs 0.97 ms per 2^20).  In the cfg-4 mix the short codewords carry 3 % of
-// the bytes and the pooling does not pay for the coarser unit of work, so RUN = 1 stays the default there
-// (profiles/r02_distribute_variants.txt).
+// of such payloads runs several times faster pooled.  In the cfg-4 mix the short codewords carry 3 % of the bytes and the
+// pooling does not pay for the coarser unit of work, so RUN = 1 stays the default there.
 // The next run is fetched one run ahead, so the counter's latency hides behind the current run.
 template <int RUN, bool DYN>
 __global__ void __launch_bounds__(kThreads, 3) rs32_crossword_distribute_kernel(const __grid_constant__ CwDistribute P) {
@@ -1325,10 +1324,10 @@ int launch_crossword_distribute(ss_rs_coder *coder, const uint8_t *data, const u
     CwDistribute P;
     P.data = data; P.data_off = data_off; P.data_len = data_len; P.spr = spr; P.rep_off = rep_off; P.n = n;
     for (int r = 0; r < 5; ++r) P.rep[r] = replica_logs[r];
-    // variant bits 0-3 (tuning; profiles/r02_distribute_variants.txt): default = a codeword per warp at a fixed stride (12.16 ms
-    // on the cfg-4 mix); 6 / 7 = runs of 8 / 4 codewords from a shared counter with the short ones pooled -- 1-2 % slower on
-    // the mix (a run of long codewords is a coarse unit of work) but 3.3x faster on batches of payloads under 1 KB, for
-    // callers that know their batch is like that
+    // variant bits 0-3 (tuning; tools/distribute_ab.py compares them): default = a codeword per warp at a fixed stride;
+    // 6 / 7 = runs of 8 / 4 codewords from a shared counter with the short ones pooled -- for the cfg-4 mix a run of long
+    // codewords is a coarse unit of work, but batches of payloads under 1 KB run several times faster, for callers that
+    // know their batch is like that
     const int vk = coder->variant & 15;
     P.next_cw = reinterpret_cast<unsigned long long *>(ctx->dev_status + 32);
     if (vk != 6 && vk != 7) {
@@ -1427,8 +1426,8 @@ int launch_rs_encode(ss_rs_coder *coder, const EncGeom &g, const TallyArgs *tall
             const uint32_t grid = static_cast<uint32_t>(ctas);
             // register budget variants (tuning knob ss_rs_set_variant): 0/2 = 40 regs, 3 = 32 regs, 4 = unconstrained
             // Register budget: 40/thread (12 CTAs of <= 128 threads per SM; the kernel needs ~47 unconstrained and fits
-            // 40 without spilling) and 64 waves measured best on B200 (profiles/r01_row_kernel_sweep.txt).  The other
-            // budgets stay selectable for tuning.
+            // 40 without spilling) and 64 waves of CTAs by default.  The other budgets and wave counts stay selectable
+            // for tuning.
             if (threads > 128) {
                 if (Rw.emit_data) rs32_encode_row_kernel<true, 256, 4><<<grid, threads, 0, st>>>(Rw);
                 else rs32_encode_row_kernel<false, 256, 4><<<grid, threads, 0, st>>>(Rw);

@@ -1,5 +1,5 @@
 // tally_kernels.cu -- quorum vote tallies, ack ingest, Crossword coverage predicate and the Raft
-// match-index commit scan, batched over millions of independent (group, slot) instances (sm_100a).
+// match-index commit scan, batched over millions of independent (group, slot) instances (sm_90a).
 //
 // What they replace (reference, josehu07/summerset @ 1daf80aa) -- work the reference does one
 // message at a time inside the replica's event loop:
@@ -304,7 +304,7 @@ raft_scan_kernel(const uint32_t *__restrict__ match, uint32_t n_peers, uint64_t 
         // ---- the rest: the last slot in (lc, upper) whose term equals curr_term (raft/messages.rs:261-263,271-274: last one
         //      wins).  Each lane walks ITS OWN group's window from the top, four terms per 128-bit load (the window rows are
         //      16-byte aligned when W % 4 == 0): a dozen instructions per step instead of a warp-wide ballot per 32 entries
-        //      and group -- the scan was issue-bound, not bandwidth-bound (profiles/r02_ncu_raft_before.txt).  Windows whose
+        //      and group -- the scan was issue-bound, not bandwidth-bound.  Windows whose
         //      size is not a multiple of four, or unaligned term arrays, take the cooperative walk below. ----
         const bool vec_ok = (W & 3u) == 0u && (reinterpret_cast<uintptr_t>(terms) & 15u) == 0u;
         if (vec_ok) {

@@ -15,9 +15,7 @@ No host synchronisation and no NCCL call sits between steps: ordering is carried
 (st.release.sys / ld.acquire.sys).  With lag = 2 the tally of step k reads the acks of step k - 2 (logs and ack buffers
 double-buffered), so ranks may drift one step apart instead of meeting at every step.
 
-Two ways to move the shard planes (profiles/r02_nvlink_probe.txt measures both per direction with traffic in both
-directions: SM stores 634 GB/s in the encode kernel's access pattern, 705 GB/s for a flat copy kernel, 711 GB/s for TMA
-bulk stores, copy engines 777 GB/s):
+Two ways to move the shard planes (tools/nvlink_probe.cu measures both per direction, with traffic in both directions):
   mode "p2p"  the encode kernel stores every remote shard straight into the follower GPU's log (fused compute + transfer,
               one kernel; NVLink-bound at the SM store rate)
   mode "ce"   the encode kernel writes the remote planes into a local staging buffer at HBM speed and a second context

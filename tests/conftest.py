@@ -10,7 +10,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run by the driver with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (select with -m gpu)")
 
 
 def _has_gpu() -> bool:
@@ -33,7 +33,7 @@ def pytest_collection_modifyitems(config, items):
 @pytest.fixture(scope="session", autouse=True)
 def _built_extension():
     """The CUDA extension is built in-tree by __graft_entry__.build(); build it here too if a test run starts
-    from a clean checkout (nvcc cross-compiles sm_100a without a GPU).  Tests never fall back to anything else."""
+    from a clean checkout (nvcc cross-compiles sm_90a without a GPU).  Tests never fall back to anything else."""
     from summerset_b200 import build as b
     b.build()
     yield

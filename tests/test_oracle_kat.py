@@ -6,7 +6,7 @@ Three groups of checks:
  2. the published algorithm of the un-vendored crate `reed-solomon-erasure ^6.0` (Cargo.toml:43):
     field constants, the Backblaze (4,2) matrix, and the crate's / JavaReedSolomon's upstream
     known-answer tests -- RECALLED from the upstream test-suites (galois tests; `test_one_encode`),
-    not present under /root/reference, hence "parity unpinned by the reference tree";
+    not present in the reference tree, hence "parity unpinned by the reference tree";
  3. the derived KAT of SURVEY.md 8c (TestData("interesting_value"), RS(3,2)).
 """
 import itertools

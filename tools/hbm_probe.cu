@@ -1,7 +1,7 @@
-// hbm_probe.cu -- what does ONE B200's HBM deliver for write-heavy SM traffic, by access pattern?
+// hbm_probe.cu -- what does ONE H100's HBM deliver for write-heavy SM traffic, by access pattern?
 //
-// The Crossword distribute kernel (cfg 4) writes 5 bytes for every byte it reads and sits at 0.78 of the measured
-// copy bandwidth; making it more parallel made it slower (profiles/r02_distribute_variants.txt).  This probe separates
+// The Crossword distribute kernel (cfg 4) writes 5 bytes for every byte it reads and stays below the measured copy
+// bandwidth; making it more parallel made it slower (tools/distribute_ab.py compares the variants).  This probe separates
 // the memory system's ceiling from the kernel's own structure:
 //   fill        write-only, grid-stride 128-bit stores (st.global / .cs / .wt)
 //   fan K       every thread loads one 16-byte vector and stores it to K destination streams that are `gap` bytes apart
@@ -10,7 +10,7 @@
 //               writes each column to K destination slots in K far-apart logs (+ row pitch), codewords of a CTA far apart
 // Reported: total DRAM bytes moved (reads + writes) / time, best of 5.
 //
-// Build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o tools/hbm_probe tools/hbm_probe.cu
+// Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tools/hbm_probe tools/hbm_probe.cu
 #include <cuda_runtime.h>
 
 #include <cstdint>

@@ -2,9 +2,9 @@
 """HBM bandwidth by traffic mix, to read the roofline fractions of kernels that are not 1:1 read:write.
 MEASURED_PEAKS.json's hbm_gbs is a COPY figure (one byte read per byte written).  The encode kernels read more than they
 write (RS(2,1) 2:1, RS(3,2) 3:2 ...), the Crossword distribute kernel writes five times what it reads.  This probe
-times, with CUDA events on one B200:
+times, with CUDA events on one H100:
     write-only   cudaMemsetAsync through ss_dev_memset
-    copy  1:1    cudaMemcpyAsync device-to-device through ss_copy_d2d, and torch's copy_ (how the driver measured)
+    copy  1:1    cudaMemcpyAsync device-to-device through ss_copy_d2d, and torch's copy_ (how MEASURED_PEAKS.json is measured)
     read-mostly  our tally kernel over 16 ack planes (128 B read per 12 B written)
 Run on a GPU box:  python tools/hbm_probe.py
 """

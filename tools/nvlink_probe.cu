@@ -1,4 +1,4 @@
-// nvlink_probe.cu -- how fast can ONE B200 move bytes into / out of a peer's HBM over NVLink, by mechanism?
+// nvlink_probe.cu -- how fast can ONE H100 move bytes into / out of a peer's HBM over NVLink, by mechanism?
 //
 // Decides how the multi-GPU accept step should deliver shard planes to the simulated follower replicas
 // (DESIGN.md section 6).  Single process, two GPUs (0 and 1) with peer access; every test moves BYTES per
@@ -11,8 +11,8 @@
 //   rows      the encode kernel's pattern: a CTA walks "codewords", each thread stores one 16-byte column into each
 //             of 4 peer planes (row pitch 1376 B) -- with and without the final per-CTA system fence
 //
-// Build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o tools/nvlink_probe tools/nvlink_probe.cu
-// Run:   gpurun --gpus 2 -- ./tools/nvlink_probe > gpurun_out/nvlink_probe.txt
+// Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tools/nvlink_probe tools/nvlink_probe.cu
+// Run:   ./tools/nvlink_probe   (on a box with two peer-capable GPUs)
 #include <cuda_runtime.h>
 
 #include <cstdint>
@@ -203,7 +203,7 @@ int main() {
     char name[160];
     for (int nsides = 1; nsides <= 2; ++nsides) {
         // local copy (HBM reference)
-        run("local copy kernel (st.cs, unroll 4, 148x16 CTAs)", sd, nsides, BYTES,
+        run("local copy kernel (st.cs, unroll 4, SMs x 16 CTAs)", sd, nsides, BYTES,
             [&](Side &s) { copy_kernel<1, 4><<<sms * 16, 256, 0, s.st>>>((const uint4 *)s.local, (uint4 *)s.local_dst, nvec); });
         run("ce   cudaMemcpyPeerAsync", sd, nsides, BYTES,
             [&](Side &s) { CK(cudaMemcpyPeerAsync(s.remote, s.peer, s.local, s.dev, BYTES, s.st)); });
