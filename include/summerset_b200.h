@@ -467,10 +467,13 @@ int ss_gossip_plan_dev(ss_ctx *ctx, uint32_t me, uint32_t population, uint32_t d
                        uint32_t n_policies, uint32_t peer_alive, uint64_t n_instances, uint32_t *targets, uint32_t *excl);
 
 /* ---- batched multi-group consensus engine ----------------------------------------------------------------------
- * The leader-side state of n_groups independent replica groups (64-slot instance window each) lives in HBM as a
- * struct of arrays; the host drives all groups together, once per event-loop turn:
- *   ss_engine_propose   one new instance per group at window position `slot`: RS-encode the request batches into the
- *                       shard planes (per-peer packed send buffers) and enter Status::Accepting under the group's
+ * The leader-side state of n_groups independent replica groups lives in HBM as a struct of arrays; the host drives all
+ * groups together, once per event-loop turn.  Paxos-family group g holds the 64 absolute slots [window_base[g],
+ * window_base[g] + 64) (window_base = the reference's start_slot, 0 at creation); every per-slot array is a RING:
+ * absolute slot s lives at position s & 63.
+ *   ss_engine_propose   one new instance per group at window position `slot` (absolute slot window_base + slot), or
+ *   ss_engine_propose_next  at each group's first Null slot: RS-encode the request batches into the shard planes
+ *                       (per-peer packed send buffers) and enter Status::Accepting under the group's
  *                       prepared ballot with an empty ack set   (multipaxos/request.rs:112-221,
  *                       rspaxos/request.rs:72-142, crossword/request.rs:82-185)
  *   ss_engine_ingest    a batch of AcceptReply records through handle_msg_accept_reply's filters
@@ -480,6 +483,7 @@ int ss_gossip_plan_dev(ss_ctx *ctx, uint32_t me, uint32_t population, uint32_t d
  *                       Crossword #acks >= majority && coverage_under_faults >= d, crossword/messages.rs:535-542),
  *                       committed |= newly, accepting &= ~newly, commit_bar = committed prefix
  *                       (multipaxos/durability.rs:161-170)
+ *   ss_engine_advance   retire committed prefixes: window_base moves forward (multipaxos/snapshot.rs:121-171)
  * Raft / CRaft engines keep match_slot / next_slot / log terms instead: ss_engine_raft_append (the leader appends
  * entries in its term), ss_engine_raft_ingest (successful AppendEntriesReply, raft/messages.rs:243-252) and
  * ss_engine_tick (commit scan raft/messages.rs:254-275,295 with quorum_cnt -- CRaft: majority + fault_tolerance,
@@ -509,12 +513,13 @@ typedef struct ss_engine_view {
     uint32_t population, threshold, data_shards, total_shards, shard_len, shard_stride, raft_window, pad0;
     uint64_t plane_stride;      /* bytes between shard planes of one proposal */
     uint64_t slot_stride;       /* bytes between the shard stores of consecutive keep slots */
+    /* per-slot words and arrays are ring-indexed: absolute slot s at bit / entry s & 63 (ss_engine_window_get) */
     uint64_t *planes;           /* [n][G]  valid-ack bit-planes */
     uint64_t *bal_prepared;     /* [G] */
     uint64_t *inst_bal;         /* [G*64] */
-    uint64_t *accepting;        /* [G]  bit s = Status::Accepting */
-    uint64_t *committed;        /* [G]  bit s = Status::Committed */
-    uint32_t *commit_bar;       /* [G] */
+    uint64_t *accepting;        /* [G]  bit s & 63 = Status::Accepting */
+    uint64_t *committed;        /* [G]  bit s & 63 = Status::Committed */
+    uint32_t *commit_bar;       /* [G]  window-relative: the absolute commit bar is window_base + commit_bar */
     uint8_t *shards;            /* [keep][T][G][shard_stride] */
     uint8_t *policy_idx;        /* Crossword [G*64]: assignment policy of each instance */
     uint32_t *match, *next_slot;/* Raft [n-1][G] */
@@ -531,13 +536,36 @@ int ss_engine_set_prepared_ballots(ss_engine *engine, const uint64_t *ballots);
 int ss_engine_set_policies(ss_engine *engine, const uint32_t *policies_host, uint32_t n_policies, int balanced);
 /* payloads: request batch of group g at payloads + g*payload_stride (data_len bytes; NULL for MultiPaxos).  policy:
  * Crossword only, [G] policy index of the new instance (NULL = 0).  *shard_planes (may be NULL) receives the base of
- * this proposal's T shard planes: shard j of group g at base + j*plane_stride + g*shard_stride. */
+ * this proposal's T shard planes: shard j of group g at base + j*plane_stride + g*shard_stride.  `slot` (< 64) is
+ * relative to each group's window base: the instance is absolute slot window_base[g] + slot, its shards go to shard
+ * store slot % keep_slots. */
 int ss_engine_propose(ss_engine *engine, uint32_t slot, const uint8_t *payloads, uint64_t payload_stride,
                       const uint8_t *policy, uint8_t **shard_planes);
+/* group g proposes at its first Null slot of [window_base[g], window_base[g]+64) (rspaxos/mod.rs:434-442);
+ * slot_out[g] (device u64, may be NULL) = that absolute slot, or UINT64_MAX when the window is full (then bit 3 of
+ * ss_ctx_device_status is set and the group is left unchanged).  Shards of this proposal go to shard store `store`
+ * (< keep_slots) -- caller-managed, so the encode stays the uniform row kernel at full speed; a full group's shards are
+ * written there too but belong to no instance.  slot_out is exactly the `slot` array ss_frame_accept_pack_dev takes:
+ * a host goes straight from the proposal to its Accept frames.  Other arguments as ss_engine_propose. */
+#define SS_DEV_STATUS_WINDOW_FULL 8u
+int ss_engine_propose_next(ss_engine *engine, uint32_t store, const uint8_t *payloads, uint64_t payload_stride,
+                           const uint8_t *policy, uint64_t *slot_out, uint8_t **shard_planes);
+/* rec_slot is window-relative, as ss_accept_reply_parse_dev emits it with this engine's window_base: 0xff and values
+ * >= 64 are dropped, rel is absolute slot window_base[g] + rel. */
 int ss_engine_ingest(ss_engine *engine, const uint32_t *rec_group, const uint8_t *rec_slot, const uint8_t *rec_peer,
                      const uint64_t *rec_ballot, uint64_t n_records);
-/* newly (may be NULL): [G] bit s = instance s committed in THIS tick (what the host logs as WalEntry::CommitSlot) */
+/* newly (may be NULL): [G] bit i = instance window_base[g] + i committed in THIS tick (what the host logs as
+ * WalEntry::CommitSlot: ss_wal_commit_pack_dev with this engine's window_base) */
 int ss_engine_tick(ss_engine *engine, uint64_t *newly);
+/* retires committed prefixes (multipaxos/snapshot.rs:121-171, start_slot advance): upto (device [G] absolute slots, or
+ * NULL = the whole committed prefix) -- k = clamp(upto[g] - window_base[g], 0, committed prefix); the k retired ring
+ * positions are cleared (committed, accepting, ack planes), window_base[g] += k and commit_bar[g] -= k. */
+int ss_engine_advance(ss_engine *engine, const uint64_t *upto);
+/* *window_base = the engine's device array [G] of window bases (valid until ss_engine_destroy); a host may install
+ * bases through it, e.g. a snapshot's start_slot on recovery, while the window holds no instance.  Until the first
+ * ss_engine_advance or ss_engine_window_get call every base is 0 and the tick does not read them.  Raft / CRaft
+ * engines (which keep their own ring) return SS_ERR_INVALID_ARG from propose_next, advance and window_get. */
+int ss_engine_window_get(ss_engine *engine, uint64_t **window_base);
 /* Raft: n_new[g] entries appended by the leader in curr_term[g]; exceeding raft_window uncommitted entries sets bit 1
  * of ss_ctx_device_status and leaves that group unchanged */
 #define SS_DEV_STATUS_RAFT_WINDOW_FULL 2u

@@ -106,8 +106,11 @@ SIGNATURES = {
     "ss_engine_set_prepared_ballots": (_i, [_vp, _vp]),
     "ss_engine_set_policies": (_i, [_vp, _vp, _u32, _i]),
     "ss_engine_propose": (_i, [_vp, _u32, _vp, _u64, _vp, C.POINTER(_vp)]),
+    "ss_engine_propose_next": (_i, [_vp, _u32, _vp, _u64, _vp, _vp, C.POINTER(_vp)]),
     "ss_engine_ingest": (_i, [_vp, _vp, _vp, _vp, _vp, _u64]),
     "ss_engine_tick": (_i, [_vp, _vp]),
+    "ss_engine_advance": (_i, [_vp, _vp]),
+    "ss_engine_window_get": (_i, [_vp, C.POINTER(_vp)]),
     "ss_engine_raft_append": (_i, [_vp, _vp]),
     "ss_engine_raft_ingest": (_i, [_vp, _vp, _vp, _vp, _u64]),
     "ss_rs_set_variant": (_i, [_vp, _i]),

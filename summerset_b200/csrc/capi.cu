@@ -980,7 +980,7 @@ int ss_ack_ingest_dev(ss_ctx *ctx, const uint32_t *rec_group, const uint8_t *rec
     if (!rec_group || !rec_slot || !rec_peer || !rec_ballot || !bal_prepared || !inst_bal || !accepting || !planes)
         return set_error(SS_ERR_INVALID_ARG, "null buffer");
     return launch_ack_ingest(ctx, rec_group, rec_slot, rec_peer, rec_ballot, n_records, bal_prepared, inst_bal,
-                             accepting, R, G, planes);
+                             accepting, nullptr, R, G, planes);
 }
 
 int ss_tally_crossword_dev(ss_ctx *ctx, const void *masks, uint32_t mask_bytes, const uint8_t *policy_idx, uint64_t n,

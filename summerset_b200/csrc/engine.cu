@@ -4,9 +4,10 @@
 // all of them together; the host (the Rust shim of INTEGRATION.md, or summerset_b200/engine.py) calls
 //
 //   ss_engine_propose   RSCodeword::from_data + compute_parity + per-peer subset_copy for every group's new instance
-//                       (multipaxos/request.rs:112-221, rspaxos/request.rs:72-142, crossword/request.rs:82-185): the
-//                       RS encode kernel writes the shard planes, one bookkeeping kernel moves the instance to
-//                       Accepting under the group's prepared ballot with an empty ack set
+//   ss_engine_propose_next  (multipaxos/request.rs:112-221, rspaxos/request.rs:72-142, crossword/request.rs:82-185): the
+//                       RS encode kernel writes the shard planes, one bookkeeping kernel moves the instance -- at a given
+//                       window position, or at the group's first Null slot (rspaxos/mod.rs:434-442) -- to Accepting
+//                       under the group's prepared ballot with an empty ack set
 //   ss_engine_ingest    handle_msg_accept_reply's filters over a batch of AcceptReply records
 //                       (multipaxos/messages.rs:377-409, rspaxos/messages.rs:402-437, crossword/messages.rs:489-530)
 //   ss_engine_tick      the commit decision for every Accepting instance and the commit_bar advance, ONE kernel:
@@ -15,9 +16,15 @@
 //                         Crossword   #acks >= majority && coverage_under_faults >= d (crossword/messages.rs:535-542)
 //                       committed |= newly, accepting &= ~newly (a committed instance drops later replies, :394-399),
 //                       commit_bar = committed prefix (multipaxos/durability.rs:161-170)
+//   ss_engine_advance   retire a committed prefix: window_base moves forward (start_slot, multipaxos/snapshot.rs:121-171)
 //   Raft / CRaft        ss_engine_raft_append (leader appends entries in its term), ss_engine_raft_ingest (successful
 //                       AppendEntriesReply: next_slot / match_slot update, raft/messages.rs:243-252), ss_engine_tick
 //                       (commit scan :254-275,295 and last_snap :298-309; CRaft thresholds craft/messages.rs:300-308)
+//
+// Paxos-family window: group g holds the absolute slots [window_base[g], window_base[g] + 64).  Every per-slot array is
+// a ring: absolute slot s lives at position s & 63 (bit s & 63 of the ack planes, accepting and committed; entry
+// g*64 + (s & 63) of inst_bal and policy_idx).  commit_bar and the tick's newly words are window-relative (bit i =
+// slot window_base + i): ring words are rotated right by window_base & 63.  At window_base == 0 both orders coincide.
 //
 // No tally, filter or shard byte is computed on the host, and nothing here is a torch op.
 #include <cstring>
@@ -35,6 +42,8 @@ struct ss_engine {
     uint32_t L = 0, ds = 0;
     // Paxos family
     uint64_t *planes = nullptr, *bal_prepared = nullptr, *inst_bal = nullptr, *accepting = nullptr, *committed = nullptr;
+    uint64_t *window_base = nullptr;        // [G] absolute slot of window position 0
+    bool windowed = false;                  // a base may be non-zero: set by ss_engine_advance / ss_engine_window_get
     uint32_t *commit_bar = nullptr;
     uint8_t *shards = nullptr;
     // Crossword
@@ -61,28 +70,86 @@ static inline uint32_t eng_grid(ss_ctx *ctx, uint64_t items) {
     return static_cast<uint32_t>(ctas);
 }
 
-// ---- propose bookkeeping: the instance at `slot` of every group enters Accepting -------------------------------
+// ring word (bit p = absolute slot with s & 63 == p) <-> window word (bit i = absolute slot base + i), r = base & 63
+__device__ __forceinline__ uint64_t ring_to_window(uint64_t x, uint32_t r) { return (x >> r) | (x << ((64u - r) & 63u)); }
+__device__ __forceinline__ uint64_t window_to_ring(uint64_t x, uint32_t r) { return (x << r) | (x >> ((64u - r) & 63u)); }
+
+// ---- propose bookkeeping: one new instance per group enters Accepting --------------------------------------------
+// slot < 64: at window position `slot`; slot == kProposeNext: at the group's first Null slot (rspaxos/mod.rs:434-442),
+// which a full window does not have -- then slot_out = UINT64_MAX, the status bit is set and the group is left as is.
+constexpr uint32_t kProposeNext = 64;
 __global__ void __launch_bounds__(kEngThreads)
-engine_propose_kernel(uint64_t *__restrict__ planes, uint32_t R, uint64_t G, uint32_t slot, const uint64_t *__restrict__ bal_prepared,
-                      uint64_t *__restrict__ inst_bal, uint64_t *__restrict__ accepting, uint64_t *__restrict__ committed,
-                      uint8_t *__restrict__ policy_idx, const uint8_t *__restrict__ new_policy) {
-    const uint64_t bit = 1ull << slot;
+engine_propose_kernel(uint64_t *__restrict__ planes, uint32_t R, uint64_t G, uint32_t slot, const uint64_t *__restrict__ window_base,
+                      const uint64_t *__restrict__ bal_prepared, uint64_t *__restrict__ inst_bal, uint64_t *__restrict__ accepting,
+                      uint64_t *__restrict__ committed, uint8_t *__restrict__ policy_idx, const uint8_t *__restrict__ new_policy,
+                      uint64_t *__restrict__ slot_out, uint32_t *status) {
+    bool full = false;
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kEngThreads;
     for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kEngThreads + threadIdx.x; g < G; g += stride) {
-        accepting[g] |= bit;                                   // Status::Accepting (request.rs: inst.status = Accepting)
-        committed[g] &= ~bit;                                  // a re-used window slot starts uncommitted
-        inst_bal[g * 64 + slot] = bal_prepared[g];             // inst.bal = bal_prepared
+        const uint64_t base = window_base[g];
+        const uint64_t acc = accepting[g], cm = committed[g];
+        uint32_t rel = slot;
+        if (slot == kProposeNext) {
+            rel = dev::commit_prefix(ring_to_window(acc | cm, static_cast<uint32_t>(base & 63u)));   // first Null position
+            if (rel == 64u) {
+                full = true;
+                if (slot_out != nullptr) slot_out[g] = ~0ull;
+                continue;
+            }
+        }
+        const uint64_t s = base + rel;
+        const uint32_t pos = static_cast<uint32_t>(s & 63u);
+        const uint64_t bit = 1ull << pos;
+        accepting[g] = acc | bit;                              // Status::Accepting (request.rs: inst.status = Accepting)
+        committed[g] = cm & ~bit;                              // a re-used window slot starts uncommitted
+        inst_bal[g * 64 + pos] = bal_prepared[g];              // inst.bal = bal_prepared
         for (uint32_t r = 0; r < R; ++r) planes[static_cast<uint64_t>(r) * G + g] &= ~bit;   // fresh accept_acks
-        if (policy_idx != nullptr) policy_idx[g * 64 + slot] = new_policy != nullptr ? new_policy[g] : 0;
+        if (policy_idx != nullptr) policy_idx[g * 64 + pos] = new_policy != nullptr ? new_policy[g] : 0;
+        if (slot_out != nullptr) slot_out[g] = s;
+    }
+    // one status write per warp, not one per full group
+    const unsigned any = __ballot_sync(__activemask(), full);
+    if (full && (threadIdx.x & 31u) == static_cast<unsigned>(__ffs(static_cast<int>(any)) - 1)) atomicOr(status, SS_DEV_STATUS_WINDOW_FULL);
+}
+
+// ---- retire the committed prefix up to upto[g] (all of it when upto is NULL) ---------------------------------------
+// multipaxos/snapshot.rs:121-171 moves start_slot past the executed prefix.  The retired ring positions are cleared in
+// every per-slot bit word, so that a later proposal there starts with no acks and the tick's prefix does not see them.
+__global__ void __launch_bounds__(kEngThreads)
+engine_advance_kernel(const uint64_t *__restrict__ upto, uint64_t *__restrict__ planes, uint32_t R, uint64_t G,
+                      uint64_t *__restrict__ window_base, uint64_t *__restrict__ accepting, uint64_t *__restrict__ committed,
+                      uint32_t *__restrict__ commit_bar) {
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kEngThreads;
+    for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kEngThreads + threadIdx.x; g < G; g += stride) {
+        const uint64_t base = window_base[g];
+        const uint64_t cm = committed[g];
+        const uint32_t r = static_cast<uint32_t>(base & 63u);
+        // only committed instances can be retired: the prefix of the committed word itself, so a commit_bar left stale
+        // by a re-proposal at a committed position never retires an uncommitted instance
+        const uint32_t bar = dev::commit_prefix(ring_to_window(cm, r));
+        uint64_t k = bar;
+        if (upto != nullptr) {
+            const uint64_t u = upto[g];
+            k = u <= base ? 0ull : (u - base < k ? u - base : k);
+        }
+        if (k == 0ull) continue;
+        const uint64_t keep = window_to_ring(k == 64ull ? 0ull : ~0ull << k, r);
+        committed[g] = cm & keep;
+        accepting[g] &= keep;
+        for (uint32_t q = 0; q < R; ++q) planes[static_cast<uint64_t>(q) * G + g] &= keep;
+        window_base[g] = base + k;
+        commit_bar[g] = bar - static_cast<uint32_t>(k);
     }
 }
 
 // ---- fused tick, threshold protocols: two groups per thread, 128-bit accesses ------------------------------------
-template <int RT>
+// WIN = false: no base can be non-zero yet (the engine never advanced nor handed out window_base), so the ring is the
+// window and the tick skips the 8 B/group load of window_base
+template <int RT, bool WIN>
 __global__ void __launch_bounds__(kEngThreads)
 engine_tick_x2_kernel(const ulonglong2 *__restrict__ planes, uint32_t R, uint64_t G2, uint32_t threshold,
-                      ulonglong2 *__restrict__ accepting, ulonglong2 *__restrict__ committed, uint2 *__restrict__ commit_bar,
-                      ulonglong2 *__restrict__ newly_out) {
+                      const ulonglong2 *__restrict__ window_base, ulonglong2 *__restrict__ accepting,
+                      ulonglong2 *__restrict__ committed, uint2 *__restrict__ commit_bar, ulonglong2 *__restrict__ newly_out) {
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kEngThreads;
     for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kEngThreads + threadIdx.x; g < G2; g += stride) {
         uint64_t a[5] = {0, 0, 0, 0, 0}, b[5] = {0, 0, 0, 0, 0};
@@ -129,14 +196,18 @@ engine_tick_x2_kernel(const ulonglong2 *__restrict__ planes, uint32_t R, uint64_
         cm.x |= newly.x; cm.y |= newly.y;
         committed[g] = cm;
         accepting[g] = make_ulonglong2(acc.x & ~newly.x, acc.y & ~newly.y);
-        commit_bar[g] = make_uint2(dev::commit_prefix(cm.x), dev::commit_prefix(cm.y));
-        if (newly_out != nullptr) newly_out[g] = newly;
+        const ulonglong2 base = WIN ? window_base[g] : make_ulonglong2(0ull, 0ull);
+        const uint32_t rx = static_cast<uint32_t>(base.x & 63u), ry = static_cast<uint32_t>(base.y & 63u);
+        commit_bar[g] = make_uint2(dev::commit_prefix(ring_to_window(cm.x, rx)), dev::commit_prefix(ring_to_window(cm.y, ry)));
+        if (newly_out != nullptr) newly_out[g] = make_ulonglong2(ring_to_window(newly.x, rx), ring_to_window(newly.y, ry));
     }
 }
 
+template <bool WIN>
 __global__ void __launch_bounds__(kEngThreads)
-engine_tick_kernel(const uint64_t *__restrict__ planes, uint32_t R, uint64_t G, uint32_t threshold, uint64_t *__restrict__ accepting,
-                   uint64_t *__restrict__ committed, uint32_t *__restrict__ commit_bar, uint64_t *__restrict__ newly_out) {
+engine_tick_kernel(const uint64_t *__restrict__ planes, uint32_t R, uint64_t G, uint32_t threshold,
+                   const uint64_t *__restrict__ window_base, uint64_t *__restrict__ accepting, uint64_t *__restrict__ committed,
+                   uint32_t *__restrict__ commit_bar, uint64_t *__restrict__ newly_out) {
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kEngThreads;
     for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kEngThreads + threadIdx.x; g < G; g += stride) {
         const uint64_t acc = accepting[g];
@@ -144,17 +215,19 @@ engine_tick_kernel(const uint64_t *__restrict__ planes, uint32_t R, uint64_t G, 
         const uint64_t cm = committed[g] | newly;
         committed[g] = cm;
         accepting[g] = acc & ~newly;
-        commit_bar[g] = dev::commit_prefix(cm);
-        if (newly_out != nullptr) newly_out[g] = newly;
+        const uint32_t r = WIN ? static_cast<uint32_t>(window_base[g] & 63u) : 0u;
+        commit_bar[g] = dev::commit_prefix(ring_to_window(cm, r));
+        if (newly_out != nullptr) newly_out[g] = ring_to_window(newly, r);
     }
 }
 
 // ---- fused tick, Crossword: coverage look-up per Accepting instance ------------------------------------------------
+template <bool WIN>
 __global__ void __launch_bounds__(kEngThreads)
 engine_tick_crossword_kernel(const uint64_t *__restrict__ planes, uint32_t R, uint64_t G, const uint8_t *__restrict__ policy_idx,
                              const uint32_t *__restrict__ lut_bits, uint32_t lut_words, uint32_t n_policies,
-                             uint64_t *__restrict__ accepting, uint64_t *__restrict__ committed, uint32_t *__restrict__ commit_bar,
-                             uint64_t *__restrict__ newly_out) {
+                             const uint64_t *__restrict__ window_base, uint64_t *__restrict__ accepting,
+                             uint64_t *__restrict__ committed, uint32_t *__restrict__ commit_bar, uint64_t *__restrict__ newly_out) {
     extern __shared__ uint32_t lut[];
     for (uint32_t i = threadIdx.x; i < lut_words; i += kEngThreads) lut[i] = lut_bits[i];
     __syncthreads();
@@ -184,8 +257,9 @@ engine_tick_crossword_kernel(const uint64_t *__restrict__ planes, uint32_t R, ui
         const uint64_t cm = committed[g] | newly;
         committed[g] = cm;
         accepting[g] = acc & ~newly;
-        commit_bar[g] = dev::commit_prefix(cm);
-        if (newly_out != nullptr) newly_out[g] = newly;
+        const uint32_t r = WIN ? static_cast<uint32_t>(window_base[g] & 63u) : 0u;
+        commit_bar[g] = dev::commit_prefix(ring_to_window(cm, r));
+        if (newly_out != nullptr) newly_out[g] = ring_to_window(newly, r);
     }
 }
 
@@ -264,7 +338,7 @@ int ss_engine_destroy(ss_engine *e) {
         cudaSetDevice(e->ctx->device);
         cudaStreamSynchronize(e->ctx->stream);
     }
-    void *bufs[] = {e->planes, e->bal_prepared, e->inst_bal, e->accepting, e->committed, e->commit_bar, e->shards, e->policy_idx,
+    void *bufs[] = {e->planes, e->bal_prepared, e->inst_bal, e->accepting, e->committed, e->window_base, e->commit_bar, e->shards, e->policy_idx,
                     e->policies, e->lut_bits, e->match, e->next_slot, e->last_commit, e->log_end, e->curr_term, e->terms,
                     e->last_snap, e->touched};
     for (void *b : bufs)
@@ -327,7 +401,8 @@ int ss_engine_create(ss_ctx *ctx, const ss_engine_config *cfg, uint64_t G, ss_en
         }
     }
     if ((rc = dalloc(&e->planes, size_t(n) * G)) || (rc = dalloc(&e->bal_prepared, G)) || (rc = dalloc(&e->inst_bal, G * 64)) ||
-        (rc = dalloc(&e->accepting, G)) || (rc = dalloc(&e->committed, G)) || (rc = dalloc(&e->commit_bar, G)))
+        (rc = dalloc(&e->accepting, G)) || (rc = dalloc(&e->committed, G)) || (rc = dalloc(&e->window_base, G)) ||
+        (rc = dalloc(&e->commit_bar, G)))
         return fail(rc);
     if (cfg->protocol != SS_PROTO_MULTIPAXOS) {
         if (cfg->data_len == 0) return fail(set_error(SS_ERR_INVALID_ARG, "data_len must be > 0 for an RS-coded protocol"));
@@ -385,18 +460,17 @@ int ss_engine_set_policies(ss_engine *e, const uint32_t *policies_host, uint32_t
                                 e->lut_bits);
 }
 
-int ss_engine_propose(ss_engine *e, uint32_t slot, const uint8_t *payloads, uint64_t payload_stride, const uint8_t *policy,
-                      uint8_t **shard_planes) {
-    if (e == nullptr) return set_error(SS_ERR_INVALID_ARG, "null engine");
-    if (e->planes == nullptr) return set_error(SS_ERR_INVALID_ARG, "not a Paxos-family engine");
-    if (slot >= 64) return set_error(SS_ERR_INVALID_ARG, "slot %u outside the 64-slot window", slot);
+// both propose calls: encode into shard store `store`, then the bookkeeping kernel at window position `slot`
+// (kProposeNext: the first Null slot)
+static int engine_propose(ss_engine *e, uint32_t store, uint32_t slot, const uint8_t *payloads, uint64_t payload_stride,
+                          const uint8_t *policy, uint64_t *slot_out, uint8_t **shard_planes) {
     ss_ctx *ctx = e->ctx;
     SS_TRY(ctx_bind(ctx));
     if (e->cfg.protocol == SS_PROTO_CROSSWORD && e->lut_bits == nullptr)
         return set_error(SS_ERR_INVALID_ARG, "ss_engine_set_policies must be called before proposing");
     if (e->coder != nullptr) {
         if (payloads == nullptr) return set_error(SS_ERR_INVALID_ARG, "null payloads");
-        uint8_t *base = e->shards + uint64_t(slot % e->cfg.keep_slots) * e->T * e->G * e->ds;
+        uint8_t *base = e->shards + uint64_t(store) * e->T * e->G * e->ds;
         // from_data + compute_parity + the per-peer packed buffers of subset_copy: data shards into planes 0..d-1,
         // parity into planes d..T-1 (rspaxos/request.rs:72-77,127-142)
         SS_TRY(ss_rs_encode_uniform_dev(e->coder, payloads, payload_stride, e->cfg.data_len, e->G, base + uint64_t(e->d) * e->G * e->ds,
@@ -405,19 +479,61 @@ int ss_engine_propose(ss_engine *e, uint32_t slot, const uint8_t *payloads, uint
     } else if (shard_planes) {
         *shard_planes = nullptr;                  // MultiPaxos sends the full batch to every peer: nothing to code
     }
-    engine_propose_kernel<<<eng_grid(ctx, e->G), kEngThreads, 0, ctx->stream>>>(e->planes, e->n, e->G, slot, e->bal_prepared, e->inst_bal,
-                                                                             e->accepting, e->committed, e->policy_idx, policy);
+    engine_propose_kernel<<<eng_grid(ctx, e->G), kEngThreads, 0, ctx->stream>>>(e->planes, e->n, e->G, slot, e->window_base,
+                                                                             e->bal_prepared, e->inst_bal, e->accepting, e->committed,
+                                                                             e->policy_idx, policy, slot_out, ctx->dev_status);
     SS_CUDA(cudaGetLastError());
     ctx->launches++;
     return SS_OK;
+}
+
+int ss_engine_propose(ss_engine *e, uint32_t slot, const uint8_t *payloads, uint64_t payload_stride, const uint8_t *policy,
+                      uint8_t **shard_planes) {
+    if (e == nullptr) return set_error(SS_ERR_INVALID_ARG, "null engine");
+    if (e->planes == nullptr) return set_error(SS_ERR_INVALID_ARG, "not a Paxos-family engine");
+    if (slot >= 64) return set_error(SS_ERR_INVALID_ARG, "slot %u outside the 64-slot window", slot);
+    const uint32_t store = e->coder != nullptr ? slot % e->cfg.keep_slots : 0;
+    return engine_propose(e, store, slot, payloads, payload_stride, policy, nullptr, shard_planes);
+}
+
+int ss_engine_propose_next(ss_engine *e, uint32_t store, const uint8_t *payloads, uint64_t payload_stride, const uint8_t *policy,
+                           uint64_t *slot_out, uint8_t **shard_planes) {
+    if (e == nullptr) return set_error(SS_ERR_INVALID_ARG, "null engine");
+    if (e->planes == nullptr) return set_error(SS_ERR_INVALID_ARG, "not a Paxos-family engine");
+    const uint32_t keep = e->cfg.keep_slots ? e->cfg.keep_slots : 1;
+    if (store >= keep) return set_error(SS_ERR_INVALID_ARG, "shard store %u >= keep_slots %u", store, keep);
+    return engine_propose(e, store, kProposeNext, payloads, payload_stride, policy, slot_out, shard_planes);
 }
 
 int ss_engine_ingest(ss_engine *e, const uint32_t *rec_group, const uint8_t *rec_slot, const uint8_t *rec_peer,
                      const uint64_t *rec_ballot, uint64_t n_records) {
     if (e == nullptr) return set_error(SS_ERR_INVALID_ARG, "null engine");
     if (e->planes == nullptr) return set_error(SS_ERR_INVALID_ARG, "not a Paxos-family engine");
-    return ss_ack_ingest_dev(e->ctx, rec_group, rec_slot, rec_peer, rec_ballot, n_records, e->bal_prepared, e->inst_bal, e->accepting,
-                             e->n, e->G, e->planes);
+    if (n_records == 0) return SS_OK;
+    if (!rec_group || !rec_slot || !rec_peer || !rec_ballot) return set_error(SS_ERR_INVALID_ARG, "null buffer");
+    return launch_ack_ingest(e->ctx, rec_group, rec_slot, rec_peer, rec_ballot, n_records, e->bal_prepared, e->inst_bal,
+                             e->accepting, e->windowed ? e->window_base : nullptr, e->n, e->G, e->planes);
+}
+
+int ss_engine_advance(ss_engine *e, const uint64_t *upto) {
+    if (e == nullptr) return set_error(SS_ERR_INVALID_ARG, "null engine");
+    if (e->planes == nullptr) return set_error(SS_ERR_INVALID_ARG, "not a Paxos-family engine");
+    ss_ctx *ctx = e->ctx;
+    SS_TRY(ctx_bind(ctx));
+    e->windowed = true;
+    engine_advance_kernel<<<eng_grid(ctx, e->G), kEngThreads, 0, ctx->stream>>>(upto, e->planes, e->n, e->G, e->window_base,
+                                                                             e->accepting, e->committed, e->commit_bar);
+    SS_CUDA(cudaGetLastError());
+    ctx->launches++;
+    return SS_OK;
+}
+
+int ss_engine_window_get(ss_engine *e, uint64_t **window_base) {
+    if (e == nullptr || window_base == nullptr) return set_error(SS_ERR_INVALID_ARG, "null argument");
+    if (e->planes == nullptr) return set_error(SS_ERR_INVALID_ARG, "not a Paxos-family engine");
+    *window_base = e->window_base;
+    e->windowed = true;                       // the host may install bases through the pointer
+    return SS_OK;
 }
 
 int ss_engine_tick(ss_engine *e, uint64_t *newly) {
@@ -438,22 +554,28 @@ int ss_engine_tick(ss_engine *e, uint64_t *newly) {
     }
     if (e->cfg.protocol == SS_PROTO_CROSSWORD) {
         if (e->lut_bits == nullptr) return set_error(SS_ERR_INVALID_ARG, "ss_engine_set_policies must be called first");
-        engine_tick_crossword_kernel<<<eng_grid(ctx, e->G), kEngThreads, e->lut_words * 4, ctx->stream>>>(
-            e->planes, e->n, e->G, e->policy_idx, e->lut_bits, e->lut_words, e->n_policies, e->accepting, e->committed, e->commit_bar, newly);
+        auto *k = e->windowed ? engine_tick_crossword_kernel<true> : engine_tick_crossword_kernel<false>;
+        k<<<eng_grid(ctx, e->G), kEngThreads, e->lut_words * 4, ctx->stream>>>(e->planes, e->n, e->G, e->policy_idx, e->lut_bits, e->lut_words,
+                                                                             e->n_policies, e->window_base, e->accepting, e->committed,
+                                                                             e->commit_bar, newly);
     } else if ((e->G & 1ull) == 0ull && (newly == nullptr || (reinterpret_cast<uintptr_t>(newly) & 15u) == 0u)) {
         const uint64_t G2 = e->G / 2;
         const uint32_t grid = static_cast<uint32_t>((G2 + kEngThreads - 1) / kEngThreads);
         const ulonglong2 *p2 = reinterpret_cast<const ulonglong2 *>(e->planes);
+        const ulonglong2 *w2 = reinterpret_cast<const ulonglong2 *>(e->window_base);
         ulonglong2 *a2 = reinterpret_cast<ulonglong2 *>(e->accepting), *c2 = reinterpret_cast<ulonglong2 *>(e->committed);
         uint2 *b2 = reinterpret_cast<uint2 *>(e->commit_bar);
         ulonglong2 *n2 = reinterpret_cast<ulonglong2 *>(newly);
-        if (e->n == 5) engine_tick_x2_kernel<5><<<grid, kEngThreads, 0, ctx->stream>>>(p2, e->n, G2, e->threshold, a2, c2, b2, n2);
-        else if (e->n == 3) engine_tick_x2_kernel<3><<<grid, kEngThreads, 0, ctx->stream>>>(p2, e->n, G2, e->threshold, a2, c2, b2, n2);
-        else if (e->n == 7) engine_tick_x2_kernel<7><<<grid, kEngThreads, 0, ctx->stream>>>(p2, e->n, G2, e->threshold, a2, c2, b2, n2);
-        else engine_tick_x2_kernel<0><<<grid, kEngThreads, 0, ctx->stream>>>(p2, e->n, G2, e->threshold, a2, c2, b2, n2);
+        const bool w = e->windowed;
+        auto *k = e->n == 5 ? (w ? engine_tick_x2_kernel<5, true> : engine_tick_x2_kernel<5, false>)
+                : e->n == 3 ? (w ? engine_tick_x2_kernel<3, true> : engine_tick_x2_kernel<3, false>)
+                : e->n == 7 ? (w ? engine_tick_x2_kernel<7, true> : engine_tick_x2_kernel<7, false>)
+                            : (w ? engine_tick_x2_kernel<0, true> : engine_tick_x2_kernel<0, false>);
+        k<<<grid, kEngThreads, 0, ctx->stream>>>(p2, e->n, G2, e->threshold, w2, a2, c2, b2, n2);
     } else {
-        engine_tick_kernel<<<eng_grid(ctx, e->G), kEngThreads, 0, ctx->stream>>>(e->planes, e->n, e->G, e->threshold, e->accepting,
-                                                                              e->committed, e->commit_bar, newly);
+        auto *k = e->windowed ? engine_tick_kernel<true> : engine_tick_kernel<false>;
+        k<<<eng_grid(ctx, e->G), kEngThreads, 0, ctx->stream>>>(e->planes, e->n, e->G, e->threshold, e->window_base, e->accepting,
+                                                             e->committed, e->commit_bar, newly);
     }
     SS_CUDA(cudaGetLastError());
     ctx->launches++;

@@ -170,6 +170,7 @@ int launch_tally_masks(ss_ctx *ctx, const void *masks, uint32_t mask_bytes, uint
 int launch_ack_ingest(ss_ctx *ctx, const uint32_t *rec_group, const uint8_t *rec_slot,
                       const uint8_t *rec_peer, const uint64_t *rec_ballot, uint64_t n_records,
                       const uint64_t *bal_prepared, const uint64_t *inst_bal, const uint64_t *accepting,
+                      const uint64_t *window_base /* NULL: rec_slot is the bit position itself */,
                       uint32_t R, uint64_t G, uint64_t *planes);
 int launch_tally_crossword(ss_ctx *ctx, const void *masks, uint32_t mask_bytes, const uint8_t *policy_idx,
                            uint64_t n, const uint32_t *policies_host, uint32_t n_policies,

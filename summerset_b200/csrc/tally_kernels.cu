@@ -147,12 +147,16 @@ __global__ void __launch_bounds__(kTallyThreads)
 ack_ingest_kernel(const uint32_t *__restrict__ rec_group, const uint8_t *__restrict__ rec_slot,
                   const uint8_t *__restrict__ rec_peer, const uint64_t *__restrict__ rec_ballot, uint64_t n_records,
                   const uint64_t *__restrict__ bal_prepared, const uint64_t *__restrict__ inst_bal,
-                  const uint64_t *__restrict__ accepting, uint32_t R, uint64_t G, uint64_t *planes) {
+                  const uint64_t *__restrict__ accepting, const uint64_t *__restrict__ window_base, uint32_t R, uint64_t G,
+                  uint64_t *planes) {
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kTallyThreads;
     for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kTallyThreads + threadIdx.x; i < n_records; i += stride) {
         const uint64_t g = rec_group[i];
-        const uint32_t s = rec_slot[i], peer = rec_peer[i];
+        uint32_t s = rec_slot[i];
+        const uint32_t peer = rec_peer[i];
         if (g >= G || s >= 64u || peer >= R) continue;            // Bitmap::get -> Err (bitmap.rs:89-97)
+        // window-relative slot -> ring position of absolute slot window_base + s (the engine's ring layout)
+        if (window_base != nullptr) s = static_cast<uint32_t>(__ldg(window_base + g) + s) & 63u;
         const uint64_t ballot = rec_ballot[i];
         if (ballot != __ldg(bal_prepared + g)) continue;          // multipaxos/messages.rs:388
         if (((__ldg(accepting + g) >> s) & 1ull) == 0ull) continue; // :394-399 status != Accepting
@@ -683,12 +687,13 @@ int launch_tally_masks(ss_ctx *ctx, const void *masks, uint32_t mask_bytes, uint
 
 int launch_ack_ingest(ss_ctx *ctx, const uint32_t *rec_group, const uint8_t *rec_slot, const uint8_t *rec_peer,
                       const uint64_t *rec_ballot, uint64_t n_records, const uint64_t *bal_prepared,
-                      const uint64_t *inst_bal, const uint64_t *accepting, uint32_t R, uint64_t G, uint64_t *planes) {
+                      const uint64_t *inst_bal, const uint64_t *accepting, const uint64_t *window_base, uint32_t R, uint64_t G,
+                      uint64_t *planes) {
     SS_TRY(ctx_bind(ctx));
     if (R == 0 || R > 16) return set_error(SS_ERR_INVALID_ARG, "n_replicas must be 1..16, got %u", R);
     if (n_records == 0) return SS_OK;
     ack_ingest_kernel<<<stream_grid(ctx, n_records), kTallyThreads, 0, ctx->stream>>>(
-        rec_group, rec_slot, rec_peer, rec_ballot, n_records, bal_prepared, inst_bal, accepting, R, G, planes);
+        rec_group, rec_slot, rec_peer, rec_ballot, n_records, bal_prepared, inst_bal, accepting, window_base, R, G, planes);
     SS_CUDA(cudaGetLastError());
     ctx->launches++;
     return SS_OK;

@@ -7,8 +7,10 @@ torch tensors (zero-copy views) so tests can read results and install state; it 
 
     LeaderEngine(ctx, protocol, G, population, ...)   protocol in {"multipaxos", "rspaxos", "crossword"}
         propose(slot, payloads[, policy])   multipaxos/request.rs:112-221, rspaxos/request.rs:72-142, crossword/request.rs:82-185
+        propose_next(store, payloads[, policy])   the same at each group's first Null slot (rspaxos/mod.rs:434-442)
         on_accept_replies(records)          handle_msg_accept_reply filters (multipaxos/messages.rs:377-409, ...)
         tick()                              commit decision + commit_bar, one kernel
+        advance([upto])                     retire committed prefixes: window_base moves on (multipaxos/snapshot.rs:121-171)
     RaftEngine(ctx, G, population[, fault_tolerance, craft])
         append(n_new) / on_append_replies(records) / tick()      raft/messages.rs:243-309, craft/messages.rs:300-308
 """
@@ -83,6 +85,17 @@ class LeaderEngine(_EngineBase):
         self.commit_bar = self._tensor(v.commit_bar, (G,), "<i4", torch.int32)
         self.shards = self._tensor(v.shards, (self.keep, self.T, G, self.ds), "|u1", torch.uint8) if v.shards else None
         self.policy_idx = self._tensor(v.policy_idx, (G * 64,), "|u1", torch.uint8)
+        self._window_base = None
+
+    @property
+    def window_base(self) -> torch.Tensor:
+        """int64 [G]: absolute slot of window position 0 per group; the per-slot words above are rings (slot s at bit
+        s & 63).  Fetched on first use: from then on the engine's tick reads the bases (until then they are all 0)."""
+        if self._window_base is None:
+            wb = C.c_void_p()
+            check(self.lib.ss_engine_window_get(self.h, C.byref(wb)))
+            self._window_base = self._tensor(wb.value, (self.G,), "<i8", torch.int64)
+        return self._window_base
 
     def set_prepared_ballots(self, ballots: torch.Tensor) -> None:
         assert ballots.is_cuda and ballots.dtype == torch.int64 and ballots.numel() == self.G
@@ -101,6 +114,24 @@ class LeaderEngine(_EngineBase):
         check(self.lib.ss_engine_propose(self.h, slot, payloads.data_ptr() if payloads is not None else None, stride,
                                          policy.data_ptr() if policy is not None else None, C.byref(base)))
         return self.shards[slot % self.keep] if self.shards is not None else None
+
+    def propose_next(self, store: int, payloads: Optional[torch.Tensor],
+                     policy: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+        """One new instance per group at its first Null slot; shards into shard store `store` (< keep_slots).
+        Returns (slot_out int64 [G]: the absolute slot, or -1 (UINT64_MAX) for a group whose window is full,
+        the store's shard planes [T, G, ds] or None for MultiPaxos)."""
+        base = C.c_void_p()
+        stride = payloads.shape[1] if payloads is not None else 0
+        slot_out = torch.empty(self.G, dtype=torch.int64, device=self.dev)
+        check(self.lib.ss_engine_propose_next(self.h, store, payloads.data_ptr() if payloads is not None else None, stride,
+                                              policy.data_ptr() if policy is not None else None, slot_out.data_ptr(),
+                                              C.byref(base)))
+        return slot_out, (self.shards[store] if self.shards is not None else None)
+
+    def advance(self, upto: Optional[torch.Tensor] = None) -> None:
+        """Retires committed prefixes up to the absolute slots upto (int64 [G]), or all of them when upto is None."""
+        assert upto is None or (upto.is_cuda and upto.dtype == torch.int64 and upto.numel() == self.G)
+        check(self.lib.ss_engine_advance(self.h, upto.data_ptr() if upto is not None else None))
 
     def on_accept_replies(self, rec_group: torch.Tensor, rec_slot: torch.Tensor, rec_peer: torch.Tensor, rec_ballot: torch.Tensor) -> None:
         assert rec_group.dtype == torch.int32 and rec_slot.dtype == torch.uint8 and rec_peer.dtype == torch.uint8 and rec_ballot.dtype == torch.int64
