@@ -42,6 +42,15 @@ __device__ __forceinline__ uint4 ldg128(const void *p) {
     return r;
 }
 
+// the same load with an L2 prefetch-size hint: the L2 fetches the whole 256-byte block around the address from DRAM
+__device__ __forceinline__ uint4 ldg128_pf256(const void *p) {
+    uint4 r;
+    asm volatile("ld.global.nc.L2::256B.v4.u32 {%0,%1,%2,%3}, [%4];"
+                 : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
+                 : "l"(p));
+    return r;
+}
+
 // streaming 128-bit store (written once, not re-read by this kernel)
 __device__ __forceinline__ void stg128_cs(void *p, const uint4 &v) {
     asm volatile("st.global.cs.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z),

@@ -24,7 +24,11 @@
 //       rs32_encode_row_kernel            uniform codewords up to 256 columns, 16-byte-aligned stride: a CTA walks
 //                                         codewords, thread = column, kernel-uniform funnel, masked tail handled by
 //                                         whichever warp has the last column block this iteration (rotating), the
-//                                         fused tally as a coalesced prologue, optional stores into peer GPUs
+//                                         fused tally (after the codeword when the planes are local, else as a
+//                                         coalesced prologue), optional stores into peer GPUs
+//       rs32_accept_bulk_kernel           the same geometry when the parity goes to local planes (the accept step):
+//                                         payload rows staged in shared memory by bulk async copies, parity rows
+//                                         written back with bulk stores, tally by a warp of its own
 //       rs32_encode_uniform_kernel        any uniform geometry: flat thread <-> column index, general masked loads
 //       rs32_encode_ragged_kernel         ragged batches: a warp per codeword, two columns per lane on long ones
 //       rs32_crossword_distribute_kernel  ragged encode + per-replica shard placement (config 4)
@@ -171,6 +175,7 @@ struct Enc32Row {
     uint32_t chunk;           // 0: codewords g = blockIdx.x + i*gridDim.x ; else CTA b owns [b*chunk, (b+1)*chunk)
     uint32_t st_mode;         // cache operator of the plane stores in replicate mode (tuning)
     uint32_t rotate;          // 1: rotate the warp -> column-block assignment per codeword (default)
+    uint32_t tally_last;      // 1: the fused tally runs after the CTA's encode loop instead of before it
     const uint64_t *planes;   // fused tally (nullptr: none); G == n
     uint32_t R, threshold;
     uint64_t *committed;
@@ -197,27 +202,28 @@ __device__ __forceinline__ void rs32_word_fast(uint32_t a, uint32_t b, uint32_t 
 
 // one column of the row kernel.  MASKED: this warp owns the codeword's last column(s): inputs past data_len
 // are zeroed, outputs past L are zeroed, and a second aligned load is issued only when it holds a valid byte.
-template <bool EMIT, bool MASKED>
+template <bool EMIT, bool MASKED, bool PF = false>
 __device__ __forceinline__ void rs32_row_column(const uint8_t *__restrict__ src, uint8_t *const (&out)[5],
                                                 uint32_t k, uint32_t o1, uint32_t o2,
                                                 uint32_t s0, uint32_t s1, uint32_t s2, int nva, int nvb, int nvc,
                                                 int onv, uint32_t st_mode = 0u) {
     // `src` is the 16-byte-aligned address at or below the payload (payload = src + s0); o1/o2 are aligned
     // offsets from src.  Loads first (pairs adjacent so the second one hits the sectors the first just
-    // brought into L1), then the byte funnels.
-    const uint4 a0 = dev::ldg128(src + k);
+    // brought into L1), then the byte funnels.  PF: the loads carry the L2 256-byte prefetch hint.
+    auto ldg = [](const uint8_t *q) { return PF ? dev::ldg128_pf256(q) : dev::ldg128(q); };
+    const uint4 a0 = ldg(src + k);
     // the second-load registers start as zeros, never as a copy of the first load: a copy would be issued right
     // behind the load and stall every later load of this column until that one has landed
     uint4 a1 = make_uint4(0u, 0u, 0u, 0u);
-    if (s0 != 0u && (!MASKED || static_cast<int>(s0) + nva > 16)) a1 = dev::ldg128(src + k + 16u);
+    if (s0 != 0u && (!MASKED || static_cast<int>(s0) + nva > 16)) a1 = ldg(src + k + 16u);
     uint4 b0 = make_uint4(0u, 0u, 0u, 0u);
-    if (!MASKED || nvb > 0) b0 = dev::ldg128(src + o1);   // a window entirely in the zero padding is never read
+    if (!MASKED || nvb > 0) b0 = ldg(src + o1);   // a window entirely in the zero padding is never read
     uint4 b1 = make_uint4(0u, 0u, 0u, 0u);
-    if (s1 != 0u && (!MASKED || static_cast<int>(s1) + nvb > 16)) b1 = dev::ldg128(src + o1 + 16u);
+    if (s1 != 0u && (!MASKED || static_cast<int>(s1) + nvb > 16)) b1 = ldg(src + o1 + 16u);
     uint4 c0 = make_uint4(0u, 0u, 0u, 0u);
-    if (!MASKED || nvc > 0) c0 = dev::ldg128(src + o2);
+    if (!MASKED || nvc > 0) c0 = ldg(src + o2);
     uint4 c1 = make_uint4(0u, 0u, 0u, 0u);
-    if (s2 != 0u && (!MASKED || static_cast<int>(s2) + nvc > 16)) c1 = dev::ldg128(src + o2 + 16u);
+    if (s2 != 0u && (!MASKED || static_cast<int>(s2) + nvc > 16)) c1 = ldg(src + o2 + 16u);
     uint4 a = s0 != 0u ? funnel16(a0, a1, s0) : a0;
     uint4 b = s1 != 0u ? funnel16(b0, b1, s1) : b0;
     uint4 c = s2 != 0u ? funnel16(c0, c1, s2) : c0;
@@ -287,7 +293,7 @@ __device__ __forceinline__ void rs32_row_pair(const uint8_t *__restrict__ src, u
     }
 }
 
-template <bool EMIT, int MAXT, int MINB, bool SEG = false>
+template <bool EMIT, int MAXT, int MINB, bool SEG = false, bool PF = false>
 __global__ void __launch_bounds__(MAXT, MINB) rs32_encode_row_kernel(const __grid_constant__ Enc32Row P) {
     const uint32_t lane = threadIdx.x & 31u, wid = threadIdx.x >> 5, nblk = blockDim.x >> 5;
     const uint32_t s1 = P.s1, s2 = P.s2;
@@ -296,8 +302,10 @@ __global__ void __launch_bounds__(MAXT, MINB) rs32_encode_row_kernel(const __gri
     // replicate mode only: the ack planes tallied below are written by peer GPUs; wait for their step flags
     if constexpr (EMIT) dev::cta_wait_flags(P.wait);
 
-    // ---- fused tally: this CTA's contiguous slice of groups, coalesced (one pass, before the encode loop) ----
-    if (P.planes != nullptr) {
+    // ---- fused tally: this CTA's contiguous slice of groups, coalesced (one pass, before the encode loop, or after
+    //      it when tally_last is set) ----
+    auto tally = [&] {
+        if (P.planes == nullptr) return;
         const uint32_t per = (P.n + gridDim.x - 1) / gridDim.x;
         const uint32_t lo = blockIdx.x * per;
         const uint32_t hi = lo + per < P.n ? lo + per : P.n;
@@ -306,7 +314,8 @@ __global__ void __launch_bounds__(MAXT, MINB) rs32_encode_row_kernel(const __gri
             P.committed[g] = w;
             if (P.commit_bar != nullptr) P.commit_bar[g] = dev::commit_prefix(w);
         }
-    }
+    };
+    if (!P.tally_last) tally();
 
     // The CTA's warps work on the same codeword, each on one 32-column block.  The block that holds the codeword's
     // last column runs the (longer) masked variant; with a fixed warp->block assignment that warp is the CTA's
@@ -360,14 +369,192 @@ __global__ void __launch_bounds__(MAXT, MINB) rs32_encode_row_kernel(const __gri
                                  EMIT ? P.plane[2] + so : nullptr, P.plane[3] + so, P.plane[4] + so};
         const uint8_t *src = P.data + static_cast<uint64_t>(g) * P.data_stride;
         if (!masked) {
-            rs32_row_column<EMIT, false>(src, out, k, o1, o2, 0u, s1, s2, 16, 16, 16, 16, P.st_mode);
+            rs32_row_column<EMIT, false, PF>(src, out, k, o1, o2, 0u, s1, s2, 16, 16, 16, 16, P.st_mode);
         } else {
-            rs32_row_column<EMIT, true>(src, out, k, o1, o2, 0u, s1, s2, clamp16(static_cast<int64_t>(P.len) - k),
+            rs32_row_column<EMIT, true, PF>(src, out, k, o1, o2, 0u, s1, s2, clamp16(static_cast<int64_t>(P.len) - k),
                                         clamp16(static_cast<int64_t>(P.len) - P.L - k),
                                         clamp16(static_cast<int64_t>(P.len) - 2ll * P.L - k),
                                         clamp16(static_cast<int64_t>(P.L) - k), P.st_mode);
         }
     }
+    if (P.tally_last) tally();
+}
+
+// ------------------------------------------------------------------------------------------------
+// RS(3,2) accept step fed by bulk async copies (the BASELINE config-3 hot kernel)
+// ------------------------------------------------------------------------------------------------
+// The row kernel above has every thread issue its own five 128-bit loads per column, wait for them, compute and store:
+// all of its memory-level parallelism comes from resident warps, each with one load batch in flight.  This kernel
+// moves whole rows instead.  A persistent CTA owns a contiguous range of codewords (sequential DRAM streams);
+//   * thread 0 streams payload rows, round_up(len,16) bytes each, into a ring of `nin` shared-memory stages with
+//     cp.async.bulk (one mbarrier per stage counts the bytes in), keeping up to nin rows per CTA in flight;
+//   * the encode warps (one thread per 16-byte column) read the three shards from the stage -- aligned 16-byte reads
+//     and the kernel-uniform byte funnel -- apply the row kernel's masking, and write both parity vectors into one of
+//     kOut output stages;
+//   * after a proxy fence and a barrier of the encode warps, thread 0 writes the two parity rows out with bulk stores
+//     (vpc*16 bytes each) and refills the stage just consumed with the payload row nin codewords ahead;
+//   * the last warp tallies the CTA's groups while the encode pipeline runs.
+// One barrier per codeword is the whole synchronisation: an input stage is refilled only after every encode thread has
+// passed the barrier that follows its reads of it, and an output stage is written again only after thread 0 has seen,
+// before an earlier barrier, that the bulk store that read it last has finished reading (cp.async.bulk.wait_group.read).
+struct Enc32Bulk {
+    const uint8_t *data;
+    uint64_t data_stride;
+    uint8_t *par0, *par1;       // parity planes 0 and 1 (16-byte aligned, padded shard slots)
+    uint64_t shard_stride;
+    uint32_t n, len, L, vpc;
+    uint32_t fast_cols;         // columns [0, fast_cols) need no masking
+    uint32_t s1, s2;            // (L & 15), (2L & 15): misalignment of shards 1 and 2
+    uint32_t chunk;             // CTA b tallies groups [b*chunk, min(n, (b+1)*chunk)) (and encodes them if !interleave)
+    uint32_t interleave;        // 1: CTA b encodes codewords b, b + gridDim.x, ...
+    uint32_t in_bytes;         // bytes copied per payload row: round_up(len, 16)
+    uint32_t in_pitch;          // bytes per input stage: in_bytes + room for the funnel's reads past the row, 128-aligned
+    uint32_t nin;               // input stages
+    const uint64_t *planes;     // fused tally (nullptr: none); G == n
+    uint32_t R, threshold;
+    uint64_t *committed;
+    uint32_t *commit_bar;
+};
+
+constexpr uint32_t kBulkOut = 4;          // output stages: a bulk store has two codewords' time to read its stage
+constexpr uint32_t kBulkHeader = 128;     // the input stages' mbarriers, ahead of the stages
+
+namespace bulk {
+__device__ __forceinline__ uint32_t smem_addr(const void *p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n"
+        "WAIT_%=:\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+        "@!p bra WAIT_%=;\n}" ::"r"(bar), "r"(parity) : "memory");
+}
+// global -> shared, completion counted in bytes on the mbarrier
+__device__ __forceinline__ void load_row(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+}
+// shared -> global, tracked by bulk groups
+__device__ __forceinline__ void store_row(void *dst, uint32_t src, uint32_t bytes) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void wait_group_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// generic-proxy writes to shared memory become visible to the bulk copies issued after the next barrier
+__device__ __forceinline__ void fence_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void encode_barrier(uint32_t nthreads) { asm volatile("bar.sync 1, %0;" ::"r"(nthreads) : "memory"); }
+}  // namespace bulk
+
+__global__ void __launch_bounds__(288) rs32_accept_bulk_kernel(const __grid_constant__ Enc32Bulk P) {
+    extern __shared__ __align__(128) uint8_t s_bulk[];
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, wid = tid >> 5;
+    const uint32_t nenc = blockDim.x - 32u;             // encode threads; the last warp tallies
+    const uint32_t lo = blockIdx.x * P.chunk;
+    const uint32_t hi = lo + P.chunk < P.n ? lo + P.chunk : P.n;
+    // codewords encoded here: lo + i*step (interleaved: step = gridDim.x from blockIdx.x; contiguous: step 1 from lo)
+    const uint32_t first = P.interleave ? blockIdx.x : lo;
+    const uint32_t step = P.interleave ? gridDim.x : 1u;
+    const uint32_t cnt = P.interleave ? (P.n - blockIdx.x + gridDim.x - 1u) / gridDim.x : hi - lo;
+    const uint32_t bar0 = bulk::smem_addr(s_bulk);
+    uint8_t *const in_base = s_bulk + kBulkHeader;
+    uint8_t *const out_base = in_base + static_cast<uint64_t>(P.nin) * P.in_pitch;
+    const uint32_t out_pitch = 2u * P.vpc * 16u;        // parity row 0, then parity row 1
+
+    if (tid == 0) {
+        for (uint32_t s = 0; s < P.nin; ++s) bulk::mbar_init(bar0 + 8u * s, 1u);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    if (wid * 32u == nenc) {
+        // ---- tally warp: this CTA's groups, coalesced, alongside the encode pipeline ----
+        if (P.planes == nullptr) return;
+        for (uint32_t g = lo + lane; g < hi; g += 32u) {
+            const uint64_t w = dev::tally_word(P.planes, P.R, P.n, g, P.threshold);
+            P.committed[g] = w;
+            if (P.commit_bar != nullptr) P.commit_bar[g] = dev::commit_prefix(w);
+        }
+        return;
+    }
+
+    auto load = [&](uint32_t dst, uint32_t g, uint32_t bar) {
+        bulk::mbar_expect_tx(bar, P.in_bytes);
+        bulk::load_row(dst, P.data + static_cast<uint64_t>(g) * P.data_stride, P.in_bytes, bar);
+    };
+    auto store = [&](uint8_t *dst, uint32_t src) { bulk::store_row(dst, src, P.vpc * 16u); };
+
+    // ---- prologue: fill the ring ----
+    if (tid == 0) {
+        const uint32_t pre = cnt < P.nin ? cnt : P.nin;
+        for (uint32_t i = 0; i < pre; ++i)
+            load(bulk::smem_addr(in_base + static_cast<uint64_t>(i) * P.in_pitch), first + i * step, bar0 + 8u * i);
+    }
+
+    auto clamp16 = [](int64_t r) { return r > 16 ? 16 : (r < 0 ? 0 : static_cast<int>(r)); };
+    const uint32_t v = tid, k = v * 16u;
+    const bool active = v < P.vpc;
+    const bool masked = v >= P.fast_cols;
+    const uint32_t s1 = P.s1, s2 = P.s2;
+    const uint32_t o1 = P.L + k - s1, o2 = 2u * P.L + k - s2;   // aligned in-row offsets of the shard 1 / 2 windows
+    const int nva = clamp16(static_cast<int64_t>(P.len) - k);
+    const int nvb = clamp16(static_cast<int64_t>(P.len) - P.L - k);
+    const int nvc = clamp16(static_cast<int64_t>(P.len) - 2ll * P.L - k);
+    const int onv = clamp16(static_cast<int64_t>(P.L) - k);
+    uint32_t s = 0, phase = 0, o = 0;
+#pragma unroll 1
+    for (uint32_t i = 0; i < cnt; ++i) {
+        bulk::mbar_wait(bar0 + 8u * s, phase);
+        const uint8_t *in = in_base + static_cast<uint64_t>(s) * P.in_pitch;
+        uint8_t *out = out_base + static_cast<uint64_t>(o) * out_pitch;
+        if (active) {
+            const uint4 a0 = *reinterpret_cast<const uint4 *>(in + k);
+            const uint4 b0 = *reinterpret_cast<const uint4 *>(in + o1);
+            const uint4 c0 = *reinterpret_cast<const uint4 *>(in + o2);
+            uint4 b = b0, c = c0;
+            if (s1 != 0u) b = funnel16(b0, *reinterpret_cast<const uint4 *>(in + o1 + 16u), s1);
+            if (s2 != 0u) c = funnel16(c0, *reinterpret_cast<const uint4 *>(in + o2 + 16u), s2);
+            uint4 a = a0;
+            if (masked) {
+                a = keep_bytes(a, nva);
+                b = keep_bytes(b, nvb);
+                c = keep_bytes(c, nvc);
+            }
+            uint4 p0, p1;
+            rs32_word_fast(a.x, b.x, c.x, p0.x, p1.x);
+            rs32_word_fast(a.y, b.y, c.y, p0.y, p1.y);
+            rs32_word_fast(a.z, b.z, c.z, p0.z, p1.z);
+            rs32_word_fast(a.w, b.w, c.w, p0.w, p1.w);
+            if (masked) {
+                p0 = keep_bytes(p0, onv);
+                p1 = keep_bytes(p1, onv);
+            }
+            *reinterpret_cast<uint4 *>(out + k) = p0;
+            *reinterpret_cast<uint4 *>(out + P.vpc * 16u + k) = p1;
+        }
+        bulk::fence_async_shared();
+        // thread 0: the bulk store that last read the output stage of codeword i + 1 has finished reading it
+        if (tid == 0) bulk::wait_group_read<kBulkOut - 2>();
+        bulk::encode_barrier(nenc);
+        if (tid == 0) {
+            const uint64_t so = static_cast<uint64_t>(first + i * step) * P.shard_stride;
+            const uint32_t src = bulk::smem_addr(out);
+            store(P.par0 + so, src);
+            store(P.par1 + so, src + P.vpc * 16u);
+            bulk::commit_group();
+            // every encode thread is past its reads of stage s: refill it
+            if (i + P.nin < cnt) load(bulk::smem_addr(in), first + (i + P.nin) * step, bar0 + 8u * s);
+        }
+        if (++s == P.nin) { s = 0; phase ^= 1u; }
+        if (++o == kBulkOut) o = 0;
+    }
+    if (tid == 0) bulk::wait_group_all();
 }
 
 struct EncRagged {
@@ -1398,13 +1585,60 @@ int launch_rs_encode(ss_rs_coder *coder, const EncGeom &g, const TallyArgs *tall
                 Rw.committed = tally->committed; Rw.commit_bar = tally->commit_bar;
             }
             Rw.wait = g.wait;
+            // The accept step proper (parity to local planes, no replication) on the bulk-copy kernel: variant bit 18
+            // selects it.  It is not the default: on an H100 it measured 2-3 % slower than the row kernel (DESIGN.md 3.1).
+            const uint32_t in_bytes = (len + 15u) & ~15u;
+            if (vpc <= 256u && !Rw.emit_data && ((coder->variant >> 18) & 1) && g.data_stride >= in_bytes) {
+                int smem_sm = 0, smem_blk = 0, smem_rsv = 0;
+                SS_CUDA(cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, ctx->device));
+                SS_CUDA(cudaDeviceGetAttribute(&smem_blk, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
+                SS_CUDA(cudaDeviceGetAttribute(&smem_rsv, cudaDevAttrReservedSharedMemoryPerBlock, ctx->device));
+                Enc32Bulk B;
+                B.data = g.data; B.data_stride = g.data_stride; B.par0 = Rw.plane[3]; B.par1 = Rw.plane[4];
+                B.shard_stride = g.shard_stride; B.n = Rw.n; B.len = len; B.L = L; B.vpc = vpc;
+                B.fast_cols = Rw.fast_cols; B.s1 = Rw.s1; B.s2 = Rw.s2;
+                B.in_bytes = in_bytes;
+                B.in_pitch = (in_bytes + 48u + 127u) & ~127u;
+                B.planes = Rw.planes; B.R = Rw.R; B.threshold = Rw.threshold; B.committed = Rw.committed;
+                B.commit_bar = Rw.commit_bar;
+                // Resident CTAs per SM (variant bits 19-20, tuning): 4 by default.  The SM's shared memory is split
+                // evenly between them; each CTA keeps kBulkOut output stages and as many input stages as fit, at most
+                // 8 -- at cfg3 (4096 B rows) that is 8 stages, up to 4 x 7 x 4 KB = 112 KB of payload in flight per SM.
+                static const uint32_t kCtasPerSm[4] = {4, 2, 3, 6};
+                const uint32_t out_bytes = kBulkOut * 2u * vpc * 16u;
+                uint32_t cps = kCtasPerSm[(coder->variant >> 19) & 3], nin = 0;
+                for (; cps >= 1; --cps) {
+                    int64_t room = static_cast<int64_t>(smem_sm) / cps - smem_rsv;
+                    if (room > smem_blk) room = smem_blk;
+                    room -= kBulkHeader + out_bytes;
+                    nin = room > 0 ? static_cast<uint32_t>(room / B.in_pitch) : 0u;
+                    if (nin > 8u) nin = 8u;
+                    if (nin >= 2u) break;
+                }
+                if (nin < 2u) return set_error(SS_ERR_UNSUPPORTED, "accept step: no room for two %u-byte stages", B.in_pitch);
+                B.nin = nin;
+                uint64_t ctas = static_cast<uint64_t>(ctx->sm_count) * cps;
+                if (ctas > g.n) ctas = g.n;
+                B.chunk = static_cast<uint32_t>((g.n + ctas - 1) / ctas);
+                ctas = (g.n + B.chunk - 1) / B.chunk;
+                B.interleave = ((coder->variant >> 21) & 1) ? 1u : 0u;       // bit 21 (tuning): interleaved codewords
+                const uint32_t smem = kBulkHeader + nin * B.in_pitch + out_bytes;
+                SS_CUDA(cudaFuncSetAttribute(rs32_accept_bulk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             static_cast<int>(smem)));
+                const uint32_t threads = ((vpc + 31u) & ~31u) + 32u;      // a thread per column + the tally warp
+                rs32_accept_bulk_kernel<<<static_cast<uint32_t>(ctas), threads, smem, st>>>(B);
+                coder->last_kernel = B.planes ? "rs32_accept_bulk_kernel+tally" : "rs32_accept_bulk_kernel";
+                SS_CUDA(cudaGetLastError());
+                ctx->launches++;
+                return SS_OK;
+            }
             const uint32_t threads = vpc > 256u ? 256u : ((vpc + 31u) & ~31u);
             if (vpc > 256u) {
                 // wide codewords: (codeword, 256-column segment) work items
                 const uint64_t items = g.n * ((vpc + 255u) / 256u);
                 uint64_t ctas = static_cast<uint64_t>(ctx->sm_count) * 8ull * 16ull;
                 if (ctas > items) ctas = items;
-                Rw.chunk = 0; Rw.st_mode = static_cast<uint32_t>((coder->variant >> 8) & 3); Rw.rotate = 0;
+                Rw.chunk = 0; Rw.st_mode = static_cast<uint32_t>((coder->variant >> 8) & 3); Rw.rotate = 0; Rw.tally_last = 0;
                 if (Rw.emit_data) rs32_encode_row_kernel<true, 256, 4, true><<<static_cast<uint32_t>(ctas), 256, 0, st>>>(Rw);
                 else rs32_encode_row_kernel<false, 256, 4, true><<<static_cast<uint32_t>(ctas), 256, 0, st>>>(Rw);
                 coder->last_kernel = Rw.planes ? "rs32_encode_row_kernel<segmented>+tally" : "rs32_encode_row_kernel<segmented>";
@@ -1416,18 +1650,24 @@ int launch_rs_encode(ss_rs_coder *coder, const EncGeom &g, const TallyArgs *tall
             uint32_t per_sm = 2048u / threads; if (per_sm > 32u) per_sm = 32u;
             const int vr = coder->variant & 15, vchunk = (coder->variant >> 4) & 1, vw = (coder->variant >> 5) & 7;
             static const uint64_t kWaves[8] = {64, 1, 32, 4, 16, 256, 128, 8};   // [0] = default, rest: tuning
-            const uint64_t waves = kWaves[vw];
+            // Local planes (the accept step): by default a CTA per codeword.  The block scheduler then hands codewords
+            // out in order, so the whole GPU reads and writes one narrow, advancing window of memory; on an H100 that
+            // measured 2.6 % faster than 64 or 256 waves of CTAs striding over the batch (DESIGN.md 3.1).
+            const uint64_t waves = (vw == 0 && !Rw.emit_data) ? (1ull << 32) : kWaves[vw];
             uint64_t ctas = static_cast<uint64_t>(ctx->sm_count) * per_sm * waves;
             if (ctas > g.n) ctas = g.n;
+            if (ctas > 0x7fffffffull) ctas = 0x7fffffffull;
             Rw.chunk = 0;
             Rw.st_mode = static_cast<uint32_t>((coder->variant >> 8) & 3);
             Rw.rotate = ((coder->variant >> 10) & 1) ? 0u : 1u;
+            // local planes: the tally goes after the CTA's codeword, so its first loads are the payload's
+            Rw.tally_last = Rw.emit_data ? 0u : 1u;
             if (vchunk) { Rw.chunk = static_cast<uint32_t>((g.n + ctas - 1) / ctas); ctas = (g.n + Rw.chunk - 1) / Rw.chunk; }
             const uint32_t grid = static_cast<uint32_t>(ctas);
             // register budget variants (tuning knob ss_rs_set_variant): 0/2 = 40 regs, 3 = 32 regs, 4 = unconstrained
             // Register budget: 40/thread (12 CTAs of <= 128 threads per SM; the kernel needs ~47 unconstrained and fits
-            // 40 without spilling) and 64 waves of CTAs by default.  The other budgets and wave counts stay selectable
-            // for tuning.
+            // 40 without spilling); a CTA per codeword for local planes, 64 waves of CTAs otherwise.  The other budgets and
+            // wave counts stay selectable for tuning.
             if (threads > 128) {
                 if (Rw.emit_data) rs32_encode_row_kernel<true, 256, 4><<<grid, threads, 0, st>>>(Rw);
                 else rs32_encode_row_kernel<false, 256, 4><<<grid, threads, 0, st>>>(Rw);
@@ -1435,7 +1675,7 @@ int launch_rs_encode(ss_rs_coder *coder, const EncGeom &g, const TallyArgs *tall
             else if (vr == 3) rs32_encode_row_kernel<false, 128, 16><<<grid, threads, 0, st>>>(Rw);   // 32 regs
             else if (vr == 6) rs32_encode_row_kernel<false, 128, 8><<<grid, threads, 0, st>>>(Rw);    // 64 regs cap
             else if (vr == 7) rs32_encode_row_kernel<false, 128, 9><<<grid, threads, 0, st>>>(Rw);    // 56 regs cap
-            else rs32_encode_row_kernel<false, 128, 12><<<grid, threads, 0, st>>>(Rw);                // 40 regs
+            else rs32_encode_row_kernel<false, 128, 12, false, true><<<grid, threads, 0, st>>>(Rw);    // 40 regs, L2 prefetch
             coder->last_kernel = Rw.planes ? "rs32_encode_row_kernel+tally" : "rs32_encode_row_kernel";
             SS_CUDA(cudaGetLastError());
             ctx->launches++;
