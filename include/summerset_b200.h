@@ -324,7 +324,7 @@ int ss_event_record(ss_ctx *ctx, void *event);
 int ss_event_wait(ss_ctx *ctx, void *event);
 /* reads (and clears) the context's device status word; synchronises the context's stream */
 #define SS_DEV_STATUS_FLAG_TIMEOUT 1u
-#define SS_DEV_STATUS_FRAME_OVERFLOW 4u   /* ss_frame_accept_pack_dev: a frame did not fit frame_stride */
+#define SS_DEV_STATUS_FRAME_OVERFLOW 4u   /* ss_frame_accept_pack_dev / _ragged_dev: a frame did not fit its room */
 int ss_ctx_device_status(ss_ctx *ctx, uint32_t *status);
 
 /* Fused encode + tally + REPLICATE (the multi-GPU accept step): as ss_accept_step_fused_dev, but shard j of the
@@ -418,6 +418,20 @@ int ss_frame_accept_pack_dev(ss_ctx *ctx, const ss_frame_spec *spec, const uint8
                              uint64_t shard_stride, const uint32_t *policies, uint32_t n_policies,
                              const uint8_t *policy_idx, uint32_t peer, const uint64_t *slot, const uint64_t *ballot,
                              uint64_t n, uint8_t *out, uint64_t frame_stride, uint64_t *frame_off, uint32_t *frame_len);
+/* The same frames / records for RAGGED codewords (spec->data_len is ignored): frame g is what the packer above writes
+ * for a codeword of data_len[g] bytes whose shard j sits at shard_planes + j*plane_stride + shard_off[g] -- the store
+ * ss_engine_propose_ragged fills -- and its RSCodeword header carries that data_len and shard_len = ceil(data_len/d)
+ * (rscoding.rs:43-72,177-199).  No frame is written for data_len[g] == 0 or slot[g] == UINT64_MAX (frame_len 0), so
+ * that call's slot_out / shard_off feed this one directly.  Packed output: frame g's region is round_up(pad + len, 16)
+ * bytes (pad: the 16-byte alignment of its first carried shard, as above); the regions follow each other in group
+ * order from out (16-byte aligned), frame_off[g] = the frame's start, *total (device u64, may be NULL) = the bytes the
+ * whole batch needs.  A frame whose region ends past out_capacity is not written: frame_len 0 and
+ * SS_DEV_STATUS_FRAME_OVERFLOW. */
+int ss_frame_accept_pack_ragged_dev(ss_ctx *ctx, const ss_frame_spec *spec, const uint8_t *shard_planes, uint64_t plane_stride,
+                                    const uint64_t *shard_off, const uint32_t *data_len, const uint32_t *policies,
+                                    uint32_t n_policies, const uint8_t *policy_idx, uint32_t peer, const uint64_t *slot,
+                                    const uint64_t *ballot, uint64_t n, uint8_t *out, uint64_t out_capacity,
+                                    uint64_t *frame_off, uint32_t *frame_len, uint64_t *total);
 
 /* AcceptReply frames -> ack records.  buf holds frames as read off the peers' connections (8-byte big-endian length +
  * body each); frame i starts at frame_off[i], came from replica frame_peer[i] of group frame_group[i].  A well-formed
@@ -550,6 +564,27 @@ int ss_engine_propose(ss_engine *engine, uint32_t slot, const uint8_t *payloads,
 #define SS_DEV_STATUS_WINDOW_FULL 8u
 int ss_engine_propose_next(ss_engine *engine, uint32_t store, const uint8_t *payloads, uint64_t payload_stride,
                            const uint8_t *policy, uint64_t *slot_out, uint8_t **shard_planes);
+/* Ragged proposals (RSPaxos / Crossword engines; others return SS_ERR_INVALID_ARG): group g's request batch is
+ * arena[data_off[g] .. +data_len[g]), of any length, as ExternalApi::get_req_batch drains it (server/external.rs:323-345)
+ * and handle_req_batch codes it (rspaxos/request.rs:72, crossword/request.rs:82; L_g = ceil(data_len[g]/d),
+ * rscoding.rs:177-199).  data_len[g] == 0: the group has nothing to propose -- slot_out[g] = UINT64_MAX, no status bit,
+ * the group is untouched.  A group with a batch proposes at its first Null slot as ss_engine_propose_next does (a full
+ * window: slot_out UINT64_MAX, SS_DEV_STATUS_WINDOW_FULL, no room taken in the store).
+ * Store: CALLER-owned, T planes at shards + j*plane_stride (plane_stride a multiple of 32, shards 16-byte aligned).
+ * Every proposing group takes a slot of SS_CW_SLOT_PITCH(L_g) bytes in each plane; shard_off[g] (device [G]) = the
+ * exclusive prefix sum of those pitches in group order, computed on the device (UINT64_MAX: the group did not propose);
+ * *need (device u64, may be NULL) = the total pitch the batch asked for.  A group whose slot would end past plane_stride
+ * is not proposed (slot_out UINT64_MAX, SS_DEV_STATUS_STORE_FULL, group unchanged); the offsets are monotone, so the
+ * groups that fit are a prefix of the proposing groups.  After the call plane j holds shard j of every proposing group
+ * at shard_off[g], zero-padded to round_up(L_g,16) (bytes from there to the pitch are not written) -- one launch of the
+ * ragged encoder (ss_rs_encode_batch_dev, SS_RS_OUT_PADDED16 | SS_RS_EMIT_DATA).  slot_out and shard_off feed
+ * ss_frame_accept_pack_ragged_dev directly.  policy: Crossword [G] policy index (NULL = 0).  No host synchronisation;
+ * per-group scratch is allocated on the first call.  Uniform and ragged proposals may be mixed on one engine
+ * (cfg.data_len sizes only the engine's own uniform store: a host that only proposes ragged batches passes 1). */
+#define SS_DEV_STATUS_STORE_FULL 16u
+int ss_engine_propose_ragged(ss_engine *engine, const uint8_t *arena, const uint64_t *data_off, const uint32_t *data_len,
+                             const uint8_t *policy, uint8_t *shards, uint64_t plane_stride, uint64_t *shard_off,
+                             uint64_t *slot_out, uint64_t *need);
 /* rec_slot is window-relative, as ss_accept_reply_parse_dev emits it with this engine's window_base: 0xff and values
  * >= 64 are dropped, rel is absolute slot window_base[g] + rel. */
 int ss_engine_ingest(ss_engine *engine, const uint32_t *rec_group, const uint8_t *rec_slot, const uint8_t *rec_peer,

@@ -97,6 +97,7 @@ SIGNATURES = {
     "ss_accept_step_fused": (_i, [_vp, _vp, _u64, _u32, _u64, _vp, _u64, _u64, _vp, _u32, _u32, _vp, _vp]),
     "ss_frame_accept_max_len": (_u64, [_vp, _u32]),
     "ss_frame_accept_pack_dev": (_i, [_vp, _vp, _vp, _u64, _u64, _vp, _u32, _vp, _u32, _vp, _vp, _u64, _vp, _u64, _vp, _vp]),
+    "ss_frame_accept_pack_ragged_dev": (_i, [_vp, _vp, _vp, _u64, _vp, _vp, _vp, _u32, _vp, _u32, _vp, _vp, _u64, _vp, _u64, _vp, _vp, _vp]),
     "ss_accept_reply_parse_dev": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _u64, _u32, _i, _vp, _vp, _vp, _vp, _vp]),
     "ss_wal_commit_pack_dev": (_i, [_vp, _vp, _vp, _u64, _u32, _vp, _vp, _vp, _u64, _vp]),
     "ss_reconstruct_serve_dev": (_i, [_vp, _vp, _u64, _u64, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _u64, _vp, _vp]),
@@ -107,6 +108,7 @@ SIGNATURES = {
     "ss_engine_set_policies": (_i, [_vp, _vp, _u32, _i]),
     "ss_engine_propose": (_i, [_vp, _u32, _vp, _u64, _vp, C.POINTER(_vp)]),
     "ss_engine_propose_next": (_i, [_vp, _u32, _vp, _u64, _vp, _vp, C.POINTER(_vp)]),
+    "ss_engine_propose_ragged": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _u64, _vp, _vp, _vp]),
     "ss_engine_ingest": (_i, [_vp, _vp, _vp, _vp, _vp, _u64]),
     "ss_engine_tick": (_i, [_vp, _vp]),
     "ss_engine_advance": (_i, [_vp, _vp]),

@@ -288,6 +288,35 @@ def _ctx_extras():
                                                 _ptr(policy_idx), peer, _ptr(slot), _ptr(ballot), n, _ptr(out), stride, _ptr(off), _ptr(ln)))
         return out, off, ln
 
+    def frame_accept_pack_ragged(self, shard_planes: torch.Tensor, shard_off: torch.Tensor, data_len: torch.Tensor, d: int, p: int,
+                                 policies: Sequence[Sequence[int]], policy_idx: Optional[torch.Tensor], peer: int, slot: torch.Tensor,
+                                 ballot: torch.Tensor, kind: int = 0, msg_variant: int = 2, with_assignment: bool = False,
+                                 out_capacity: Optional[int] = None):
+        """Accept / WAL AcceptData frames for ragged codewords, packed back to back.  shard_planes uint8 [d+p, plane_stride]
+        (the store LeaderEngine.propose_ragged fills); shard_off int64 [n], data_len int32 [n], slot / ballot int64 [n].
+        out_capacity None: room for the largest frames the lengths allow (reads data_len back to the host).  Returns
+        (out uint8 [out_capacity], frame_off int64 [n], frame_len int32 [n], total int64 [1])."""
+        T, ps = shard_planes.shape
+        assert T == d + p and shard_planes.is_contiguous() and shard_planes.dtype == torch.uint8
+        assert shard_off.dtype == torch.int64 and data_len.dtype == torch.int32
+        n = data_len.numel()
+        pol = np.ascontiguousarray(np.array(policies, dtype=np.uint32))
+        dev = shard_planes.device
+        pol_dev = torch.from_numpy(pol.view(np.int32)).to(dev)
+        spec = _lib.FrameSpec(kind, msg_variant, d, p, 0, pol.shape[1], 1 if with_assignment else 0, T)
+        if out_capacity is None:
+            L = (data_len.cpu().numpy().astype(np.int64) + d - 1) // d
+            per = 8 + 44 + T + T * (5 + L) + 1 + (5 + pol.shape[1] * 19 if with_assignment else 0) + 15
+            out_capacity = max(16, int(((per + 15) // 16 * 16).sum()))
+        out = torch.full((out_capacity,), 0xA5, dtype=torch.uint8, device=dev)      # the C ABI does not require a zeroed buffer
+        off = torch.empty(n, dtype=torch.int64, device=dev)
+        ln = torch.empty(n, dtype=torch.int32, device=dev)
+        total = torch.empty(1, dtype=torch.int64, device=dev)
+        check(self.lib.ss_frame_accept_pack_ragged_dev(self.h, C.byref(spec), _ptr(shard_planes), ps, _ptr(shard_off), _ptr(data_len),
+                                                       _ptr(pol_dev), pol.shape[0], _ptr(policy_idx), peer, _ptr(slot), _ptr(ballot), n,
+                                                       _ptr(out), out_capacity, _ptr(off), _ptr(ln), _ptr(total)))
+        return out, off, ln, total
+
     def accept_reply_parse(self, buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor, frame_peer: torch.Tensor,
                            window_base: torch.Tensor, reply_variant: int = 3, with_size: bool = False):
         """AcceptReply frames -> (rec_group int32, rec_slot uint8, rec_peer uint8, rec_ballot int64, rec_kind int32)."""
@@ -324,6 +353,7 @@ def _ctx_extras():
         return mask, out
 
     Context.frame_accept_pack = frame_accept_pack
+    Context.frame_accept_pack_ragged = frame_accept_pack_ragged
     Context.accept_reply_parse = accept_reply_parse
     Context.wal_commit_pack = wal_commit_pack
     Context.reconstruct_serve = reconstruct_serve

@@ -46,6 +46,10 @@ struct ss_engine {
     bool windowed = false;                  // a base may be non-zero: set by ss_engine_advance / ss_engine_window_get
     uint32_t *commit_bar = nullptr;
     uint8_t *shards = nullptr;
+    // ragged proposals: allocated on the first ss_engine_propose_ragged call
+    uint32_t *rg_len = nullptr;             // [G] effective length (0 = the group does not propose)
+    uint64_t *rg_partials = nullptr;        // [scan_tiles(G)] tile sums of the pitch scan
+    uint64_t *rg_need = nullptr;            // [1] total pitch, when the caller does not ask for it
     // Crossword
     uint8_t *policy_idx = nullptr;          // [G*64]
     uint32_t *policies = nullptr, *lut_bits = nullptr;
@@ -75,8 +79,34 @@ __device__ __forceinline__ uint64_t ring_to_window(uint64_t x, uint32_t r) { ret
 __device__ __forceinline__ uint64_t window_to_ring(uint64_t x, uint32_t r) { return (x << r) | (x >> ((64u - r) & 63u)); }
 
 // ---- propose bookkeeping: one new instance per group enters Accepting --------------------------------------------
-// slot < 64: at window position `slot`; slot == kProposeNext: at the group's first Null slot (rspaxos/mod.rs:434-442),
-// which a full window does not have -- then slot_out = UINT64_MAX, the status bit is set and the group is left as is.
+// window position of the group's first Null slot (rspaxos/mod.rs:434-442); 64 = the window is full
+__device__ __forceinline__ uint32_t first_null(uint64_t acc, uint64_t cm, uint64_t base) {
+    return dev::commit_prefix(ring_to_window(acc | cm, static_cast<uint32_t>(base & 63u)));
+}
+
+// instance s of group g enters Accepting; acc / cm are the group's accepting / committed words as loaded
+__device__ __forceinline__ void enter_accepting(uint64_t g, uint64_t s, uint64_t acc, uint64_t cm, uint64_t *__restrict__ planes,
+                                                uint32_t R, uint64_t G, const uint64_t *__restrict__ bal_prepared,
+                                                uint64_t *__restrict__ inst_bal, uint64_t *__restrict__ accepting,
+                                                uint64_t *__restrict__ committed, uint8_t *__restrict__ policy_idx,
+                                                const uint8_t *__restrict__ new_policy) {
+    const uint32_t pos = static_cast<uint32_t>(s & 63u);
+    const uint64_t bit = 1ull << pos;
+    accepting[g] = acc | bit;                              // Status::Accepting (request.rs: inst.status = Accepting)
+    committed[g] = cm & ~bit;                              // a re-used window slot starts uncommitted
+    inst_bal[g * 64 + pos] = bal_prepared[g];              // inst.bal = bal_prepared
+    for (uint32_t r = 0; r < R; ++r) planes[static_cast<uint64_t>(r) * G + g] &= ~bit;   // fresh accept_acks
+    if (policy_idx != nullptr) policy_idx[g * 64 + pos] = new_policy != nullptr ? new_policy[g] : 0;
+}
+
+// one status write per warp, not one per flagged group
+__device__ __forceinline__ void warp_status(bool flag, uint32_t bit, uint32_t *status) {
+    const unsigned any = __ballot_sync(__activemask(), flag);
+    if (flag && (threadIdx.x & 31u) == static_cast<unsigned>(__ffs(static_cast<int>(any)) - 1)) atomicOr(status, bit);
+}
+
+// slot < 64: at window position `slot`; slot == kProposeNext: at the group's first Null slot, which a full window does
+// not have -- then slot_out = UINT64_MAX, the status bit is set and the group is left as is.
 constexpr uint32_t kProposeNext = 64;
 __global__ void __launch_bounds__(kEngThreads)
 engine_propose_kernel(uint64_t *__restrict__ planes, uint32_t R, uint64_t G, uint32_t slot, const uint64_t *__restrict__ window_base,
@@ -90,7 +120,7 @@ engine_propose_kernel(uint64_t *__restrict__ planes, uint32_t R, uint64_t G, uin
         const uint64_t acc = accepting[g], cm = committed[g];
         uint32_t rel = slot;
         if (slot == kProposeNext) {
-            rel = dev::commit_prefix(ring_to_window(acc | cm, static_cast<uint32_t>(base & 63u)));   // first Null position
+            rel = first_null(acc, cm, base);
             if (rel == 64u) {
                 full = true;
                 if (slot_out != nullptr) slot_out[g] = ~0ull;
@@ -98,18 +128,154 @@ engine_propose_kernel(uint64_t *__restrict__ planes, uint32_t R, uint64_t G, uin
             }
         }
         const uint64_t s = base + rel;
-        const uint32_t pos = static_cast<uint32_t>(s & 63u);
-        const uint64_t bit = 1ull << pos;
-        accepting[g] = acc | bit;                              // Status::Accepting (request.rs: inst.status = Accepting)
-        committed[g] = cm & ~bit;                              // a re-used window slot starts uncommitted
-        inst_bal[g * 64 + pos] = bal_prepared[g];              // inst.bal = bal_prepared
-        for (uint32_t r = 0; r < R; ++r) planes[static_cast<uint64_t>(r) * G + g] &= ~bit;   // fresh accept_acks
-        if (policy_idx != nullptr) policy_idx[g * 64 + pos] = new_policy != nullptr ? new_policy[g] : 0;
+        enter_accepting(g, s, acc, cm, planes, R, G, bal_prepared, inst_bal, accepting, committed, policy_idx, new_policy);
         if (slot_out != nullptr) slot_out[g] = s;
     }
-    // one status write per warp, not one per full group
-    const unsigned any = __ballot_sync(__activemask(), full);
-    if (full && (threadIdx.x & 31u) == static_cast<unsigned>(__ffs(static_cast<int>(any)) - 1)) atomicOr(status, SS_DEV_STATUS_WINDOW_FULL);
+    warp_status(full, SS_DEV_STATUS_WINDOW_FULL, status);
+}
+
+// ---- ragged proposals (ss_engine_propose_ragged) ------------------------------------------------------------------
+// 1. prepare: a group proposes when it has a batch (data_len > 0) and its window a Null slot; its effective length is
+//    then data_len, its pitch SS_CW_SLOT_PITCH(ceil(data_len / d)), else both are 0.  The pitches go to shard_off, which
+//    the scan then turns into slot offsets in place.
+__global__ void __launch_bounds__(kEngThreads)
+engine_ragged_prepare_kernel(const uint32_t *__restrict__ data_len, uint64_t G, uint32_t d, const uint64_t *__restrict__ window_base,
+                             const uint64_t *__restrict__ accepting, const uint64_t *__restrict__ committed,
+                             uint32_t *__restrict__ eff_len, uint64_t *__restrict__ pitch, uint32_t *status) {
+    bool full = false;
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kEngThreads;
+    for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kEngThreads + threadIdx.x; g < G; g += stride) {
+        uint32_t len = data_len[g];
+        if (len != 0u && first_null(accepting[g], committed[g], window_base[g]) == 64u) {
+            full = true;
+            len = 0u;
+        }
+        eff_len[g] = len;
+        pitch[g] = len == 0u ? 0ull : SS_CW_SLOT_PITCH((static_cast<uint64_t>(len) + d - 1u) / d);
+    }
+    warp_status(full, SS_DEV_STATUS_WINDOW_FULL, status);
+}
+
+// 3. clamp + bookkeeping: shard_off holds the exclusive prefix of the pitches.  A proposing group whose slot ends past
+//    the plane capacity is dropped (effective length 0, status bit); the others enter Accepting at their first Null slot.
+//    Groups that do not propose get shard_off = slot_out = UINT64_MAX.
+__global__ void __launch_bounds__(kEngThreads)
+engine_ragged_commit_kernel(uint32_t *__restrict__ eff_len, uint64_t *__restrict__ shard_off, uint64_t capacity, uint32_t d,
+                            uint64_t *__restrict__ planes, uint32_t R, uint64_t G, const uint64_t *__restrict__ window_base,
+                            const uint64_t *__restrict__ bal_prepared, uint64_t *__restrict__ inst_bal,
+                            uint64_t *__restrict__ accepting, uint64_t *__restrict__ committed, uint8_t *__restrict__ policy_idx,
+                            const uint8_t *__restrict__ new_policy, uint64_t *__restrict__ slot_out, uint32_t *status) {
+    bool over = false;
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kEngThreads;
+    for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kEngThreads + threadIdx.x; g < G; g += stride) {
+        const uint32_t len = eff_len[g];
+        const uint64_t off = shard_off[g];
+        const uint64_t pitch = SS_CW_SLOT_PITCH((static_cast<uint64_t>(len) + d - 1u) / d);
+        if (len == 0u || off > capacity || pitch > capacity - off) {
+            if (len != 0u) {
+                over = true;
+                eff_len[g] = 0u;                               // the encode skips it
+            }
+            shard_off[g] = ~0ull;
+            slot_out[g] = ~0ull;
+            continue;
+        }
+        const uint64_t base = window_base[g];
+        const uint64_t acc = accepting[g], cm = committed[g];
+        const uint64_t s = base + first_null(acc, cm, base);   // not full: the prepare kernel checked the same words
+        enter_accepting(g, s, acc, cm, planes, R, G, bal_prepared, inst_bal, accepting, committed, policy_idx, new_policy);
+        slot_out[g] = s;
+    }
+    warp_status(over, SS_DEV_STATUS_STORE_FULL, status);
+}
+
+// ---- exclusive scan of u64 values, in place: reduce / scan / add ------------------------------------------------------
+// Tiles of kScanTile values: the first pass writes each tile's sum, one CTA scans the sums (and writes the total), the
+// last pass scans each tile again from its base.  Integer sums in a fixed order: the result is exactly numpy's
+// cumsum shifted by one, on every run.
+constexpr int kScanThreads = 256, kScanItems = 8, kScanTile = kScanThreads * kScanItems;
+
+// exclusive scan of one value per thread across the CTA; *total (shared) receives the CTA's sum
+__device__ __forceinline__ uint64_t cta_exclusive_scan(uint64_t v, uint64_t *warp_sums, uint64_t *total) {
+    const uint32_t lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
+    uint64_t x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint64_t y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= static_cast<uint32_t>(o)) x += y;
+    }
+    if (lane == 31u) warp_sums[wid] = x;
+    __syncthreads();
+    if (wid == 0) {
+        uint64_t w = lane < kScanThreads / 32 ? warp_sums[lane] : 0ull;
+#pragma unroll
+        for (int o = 1; o < kScanThreads / 32; o <<= 1) {
+            const uint64_t y = __shfl_up_sync(0xffffffffu, w, o);
+            if (lane >= static_cast<uint32_t>(o)) w += y;
+        }
+        if (lane < kScanThreads / 32) warp_sums[lane] = w;           // inclusive over warps
+        if (lane == kScanThreads / 32 - 1) *total = w;
+    }
+    __syncthreads();
+    const uint64_t before = wid == 0 ? 0ull : warp_sums[wid - 1];
+    const uint64_t r = before + x - v;
+    __syncthreads();                                                 // warp_sums / total may be reused by the caller
+    return r;
+}
+
+__global__ void __launch_bounds__(kScanThreads) scan_tile_sum_kernel(const uint64_t *__restrict__ x, uint64_t n,
+                                                                     uint64_t *__restrict__ partials) {
+    __shared__ uint64_t warp_sums[kScanThreads / 32], total;
+    const uint64_t t0 = static_cast<uint64_t>(blockIdx.x) * kScanTile;
+    uint64_t s = 0;
+#pragma unroll
+    for (int i = 0; i < kScanItems; ++i) {
+        const uint64_t k = t0 + static_cast<uint64_t>(i) * kScanThreads + threadIdx.x;
+        if (k < n) s += x[k];
+    }
+    cta_exclusive_scan(s, warp_sums, &total);
+    if (threadIdx.x == 0) partials[blockIdx.x] = total;
+}
+
+__global__ void __launch_bounds__(kScanThreads) scan_partials_kernel(uint64_t *__restrict__ partials, uint64_t tiles,
+                                                                     uint64_t *__restrict__ total_out) {
+    __shared__ uint64_t warp_sums[kScanThreads / 32], total;
+    uint64_t carry = 0;
+    for (uint64_t c = 0; c < tiles; c += kScanThreads) {
+        const uint64_t k = c + threadIdx.x;
+        const uint64_t v = k < tiles ? partials[k] : 0ull;
+        const uint64_t e = cta_exclusive_scan(v, warp_sums, &total);
+        if (k < tiles) partials[k] = carry + e;
+        carry += total;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0 && total_out != nullptr) *total_out = carry;
+}
+
+__global__ void __launch_bounds__(kScanThreads) scan_tile_apply_kernel(uint64_t *__restrict__ x, uint64_t n,
+                                                                       const uint64_t *__restrict__ partials) {
+    __shared__ uint64_t tile[kScanTile + kScanTile / 32];            // one pad word per 32: the per-thread runs avoid bank conflicts
+    __shared__ uint64_t warp_sums[kScanThreads / 32], total;
+    auto at = [](uint32_t i) { return i + (i >> 5); };
+    const uint64_t t0 = static_cast<uint64_t>(blockIdx.x) * kScanTile;
+#pragma unroll
+    for (int i = 0; i < kScanItems; ++i) {
+        const uint32_t j = static_cast<uint32_t>(i) * kScanThreads + threadIdx.x;
+        tile[at(j)] = t0 + j < n ? x[t0 + j] : 0ull;
+    }
+    __syncthreads();
+    uint64_t v[kScanItems], s = 0;
+#pragma unroll
+    for (int i = 0; i < kScanItems; ++i) { v[i] = tile[at(threadIdx.x * kScanItems + i)]; s += v[i]; }
+    uint64_t run = partials[blockIdx.x] + cta_exclusive_scan(s, warp_sums, &total);
+#pragma unroll
+    for (int i = 0; i < kScanItems; ++i) { tile[at(threadIdx.x * kScanItems + i)] = run; run += v[i]; }
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < kScanItems; ++i) {
+        const uint32_t j = static_cast<uint32_t>(i) * kScanThreads + threadIdx.x;
+        if (t0 + j < n) x[t0 + j] = tile[at(j)];
+    }
 }
 
 // ---- retire the committed prefix up to upto[g] (all of it when upto is NULL) ---------------------------------------
@@ -326,6 +492,24 @@ static int dalloc(T **p, size_t count, bool zero = true) {
     return SS_OK;
 }
 
+uint64_t scan_tiles(uint64_t n) { return (n + kScanTile - 1) / kScanTile; }
+
+int launch_exclusive_scan_u64(ss_ctx *ctx, uint64_t *x, uint64_t n, uint64_t *partials, uint64_t *total) {
+    const uint64_t tiles = scan_tiles(n);
+    if (tiles == 0) {
+        if (total != nullptr) SS_CUDA(cudaMemsetAsync(total, 0, 8, ctx->stream));
+        return SS_OK;
+    }
+    if (tiles > 0x7fffffffull) return set_error(SS_ERR_INVALID_ARG, "scan of %llu values is too long", (unsigned long long)n);
+    const uint32_t grid = static_cast<uint32_t>(tiles);
+    scan_tile_sum_kernel<<<grid, kScanThreads, 0, ctx->stream>>>(x, n, partials);
+    scan_partials_kernel<<<1, kScanThreads, 0, ctx->stream>>>(partials, tiles, total);
+    scan_tile_apply_kernel<<<grid, kScanThreads, 0, ctx->stream>>>(x, n, partials);
+    SS_CUDA(cudaGetLastError());
+    ctx->launches += 3;
+    return SS_OK;
+}
+
 }  // namespace ssb
 
 using namespace ssb;
@@ -340,7 +524,7 @@ int ss_engine_destroy(ss_engine *e) {
     }
     void *bufs[] = {e->planes, e->bal_prepared, e->inst_bal, e->accepting, e->committed, e->window_base, e->commit_bar, e->shards, e->policy_idx,
                     e->policies, e->lut_bits, e->match, e->next_slot, e->last_commit, e->log_end, e->curr_term, e->terms,
-                    e->last_snap, e->touched};
+                    e->last_snap, e->touched, e->rg_len, e->rg_partials, e->rg_need};
     for (void *b : bufs)
         if (b) cudaFree(b);
     if (e->coder) ss_rs_coder_destroy(e->coder);
@@ -503,6 +687,39 @@ int ss_engine_propose_next(ss_engine *e, uint32_t store, const uint8_t *payloads
     const uint32_t keep = e->cfg.keep_slots ? e->cfg.keep_slots : 1;
     if (store >= keep) return set_error(SS_ERR_INVALID_ARG, "shard store %u >= keep_slots %u", store, keep);
     return engine_propose(e, store, kProposeNext, payloads, payload_stride, policy, slot_out, shard_planes);
+}
+
+int ss_engine_propose_ragged(ss_engine *e, const uint8_t *arena, const uint64_t *data_off, const uint32_t *data_len,
+                             const uint8_t *policy, uint8_t *shards, uint64_t plane_stride, uint64_t *shard_off,
+                             uint64_t *slot_out, uint64_t *need) {
+    if (e == nullptr) return set_error(SS_ERR_INVALID_ARG, "null engine");
+    if (e->planes == nullptr || e->coder == nullptr) return set_error(SS_ERR_INVALID_ARG, "ragged proposals need an RSPaxos or Crossword engine");
+    if (!arena || !data_off || !data_len || !shards || !shard_off || !slot_out) return set_error(SS_ERR_INVALID_ARG, "null buffer");
+    if ((plane_stride & 31u) || plane_stride == 0) return set_error(SS_ERR_INVALID_ARG, "plane_stride must be a non-zero multiple of 32");
+    if (reinterpret_cast<uintptr_t>(shards) & 15u) return set_error(SS_ERR_INVALID_ARG, "the shard store must be 16-byte aligned");
+    if (e->cfg.protocol == SS_PROTO_CROSSWORD && e->lut_bits == nullptr)
+        return set_error(SS_ERR_INVALID_ARG, "ss_engine_set_policies must be called before proposing");
+    ss_ctx *ctx = e->ctx;
+    SS_TRY(ctx_bind(ctx));
+    if (e->rg_len == nullptr) SS_TRY(dalloc(&e->rg_len, e->G, false));
+    if (e->rg_partials == nullptr) SS_TRY(dalloc(&e->rg_partials, scan_tiles(e->G), false));
+    if (e->rg_need == nullptr) SS_TRY(dalloc(&e->rg_need, 1, false));
+    const uint32_t grid = eng_grid(ctx, e->G);
+    engine_ragged_prepare_kernel<<<grid, kEngThreads, 0, ctx->stream>>>(data_len, e->G, e->d, e->window_base, e->accepting, e->committed,
+                                                                      e->rg_len, shard_off, ctx->dev_status);
+    SS_CUDA(cudaGetLastError());
+    ctx->launches++;
+    SS_TRY(launch_exclusive_scan_u64(ctx, shard_off, e->G, e->rg_partials, need != nullptr ? need : e->rg_need));
+    engine_ragged_commit_kernel<<<grid, kEngThreads, 0, ctx->stream>>>(e->rg_len, shard_off, plane_stride, e->d, e->planes, e->n, e->G,
+                                                                     e->window_base, e->bal_prepared, e->inst_bal, e->accepting,
+                                                                     e->committed, e->policy_idx, policy, slot_out, ctx->dev_status);
+    SS_CUDA(cudaGetLastError());
+    ctx->launches++;
+    // from_data + compute_parity + subset_copy's per-peer buffers for every proposing group, one launch: data shards into
+    // planes 0..d-1, parity into planes d..T-1, each at the group's slot (rspaxos/request.rs:72-77,127-142,
+    // crossword/request.rs:82-87,164-185)
+    return ss_rs_encode_batch_dev(e->coder, arena, data_off, e->rg_len, e->G, shards + uint64_t(e->d) * plane_stride, plane_stride,
+                                  shard_off, SS_RS_OUT_PADDED16 | SS_RS_EMIT_DATA);
 }
 
 int ss_engine_ingest(ss_engine *e, const uint32_t *rec_group, const uint8_t *rec_slot, const uint8_t *rec_peer,

@@ -128,6 +128,11 @@ void ctx_retain(ss_ctx *ctx);                           // a handle (coder, engi
 void ctx_release(ss_ctx *ctx);                          // ... and stops; tears ctx down if it was destroyed meanwhile
 int ctx_scratch(ss_ctx *ctx, size_t bytes, void **out); // grow-only scratch
 
+// exclusive prefix sum of x[0..n) in place (engine.cu); partials: scan_tiles(n) words of device scratch; total (device,
+// may be NULL) = the sum of all n values.  Deterministic: integer sums in a fixed order.
+uint64_t scan_tiles(uint64_t n);
+int launch_exclusive_scan_u64(ss_ctx *ctx, uint64_t *x, uint64_t n, uint64_t *partials, uint64_t *total);
+
 // ---- kernel launchers (defined in the .cu files) ---------------------------------------------
 struct EncGeom {
     // sources: payload arena

@@ -7,6 +7,9 @@
 //                               codeword carrying exactly the shards of the peer's assignment (subset_copy(.., false),
 //                               rspaxos/request.rs:127-142, crossword/request.rs:164-185; encoding utils/rscoding.rs:43-72,
 //                               assignment Vec<Bitmap> utils/bitmap.rs:20-30)
+//   frame_size_ragged_kernel    the same frames for ragged codewords (data_len per codeword), packed back to back:
+//   frame_pack_ragged_kernel    exact sizes, an exclusive scan of the 16-byte regions (engine.cu), then the frames;
+//                               both share frame_layout / frame_write with frame_pack_kernel
 //   accept_reply_parse_kernel   AcceptReply frames -> (group, window slot, peer, ballot) records for ss_ack_ingest_dev /
 //                               ss_engine_ingest (rspaxos/mod.rs:290-291, crossword/mod.rs:365-373)
 //   wal_commit_pack_kernel      newly committed instances -> WalEntry::CommitSlot{slot} records (rspaxos/mod.rs:231)
@@ -75,94 +78,158 @@ struct PackArgs {
     const uint64_t *slot, *ballot;
     uint64_t n;
     uint8_t *out;
-    uint64_t frame_stride;
+    uint64_t frame_stride;          // uniform: frame g inside out[g*frame_stride ..)
     uint64_t *frame_off;
     uint32_t *frame_len;
     uint32_t *status;               // context's device status word
+    // ragged: shard j of codeword g at planes + j*plane_stride + shard_off[g], data_len[g] bytes; packed regions in out
+    const uint64_t *shard_off;
+    const uint32_t *lens;
+    uint64_t capacity;
 };
+
+// where the bytes of frame g go, known before a byte is written
+struct FrameLayout {
+    const uint32_t *pol;            // the codeword's policy row
+    uint32_t mask;                  // shards carried for this peer
+    uint32_t h;                     // fixed fields after the length prefix
+    uint32_t some_len;              // Some tag + byte length of one carried shard
+    uint32_t pad;                   // bytes before the frame that put its first carried shard on a 16-byte boundary
+    uint64_t len;                   // frame bytes: 8-byte length prefix + body
+};
+
+__device__ __forceinline__ FrameLayout frame_layout(const PackArgs &A, uint64_t g, uint32_t data_len, uint32_t L) {
+    FrameLayout F;
+    const uint32_t T = A.d + A.p;
+    uint32_t k = A.policy_idx != nullptr ? A.policy_idx[g] : 0u;
+    if (k >= A.n_policies) k = 0u;
+    F.pol = A.policies + static_cast<uint64_t>(k) * A.population;
+    F.mask = __ldg(F.pol + A.peer) & (T >= 32u ? 0xffffffffu : ((1u << T) - 1u));
+    F.h = (A.kind == SS_FRAME_PEER_ACCEPT ? 1u : 0u) + static_cast<uint32_t>(wv_len(A.variant) + wv_len(__ldg(A.slot + g)) +
+          wv_len(__ldg(A.ballot + g))) + 2u + static_cast<uint32_t>(wv_len(data_len) + wv_len(L) + wv_len(T));
+    F.some_len = 1u + static_cast<uint32_t>(wv_len(L));
+    // bytes before the first carried shard's payload decide the padding that makes that payload 16-byte aligned
+    const uint32_t first = F.mask ? static_cast<uint32_t>(__ffs(F.mask) - 1) : T;
+    const uint32_t pre = 8u + F.h + first + (F.mask ? F.some_len : 0u);
+    F.pad = (16u - (pre & 15u)) & 15u;
+    uint32_t asg_len = 0;
+    if (A.with_assignment) {
+        const uint32_t nblocks = (A.assign_size + 63u) / 64u;
+        asg_len = static_cast<uint32_t>(wv_len(A.population));
+        for (uint32_t r = 0; r < A.population; ++r)
+            asg_len += static_cast<uint32_t>(wv_len(A.assign_size) + wv_len(nblocks) + wv_len(F.pol[r])) + (nblocks > 1u ? nblocks - 1u : 0u);
+    }
+    const uint32_t carried = static_cast<uint32_t>(__popc(F.mask));
+    F.len = 8u + static_cast<uint64_t>(F.h) + (T - carried) + static_cast<uint64_t>(carried) * (F.some_len + L) + 1u + asg_len;
+    return F;
+}
+
+// one warp writes frame g at f (its length prefix first); shard j is read from shards + j*plane_stride
+__device__ __forceinline__ void frame_write(const PackArgs &A, const FrameLayout &F, uint64_t g, uint32_t data_len, uint32_t L,
+                                            const uint8_t *shards, uint8_t *f, uint32_t lane) {
+    const uint32_t T = A.d + A.p;
+    if (lane == 0u) {                                                            // fixed fields (at most 41 bytes)
+        uint32_t w = 8u;
+        if (A.kind == SS_FRAME_PEER_ACCEPT) f[w++] = 0;                          // PeerMessage::Msg
+        w += wv_put(f + w, A.variant);
+        w += wv_put(f + w, __ldg(A.slot + g));
+        w += wv_put(f + w, __ldg(A.ballot + g));
+        f[w++] = static_cast<uint8_t>(A.d);
+        f[w++] = static_cast<uint8_t>(A.p);
+        w += wv_put(f + w, data_len);
+        w += wv_put(f + w, L);
+        wv_put(f + w, T);
+    }
+    uint32_t at = 8u + F.h;                                                      // running offset inside the frame
+    for (uint32_t j = 0; j < T; ++j) {
+        if (!((F.mask >> j) & 1u)) {
+            if (lane == 0u) f[at] = 0;                                           // None
+            at += 1u;
+            continue;
+        }
+        if (lane == 0u) { f[at] = 1; wv_put(f + at + 1u, L); }                   // Some(bytes): tag, length
+        at += F.some_len;
+        warp_copy_bytes(f + at, shards + static_cast<uint64_t>(j) * A.plane_stride, L, lane);
+        at += L;
+    }
+    if (lane == 0u) f[at] = 0;                                                   // data_copy: None
+    at += 1u;
+    if (A.with_assignment && lane == 0u) {                                       // assignment: Vec<Bitmap>
+        uint32_t w = at;
+        w += wv_put(f + w, A.population);
+        const uint32_t nblocks = (A.assign_size + 63u) / 64u;
+        for (uint32_t r = 0; r < A.population; ++r) {
+            w += wv_put(f + w, A.assign_size);
+            w += wv_put(f + w, nblocks);
+            for (uint32_t b = 0; b < nblocks; ++b) w += wv_put(f + w, b == 0u ? F.pol[r] : 0u);
+        }
+    }
+    const uint64_t body = F.len - 8u;
+    if (lane < 8u) f[lane] = static_cast<uint8_t>(body >> (8u * (7u - lane)));
+}
 
 __global__ void __launch_bounds__(kWireThreads) frame_pack_kernel(const __grid_constant__ PackArgs A) {
     const uint32_t lane = threadIdx.x & 31u;
     const uint64_t warp = (static_cast<uint64_t>(blockIdx.x) * kWireThreads + threadIdx.x) >> 5;
     const uint64_t nwarps = (static_cast<uint64_t>(gridDim.x) * kWireThreads) >> 5;
-    const uint32_t T = A.d + A.p;
     for (uint64_t g = warp; g < A.n; g += nwarps) {
-        uint32_t k = A.policy_idx != nullptr ? A.policy_idx[g] : 0u;
-        if (k >= A.n_policies) k = 0u;
-        const uint32_t *pol = A.policies + static_cast<uint64_t>(k) * A.population;
-        const uint32_t mask = __ldg(pol + A.peer) & (T >= 32u ? 0xffffffffu : ((1u << T) - 1u));
-        // fixed fields (every lane builds them; at most 41 bytes)
-        uint8_t hdr[44];
-        int h = 0;
-        if (A.kind == SS_FRAME_PEER_ACCEPT) hdr[h++] = 0;                       // PeerMessage::Msg
-        h += wv_put(hdr + h, A.variant);
-        h += wv_put(hdr + h, __ldg(A.slot + g));
-        h += wv_put(hdr + h, __ldg(A.ballot + g));
-        hdr[h++] = static_cast<uint8_t>(A.d);
-        hdr[h++] = static_cast<uint8_t>(A.p);
-        h += wv_put(hdr + h, A.data_len);
-        h += wv_put(hdr + h, A.L);
-        h += wv_put(hdr + h, T);
-        const uint32_t some_len = 1u + static_cast<uint32_t>(wv_len(A.L));       // Some tag + byte length
-        // bytes before the first carried shard's payload decide the padding that makes that payload 16-byte aligned
-        const uint32_t first = mask ? static_cast<uint32_t>(__ffs(mask) - 1) : T;
-        const uint32_t pre = 8u + static_cast<uint32_t>(h) + first + (mask ? some_len : 0u);
-        const uint32_t pad = (16u - (pre & 15u)) & 15u;
-        // the frame must fit its slot: its length is known before a byte is written
-        uint32_t asg_len = 0;
-        if (A.with_assignment) {
-            const uint32_t nblocks = (A.assign_size + 63u) / 64u;
-            asg_len = static_cast<uint32_t>(wv_len(A.population));
-            for (uint32_t r = 0; r < A.population; ++r)
-                asg_len += static_cast<uint32_t>(wv_len(A.assign_size) + wv_len(nblocks) + wv_len(pol[r])) + (nblocks > 1u ? nblocks - 1u : 0u);
-        }
-        const uint32_t carried = static_cast<uint32_t>(__popc(mask));
-        const uint64_t need = static_cast<uint64_t>(pad) + 8u + static_cast<uint32_t>(h) + (T - carried) +
-                              static_cast<uint64_t>(carried) * (some_len + A.L) + 1u + asg_len;
-        if (need > A.frame_stride) {
+        const FrameLayout F = frame_layout(A, g, A.data_len, A.L);
+        // the frame must fit its slot
+        if (F.pad + F.len > A.frame_stride) {
             if (lane == 0u) {
                 A.frame_off[g] = g * A.frame_stride;
                 A.frame_len[g] = 0;                                              // nothing written for this codeword
-                atomicOr(A.status, 4u);                                          // SS_DEV_STATUS_FRAME_OVERFLOW
+                atomicOr(A.status, SS_DEV_STATUS_FRAME_OVERFLOW);
             }
             continue;
         }
-        uint8_t *f = A.out + g * A.frame_stride + pad;
-        for (uint32_t i = lane; i < static_cast<uint32_t>(h); i += 32u) f[8u + i] = hdr[i];
-        uint32_t at = 8u + static_cast<uint32_t>(h);                             // running offset inside the frame
-        for (uint32_t j = 0; j < T; ++j) {
-            if (!((mask >> j) & 1u)) {
-                if (lane == 0u) f[at] = 0;                                       // None
-                at += 1u;
-                continue;
-            }
-            if (lane == 0u) { f[at] = 1; wv_put(f + at + 1u, A.L); }             // Some(bytes): tag, length
-            at += some_len;
-            warp_copy_bytes(f + at, A.planes + static_cast<uint64_t>(j) * A.plane_stride + g * A.shard_stride, A.L, lane);
-            at += A.L;
-        }
-        if (lane == 0u) f[at] = 0;                                               // data_copy: None
-        at += 1u;
-        if (A.with_assignment) {                                                 // assignment: Vec<Bitmap>
-            uint32_t w = at;
-            if (lane == 0u) {
-                w += wv_put(f + w, A.population);
-                const uint32_t nblocks = (A.assign_size + 63u) / 64u;
-                for (uint32_t r = 0; r < A.population; ++r) {
-                    w += wv_put(f + w, A.assign_size);
-                    w += wv_put(f + w, nblocks);
-                    for (uint32_t b = 0; b < nblocks; ++b) w += wv_put(f + w, b == 0u ? pol[r] : 0u);
-                }
-            }
-            at = __shfl_sync(0xffffffffu, w, 0);
-        }
-        const uint64_t body = at - 8u;
-        if (lane < 8u) f[lane] = static_cast<uint8_t>(body >> (8u * (7u - lane)));
+        frame_write(A, F, g, A.data_len, A.L, A.planes + g * A.shard_stride, A.out + g * A.frame_stride + F.pad, lane);
         if (lane == 0u) {
-            A.frame_off[g] = g * A.frame_stride + pad;
-            A.frame_len[g] = at;
+            A.frame_off[g] = g * A.frame_stride + F.pad;
+            A.frame_len[g] = static_cast<uint32_t>(F.len);
         }
     }
+}
+
+// ragged, pass 1 (a thread per codeword): each frame's region round_up(pad + len, 16) into frame_off (the scan's input)
+// and its length into frame_len; 0 for the frames that are not written
+__global__ void __launch_bounds__(kWireThreads) frame_size_ragged_kernel(const __grid_constant__ PackArgs A) {
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kWireThreads;
+    for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kWireThreads + threadIdx.x; g < A.n; g += stride) {
+        const uint32_t len = __ldg(A.lens + g);
+        uint64_t region = 0;
+        uint32_t flen = 0;
+        if (len != 0u && __ldg(A.slot + g) != ~0ull) {
+            const FrameLayout F = frame_layout(A, g, len, (len + A.d - 1u) / A.d);
+            region = (F.pad + F.len + 15u) & ~15ull;
+            flen = static_cast<uint32_t>(F.len);
+        }
+        A.frame_off[g] = region;
+        A.frame_len[g] = flen;
+    }
+}
+
+// ragged, pass 2 (a warp per codeword): frame_off now holds the region's start
+__global__ void __launch_bounds__(kWireThreads) frame_pack_ragged_kernel(const __grid_constant__ PackArgs A) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint64_t warp = (static_cast<uint64_t>(blockIdx.x) * kWireThreads + threadIdx.x) >> 5;
+    const uint64_t nwarps = (static_cast<uint64_t>(gridDim.x) * kWireThreads) >> 5;
+    bool over = false;
+    for (uint64_t g = warp; g < A.n; g += nwarps) {
+        if (A.frame_len[g] == 0u) continue;                                      // skipped codeword
+        const uint32_t len = __ldg(A.lens + g), L = (len + A.d - 1u) / A.d;
+        const FrameLayout F = frame_layout(A, g, len, L);
+        const uint64_t off = A.frame_off[g], region = (F.pad + F.len + 15u) & ~15ull;
+        __syncwarp();                                                            // every lane has read frame_off / frame_len
+        if (off > A.capacity || region > A.capacity - off) {
+            over = true;
+            if (lane == 0u) A.frame_len[g] = 0;                                  // nothing written for this codeword
+            continue;
+        }
+        frame_write(A, F, g, len, L, A.planes + __ldg(A.shard_off + g), A.out + off + F.pad, lane);
+        if (lane == 0u) A.frame_off[g] = off + F.pad;
+    }
+    if (over && lane == 0u) atomicOr(A.status, SS_DEV_STATUS_FRAME_OVERFLOW);
 }
 
 struct ParseArgs {
@@ -352,6 +419,47 @@ int ss_frame_accept_pack_dev(ss_ctx *ctx, const ss_frame_spec *s, const uint8_t 
     A.slot = slot; A.ballot = ballot; A.n = n; A.out = out; A.frame_stride = frame_stride; A.frame_off = frame_off; A.frame_len = frame_len;
     if (shard_stride < ((uint64_t(A.L) + 15) & ~uint64_t(15))) return set_error(SS_ERR_INVALID_ARG, "shard_stride shorter than a padded shard");
     frame_pack_kernel<<<wire_grid(ctx, n, kWireThreads / 32), kWireThreads, 0, ctx->stream>>>(A);
+    SS_CUDA(cudaGetLastError());
+    ctx->launches++;
+    return SS_OK;
+}
+
+int ss_frame_accept_pack_ragged_dev(ss_ctx *ctx, const ss_frame_spec *s, const uint8_t *shard_planes, uint64_t plane_stride,
+                                    const uint64_t *shard_off, const uint32_t *data_len, const uint32_t *policies,
+                                    uint32_t n_policies, const uint8_t *policy_idx, uint32_t peer, const uint64_t *slot,
+                                    const uint64_t *ballot, uint64_t n, uint8_t *out, uint64_t out_capacity,
+                                    uint64_t *frame_off, uint32_t *frame_len, uint64_t *total) {
+    if (ctx == nullptr || s == nullptr) return set_error(SS_ERR_INVALID_ARG, "null context or spec");
+    SS_TRY(ctx_bind(ctx));
+    if (n == 0) {
+        if (total != nullptr) SS_CUDA(cudaMemsetAsync(total, 0, 8, ctx->stream));
+        return SS_OK;
+    }
+    if (!shard_planes || !shard_off || !data_len || !policies || !slot || !ballot || !out || !frame_off || !frame_len)
+        return set_error(SS_ERR_INVALID_ARG, "null buffer");
+    const uint32_t T = s->data_shards + s->parity_shards;
+    if (s->data_shards == 0 || T > 32) return set_error(SS_ERR_INVALID_ARG, "shard counts must satisfy 1 <= d, d+p <= 32");
+    if (s->kind != SS_FRAME_PEER_ACCEPT && s->kind != SS_FRAME_WAL_ACCEPT_DATA) return set_error(SS_ERR_INVALID_ARG, "unknown frame kind %u", s->kind);
+    if (s->population == 0 || s->population > 32 || peer >= s->population || n_policies == 0)
+        return set_error(SS_ERR_INVALID_ARG, "bad population / peer / policy table");
+    if (s->with_assignment && (s->assign_size == 0 || s->assign_size > 64)) return set_error(SS_ERR_INVALID_ARG, "assignment bitmaps must have 1..64 bits");
+    if ((reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(shard_planes) | plane_stride) & 15u)
+        return set_error(SS_ERR_INVALID_ARG, "buffers and plane_stride must be 16-byte aligned");
+    PackArgs A{};
+    A.status = ctx->dev_status;
+    A.planes = shard_planes; A.plane_stride = plane_stride;
+    A.d = s->data_shards; A.p = s->parity_shards;
+    A.kind = s->kind; A.variant = s->msg_variant; A.policies = policies; A.policy_idx = policy_idx; A.n_policies = n_policies;
+    A.population = s->population; A.peer = peer; A.with_assignment = s->with_assignment; A.assign_size = s->assign_size;
+    A.slot = slot; A.ballot = ballot; A.n = n; A.out = out; A.frame_off = frame_off; A.frame_len = frame_len;
+    A.shard_off = shard_off; A.lens = data_len; A.capacity = out_capacity;
+    void *scr = nullptr;
+    SS_TRY(ctx_scratch(ctx, scan_tiles(n) * 8, &scr));
+    frame_size_ragged_kernel<<<wire_grid(ctx, n, kWireThreads), kWireThreads, 0, ctx->stream>>>(A);
+    SS_CUDA(cudaGetLastError());
+    ctx->launches++;
+    SS_TRY(launch_exclusive_scan_u64(ctx, frame_off, n, static_cast<uint64_t *>(scr), total));
+    frame_pack_ragged_kernel<<<wire_grid(ctx, n, kWireThreads / 32), kWireThreads, 0, ctx->stream>>>(A);
     SS_CUDA(cudaGetLastError());
     ctx->launches++;
     return SS_OK;

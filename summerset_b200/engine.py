@@ -8,6 +8,7 @@ torch tensors (zero-copy views) so tests can read results and install state; it 
     LeaderEngine(ctx, protocol, G, population, ...)   protocol in {"multipaxos", "rspaxos", "crossword"}
         propose(slot, payloads[, policy])   multipaxos/request.rs:112-221, rspaxos/request.rs:72-142, crossword/request.rs:82-185
         propose_next(store, payloads[, policy])   the same at each group's first Null slot (rspaxos/mod.rs:434-442)
+        propose_ragged(arena, data_off, data_len, store[, policy])   variable-length batches into a caller-owned store
         on_accept_replies(records)          handle_msg_accept_reply filters (multipaxos/messages.rs:377-409, ...)
         tick()                              commit decision + commit_bar, one kernel
         advance([upto])                     retire committed prefixes: window_base moves on (multipaxos/snapshot.rs:121-171)
@@ -127,6 +128,24 @@ class LeaderEngine(_EngineBase):
                                               policy.data_ptr() if policy is not None else None, slot_out.data_ptr(),
                                               C.byref(base)))
         return slot_out, (self.shards[store] if self.shards is not None else None)
+
+    def propose_ragged(self, arena: torch.Tensor, data_off: torch.Tensor, data_len: torch.Tensor, store: torch.Tensor,
+                       policy: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """Ragged request batches (RSPaxos / Crossword): group g proposes arena[data_off[g] : +data_len[g]] at its first
+        Null slot, or nothing when data_len[g] == 0.  store: caller-owned uint8 [T, plane_stride] (plane_stride a
+        multiple of 32); shard j of a proposing group lands at store[j, shard_off[g]:], zero-padded to 16 bytes.
+        Returns (slot_out int64 [G], shard_off int64 [G], need int64 [1]); -1 (UINT64_MAX) marks a group that did not
+        propose, need = the total slot pitch the batch asked for."""
+        assert arena.is_cuda and arena.dtype == torch.uint8
+        assert data_off.dtype == torch.int64 and data_len.dtype == torch.int32 and data_len.numel() == self.G
+        assert store.dtype == torch.uint8 and store.dim() == 2 and store.shape[0] == self.T and store.is_contiguous()
+        slot_out = torch.empty(self.G, dtype=torch.int64, device=self.dev)
+        shard_off = torch.empty(self.G, dtype=torch.int64, device=self.dev)
+        need = torch.empty(1, dtype=torch.int64, device=self.dev)
+        check(self.lib.ss_engine_propose_ragged(self.h, arena.data_ptr(), data_off.data_ptr(), data_len.data_ptr(),
+                                                policy.data_ptr() if policy is not None else None, store.data_ptr(),
+                                                store.shape[1], shard_off.data_ptr(), slot_out.data_ptr(), need.data_ptr()))
+        return slot_out, shard_off, need
 
     def advance(self, upto: Optional[torch.Tensor] = None) -> None:
         """Retires committed prefixes up to the absolute slots upto (int64 [G]), or all of them when upto is None."""
