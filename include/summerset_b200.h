@@ -617,6 +617,8 @@ int ss_engine_raft_ingest(ss_engine *engine, const uint32_t *rec_group, const ui
  *   bits 5-7  row kernel waves of CTAs per resident set: {64 (default), 1, 32, 4, 16, 256, 128, 8}
  *   bits 8-9  cache operator of the plane stores in replicate mode: .cs (default), write-back, .cg, .wt
  *   bit 10    row kernel: fixed instead of rotating warp -> column-block assignment
+ *   bit 18    the accept step (parity to local planes, up to 256 columns) on the bulk-copy kernel instead of the row kernel;
+ *             bits 19-20 its resident CTAs per SM {4 (default), 2, 3, 6}, bit 21 interleaved instead of contiguous codewords
  *   ss_crossword_distribute_dev, bits 0-3: 6 / 7 = a warp takes runs of 8 / 4 codewords from a shared counter and pools the
  *             short ones into shared passes (3.3x on batches of sub-KB payloads, 1-2 % behind on mixed sizes), 4 = the
  *             general (any code) kernel also for RS(3,2) / n = 5

@@ -666,9 +666,7 @@ static int engine_propose(ss_engine *e, uint32_t store, uint32_t slot, const uin
     engine_propose_kernel<<<eng_grid(ctx, e->G), kEngThreads, 0, ctx->stream>>>(e->planes, e->n, e->G, slot, e->window_base,
                                                                              e->bal_prepared, e->inst_bal, e->accepting, e->committed,
                                                                              e->policy_idx, policy, slot_out, ctx->dev_status);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int ss_engine_propose(ss_engine *e, uint32_t slot, const uint8_t *payloads, uint64_t payload_stride, const uint8_t *policy,
@@ -707,14 +705,12 @@ int ss_engine_propose_ragged(ss_engine *e, const uint8_t *arena, const uint64_t 
     const uint32_t grid = eng_grid(ctx, e->G);
     engine_ragged_prepare_kernel<<<grid, kEngThreads, 0, ctx->stream>>>(data_len, e->G, e->d, e->window_base, e->accepting, e->committed,
                                                                       e->rg_len, shard_off, ctx->dev_status);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
+    SS_TRY(launched(ctx));
     SS_TRY(launch_exclusive_scan_u64(ctx, shard_off, e->G, e->rg_partials, need != nullptr ? need : e->rg_need));
     engine_ragged_commit_kernel<<<grid, kEngThreads, 0, ctx->stream>>>(e->rg_len, shard_off, plane_stride, e->d, e->planes, e->n, e->G,
                                                                      e->window_base, e->bal_prepared, e->inst_bal, e->accepting,
                                                                      e->committed, e->policy_idx, policy, slot_out, ctx->dev_status);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
+    SS_TRY(launched(ctx));
     // from_data + compute_parity + subset_copy's per-peer buffers for every proposing group, one launch: data shards into
     // planes 0..d-1, parity into planes d..T-1, each at the group's slot (rspaxos/request.rs:72-77,127-142,
     // crossword/request.rs:82-87,164-185)
@@ -740,9 +736,7 @@ int ss_engine_advance(ss_engine *e, const uint64_t *upto) {
     e->windowed = true;
     engine_advance_kernel<<<eng_grid(ctx, e->G), kEngThreads, 0, ctx->stream>>>(upto, e->planes, e->n, e->G, e->window_base,
                                                                              e->accepting, e->committed, e->commit_bar);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int ss_engine_window_get(ss_engine *e, uint64_t **window_base) {
@@ -765,9 +759,7 @@ int ss_engine_tick(ss_engine *e, uint64_t *newly) {
         if (e->n_peers <= 4) engine_raft_snap_kernel<4><<<grid, kEngThreads, 0, ctx->stream>>>(e->match, e->n_peers, e->G, e->touched, e->last_snap);
         else if (e->n_peers <= 8) engine_raft_snap_kernel<8><<<grid, kEngThreads, 0, ctx->stream>>>(e->match, e->n_peers, e->G, e->touched, e->last_snap);
         else engine_raft_snap_kernel<16><<<grid, kEngThreads, 0, ctx->stream>>>(e->match, e->n_peers, e->G, e->touched, e->last_snap);
-        SS_CUDA(cudaGetLastError());
-        ctx->launches++;
-        return SS_OK;
+        return launched(ctx);
     }
     if (e->cfg.protocol == SS_PROTO_CROSSWORD) {
         if (e->lut_bits == nullptr) return set_error(SS_ERR_INVALID_ARG, "ss_engine_set_policies must be called first");
@@ -794,9 +786,7 @@ int ss_engine_tick(ss_engine *e, uint64_t *newly) {
         k<<<eng_grid(ctx, e->G), kEngThreads, 0, ctx->stream>>>(e->planes, e->n, e->G, e->threshold, e->window_base, e->accepting,
                                                              e->committed, e->commit_bar, newly);
     }
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int ss_engine_raft_append(ss_engine *e, const uint32_t *n_new) {
@@ -806,9 +796,7 @@ int ss_engine_raft_append(ss_engine *e, const uint32_t *n_new) {
     SS_TRY(ctx_bind(ctx));
     engine_raft_append_kernel<<<eng_grid(ctx, e->G), kEngThreads, 0, ctx->stream>>>(n_new, e->G, e->W, e->curr_term, e->last_commit,
                                                                                  e->log_end, e->terms, ctx->dev_status);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int ss_engine_raft_ingest(ss_engine *e, const uint32_t *rec_group, const uint8_t *rec_peer, const uint32_t *rec_end_slot,
@@ -821,9 +809,7 @@ int ss_engine_raft_ingest(ss_engine *e, const uint32_t *rec_group, const uint8_t
     SS_TRY(ctx_bind(ctx));
     engine_raft_ingest_kernel<<<eng_grid(ctx, n_records), kEngThreads, 0, ctx->stream>>>(rec_group, rec_peer, rec_end_slot, n_records,
                                                                                       e->n_peers, e->G, e->next_slot, e->match, e->touched);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 }  // extern "C"

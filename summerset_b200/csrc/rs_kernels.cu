@@ -1178,6 +1178,35 @@ static int dispatch_p(int p, F &&f) {
     }
 }
 
+// f(integral_constant<D>, integral_constant<Code>): a compile-time cluster code at its exact width, any other code
+// (kCodeGeneric) at dispatch_d's capacity for d.  The NVRTC code (kCodeJit) is launched by the callers themselves.
+template <typename F>
+static int dispatch_code(int sc, int d, F &&f) {
+    auto fixed = [&](auto CC) { return f(std::integral_constant<int, static_code_d(decltype(CC)::value)>{}, CC); };
+    switch (sc) {
+        case kCode21: return fixed(std::integral_constant<int, kCode21>{});
+        case kCode43: return fixed(std::integral_constant<int, kCode43>{});
+        case kCode54: return fixed(std::integral_constant<int, kCode54>{});
+        case kCode42: return fixed(std::integral_constant<int, kCode42>{});
+        case kCode31: return fixed(std::integral_constant<int, kCode31>{});
+        default: return dispatch_d(d, [&](auto DC) { return f(DC, std::integral_constant<int, kCodeGeneric>{}); });
+    }
+}
+
+// the fused-tally fields of an encode kernel's parameters (t == nullptr: no tally)
+template <typename Args>
+static void set_tally(Args &a, const TallyArgs *t) {
+    const TallyArgs none;
+    if (t == nullptr) t = &none;
+    a.planes = t->planes; a.R = t->R; a.threshold = t->threshold; a.committed = t->committed; a.commit_bar = t->commit_bar;
+}
+
+// base of shard plane j of a uniform batch: the caller's explicit plane bases, or parity plane j - d
+static uint8_t *out_plane(const EncGeom &g, int d, int j) {
+    if (g.plane_ptrs != nullptr) return g.plane_ptrs[j];
+    return g.parity + (static_cast<int64_t>(j) - d) * static_cast<int64_t>(g.plane_stride);
+}
+
 
 // ------------------------------------------------------------------------------------------------
 // Crossword distribute (BASELINE config 4, n = 5 replicas, RS(3,2), T = 5 total shards, dj = 1):
@@ -1486,27 +1515,12 @@ int launch_crossword_distribute(ss_rs_coder *coder, const uint8_t *data, const u
         for (uint32_t r = 0; r < 16; ++r) Gp.rep[r] = r < n_replicas ? replica_logs[r] : nullptr;
         const uint32_t grid = ragged_grid(ctx, n);
         const int sc = ((coder->variant >> 11) & 1) ? kCodeGeneric : coder->static_code;
-        auto go_static = [&](auto CC) {
-            constexpr int C = decltype(CC)::value;
-            crossword_distribute_generic_kernel<static_code_d(C), C><<<grid, kThreads, 0, ctx->stream>>>(Gp);
-            coder->last_kernel = "crossword_distribute_generic_kernel<static>";
-        };
-        switch (sc) {
-            case kCode21: go_static(std::integral_constant<int, kCode21>{}); break;
-            case kCode43: go_static(std::integral_constant<int, kCode43>{}); break;
-            case kCode54: go_static(std::integral_constant<int, kCode54>{}); break;
-            case kCode42: go_static(std::integral_constant<int, kCode42>{}); break;
-            case kCode31: go_static(std::integral_constant<int, kCode31>{}); break;
-            default:
-                SS_TRY(dispatch_d(coder->d, [&](auto DC) {
-                    crossword_distribute_generic_kernel<decltype(DC)::value, kCodeGeneric><<<grid, kThreads, 0, ctx->stream>>>(Gp);
-                    return SS_OK;
-                }));
-                coder->last_kernel = "crossword_distribute_generic_kernel";
-        }
-        SS_CUDA(cudaGetLastError());
-        ctx->launches++;
-        return SS_OK;
+        SS_TRY(dispatch_code(sc, coder->d, [&](auto DC, auto CC) {
+            crossword_distribute_generic_kernel<decltype(DC)::value, decltype(CC)::value><<<grid, kThreads, 0, ctx->stream>>>(Gp);
+            return SS_OK;
+        }));
+        coder->last_kernel = sc != kCodeGeneric ? "crossword_distribute_generic_kernel<static>" : "crossword_distribute_generic_kernel";
+        return launched(ctx);
     }
     CwDistribute P;
     P.data = data; P.data_off = data_off; P.data_len = data_len; P.spr = spr; P.rep_off = rep_off; P.n = n;
@@ -1531,402 +1545,361 @@ int launch_crossword_distribute(ss_rs_coder *coder, const uint8_t *data, const u
         else rs32_crossword_distribute_kernel<8, true><<<static_cast<uint32_t>(ctas), kThreads, 0, ctx->stream>>>(P);
         coder->last_kernel = vk == 7 ? "rs32_crossword_distribute_kernel<4,dynamic>" : "rs32_crossword_distribute_kernel<8,dynamic>";
     }
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
+    return launched(ctx);
+}
+
+// ---- batched encode: launch_rs_encode validates a batch and routes it to one of the four kernel families below ----
+
+// RS(3,2) in the row geometry: the bulk-copy accept kernel (variant bit 18), the segmented row kernel for codewords over
+// 256 columns, else the row kernel
+static int encode_rs32_row(ss_rs_coder *coder, const EncGeom &g, const TallyArgs *tally, uint32_t len, uint32_t L,
+                           uint32_t vpc) {
+    ss_ctx *ctx = coder->ctx;
+    cudaStream_t st = ctx->stream;
+    Enc32Row Rw;
+    Rw.data = g.data; Rw.data_stride = g.data_stride; Rw.shard_stride = g.shard_stride;
+    for (int j = 0; j < 5; ++j) Rw.plane[j] = out_plane(g, 3, j);
+    Rw.n = static_cast<uint32_t>(g.n); Rw.len = len; Rw.L = L; Rw.vpc = vpc;
+    const uint32_t lim = (len - 2u * L) < L ? (len - 2u * L) : L;     // bytes of shard 2 inside the payload
+    Rw.fast_cols = len >= 2u * L ? lim / 16u : 0u;
+    Rw.s1 = L & 15u; Rw.s2 = (2u * L) & 15u;
+    Rw.emit_data = ((g.flags & SS_RS_EMIT_DATA) || g.plane_ptrs != nullptr) ? 1u : 0u;
+    set_tally(Rw, tally);
+    Rw.wait = g.wait;
+    // The accept step proper (parity to local planes, no replication) on the bulk-copy kernel: variant bit 18
+    // selects it.  It is not the default: on an H100 it measured 2-3 % slower than the row kernel (DESIGN.md 3.1).
+    const uint32_t in_bytes = (len + 15u) & ~15u;
+    if (vpc <= 256u && !Rw.emit_data && ((coder->variant >> 18) & 1) && g.data_stride >= in_bytes) {
+        int smem_sm = 0, smem_blk = 0, smem_rsv = 0;
+        SS_CUDA(cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, ctx->device));
+        SS_CUDA(cudaDeviceGetAttribute(&smem_blk, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
+        SS_CUDA(cudaDeviceGetAttribute(&smem_rsv, cudaDevAttrReservedSharedMemoryPerBlock, ctx->device));
+        Enc32Bulk B;
+        B.data = g.data; B.data_stride = g.data_stride; B.par0 = Rw.plane[3]; B.par1 = Rw.plane[4];
+        B.shard_stride = g.shard_stride; B.n = Rw.n; B.len = len; B.L = L; B.vpc = vpc;
+        B.fast_cols = Rw.fast_cols; B.s1 = Rw.s1; B.s2 = Rw.s2;
+        B.in_bytes = in_bytes;
+        B.in_pitch = (in_bytes + 48u + 127u) & ~127u;
+        set_tally(B, tally);
+        // Resident CTAs per SM (variant bits 19-20, tuning): 4 by default.  The SM's shared memory is split
+        // evenly between them; each CTA keeps kBulkOut output stages and as many input stages as fit, at most
+        // 8 -- at cfg3 (4096 B rows) that is 8 stages, up to 4 x 7 x 4 KB = 112 KB of payload in flight per SM.
+        static const uint32_t kCtasPerSm[4] = {4, 2, 3, 6};
+        const uint32_t out_bytes = kBulkOut * 2u * vpc * 16u;
+        uint32_t cps = kCtasPerSm[(coder->variant >> 19) & 3], nin = 0;
+        for (; cps >= 1; --cps) {
+            int64_t room = static_cast<int64_t>(smem_sm) / cps - smem_rsv;
+            if (room > smem_blk) room = smem_blk;
+            room -= kBulkHeader + out_bytes;
+            nin = room > 0 ? static_cast<uint32_t>(room / B.in_pitch) : 0u;
+            if (nin > 8u) nin = 8u;
+            if (nin >= 2u) break;
+        }
+        if (nin < 2u) return set_error(SS_ERR_UNSUPPORTED, "accept step: no room for two %u-byte stages", B.in_pitch);
+        B.nin = nin;
+        uint64_t ctas = static_cast<uint64_t>(ctx->sm_count) * cps;
+        if (ctas > g.n) ctas = g.n;
+        B.chunk = static_cast<uint32_t>((g.n + ctas - 1) / ctas);
+        ctas = (g.n + B.chunk - 1) / B.chunk;
+        B.interleave = ((coder->variant >> 21) & 1) ? 1u : 0u;       // bit 21 (tuning): interleaved codewords
+        const uint32_t smem = kBulkHeader + nin * B.in_pitch + out_bytes;
+        SS_CUDA(cudaFuncSetAttribute(rs32_accept_bulk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     static_cast<int>(smem)));
+        const uint32_t threads = ((vpc + 31u) & ~31u) + 32u;      // a thread per column + the tally warp
+        rs32_accept_bulk_kernel<<<static_cast<uint32_t>(ctas), threads, smem, st>>>(B);
+        coder->last_kernel = B.planes ? "rs32_accept_bulk_kernel+tally" : "rs32_accept_bulk_kernel";
+        return launched(ctx);
+    }
+    const uint32_t threads = vpc > 256u ? 256u : ((vpc + 31u) & ~31u);
+    if (vpc > 256u) {
+        // wide codewords: (codeword, 256-column segment) work items
+        const uint64_t items = g.n * ((vpc + 255u) / 256u);
+        uint64_t ctas = static_cast<uint64_t>(ctx->sm_count) * 8ull * 16ull;
+        if (ctas > items) ctas = items;
+        Rw.chunk = 0; Rw.st_mode = static_cast<uint32_t>((coder->variant >> 8) & 3); Rw.rotate = 0; Rw.tally_last = 0;
+        if (Rw.emit_data) rs32_encode_row_kernel<true, 256, 4, true><<<static_cast<uint32_t>(ctas), 256, 0, st>>>(Rw);
+        else rs32_encode_row_kernel<false, 256, 4, true><<<static_cast<uint32_t>(ctas), 256, 0, st>>>(Rw);
+        coder->last_kernel = Rw.planes ? "rs32_encode_row_kernel<segmented>+tally" : "rs32_encode_row_kernel<segmented>";
+        return launched(ctx);
+    }
+    // resident CTAs per SM (2048 threads, 32 CTAs) x a few waves; every CTA strides over codewords
+    uint32_t per_sm = 2048u / threads; if (per_sm > 32u) per_sm = 32u;
+    const int vr = coder->variant & 15, vchunk = (coder->variant >> 4) & 1, vw = (coder->variant >> 5) & 7;
+    static const uint64_t kWaves[8] = {64, 1, 32, 4, 16, 256, 128, 8};   // [0] = default, rest: tuning
+    // Local planes (the accept step): by default a CTA per codeword.  The block scheduler then hands codewords
+    // out in order, so the whole GPU reads and writes one narrow, advancing window of memory; on an H100 that
+    // measured 2.6 % faster than 64 or 256 waves of CTAs striding over the batch (DESIGN.md 3.1).
+    const uint64_t waves = (vw == 0 && !Rw.emit_data) ? (1ull << 32) : kWaves[vw];
+    uint64_t ctas = static_cast<uint64_t>(ctx->sm_count) * per_sm * waves;
+    if (ctas > g.n) ctas = g.n;
+    if (ctas > 0x7fffffffull) ctas = 0x7fffffffull;
+    Rw.chunk = 0;
+    Rw.st_mode = static_cast<uint32_t>((coder->variant >> 8) & 3);
+    Rw.rotate = ((coder->variant >> 10) & 1) ? 0u : 1u;
+    // local planes: the tally goes after the CTA's codeword, so its first loads are the payload's
+    Rw.tally_last = Rw.emit_data ? 0u : 1u;
+    if (vchunk) { Rw.chunk = static_cast<uint32_t>((g.n + ctas - 1) / ctas); ctas = (g.n + Rw.chunk - 1) / Rw.chunk; }
+    const uint32_t grid = static_cast<uint32_t>(ctas);
+    // Register budget: 40/thread (12 CTAs of <= 128 threads per SM; the kernel needs ~47 unconstrained and fits
+    // 40 without spilling); a CTA per codeword for local planes, 64 waves of CTAs otherwise.  The other budgets
+    // (variant bits 0-3: 3 = 32 regs, 6 = 64, 7 = 56) and wave counts stay selectable for tuning.
+    if (threads > 128) {
+        if (Rw.emit_data) rs32_encode_row_kernel<true, 256, 4><<<grid, threads, 0, st>>>(Rw);
+        else rs32_encode_row_kernel<false, 256, 4><<<grid, threads, 0, st>>>(Rw);
+    } else if (Rw.emit_data) rs32_encode_row_kernel<true, 128, 8><<<grid, threads, 0, st>>>(Rw);
+    else if (vr == 3) rs32_encode_row_kernel<false, 128, 16><<<grid, threads, 0, st>>>(Rw);   // 32 regs
+    else if (vr == 6) rs32_encode_row_kernel<false, 128, 8><<<grid, threads, 0, st>>>(Rw);    // 64 regs cap
+    else if (vr == 7) rs32_encode_row_kernel<false, 128, 9><<<grid, threads, 0, st>>>(Rw);    // 56 regs cap
+    else rs32_encode_row_kernel<false, 128, 12, false, true><<<grid, threads, 0, st>>>(Rw);    // 40 regs, L2 prefetch
+    coder->last_kernel = Rw.planes ? "rs32_encode_row_kernel+tally" : "rs32_encode_row_kernel";
+    return launched(ctx);
+}
+
+// Other codes with d <= 8 in the row geometry: the packed or the row layout, each as a compile-time cluster code, the
+// coder's own NVRTC specialisation or with run-time coefficient masks
+static int encode_horner_row(ss_rs_coder *coder, const EncGeom &g, const TallyArgs *tally, uint32_t len, uint32_t L,
+                             uint32_t vpc) {
+    ss_ctx *ctx = coder->ctx;
+    cudaStream_t st = ctx->stream;
+    const int d = coder->d, p = coder->p;
+    EncRowGen Rg;
+    Rg.data = g.data; Rg.data_stride = g.data_stride;
+    for (int j = 0; j < 16; ++j) Rg.plane[j] = j < d + p ? out_plane(g, d, j) : nullptr;
+    Rg.emit_data = ((g.flags & SS_RS_EMIT_DATA) || g.plane_ptrs != nullptr) ? 1u : 0u;
+    Rg.wait = g.wait;
+    Rg.shard_stride = g.shard_stride; Rg.n = static_cast<uint32_t>(g.n); Rg.len = len; Rg.L = L; Rg.vpc = vpc;
+    // columns whose every source window lies inside the payload and whose output vector is complete
+    const uint64_t last_shard_bytes = static_cast<uint64_t>(len) >= static_cast<uint64_t>(d - 1) * L
+                                          ? static_cast<uint64_t>(len) - static_cast<uint64_t>(d - 1) * L : 0;
+    Rg.fast_cols = static_cast<uint32_t>((last_shard_bytes < L ? last_shard_bytes : L) / 16u);
+    Rg.d = static_cast<uint32_t>(d); Rg.p = static_cast<uint32_t>(p);
+    Rg.hmT8 = static_cast<const uint32_t *>(coder->enc_hmT8);
+    for (int j = 0; j < kMaxP; ++j) Rg.top[j] = coder->enc_top[j];
+    set_tally(Rg, tally);
+    // which flavour of the kernels: a compile-time cluster code, the coder's own NVRTC specialisation (any other
+    // matrix; compiled on first use), or run-time coefficient masks (variant bit 11 forces them, bit 17 skips NVRTC)
+    int sc = ((coder->variant >> 11) & 1) ? kCodeGeneric : coder->static_code;
+    const bool jit_allowed = sc == kCodeGeneric && !((coder->variant >> 11) & 1) && !((coder->variant >> 17) & 1);
+    auto launch_jit = [&](int which, uint32_t grid_x, uint32_t block_x) -> int {
+        void *args[] = {&Rg};
+        SS_CUDA(cudaLaunchKernel(reinterpret_cast<const void *>(coder->jit_kernel[which]), dim3(grid_x), dim3(block_x), args, 0, st));
+        return SS_OK;
+    };
+    // Packed flavour when the one-codeword-per-pass layout would idle or mask a good part of the lanes
+    // (bit 13 forces it off, bit 14 forces it on).
+    const uint32_t fc = Rg.fast_cols;
+    const uint32_t row_threads = vpc > 256u ? 256u : ((vpc + 31u) & ~31u);    // wider codewords: 256-column segments
+    bool packed = (fc != vpc || row_threads != vpc) && vpc <= 256u;
+    if ((coder->variant >> 13) & 1) packed = false;
+    if ((coder->variant >> 14) & 1) packed = true;
+    // software-pipelined main loop: always when every shard is 16-byte aligned; bit 15 selects it for unaligned too
+    const bool pipe = (L & 15u) == 0u || ((coder->variant >> 15) & 1);
+    if (jit_allowed) {
+        // the one instance this geometry needs (compiled by NVRTC on first use, ~1 s; then cached in the coder)
+        const int which = packed ? ((L & 15u) == 0u ? 2 : pipe ? 3 : 4) : (row_threads > 128u ? 1 : 0);
+        if (jit_ensure(coder, which) == SS_OK) sc = kCodeJit;
+    }
+    if (packed) {
+        // threads: the multiple of 32 (<= 256) that wastes the fewest lanes; ties go to the larger CTA
+        uint32_t T = 256, m = fc ? 256u / fc : 0u;
+        if (fc) {
+            double best = -1.0;
+            for (uint32_t t = 256; t >= 64; t -= 32) {
+                const uint32_t mm = t / fc;
+                const double eff = static_cast<double>(mm * fc) / t;
+                if (eff > best + 1e-9) { best = eff; T = t; m = mm; }
+            }
+        }
+        Rg.pack_m = m;
+        Rg.ntail = vpc - fc;
+        const uint64_t tail_items = g.n * Rg.ntail;
+        const uint64_t tail_ctas = (tail_items + T - 1) / T;
+        uint64_t main_ctas = 0;
+        if (m) {
+            const uint32_t dcap = d <= 2 ? 2 : d == 3 ? 3 : d == 4 ? 4 : d <= 6 ? 6 : 8;      // dispatch_d's capacity
+            const uint32_t dt = sc != kCodeGeneric ? static_cast<uint32_t>(d) : dcap;       // static and NVRTC kernels are exact-width
+            const uint32_t reg_need = 4u * dt + ((L & 15u) == 0u ? 4u * dt : 8u * dt - 4u) + 22u;
+            uint32_t rb = 65536u / (256u * reg_need); rb = rb > 6u ? 6u : (rb < 1u ? 1u : rb);
+            if (!pipe) rb = dt <= 3 ? 6u : dt <= 5 ? 5u : dt <= 6 ? 4u : 3u;
+            const uint32_t resident_threads = 256u * rb;
+            main_ctas = static_cast<uint64_t>(ctx->sm_count) * (resident_threads / T) * 64ull;
+            const uint64_t need = (g.n + m - 1) / m;
+            if (main_ctas > need) main_ctas = need;
+        }
+        if (tail_ctas + main_ctas <= 0x7fffffffull) {
+            Rg.tail_ctas = static_cast<uint32_t>(tail_ctas);
+            const uint32_t grid = static_cast<uint32_t>(tail_ctas + main_ctas);
+            if (sc == kCodeJit) SS_TRY(launch_jit((L & 15u) == 0u ? 2 : pipe ? 3 : 4, grid, T));
+            else SS_TRY(dispatch_code(sc, d, [&](auto DC, auto CC) {
+                constexpr int kD = decltype(DC)::value, kC = decltype(CC)::value;
+                if ((L & 15u) == 0u) horner_encode_packed_kernel<kD, kC, true, true><<<grid, T, 0, st>>>(Rg);
+                else if (pipe) horner_encode_packed_kernel<kD, kC, false, true><<<grid, T, 0, st>>>(Rg);
+                else horner_encode_packed_kernel<kD, kC, false, false><<<grid, T, 0, st>>>(Rg);
+                return SS_OK;
+            }));
+            if (sc == kCodeJit)
+                coder->last_kernel = Rg.planes ? "horner_encode_packed_kernel<nvrtc>+tally" : "horner_encode_packed_kernel<nvrtc>";
+            else if (sc != kCodeGeneric)
+                coder->last_kernel = Rg.planes ? "horner_encode_packed_kernel<static code>+tally" : "horner_encode_packed_kernel<static code>";
+            else
+                coder->last_kernel = Rg.planes ? "horner_encode_packed_kernel+tally" : "horner_encode_packed_kernel";
+            return launched(ctx);
+        }
+    }
+    Rg.pack_m = 0; Rg.tail_ctas = 0; Rg.ntail = 0;
+    const uint32_t threads = row_threads;
+    if (sc == kCodeJit && jit_ensure(coder, threads > 128u ? 1 : 0) != SS_OK) sc = kCodeGeneric;   // (packed grid did not fit)
+    uint32_t per_sm = 2048u / threads; if (per_sm > 32u) per_sm = 32u;
+    uint64_t ctas = static_cast<uint64_t>(ctx->sm_count) * per_sm * 64ull;
+    if (ctas > g.n) ctas = g.n;
+    const uint32_t grid = static_cast<uint32_t>(ctas);
+    // register budget (variant bits 0-3): threads <= 128: 0 = 12 CTAs/SM (40 regs), 2 = 10 (48), 3 = 8 (64), 4 = 6 (80)
+    const int vbits = coder->variant & 15;
+    if (sc == kCodeJit) SS_TRY(launch_jit(threads > 128 ? 1 : 0, grid, threads));
+    else SS_TRY(dispatch_code(sc, d, [&](auto DC, auto CC) {
+        constexpr int kD = decltype(DC)::value, kC = decltype(CC)::value;
+        // default budget by width: spill-free at 40 registers up to d = 4, 48 for 5, 64 for 6, 80 beyond
+        const int vdef = kD <= 4 ? 0 : kD == 5 ? 2 : kD == 6 ? 3 : 4;
+        const int vb = (vbits >= 2 && vbits <= 4) ? vbits : vdef;      // other values select other kernels' knobs
+        if (threads > 128) horner_encode_row_kernel<kD, kC, 256, 3><<<grid, threads, 0, st>>>(Rg);
+        else if (vb == 2) horner_encode_row_kernel<kD, kC, 128, 10><<<grid, threads, 0, st>>>(Rg);
+        else if (vb == 3) horner_encode_row_kernel<kD, kC, 128, 8><<<grid, threads, 0, st>>>(Rg);
+        else if (vb == 4) horner_encode_row_kernel<kD, kC, 128, 6><<<grid, threads, 0, st>>>(Rg);
+        else horner_encode_row_kernel<kD, kC, 128, 12><<<grid, threads, 0, st>>>(Rg);
+        return SS_OK;
+    }));
+    if (sc == kCodeJit)
+        coder->last_kernel = Rg.planes ? "horner_encode_row_kernel<nvrtc>+tally" : "horner_encode_row_kernel<nvrtc>";
+    else if (sc != kCodeGeneric)
+        coder->last_kernel = Rg.planes ? "horner_encode_row_kernel<static code>+tally" : "horner_encode_row_kernel<static code>";
+    else
+        coder->last_kernel = Rg.planes ? "horner_encode_row_kernel+tally" : "horner_encode_row_kernel";
+    return launched(ctx);
+}
+
+// Any uniform geometry, a thread per flat column index; chunked so that a launch's n_chunk * vpc fits in 32 bits.  The
+// fused tally rides on the first launch.
+static int encode_flat(ss_rs_coder *coder, const EncGeom &g, const TallyArgs *tally, uint32_t len, uint32_t L,
+                       uint32_t vpc) {
+    ss_ctx *ctx = coder->ctx;
+    const int d = coder->d, p = coder->p;
+    const uint64_t max_cw = vpc ? (0xffffff00ull / vpc) : g.n;
+    uint64_t done = 0;
+    bool tally_pending = tally != nullptr;
+    do {
+        const uint64_t nc = (g.n - done) < max_cw ? (g.n - done) : max_cw;
+        EncUniform E;
+        E.data = g.data + done * g.data_stride;
+        E.data_stride = g.data_stride;
+        E.len = len; E.L = L; E.vpc = vpc;
+        E.parity = g.parity + done * g.shard_stride;
+        E.plane_stride = g.plane_stride; E.shard_stride = g.shard_stride;
+        E.n = nc;
+        E.total = static_cast<uint32_t>(nc * vpc);
+        E.padded = ((g.flags & SS_RS_OUT_PADDED16) ? 1u : 0u) | ((g.flags & SS_RS_EMIT_DATA) ? 2u : 0u);
+        set_tally(E, tally_pending ? tally : nullptr);
+        E.G = 0;
+        uint64_t threads = E.total;
+        if (tally_pending) {
+            if (tally->G > 0xffffff00ull) return set_error(SS_ERR_INVALID_ARG, "too many groups for one fused launch");
+            E.G = tally->G;
+            if (threads < tally->G) threads = tally->G;
+            tally_pending = false;
+        }
+        if (threads == 0) break;
+        const uint32_t grid = static_cast<uint32_t>((threads + kThreads - 1) / kThreads);
+        const uint32_t *prog = static_cast<const uint32_t *>(coder->enc_prog);
+        if (coder->is_rs32) {
+            rs32_encode_uniform_kernel<<<grid, kThreads, 0, ctx->stream>>>(E);
+            coder->last_kernel = E.planes ? "rs32_encode_uniform_kernel+tally" : "rs32_encode_uniform_kernel";
+        } else if (d <= 8 && (coder->variant & 15) != 5) {
+            SS_TRY(dispatch_d(d, [&](auto DC) {
+                horner_encode_uniform_kernel<decltype(DC)::value><<<grid, kThreads, 0, ctx->stream>>>(E, prog, d, p);
+                return SS_OK;
+            }));
+            coder->last_kernel = "horner_encode_uniform_kernel";
+        } else {
+            SS_TRY(dispatch_p(p, [&](auto PC) {
+                generic_encode_uniform_kernel<decltype(PC)::value><<<grid, kThreads, 0, ctx->stream>>>(E, prog, d, p);
+                return SS_OK;
+            }));
+            coder->last_kernel = "generic_encode_uniform_kernel";
+        }
+        SS_TRY(launched(ctx));
+        done += nc;
+    } while (done < g.n);
     return SS_OK;
 }
 
-int launch_rs_encode(ss_rs_coder *coder, const EncGeom &g, const TallyArgs *tally) {
+// Ragged batches, a warp per codeword; the fused tally is a launch of its own
+static int encode_ragged(ss_rs_coder *coder, const EncGeom &g, const TallyArgs *tally) {
     ss_ctx *ctx = coder->ctx;
-    SS_TRY(ctx_bind(ctx));
-    if (!coder->batch_ok)
-        return set_error(SS_ERR_UNSUPPORTED, "batched encode needs d <= %d, p <= %d (coder is %d,%d)", kMaxD,
-                         kMaxP, coder->d, coder->p);
     const int d = coder->d, p = coder->p;
-    const bool padded = (g.flags & SS_RS_OUT_PADDED16) != 0u;
-    if (padded && ((reinterpret_cast<uintptr_t>(g.parity) | g.plane_stride) & 15u))
-        return set_error(SS_ERR_INVALID_ARG, "SS_RS_OUT_PADDED16 needs 16-byte aligned parity base and plane_stride");
-    const bool use_rs32 = coder->is_rs32;
-    cudaStream_t st = ctx->stream;
-
-    if (g.data_off == nullptr) {
-        // ---- uniform geometry: flat column index ----
-        const uint32_t len = g.uni_len;
-        if (len == 0u || g.n == 0u) {
-            if (tally == nullptr || tally->planes == nullptr) return SS_OK;
-        }
-        if (len >= 0x7fffffffu) return set_error(SS_ERR_INVALID_ARG, "data_len too large");
-        const uint32_t L = len == 0u ? 0u : (len + static_cast<uint32_t>(d) - 1u) / static_cast<uint32_t>(d);
-        const uint32_t vpc = (L + 15u) >> 4;
-        if (padded && (g.shard_stride & 15u))
-            return set_error(SS_ERR_INVALID_ARG, "SS_RS_OUT_PADDED16 needs shard_stride %% 16 == 0");
-        if (padded && g.shard_stride < static_cast<uint64_t>(vpc) * 16u)
-            return set_error(SS_ERR_INVALID_ARG, "shard_stride %llu < padded shard length %u",
-                             (unsigned long long)g.shard_stride, vpc * 16u);
-
-        // ---- RS(3,2) row kernel: aligned uniform geometry, codewords up to 256 columns ----
-        if (use_rs32 && (coder->variant & 15) != 1 && padded && vpc >= 1 && g.n <= 0xffffffffull &&
-            ((reinterpret_cast<uintptr_t>(g.data) | g.data_stride) & 15u) == 0u &&
-            (tally == nullptr || tally->planes == nullptr || tally->G == g.n)) {
-            Enc32Row Rw;
-            Rw.data = g.data; Rw.data_stride = g.data_stride; Rw.shard_stride = g.shard_stride;
-            for (int j = 0; j < 5; ++j) {
-                if (g.plane_ptrs != nullptr) Rw.plane[j] = g.plane_ptrs[j];
-                else Rw.plane[j] = g.parity + (static_cast<int64_t>(j) - 3) * static_cast<int64_t>(g.plane_stride);
-            }
-            Rw.n = static_cast<uint32_t>(g.n); Rw.len = len; Rw.L = L; Rw.vpc = vpc;
-            const uint32_t lim = (len - 2u * L) < L ? (len - 2u * L) : L;     // bytes of shard 2 inside the payload
-            Rw.fast_cols = len >= 2u * L ? lim / 16u : 0u;
-            Rw.s1 = L & 15u; Rw.s2 = (2u * L) & 15u;
-            Rw.emit_data = ((g.flags & SS_RS_EMIT_DATA) || g.plane_ptrs != nullptr) ? 1u : 0u;
-            Rw.planes = nullptr; Rw.R = 0; Rw.threshold = 0; Rw.committed = nullptr; Rw.commit_bar = nullptr;
-            if (tally != nullptr && tally->planes != nullptr) {
-                Rw.planes = tally->planes; Rw.R = tally->R; Rw.threshold = tally->threshold;
-                Rw.committed = tally->committed; Rw.commit_bar = tally->commit_bar;
-            }
-            Rw.wait = g.wait;
-            // The accept step proper (parity to local planes, no replication) on the bulk-copy kernel: variant bit 18
-            // selects it.  It is not the default: on an H100 it measured 2-3 % slower than the row kernel (DESIGN.md 3.1).
-            const uint32_t in_bytes = (len + 15u) & ~15u;
-            if (vpc <= 256u && !Rw.emit_data && ((coder->variant >> 18) & 1) && g.data_stride >= in_bytes) {
-                int smem_sm = 0, smem_blk = 0, smem_rsv = 0;
-                SS_CUDA(cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, ctx->device));
-                SS_CUDA(cudaDeviceGetAttribute(&smem_blk, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
-                SS_CUDA(cudaDeviceGetAttribute(&smem_rsv, cudaDevAttrReservedSharedMemoryPerBlock, ctx->device));
-                Enc32Bulk B;
-                B.data = g.data; B.data_stride = g.data_stride; B.par0 = Rw.plane[3]; B.par1 = Rw.plane[4];
-                B.shard_stride = g.shard_stride; B.n = Rw.n; B.len = len; B.L = L; B.vpc = vpc;
-                B.fast_cols = Rw.fast_cols; B.s1 = Rw.s1; B.s2 = Rw.s2;
-                B.in_bytes = in_bytes;
-                B.in_pitch = (in_bytes + 48u + 127u) & ~127u;
-                B.planes = Rw.planes; B.R = Rw.R; B.threshold = Rw.threshold; B.committed = Rw.committed;
-                B.commit_bar = Rw.commit_bar;
-                // Resident CTAs per SM (variant bits 19-20, tuning): 4 by default.  The SM's shared memory is split
-                // evenly between them; each CTA keeps kBulkOut output stages and as many input stages as fit, at most
-                // 8 -- at cfg3 (4096 B rows) that is 8 stages, up to 4 x 7 x 4 KB = 112 KB of payload in flight per SM.
-                static const uint32_t kCtasPerSm[4] = {4, 2, 3, 6};
-                const uint32_t out_bytes = kBulkOut * 2u * vpc * 16u;
-                uint32_t cps = kCtasPerSm[(coder->variant >> 19) & 3], nin = 0;
-                for (; cps >= 1; --cps) {
-                    int64_t room = static_cast<int64_t>(smem_sm) / cps - smem_rsv;
-                    if (room > smem_blk) room = smem_blk;
-                    room -= kBulkHeader + out_bytes;
-                    nin = room > 0 ? static_cast<uint32_t>(room / B.in_pitch) : 0u;
-                    if (nin > 8u) nin = 8u;
-                    if (nin >= 2u) break;
-                }
-                if (nin < 2u) return set_error(SS_ERR_UNSUPPORTED, "accept step: no room for two %u-byte stages", B.in_pitch);
-                B.nin = nin;
-                uint64_t ctas = static_cast<uint64_t>(ctx->sm_count) * cps;
-                if (ctas > g.n) ctas = g.n;
-                B.chunk = static_cast<uint32_t>((g.n + ctas - 1) / ctas);
-                ctas = (g.n + B.chunk - 1) / B.chunk;
-                B.interleave = ((coder->variant >> 21) & 1) ? 1u : 0u;       // bit 21 (tuning): interleaved codewords
-                const uint32_t smem = kBulkHeader + nin * B.in_pitch + out_bytes;
-                SS_CUDA(cudaFuncSetAttribute(rs32_accept_bulk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             static_cast<int>(smem)));
-                const uint32_t threads = ((vpc + 31u) & ~31u) + 32u;      // a thread per column + the tally warp
-                rs32_accept_bulk_kernel<<<static_cast<uint32_t>(ctas), threads, smem, st>>>(B);
-                coder->last_kernel = B.planes ? "rs32_accept_bulk_kernel+tally" : "rs32_accept_bulk_kernel";
-                SS_CUDA(cudaGetLastError());
-                ctx->launches++;
-                return SS_OK;
-            }
-            const uint32_t threads = vpc > 256u ? 256u : ((vpc + 31u) & ~31u);
-            if (vpc > 256u) {
-                // wide codewords: (codeword, 256-column segment) work items
-                const uint64_t items = g.n * ((vpc + 255u) / 256u);
-                uint64_t ctas = static_cast<uint64_t>(ctx->sm_count) * 8ull * 16ull;
-                if (ctas > items) ctas = items;
-                Rw.chunk = 0; Rw.st_mode = static_cast<uint32_t>((coder->variant >> 8) & 3); Rw.rotate = 0; Rw.tally_last = 0;
-                if (Rw.emit_data) rs32_encode_row_kernel<true, 256, 4, true><<<static_cast<uint32_t>(ctas), 256, 0, st>>>(Rw);
-                else rs32_encode_row_kernel<false, 256, 4, true><<<static_cast<uint32_t>(ctas), 256, 0, st>>>(Rw);
-                coder->last_kernel = Rw.planes ? "rs32_encode_row_kernel<segmented>+tally" : "rs32_encode_row_kernel<segmented>";
-                SS_CUDA(cudaGetLastError());
-                ctx->launches++;
-                return SS_OK;
-            }
-            // resident CTAs per SM (2048 threads, 32 CTAs) x a few waves; every CTA strides over codewords
-            uint32_t per_sm = 2048u / threads; if (per_sm > 32u) per_sm = 32u;
-            const int vr = coder->variant & 15, vchunk = (coder->variant >> 4) & 1, vw = (coder->variant >> 5) & 7;
-            static const uint64_t kWaves[8] = {64, 1, 32, 4, 16, 256, 128, 8};   // [0] = default, rest: tuning
-            // Local planes (the accept step): by default a CTA per codeword.  The block scheduler then hands codewords
-            // out in order, so the whole GPU reads and writes one narrow, advancing window of memory; on an H100 that
-            // measured 2.6 % faster than 64 or 256 waves of CTAs striding over the batch (DESIGN.md 3.1).
-            const uint64_t waves = (vw == 0 && !Rw.emit_data) ? (1ull << 32) : kWaves[vw];
-            uint64_t ctas = static_cast<uint64_t>(ctx->sm_count) * per_sm * waves;
-            if (ctas > g.n) ctas = g.n;
-            if (ctas > 0x7fffffffull) ctas = 0x7fffffffull;
-            Rw.chunk = 0;
-            Rw.st_mode = static_cast<uint32_t>((coder->variant >> 8) & 3);
-            Rw.rotate = ((coder->variant >> 10) & 1) ? 0u : 1u;
-            // local planes: the tally goes after the CTA's codeword, so its first loads are the payload's
-            Rw.tally_last = Rw.emit_data ? 0u : 1u;
-            if (vchunk) { Rw.chunk = static_cast<uint32_t>((g.n + ctas - 1) / ctas); ctas = (g.n + Rw.chunk - 1) / Rw.chunk; }
-            const uint32_t grid = static_cast<uint32_t>(ctas);
-            // register budget variants (tuning knob ss_rs_set_variant): 0/2 = 40 regs, 3 = 32 regs, 4 = unconstrained
-            // Register budget: 40/thread (12 CTAs of <= 128 threads per SM; the kernel needs ~47 unconstrained and fits
-            // 40 without spilling); a CTA per codeword for local planes, 64 waves of CTAs otherwise.  The other budgets and
-            // wave counts stay selectable for tuning.
-            if (threads > 128) {
-                if (Rw.emit_data) rs32_encode_row_kernel<true, 256, 4><<<grid, threads, 0, st>>>(Rw);
-                else rs32_encode_row_kernel<false, 256, 4><<<grid, threads, 0, st>>>(Rw);
-            } else if (Rw.emit_data) rs32_encode_row_kernel<true, 128, 8><<<grid, threads, 0, st>>>(Rw);
-            else if (vr == 3) rs32_encode_row_kernel<false, 128, 16><<<grid, threads, 0, st>>>(Rw);   // 32 regs
-            else if (vr == 6) rs32_encode_row_kernel<false, 128, 8><<<grid, threads, 0, st>>>(Rw);    // 64 regs cap
-            else if (vr == 7) rs32_encode_row_kernel<false, 128, 9><<<grid, threads, 0, st>>>(Rw);    // 56 regs cap
-            else rs32_encode_row_kernel<false, 128, 12, false, true><<<grid, threads, 0, st>>>(Rw);    // 40 regs, L2 prefetch
-            coder->last_kernel = Rw.planes ? "rs32_encode_row_kernel+tally" : "rs32_encode_row_kernel";
-            SS_CUDA(cudaGetLastError());
-            ctx->launches++;
-            return SS_OK;
-        }
-
-        // ---- generic row kernel: any code with d <= 8, aligned uniform geometry, codewords up to 256 columns ----
-        if (!use_rs32 && d <= 8 && coder->enc_hmT8 != nullptr && (coder->variant & 15) != 5 && (coder->variant & 15) != 1 &&
-            padded && vpc >= 1 && g.n <= 0xffffffffull &&
-            ((reinterpret_cast<uintptr_t>(g.data) | g.data_stride) & 15u) == 0u &&
-            (tally == nullptr || tally->planes == nullptr || tally->G == g.n)) {
-            EncRowGen Rg;
-            Rg.data = g.data; Rg.data_stride = g.data_stride;
-            for (int j = 0; j < 16; ++j) {
-                if (j >= d + p) Rg.plane[j] = nullptr;
-                else if (g.plane_ptrs != nullptr) Rg.plane[j] = g.plane_ptrs[j];
-                else Rg.plane[j] = g.parity + (static_cast<int64_t>(j) - d) * static_cast<int64_t>(g.plane_stride);
-            }
-            Rg.emit_data = ((g.flags & SS_RS_EMIT_DATA) || g.plane_ptrs != nullptr) ? 1u : 0u;
-            Rg.wait = g.wait;
-            Rg.shard_stride = g.shard_stride; Rg.n = static_cast<uint32_t>(g.n); Rg.len = len; Rg.L = L; Rg.vpc = vpc;
-            // columns whose every source window lies inside the payload and whose output vector is complete
-            const uint64_t last_shard_bytes = static_cast<uint64_t>(len) >= static_cast<uint64_t>(d - 1) * L
-                                                  ? static_cast<uint64_t>(len) - static_cast<uint64_t>(d - 1) * L : 0;
-            Rg.fast_cols = static_cast<uint32_t>((last_shard_bytes < L ? last_shard_bytes : L) / 16u);
-            Rg.d = static_cast<uint32_t>(d); Rg.p = static_cast<uint32_t>(p);
-            Rg.hmT8 = static_cast<const uint32_t *>(coder->enc_hmT8);
-            for (int j = 0; j < kMaxP; ++j) Rg.top[j] = coder->enc_top[j];
-            Rg.planes = nullptr; Rg.R = 0; Rg.threshold = 0; Rg.committed = nullptr; Rg.commit_bar = nullptr;
-            if (tally != nullptr && tally->planes != nullptr) {
-                Rg.planes = tally->planes; Rg.R = tally->R; Rg.threshold = tally->threshold;
-                Rg.committed = tally->committed; Rg.commit_bar = tally->commit_bar;
-            }
-            // which flavour of the kernels: a compile-time cluster code, the coder's own NVRTC specialisation (any other
-            // matrix; compiled on first use), or run-time coefficient masks (variant bit 11 forces them, bit 17 skips NVRTC)
-            int sc = ((coder->variant >> 11) & 1) ? kCodeGeneric : coder->static_code;
-            const bool jit_allowed = sc == kCodeGeneric && !((coder->variant >> 11) & 1) && !((coder->variant >> 17) & 1);
-            auto launch_jit = [&](int which, uint32_t grid_x, uint32_t block_x) -> int {
-                void *args[] = {&Rg};
-                SS_CUDA(cudaLaunchKernel(reinterpret_cast<const void *>(coder->jit_kernel[which]), dim3(grid_x), dim3(block_x), args, 0, st));
-                return SS_OK;
-            };
-            // Packed flavour when the one-codeword-per-pass layout would idle or mask a good part of the lanes
-            // (bit 13 forces it off, bit 14 forces it on).
-            const uint32_t fc = Rg.fast_cols;
-            const uint32_t row_threads = vpc > 256u ? 256u : ((vpc + 31u) & ~31u);    // wider codewords: 256-column segments
-            bool packed = (fc != vpc || row_threads != vpc) && vpc <= 256u;
-            if ((coder->variant >> 13) & 1) packed = false;
-            if ((coder->variant >> 14) & 1) packed = true;
-            // software-pipelined main loop: always when every shard is 16-byte aligned; bit 15 selects it for unaligned too
-            const bool pipe = (L & 15u) == 0u || ((coder->variant >> 15) & 1);
-            if (jit_allowed) {
-                // the one instance this geometry needs (compiled by NVRTC on first use, ~1 s; then cached in the coder)
-                const int which = packed ? ((L & 15u) == 0u ? 2 : pipe ? 3 : 4) : (row_threads > 128u ? 1 : 0);
-                if (jit_ensure(coder, which) == SS_OK) sc = kCodeJit;
-            }
-            if (packed) {
-                // threads: the multiple of 32 (<= 256) that wastes the fewest lanes; ties go to the larger CTA
-                uint32_t T = 256, m = fc ? 256u / fc : 0u;
-                if (fc) {
-                    double best = -1.0;
-                    for (uint32_t t = 256; t >= 64; t -= 32) {
-                        const uint32_t mm = t / fc;
-                        const double eff = static_cast<double>(mm * fc) / t;
-                        if (eff > best + 1e-9) { best = eff; T = t; m = mm; }
-                    }
-                }
-                Rg.pack_m = m;
-                Rg.ntail = vpc - fc;
-                const uint64_t tail_items = g.n * Rg.ntail;
-                const uint64_t tail_ctas = (tail_items + T - 1) / T;
-                uint64_t main_ctas = 0;
-                if (m) {
-                    const uint32_t dcap = d <= 2 ? 2 : d == 3 ? 3 : d == 4 ? 4 : d <= 6 ? 6 : 8;      // dispatch_d's capacity
-                    const uint32_t dt = sc != kCodeGeneric ? static_cast<uint32_t>(d) : dcap;       // static and NVRTC kernels are exact-width
-                    const uint32_t reg_need = 4u * dt + ((L & 15u) == 0u ? 4u * dt : 8u * dt - 4u) + 22u;
-                    uint32_t rb = 65536u / (256u * reg_need); rb = rb > 6u ? 6u : (rb < 1u ? 1u : rb);
-                    if (!pipe) rb = dt <= 3 ? 6u : dt <= 5 ? 5u : dt <= 6 ? 4u : 3u;
-                    const uint32_t resident_threads = 256u * rb;
-                    main_ctas = static_cast<uint64_t>(ctx->sm_count) * (resident_threads / T) * 64ull;
-                    const uint64_t need = (g.n + m - 1) / m;
-                    if (main_ctas > need) main_ctas = need;
-                }
-                if (tail_ctas + main_ctas <= 0x7fffffffull) {
-                    Rg.tail_ctas = static_cast<uint32_t>(tail_ctas);
-                    const uint32_t grid = static_cast<uint32_t>(tail_ctas + main_ctas);
-                    auto gop = [&](auto DC, auto CC) {
-                        constexpr int kD = decltype(DC)::value, kC = decltype(CC)::value;
-                        if ((L & 15u) == 0u) horner_encode_packed_kernel<kD, kC, true, true><<<grid, T, 0, st>>>(Rg);
-                        else if (pipe) horner_encode_packed_kernel<kD, kC, false, true><<<grid, T, 0, st>>>(Rg);
-                        else horner_encode_packed_kernel<kD, kC, false, false><<<grid, T, 0, st>>>(Rg);
-                    };
-                    auto gop_static = [&](auto CC) {
-                        constexpr int C = decltype(CC)::value;
-                        gop(std::integral_constant<int, static_code_d(C)>{}, CC);
-                    };
-                    switch (sc) {
-                        case kCodeJit: SS_TRY(launch_jit((L & 15u) == 0u ? 2 : pipe ? 3 : 4, grid, T)); break;
-                        case kCode21: gop_static(std::integral_constant<int, kCode21>{}); break;
-                        case kCode43: gop_static(std::integral_constant<int, kCode43>{}); break;
-                        case kCode54: gop_static(std::integral_constant<int, kCode54>{}); break;
-                        case kCode42: gop_static(std::integral_constant<int, kCode42>{}); break;
-                        case kCode31: gop_static(std::integral_constant<int, kCode31>{}); break;
-                        default:
-                            SS_TRY(dispatch_d(d, [&](auto DC) {
-                                gop(DC, std::integral_constant<int, kCodeGeneric>{});
-                                return SS_OK;
-                            }));
-                    }
-                    if (sc == kCodeJit)
-                        coder->last_kernel = Rg.planes ? "horner_encode_packed_kernel<nvrtc>+tally" : "horner_encode_packed_kernel<nvrtc>";
-                    else if (sc != kCodeGeneric)
-                        coder->last_kernel = Rg.planes ? "horner_encode_packed_kernel<static code>+tally" : "horner_encode_packed_kernel<static code>";
-                    else
-                        coder->last_kernel = Rg.planes ? "horner_encode_packed_kernel+tally" : "horner_encode_packed_kernel";
-                    SS_CUDA(cudaGetLastError());
-                    ctx->launches++;
-                    return SS_OK;
-                }
-            }
-            Rg.pack_m = 0; Rg.tail_ctas = 0; Rg.ntail = 0;
-            const uint32_t threads = row_threads;
-            if (sc == kCodeJit && jit_ensure(coder, threads > 128u ? 1 : 0) != SS_OK) sc = kCodeGeneric;   // (packed grid did not fit)
-            uint32_t per_sm = 2048u / threads; if (per_sm > 32u) per_sm = 32u;
-            uint64_t ctas = static_cast<uint64_t>(ctx->sm_count) * per_sm * 64ull;
-            if (ctas > g.n) ctas = g.n;
-            const uint32_t grid = static_cast<uint32_t>(ctas);
-            // register budget (variant bits 0-3): threads <= 128: 0 = 12 CTAs/SM (40 regs), 2 = 10 (48), 3 = 8 (64), 4 = 6 (80)
-            const int vbits = coder->variant & 15;
-            auto go = [&](auto DC, auto CC) {
-                constexpr int kD = decltype(DC)::value, kC = decltype(CC)::value;
-                // default budget by width: spill-free at 40 registers up to d = 4, 48 for 5, 64 for 6, 80 beyond
-                const int vdef = kD <= 4 ? 0 : kD == 5 ? 2 : kD == 6 ? 3 : 4;
-                const int vb = (vbits >= 2 && vbits <= 4) ? vbits : vdef;      // other values select other kernels' knobs
-                if (threads > 128) horner_encode_row_kernel<kD, kC, 256, 3><<<grid, threads, 0, st>>>(Rg);
-                else if (vb == 2) horner_encode_row_kernel<kD, kC, 128, 10><<<grid, threads, 0, st>>>(Rg);
-                else if (vb == 3) horner_encode_row_kernel<kD, kC, 128, 8><<<grid, threads, 0, st>>>(Rg);
-                else if (vb == 4) horner_encode_row_kernel<kD, kC, 128, 6><<<grid, threads, 0, st>>>(Rg);
-                else horner_encode_row_kernel<kD, kC, 128, 12><<<grid, threads, 0, st>>>(Rg);
-            };
-            auto go_static = [&](auto CC) {
-                constexpr int C = decltype(CC)::value;
-                go(std::integral_constant<int, static_code_d(C)>{}, CC);
-            };
-            switch (sc) {
-                case kCodeJit: SS_TRY(launch_jit(threads > 128 ? 1 : 0, grid, threads)); break;
-                case kCode21: go_static(std::integral_constant<int, kCode21>{}); break;
-                case kCode43: go_static(std::integral_constant<int, kCode43>{}); break;
-                case kCode54: go_static(std::integral_constant<int, kCode54>{}); break;
-                case kCode42: go_static(std::integral_constant<int, kCode42>{}); break;
-                case kCode31: go_static(std::integral_constant<int, kCode31>{}); break;
-                default:
-                    SS_TRY(dispatch_d(d, [&](auto DC) {
-                        go(DC, std::integral_constant<int, kCodeGeneric>{});
-                        return SS_OK;
-                    }));
-            }
-            if (sc == kCodeJit)
-                coder->last_kernel = Rg.planes ? "horner_encode_row_kernel<nvrtc>+tally" : "horner_encode_row_kernel<nvrtc>";
-            else if (sc != kCodeGeneric)
-                coder->last_kernel = Rg.planes ? "horner_encode_row_kernel<static code>+tally" : "horner_encode_row_kernel<static code>";
-            else
-                coder->last_kernel = Rg.planes ? "horner_encode_row_kernel+tally" : "horner_encode_row_kernel";
-            SS_CUDA(cudaGetLastError());
-            ctx->launches++;
-            return SS_OK;
-        }
-        // chunk so that n_chunk * vpc fits in 32 bits
-        const uint64_t max_cw = vpc ? (0xffffff00ull / vpc) : g.n;
-        uint64_t done = 0;
-        bool tally_pending = tally != nullptr && tally->planes != nullptr;
-        do {
-            const uint64_t nc = (g.n - done) < max_cw ? (g.n - done) : max_cw;
-            EncUniform E;
-            E.data = g.data + done * g.data_stride;
-            E.data_stride = g.data_stride;
-            E.len = len; E.L = L; E.vpc = vpc;
-            E.parity = g.parity + done * g.shard_stride;
-            E.plane_stride = g.plane_stride; E.shard_stride = g.shard_stride;
-            E.n = nc;
-            E.total = static_cast<uint32_t>(nc * vpc);
-            E.padded = (padded ? 1u : 0u) | ((g.flags & SS_RS_EMIT_DATA) ? 2u : 0u);
-            E.planes = nullptr; E.R = 0; E.threshold = 0; E.G = 0; E.committed = nullptr; E.commit_bar = nullptr;
-            uint64_t threads = E.total;
-            if (tally_pending) {
-                if (tally->G > 0xffffff00ull) return set_error(SS_ERR_INVALID_ARG, "too many groups for one fused launch");
-                E.planes = tally->planes; E.R = tally->R; E.threshold = tally->threshold; E.G = tally->G;
-                E.committed = tally->committed; E.commit_bar = tally->commit_bar;
-                if (threads < tally->G) threads = tally->G;
-                tally_pending = false;
-            }
-            if (threads == 0) break;
-            const uint32_t grid = static_cast<uint32_t>((threads + kThreads - 1) / kThreads);
-            if (use_rs32) {
-                rs32_encode_uniform_kernel<<<grid, kThreads, 0, st>>>(E);
-                coder->last_kernel = E.planes ? "rs32_encode_uniform_kernel+tally" : "rs32_encode_uniform_kernel";
-            } else if (d <= 8 && (coder->variant & 15) != 5) {
-                const uint32_t *prog = static_cast<const uint32_t *>(coder->enc_prog);
-                SS_TRY(dispatch_d(d, [&](auto DC) {
-                    horner_encode_uniform_kernel<decltype(DC)::value><<<grid, kThreads, 0, st>>>(E, prog, d, p);
-                    return SS_OK;
-                }));
-                coder->last_kernel = "horner_encode_uniform_kernel";
-            } else {
-                const uint32_t *prog = static_cast<const uint32_t *>(coder->enc_prog);
-                SS_TRY(dispatch_p(p, [&](auto PC) {
-                    generic_encode_uniform_kernel<decltype(PC)::value><<<grid, kThreads, 0, st>>>(E, prog, d, p);
-                    return SS_OK;
-                }));
-                coder->last_kernel = "generic_encode_uniform_kernel";
-            }
-            SS_CUDA(cudaGetLastError());
-            ctx->launches++;
-            done += nc;
-        } while (done < g.n);
-        return SS_OK;
-    }
-
-    // ---- ragged geometry: a warp per codeword ----
     if (g.n == 0) return SS_OK;
     if (g.data_len == nullptr || g.par_off == nullptr)
         return set_error(SS_ERR_INVALID_ARG, "ragged encode needs data_off, data_len and par_off");
     EncRagged E;
     E.data = g.data; E.data_off = g.data_off; E.data_len = g.data_len;
     E.parity = g.parity; E.plane_stride = g.plane_stride; E.par_off = g.par_off;
-    E.n = g.n; E.padded = (padded ? 1u : 0u) | ((g.flags & SS_RS_EMIT_DATA) ? 2u : 0u);
+    E.n = g.n; E.padded = ((g.flags & SS_RS_OUT_PADDED16) ? 1u : 0u) | ((g.flags & SS_RS_EMIT_DATA) ? 2u : 0u);
     const uint32_t grid = ragged_grid(ctx, g.n);
-    if (use_rs32) {
-        rs32_encode_ragged_kernel<<<grid, kThreads, 0, st>>>(E);
+    const uint32_t *prog = static_cast<const uint32_t *>(coder->enc_prog);
+    if (coder->is_rs32) {
+        rs32_encode_ragged_kernel<<<grid, kThreads, 0, ctx->stream>>>(E);
         coder->last_kernel = "rs32_encode_ragged_kernel";
     } else if (d <= 8 && (coder->variant & 15) != 5) {
-        const uint32_t *prog = static_cast<const uint32_t *>(coder->enc_prog);
         SS_TRY(dispatch_d(d, [&](auto DC) {
-            horner_encode_ragged_kernel<decltype(DC)::value><<<grid, kThreads, 0, st>>>(E, prog, d, p);
+            horner_encode_ragged_kernel<decltype(DC)::value><<<grid, kThreads, 0, ctx->stream>>>(E, prog, d, p);
             return SS_OK;
         }));
         coder->last_kernel = "horner_encode_ragged_kernel";
     } else {
-        const uint32_t *prog = static_cast<const uint32_t *>(coder->enc_prog);
         SS_TRY(dispatch_p(p, [&](auto PC) {
-            generic_encode_ragged_kernel<decltype(PC)::value><<<grid, kThreads, 0, st>>>(E, prog, d, p);
+            generic_encode_ragged_kernel<decltype(PC)::value><<<grid, kThreads, 0, ctx->stream>>>(E, prog, d, p);
             return SS_OK;
         }));
         coder->last_kernel = "generic_encode_ragged_kernel";
     }
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    if (tally != nullptr && tally->planes != nullptr)
-        return launch_tally_planes(ctx, tally->planes, tally->R, tally->G, tally->threshold, tally->committed,
-                                   tally->commit_bar);
-    return SS_OK;
+    SS_TRY(launched(ctx));
+    if (tally == nullptr) return SS_OK;
+    return launch_tally_planes(ctx, tally->planes, tally->R, tally->G, tally->threshold, tally->committed, tally->commit_bar);
+}
+
+int launch_rs_encode(ss_rs_coder *coder, const EncGeom &g, const TallyArgs *tally) {
+    SS_TRY(ctx_bind(coder->ctx));
+    if (!coder->batch_ok)
+        return set_error(SS_ERR_UNSUPPORTED, "batched encode needs d <= %d, p <= %d (coder is %d,%d)", kMaxD,
+                         kMaxP, coder->d, coder->p);
+    const bool padded = (g.flags & SS_RS_OUT_PADDED16) != 0u;
+    if (padded && ((reinterpret_cast<uintptr_t>(g.parity) | g.plane_stride) & 15u))
+        return set_error(SS_ERR_INVALID_ARG, "SS_RS_OUT_PADDED16 needs 16-byte aligned parity base and plane_stride");
+    if (tally != nullptr && tally->planes == nullptr) tally = nullptr;     // no ack planes: nothing to tally
+    if (g.data_off != nullptr) return encode_ragged(coder, g, tally);
+
+    // uniform geometry
+    const uint32_t len = g.uni_len;
+    if ((len == 0u || g.n == 0u) && tally == nullptr) return SS_OK;
+    if (len >= 0x7fffffffu) return set_error(SS_ERR_INVALID_ARG, "data_len too large");
+    const uint32_t d = static_cast<uint32_t>(coder->d);
+    const uint32_t L = len == 0u ? 0u : (len + d - 1u) / d;
+    const uint32_t vpc = (L + 15u) >> 4;
+    if (padded && (g.shard_stride & 15u))
+        return set_error(SS_ERR_INVALID_ARG, "SS_RS_OUT_PADDED16 needs shard_stride %% 16 == 0");
+    if (padded && g.shard_stride < static_cast<uint64_t>(vpc) * 16u)
+        return set_error(SS_ERR_INVALID_ARG, "shard_stride %llu < padded shard length %u",
+                         (unsigned long long)g.shard_stride, vpc * 16u);
+    // The row kernels take 16-byte aligned payload rows into padded shard slots, codewords of at least one column,
+    // a batch whose size fits 32 bits, and a fused tally over exactly the batch's groups.  Variant bits 0-3 = 1 select
+    // the flat kernels instead, 5 the bit-plane ones.
+    const int vk = coder->variant & 15;
+    const bool row_geometry = padded && vpc >= 1 && g.n <= 0xffffffffull &&
+                              ((reinterpret_cast<uintptr_t>(g.data) | g.data_stride) & 15u) == 0u &&
+                              (tally == nullptr || tally->G == g.n);
+    const bool rs32_row = coder->is_rs32 && vk != 1 && row_geometry;
+    const bool horner_row = !coder->is_rs32 && d <= 8 && coder->enc_hmT8 != nullptr && vk != 5 && vk != 1 && row_geometry;
+    if (rs32_row) return encode_rs32_row(coder, g, tally, len, L, vpc);
+    if (horner_row) return encode_horner_row(coder, g, tally, len, L, vpc);
+    return encode_flat(coder, g, tally, len, L, vpc);
 }
 
 int launch_rs_reconstruct(ss_rs_coder *coder, uint8_t *shards, uint64_t plane_stride, const uint64_t *off,
@@ -1957,20 +1930,19 @@ int launch_rs_reconstruct(ss_rs_coder *coder, uint8_t *shards, uint64_t plane_st
     if (coder->d <= 4 && A.fast_progs != nullptr && (coder->variant & 15) != 5 && (coder->variant & 15) != 8) {
         const bool smem = A.fast_bytes <= 40u * 1024u;
         const size_t sb = smem ? A.fast_bytes : 0;
-#define SS_SMALL(DD)                                                                                       \
-        do {                                                                                                   \
-            const bool pair = A.padded && ((coder->variant >> 16) & 1);    /* bit 16: two columns per lane and pass */      \
-            if (smem && pair) rs_reconstruct_small_kernel<DD, true, true, true><<<grid, kThreads, sb, ctx->stream>>>(A);         \
-            else if (smem && A.padded) rs_reconstruct_small_kernel<DD, true, true, false><<<grid, kThreads, sb, ctx->stream>>>(A); \
-            else if (smem) rs_reconstruct_small_kernel<DD, true, false, false><<<grid, kThreads, sb, ctx->stream>>>(A);          \
-            else if (pair) rs_reconstruct_small_kernel<DD, false, true, true><<<grid, kThreads, 0, ctx->stream>>>(A);            \
-            else if (A.padded) rs_reconstruct_small_kernel<DD, false, true, false><<<grid, kThreads, 0, ctx->stream>>>(A);       \
-            else rs_reconstruct_small_kernel<DD, false, false, false><<<grid, kThreads, 0, ctx->stream>>>(A);                    \
-        } while (0)
-        if (coder->d <= 2) SS_SMALL(2);
-        else if (coder->d == 3) SS_SMALL(3);
-        else SS_SMALL(4);
-#undef SS_SMALL
+        const bool pair = A.padded && ((coder->variant >> 16) & 1);    // bit 16: two columns per lane and pass
+        auto small = [&](auto DC) {
+            constexpr int kD = decltype(DC)::value;
+            if (smem && pair) rs_reconstruct_small_kernel<kD, true, true, true><<<grid, kThreads, sb, ctx->stream>>>(A);
+            else if (smem && A.padded) rs_reconstruct_small_kernel<kD, true, true, false><<<grid, kThreads, sb, ctx->stream>>>(A);
+            else if (smem) rs_reconstruct_small_kernel<kD, true, false, false><<<grid, kThreads, sb, ctx->stream>>>(A);
+            else if (pair) rs_reconstruct_small_kernel<kD, false, true, true><<<grid, kThreads, 0, ctx->stream>>>(A);
+            else if (A.padded) rs_reconstruct_small_kernel<kD, false, true, false><<<grid, kThreads, 0, ctx->stream>>>(A);
+            else rs_reconstruct_small_kernel<kD, false, false, false><<<grid, kThreads, 0, ctx->stream>>>(A);
+        };
+        if (coder->d <= 2) small(std::integral_constant<int, 2>{});
+        else if (coder->d == 3) small(std::integral_constant<int, 3>{});
+        else small(std::integral_constant<int, 4>{});
         coder->last_kernel = smem ? "rs_reconstruct_small_kernel(smem programs)" : "rs_reconstruct_small_kernel";
     } else if (coder->d <= 8 && (coder->variant & 15) != 5) {
         SS_TRY(dispatch_d(coder->d, [&](auto DC) {
@@ -1985,9 +1957,7 @@ int launch_rs_reconstruct(ss_rs_coder *coder, uint8_t *shards, uint64_t plane_st
         }));
         coder->last_kernel = "generic_reconstruct_kernel";
     }
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int launch_rs_reconstruct_uniform(ss_rs_coder *coder, uint8_t *shards, uint64_t plane_stride, uint64_t shard_stride,
@@ -2019,9 +1989,7 @@ int launch_rs_reconstruct_uniform(ss_rs_coder *coder, uint8_t *shards, uint64_t 
             else rs32_reconstruct_row_kernel<false, 128, 12><<<grid, threads, 0, ctx->stream>>>(P);
         }
         coder->last_kernel = "rs32_reconstruct_row_kernel";
-        SS_CUDA(cudaGetLastError());
-        ctx->launches++;
-        return SS_OK;
+        return launched(ctx);
     }
     // any other code: the per-pattern program kernels over synthesised offsets
     void *scr = nullptr;
@@ -2030,8 +1998,7 @@ int launch_rs_reconstruct_uniform(ss_rs_coder *coder, uint8_t *shards, uint64_t 
     uint32_t *len = reinterpret_cast<uint32_t *>(off + n);
     uint64_t mg = (n + 255) / 256; if (mg > 4096) mg = 4096;
     uniform_meta_kernel<<<static_cast<uint32_t>(mg), 256, 0, ctx->stream>>>(off, len, n, shard_stride, data_len);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
+    SS_TRY(launched(ctx));
     return launch_rs_reconstruct(coder, shards, plane_stride, off, len, present, n, data_only, status, SS_RS_OUT_PADDED16);
 }
 

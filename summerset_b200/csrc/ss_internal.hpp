@@ -128,6 +128,13 @@ void ctx_retain(ss_ctx *ctx);                           // a handle (coder, engi
 void ctx_release(ss_ctx *ctx);                          // ... and stops; tears ctx down if it was destroyed meanwhile
 int ctx_scratch(ss_ctx *ctx, size_t bytes, void **out); // grow-only scratch
 
+// closes every kernel launch: reports a launch error, else counts the launch (ss_ctx_launch_count)
+inline int launched(ss_ctx *ctx) {
+    SS_CUDA(cudaGetLastError());
+    ctx->launches++;
+    return SS_OK;
+}
+
 // exclusive prefix sum of x[0..n) in place (engine.cu); partials: scan_tiles(n) words of device scratch; total (device,
 // may be NULL) = the sum of all n values.  Deterministic: integer sums in a fixed order.
 uint64_t scan_tiles(uint64_t n);

@@ -596,18 +596,14 @@ int launch_flag_signal(ss_ctx *ctx, const ss_step_sync *sync) {
         if (A.flag[i] == nullptr || (reinterpret_cast<uintptr_t>(A.flag[i]) & 7u))
             return set_error(SS_ERR_INVALID_ARG, "signal flag %u is null or not 8-byte aligned", i);
     flag_signal_kernel<<<1, 32, 0, ctx->stream>>>(A);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int launch_flag_wait(ss_ctx *ctx, const dev::FlagWait &w) {
     if (w.flags == nullptr) return SS_OK;
     SS_TRY(ctx_bind(ctx));
     flag_wait_kernel<<<1, 32, 0, ctx->stream>>>(w);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int launch_follower_ack(ss_ctx *ctx, const uint64_t *ack_src, uint64_t *const *ack_dst, uint32_t R, uint64_t G,
@@ -627,9 +623,7 @@ int launch_follower_ack(ss_ctx *ctx, const uint64_t *ack_src, uint64_t *const *a
     const uint64_t cap = static_cast<uint64_t>(ctx->sm_count) * 2ull;     // small, latency-bound: two CTAs per SM are plenty
     if (ctas > cap) ctas = cap;
     follower_ack_kernel<<<static_cast<uint32_t>(ctas), kTallyThreads, 0, ctx->stream>>>(A);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 static inline uint32_t stream_grid(ss_ctx *ctx, uint64_t items) {
@@ -657,14 +651,10 @@ int launch_tally_planes(ss_ctx *ctx, const uint64_t *planes, uint32_t R, uint64_
         else if (R == 3) tally_planes_x2_kernel<3><<<grid, kTallyThreads, 0, ctx->stream>>>(p2, R, G2, thr, c2, b2);
         else if (R == 7) tally_planes_x2_kernel<7><<<grid, kTallyThreads, 0, ctx->stream>>>(p2, R, G2, thr, c2, b2);
         else tally_planes_x2_kernel<0><<<grid, kTallyThreads, 0, ctx->stream>>>(p2, R, G2, thr, c2, b2);
-        SS_CUDA(cudaGetLastError());
-        ctx->launches++;
-        return SS_OK;
+        return launched(ctx);
     }
     tally_planes_kernel<<<stream_grid(ctx, G), kTallyThreads, 0, ctx->stream>>>(planes, R, G, thr, committed, commit_bar);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int launch_tally_masks(ss_ctx *ctx, const void *masks, uint32_t mask_bytes, uint64_t n, uint32_t thr,
@@ -680,9 +670,7 @@ int launch_tally_masks(ss_ctx *ctx, const void *masks, uint32_t mask_bytes, uint
     } else {
         return set_error(SS_ERR_INVALID_ARG, "mask_bytes must be 1 or 2, got %u", mask_bytes);
     }
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int launch_ack_ingest(ss_ctx *ctx, const uint32_t *rec_group, const uint8_t *rec_slot, const uint8_t *rec_peer,
@@ -694,9 +682,7 @@ int launch_ack_ingest(ss_ctx *ctx, const uint32_t *rec_group, const uint8_t *rec
     if (n_records == 0) return SS_OK;
     ack_ingest_kernel<<<stream_grid(ctx, n_records), kTallyThreads, 0, ctx->stream>>>(
         rec_group, rec_slot, rec_peer, rec_ballot, n_records, bal_prepared, inst_bal, accepting, window_base, R, G, planes);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int launch_tally_crossword(ss_ctx *ctx, const void *masks, uint32_t mask_bytes, const uint8_t *policy_idx,
@@ -724,8 +710,7 @@ int launch_tally_crossword(ss_ctx *ctx, const void *masks, uint32_t mask_bytes, 
     SS_CUDA(cudaMemsetAsync(d_lut, 0, lut_words * 4, ctx->stream));
     crossword_lut_kernel<<<(entries + 127) / 128, 128, 0, ctx->stream>>>(d_pol, n_policies, n_replicas, T, d, majority,
                                                                          f, balanced, d_lut);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
+    SS_TRY(launched(ctx));
     const uint32_t grid = stream_grid(ctx, ((n + 63) / 64) * 8);
     const size_t smem = lut_words * 4;
     if (mask_bytes == 1)
@@ -736,9 +721,7 @@ int launch_tally_crossword(ss_ctx *ctx, const void *masks, uint32_t mask_bytes, 
         tally_crossword_kernel<uint16_t><<<grid, kTallyThreads, smem, ctx->stream>>>(
             static_cast<const uint16_t *>(masks), policy_idx, n, d_lut, lut_words, n_policies, n_replicas,
             reinterpret_cast<uint8_t *>(commit_bits));
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int launch_raft_scan(ss_ctx *ctx, const uint32_t *match, uint32_t n_peers, uint64_t G, const uint32_t *last_commit,
@@ -761,9 +744,7 @@ int launch_raft_scan(ss_ctx *ctx, const uint32_t *match, uint32_t n_peers, uint6
     else if (n_peers <= 8) SS_RAFT_LAUNCH(8);
     else SS_RAFT_LAUNCH(16);
 #undef SS_RAFT_LAUNCH
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int launch_raft_scan_ring(ss_ctx *ctx, const uint32_t *match, uint32_t n_peers, uint64_t G, const uint32_t *last_commit,
@@ -779,9 +760,7 @@ int launch_crossword_lut(ss_ctx *ctx, const uint32_t *d_policies, uint32_t n_pol
     SS_CUDA(cudaMemsetAsync(d_lut_bits, 0, ((entries + 31) / 32) * 4, ctx->stream));
     crossword_lut_kernel<<<(entries + 127) / 128, 128, 0, ctx->stream>>>(d_policies, n_policies, n_replicas, T, d, majority, f,
                                                                          balanced, d_lut_bits);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int launch_kth_match(ss_ctx *ctx, const uint32_t *match, uint32_t n_peers, uint64_t G, uint32_t k, uint32_t *out) {
@@ -795,9 +774,7 @@ int launch_kth_match(ss_ctx *ctx, const uint32_t *match, uint32_t n_peers, uint6
     else if (n_peers <= 6) kth_match_kernel<6><<<grid, kTallyThreads, 0, ctx->stream>>>(match, n_peers, G, k, out);
     else if (n_peers <= 8) kth_match_kernel<8><<<grid, kTallyThreads, 0, ctx->stream>>>(match, n_peers, G, k, out);
     else kth_match_kernel<16><<<grid, kTallyThreads, 0, ctx->stream>>>(match, n_peers, G, k, out);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int launch_prepare_merge(ss_ctx *ctx, const uint64_t *vote_bal, const uint32_t *vote_mask, uint32_t R, uint64_t N,
@@ -809,9 +786,7 @@ int launch_prepare_merge(ss_ctx *ctx, const uint64_t *vote_bal, const uint32_t *
     if (N == 0) return SS_OK;
     prepare_merge_kernel<<<stream_grid(ctx, N), kTallyThreads, 0, ctx->stream>>>(vote_bal, vote_mask, R, N, acks_cnt, d,
                                                                                 population, f, max_bal, merged, action);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int launch_frame_accept(ss_ctx *ctx, const uint8_t *plane, uint64_t shard_stride, uint32_t shard_idx, uint32_t d, uint32_t p,
@@ -834,9 +809,7 @@ int launch_frame_accept(ss_ctx *ctx, const uint8_t *plane, uint64_t shard_stride
     const uint64_t cap = static_cast<uint64_t>(ctx->sm_count) * 8ull * 8ull;
     if (ctas > cap) ctas = cap;
     frame_accept_kernel<<<static_cast<uint32_t>(ctas), kTallyThreads, 0, ctx->stream>>>(A);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int launch_gossip_plan(ss_ctx *ctx, uint32_t me, uint32_t population, uint32_t d, const uint8_t *src_peer,
@@ -854,9 +827,7 @@ int launch_gossip_plan(ss_ctx *ctx, uint32_t me, uint32_t population, uint32_t d
     gossip_plan_kernel<<<stream_grid(ctx, N), kTallyThreads, 0, ctx->stream>>>(
         me, population, d, src_peer, avail, policy_idx, static_cast<const uint32_t *>(scratch), n_policies, peer_alive, N,
         targets, excl);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 }  // namespace ssb

@@ -419,9 +419,7 @@ int ss_frame_accept_pack_dev(ss_ctx *ctx, const ss_frame_spec *s, const uint8_t 
     A.slot = slot; A.ballot = ballot; A.n = n; A.out = out; A.frame_stride = frame_stride; A.frame_off = frame_off; A.frame_len = frame_len;
     if (shard_stride < ((uint64_t(A.L) + 15) & ~uint64_t(15))) return set_error(SS_ERR_INVALID_ARG, "shard_stride shorter than a padded shard");
     frame_pack_kernel<<<wire_grid(ctx, n, kWireThreads / 32), kWireThreads, 0, ctx->stream>>>(A);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int ss_frame_accept_pack_ragged_dev(ss_ctx *ctx, const ss_frame_spec *s, const uint8_t *shard_planes, uint64_t plane_stride,
@@ -456,13 +454,10 @@ int ss_frame_accept_pack_ragged_dev(ss_ctx *ctx, const ss_frame_spec *s, const u
     void *scr = nullptr;
     SS_TRY(ctx_scratch(ctx, scan_tiles(n) * 8, &scr));
     frame_size_ragged_kernel<<<wire_grid(ctx, n, kWireThreads), kWireThreads, 0, ctx->stream>>>(A);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
+    SS_TRY(launched(ctx));
     SS_TRY(launch_exclusive_scan_u64(ctx, frame_off, n, static_cast<uint64_t *>(scr), total));
     frame_pack_ragged_kernel<<<wire_grid(ctx, n, kWireThreads / 32), kWireThreads, 0, ctx->stream>>>(A);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int ss_accept_reply_parse_dev(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
@@ -479,9 +474,7 @@ int ss_accept_reply_parse_dev(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len,
     A.window_base = window_base; A.n_frames = n_frames; A.G = n_groups; A.reply_variant = reply_variant; A.with_size = with_size ? 1u : 0u;
     A.rec_group = rec_group; A.rec_slot = rec_slot; A.rec_peer = rec_peer; A.rec_ballot = rec_ballot; A.rec_kind = rec_kind;
     accept_reply_parse_kernel<<<wire_grid(ctx, n_frames, kWireThreads), kWireThreads, 0, ctx->stream>>>(A);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int ss_wal_commit_pack_dev(ss_ctx *ctx, const uint64_t *newly, const uint64_t *window_base, uint64_t n_groups, uint32_t commit_variant,
@@ -493,9 +486,7 @@ int ss_wal_commit_pack_dev(ss_ctx *ctx, const uint64_t *newly, const uint64_t *w
     if (n_groups == 0) return SS_OK;
     wal_commit_pack_kernel<<<wire_grid(ctx, n_groups, kWireThreads), kWireThreads, 0, ctx->stream>>>(
         newly, window_base, n_groups, commit_variant, entries, entry_group, entry_len, capacity, reinterpret_cast<unsigned long long *>(n_entries));
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 int ss_reconstruct_serve_dev(ss_ctx *ctx, const uint8_t *shard_planes, uint64_t plane_stride, uint64_t shard_stride, uint32_t total_shards,
@@ -515,9 +506,7 @@ int ss_reconstruct_serve_dev(ss_ctx *ctx, const uint8_t *shard_planes, uint64_t 
     A.req_group = req_group; A.req_held = req_held; A.req_excl = req_excl; A.req_status = req_status; A.reply_off = reply_off;
     A.n = n_requests; A.reply_mask = reply_mask; A.out = out;
     reconstruct_serve_kernel<<<wire_grid(ctx, n_requests, kWireThreads / 32), kWireThreads, 0, ctx->stream>>>(A);
-    SS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return SS_OK;
+    return launched(ctx);
 }
 
 }  // extern "C"
