@@ -238,7 +238,8 @@ int ss_ack_ingest_dev(ss_ctx *ctx, const uint32_t *rec_group, const uint8_t *rec
  * crossword/mod.rs:866-888, or the single init_assignment when unbalanced, adaptive.rs:129-131).
  * policy_idx[i] selects instance i's policy; masks[i] = which replicas acked.
  * balanced != 0 uses the reference's closed form (:28-33), else the subset enumeration (:35-61).
- * commit iff #acks >= majority && coverage >= data_shards.  n_replicas <= 12, n_policies <= 16. */
+ * commit iff #acks >= majority && coverage >= data_shards.  n_replicas <= 12, n_policies <= 16.
+ * An instance with policy_idx[i] >= n_policies never commits. */
 int ss_tally_crossword_dev(ss_ctx *ctx, const void *masks, uint32_t mask_bytes,
                            const uint8_t *policy_idx, uint64_t n_instances,
                            const uint32_t *policies_host, uint32_t n_policies, uint32_t n_replicas,
@@ -397,7 +398,8 @@ int ss_frame_accept_batch_dev(ss_ctx *ctx, const uint8_t *shard_plane, uint64_t 
  * policies[policy_idx[g]][peer] names (what subset_copy(.., false) builds for that peer: one shard in RSPaxos,
  * rspaxos/request.rs:127-142; spr shards in Crossword, crossword/request.rs:164-185), data_copy None, encoded per
  * utils/rscoding.rs:43-72; with_assignment appends assignment: Vec<Bitmap> = that policy row (utils/bitmap.rs:20-30).
- * policies: DEVICE array [n_policies][population] of shard bitmasks; policy_idx: device [n] or NULL (policy 0).
+ * policies: DEVICE array [n_policies][population] of shard bitmasks; policy_idx: device [n] or NULL (policy 0); an
+ * index >= n_policies also selects policy 0 (here and in ss_frame_accept_pack_ragged_dev).
  * Frame g is written inside out[g*frame_stride ..) at frame_off[g] (placed so that its first shard's bytes are 16-byte
  * aligned) and is frame_len[g] bytes long; frame_stride >= ss_frame_accept_max_len(spec, max shards per frame) -- a
  * frame that would not fit its slot is not written: frame_len[g] = 0 and bit 2 of ss_ctx_device_status is set.
@@ -472,7 +474,7 @@ int ss_reconstruct_serve_dev(ss_ctx *ctx, const uint8_t *shard_planes, uint64_t 
 /* Crossword follower gossip planning (SURVEY 8f-4; crossword/gossiping.rs:35-84 gossip_targets_excl) for
  * n_instances committed-but-incomplete instances of replica `me`: walking peers me+1, me+2, ... (mod population) and
  * skipping the instance's source peer (src_peer[i]) and peers absent from `peer_alive`, a peer is selected when its
- * assigned shards (policies[policy_idx[i]][peer], as in ss_tally_crossword_dev) include one not yet held/asked for;
+ * assigned shards (policies[policy_idx[i]][peer]; an index >= n_policies selects policy 0) include one not yet held/asked for;
  * excl[peer*N + i] = the availability map at that moment (what the Reconstruct message tells the peer to leave out,
  * crossword/messages.rs:577-632); the walk stops once data_shards shards are covered.  targets[i] = selected peers.
  * excl entries of unselected peers are left untouched. */
@@ -549,7 +551,8 @@ int ss_engine_set_prepared_ballots(ss_engine *engine, const uint64_t *ballots);
  * ss_tally_crossword_dev) and whether the balanced closed form applies (crossword/mod.rs:849-850) */
 int ss_engine_set_policies(ss_engine *engine, const uint32_t *policies_host, uint32_t n_policies, int balanced);
 /* payloads: request batch of group g at payloads + g*payload_stride (data_len bytes; NULL for MultiPaxos).  policy:
- * Crossword only, [G] policy index of the new instance (NULL = 0).  *shard_planes (may be NULL) receives the base of
+ * Crossword only, [G] policy index of the new instance (NULL = 0; an index >= n_policies is stored as given, and
+ * ss_engine_tick never commits that instance).  *shard_planes (may be NULL) receives the base of
  * this proposal's T shard planes: shard j of group g at base + j*plane_stride + g*shard_stride.  `slot` (< 64) is
  * relative to each group's window base: the instance is absolute slot window_base[g] + slot, its shards go to shard
  * store slot % keep_slots. */

@@ -8,62 +8,61 @@ import pytest
 import torch
 
 ROOT = Path(__file__).resolve().parent.parent
-BIN = ROOT / "tests" / "cpp" / "test_rscoding"
 
 
-def _build():
+# The executables are built into a per-module temporary directory, never into the source tree: the tree the suite
+# runs from may be read-only, and a binary left there by an earlier run (or another user) must not be reused.
+@pytest.fixture(scope="module")
+def out_dir(tmp_path_factory):
     from summerset_b200 import build as b
     b.build()
-    src = ROOT / "tests" / "cpp" / "test_rscoding.cpp"
-    hdr = ROOT / "summerset_b200" / "host" / "summerset_host.hpp"
-    if BIN.exists() and BIN.stat().st_mtime > max(src.stat().st_mtime, hdr.stat().st_mtime):
-        return
+    return tmp_path_factory.mktemp("cpp_host")
+
+
+@pytest.fixture(scope="module")
+def cpp_bin(out_dir):
+    exe = out_dir / "test_rscoding"
     gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-    subprocess.run([gxx, "-std=c++17", "-O1", "-Wall", str(src), "-o", str(BIN), f"-L{ROOT / 'summerset_b200'}",
-                    "-lsummerset_b200", f"-Wl,-rpath,{ROOT / 'summerset_b200'}"], check=True)
+    subprocess.run([gxx, "-std=c++17", "-O1", "-Wall", str(ROOT / "tests" / "cpp" / "test_rscoding.cpp"), "-o", str(exe),
+                    f"-L{ROOT / 'summerset_b200'}", "-lsummerset_b200", f"-Wl,-rpath,{ROOT / 'summerset_b200'}"], check=True)
+    return exe
 
 
-def test_cpp_host_mirror_bookkeeping():
-    _build()
+@pytest.fixture(scope="module")
+def demo_bin(out_dir):
+    exe = out_dir / "c_abi_demo"
+    gcc = "/usr/bin/gcc" if os.path.exists("/usr/bin/gcc") else "gcc"
+    subprocess.run([gcc, "-O2", "-Wall", "-std=c11", str(ROOT / "examples" / "c_abi_demo.c"), f"-I{ROOT / 'include'}",
+                    f"-L{ROOT / 'summerset_b200'}", "-lsummerset_b200", f"-Wl,-rpath,{ROOT / 'summerset_b200'}",
+                    "-o", str(exe)], check=True)
+    return exe
+
+
+def test_cpp_host_mirror_bookkeeping(cpp_bin):
     env = dict(os.environ)
     if not torch.cuda.is_available():
         env["SS_EXPECT_NO_GPU"] = "1"
-    r = subprocess.run([str(BIN), "host"], capture_output=True, text=True, env=env, timeout=120)
+    r = subprocess.run([str(cpp_bin), "host"], capture_output=True, text=True, env=env, timeout=120)
     assert r.returncode == 0, r.stdout + r.stderr
 
 
 @pytest.mark.gpu
-def test_cpp_reference_tests_on_gpu():
-    _build()
-    r = subprocess.run([str(BIN), "gpu"], capture_output=True, text=True, timeout=300)
+def test_cpp_reference_tests_on_gpu(cpp_bin):
+    r = subprocess.run([str(cpp_bin), "gpu"], capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "gpu: 0 failure(s)" in r.stdout
 
 
-DEMO = ROOT / "examples" / "c_abi_demo"
-
-
-def _build_demo():
-    from summerset_b200 import build as b
-    b.build()
-    gcc = "/usr/bin/gcc" if os.path.exists("/usr/bin/gcc") else "gcc"
-    subprocess.run([gcc, "-O2", "-Wall", "-std=c11", str(ROOT / "examples" / "c_abi_demo.c"), f"-I{ROOT / 'include'}",
-                    f"-L{ROOT / 'summerset_b200'}", "-lsummerset_b200", f"-Wl,-rpath,{ROOT / 'summerset_b200'}",
-                    "-o", str(DEMO)], check=True)
-
-
-def test_plain_c_client_compiles_and_refuses_without_gpu():
+def test_plain_c_client_compiles_and_refuses_without_gpu(demo_bin):
     """the header is valid C11 and a plain-C client links; without a GPU it gets SS_ERR_NO_DEVICE, never a fallback"""
-    _build_demo()
     if not torch.cuda.is_available():
-        r = subprocess.run([str(DEMO)], capture_output=True, text=True, timeout=60)
+        r = subprocess.run([str(demo_bin)], capture_output=True, text=True, timeout=60)
         assert r.returncode == 3 and "no CPU fallback" in r.stderr
 
 
 @pytest.mark.gpu
-def test_plain_c_client_on_gpu():
-    _build_demo()
-    r = subprocess.run([str(DEMO)], capture_output=True, text=True, timeout=120)
+def test_plain_c_client_on_gpu(demo_bin):
+    r = subprocess.run([str(demo_bin)], capture_output=True, text=True, timeout=120)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "bit-exact" in r.stdout and "verify after encode: ok" in r.stdout and "-> -10" in r.stdout
 

@@ -163,14 +163,53 @@ def test_crossword_engine_matches_incremental_handler(ctx, oracle, population, T
     eng.close()
 
 
-@pytest.mark.parametrize("population,f,craft", [(7, 0, False), (5, 0, False), (3, 0, False), (5, 1, True), (7, 2, True), (9, 1, True)])
-def test_raft_engine_matches_per_reply_handler(ctx, oracle, population, f, craft):
+def _raft_append(rng, W, curr_term, last_commit, log_end, terms):
+    """The leader appends half to a full ring per group, never more than the ring can hold: n_new, and the host model's
+    log_end and terms (ring position (log_end + i) & (W-1)) updated in place."""
+    G = len(log_end)
+    room = (W - (log_end - last_commit - 1)).astype(np.int64)
+    n_new = np.minimum(rng.integers((W + 1) // 2, W + 1, G), room).astype(np.uint32)
+    n_new[rng.random(G) < 0.1] = 0
+    wrote = ((np.arange(W)[None, :] - log_end[:, None].astype(np.int64)) & (W - 1)) < n_new[:, None]
+    terms[wrote] = np.broadcast_to(curr_term[:, None], terms.shape)[wrote]
+    log_end += n_new
+    return n_new
+
+
+def _raft_rewrite_tail(rng, W, curr_term, last_commit, log_end, terms):
+    """A new leader inherits a tail with older-term entries: rewrite half the uncommitted entries of 30 % of the groups."""
+    G = len(log_end)
+    off = (np.arange(W)[None, :] - (last_commit[:, None].astype(np.int64) + 1)) & (W - 1)
+    tail = off < (log_end - last_commit - 1)[:, None].astype(np.int64)
+    old = tail & (rng.random(G) < 0.3)[:, None] & (rng.random((G, W)) < 0.5)
+    terms[old] = np.broadcast_to(curr_term[:, None] - 1, terms.shape)[old]
+
+
+def _raft_replies(rng, P, log_end):
+    """Successful AppendEntriesReplies: a few out-of-range groups and peers, end_slot in [0, log_end) (a follower never
+    acknowledges past the leader's log), mostly near the top of the log, some stale."""
+    G = len(log_end)
+    nrec = 6 * G * (P + 1)
+    rg = rng.integers(0, G + 3, nrec).astype(np.uint32)
+    rp = rng.integers(0, P + 1, nrec).astype(np.uint8)
+    hi = log_end[np.minimum(rg, G - 1)].astype(np.int64)
+    rend = np.where(rng.random(nrec) < 0.7, np.maximum(hi - rng.geometric(0.3, nrec), 0),
+                    rng.integers(0, 1 << 30, nrec) % hi).astype(np.uint32)
+    return rg, rp, rend
+
+
+@pytest.mark.parametrize("W", [1, 2, 4, 8, 64, 4096])
+@pytest.mark.parametrize("population", range(2, 13))
+def test_raft_engine_matches_per_reply_handler(ctx, oracle, population, W):
     """Appends + batches of successful AppendEntriesReplies (duplicates, stale end_slots, out-of-range peers) over several
-    ticks: match_slot / next_slot / last_commit / last_snap equal the per-reply handler's end state, with adversarial
-    term rings (older-term entries inside the uncommitted tail)."""
+    ticks: match_slot / next_slot / last_commit / last_snap and the term ring equal the per-reply handler's end state,
+    with adversarial term rings (older-term entries inside the uncommitted tail).  The logs grow to several times the
+    window, so every ring index wraps.  Odd populations from 5 up run CRaft (threshold majority + f)."""
     from summerset_b200.engine import RaftEngine
-    rng = np.random.default_rng(population * 7 + f)
-    G, W, P = 1500, 64, population - 1
+    craft = population >= 5 and population % 2 == 1
+    f = min(2, population - population // 2 - 1) if craft else 0
+    rng = np.random.default_rng(population * 7 + W)
+    G, P = 1500, population - 1
     eng = RaftEngine(ctx, G, population, f, craft, W)
     majority = population // 2 + 1
     thr = majority + f if craft else majority
@@ -181,29 +220,16 @@ def test_raft_engine_matches_per_reply_handler(ctx, oracle, population, f, craft
     next_slot = np.ones((P, G), dtype=np.uint32); match = np.zeros((P, G), dtype=np.uint32)
     last_commit = np.zeros(G, dtype=np.uint32); last_snap = np.zeros(G, dtype=np.uint32)
     log_end = np.ones(G, dtype=np.uint32); terms = np.zeros((G, W), dtype=np.uint32)
-    for rnd in range(6):
-        # the leader appends 0..10 entries per group, never more than the ring can hold
-        room = W - (log_end - last_commit - 1)
-        n_new = np.minimum(rng.integers(0, 11, G).astype(np.uint32), room).astype(np.uint32)
+    for rnd in range(10):
+        n_new = _raft_append(rng, W, curr_term, last_commit, log_end, terms)
         eng.append(_t(n_new))
-        for g in range(G):
-            for i in range(int(n_new[g])):
-                terms[g, (log_end[g] + i) % W] = curr_term[g]
-        log_end += n_new
+        torch.cuda.synchronize()
+        assert (eng.log_end.cpu().numpy().view(np.uint32) == log_end).all(), rnd
+        assert (eng.terms.cpu().numpy().view(np.uint32) == terms).all(), rnd
         if rnd == 2:
-            # a new leader inherits a tail with older-term entries: rewrite part of the uncommitted tail and move on a term
-            sel = rng.random(G) < 0.3
-            for g in np.nonzero(sel)[0]:
-                for s in range(int(last_commit[g]) + 1, int(log_end[g])):
-                    if rng.random() < 0.5:
-                        terms[g, s % W] = curr_term[g] - 1
+            _raft_rewrite_tail(rng, W, curr_term, last_commit, log_end, terms)
             eng.terms.copy_(_t(terms))
-        nrec = 25000
-        rg = rng.integers(0, G + 3, nrec).astype(np.uint32)                # a few out-of-range groups
-        rp = rng.integers(0, P + 1, nrec).astype(np.uint8)                # P = out-of-range peer
-        gi = np.minimum(rg, G - 1)
-        hi = np.maximum(log_end[gi], 2)
-        rend = (rng.integers(0, 1 << 30, nrec) % hi).astype(np.uint32)    # end_slot in [0, log_end)
+        rg, rp, rend = _raft_replies(rng, P, log_end)
         eng.on_append_replies(_t(rg), torch.from_numpy(rp).to(DEV), _t(rend))
         lc, ls = eng.tick()
         torch.cuda.synchronize()
@@ -212,8 +238,8 @@ def test_raft_engine_matches_per_reply_handler(ctx, oracle, population, f, craft
         assert (eng.match.cpu().numpy().view(np.uint32) == match).all(), rnd
         assert (lc.cpu().numpy().view(np.uint32) == last_commit).all(), rnd
         assert (ls.cpu().numpy().view(np.uint32) == last_snap).all(), rnd
-        assert (eng.log_end.cpu().numpy().view(np.uint32) == log_end).all()
-    assert (last_commit > 0).mean() > 0.3
+    # the ring wrapped: logs several windows long, commits past the first window
+    assert (log_end > 3 * W).mean() > 0.9 and (last_commit > W).mean() > 0.9
     assert ctx.device_status() == 0
     # appending past the ring's capacity is refused and reported
     eng.append(_t(np.full(G, W + 1, dtype=np.uint32)))

@@ -113,8 +113,12 @@ def test_ack_ingest_matches_stream_handler(ctx, oracle):
 
 @pytest.mark.parametrize("balanced", [True, False])
 def test_crossword_matches_oracle(ctx, oracle, balanced):
+    """Up to 12 replicas and 16 policies (a 16 x 2^12-bit LUT, 8 KB of shared memory).  A policy_idx >= n_policies
+    never commits, as in the engine tick."""
     rng = np.random.default_rng(17)
-    for n, T, d, f in [(5, 5, 3, 2), (5, 5, 3, 1), (5, 5, 3, 0), (7, 7, 4, 3), (3, 3, 2, 1), (5, 10, 6, 2), (9, 9, 5, 2)]:
+    for n, T, d, f, K in [(5, 5, 3, 2, 0), (5, 5, 3, 1, 0), (5, 5, 3, 0, 0), (7, 7, 4, 3, 0), (3, 3, 2, 1, 0), (5, 10, 6, 2, 0),
+                          (9, 9, 5, 2, 0), (10, 10, 6, 2, 0), (11, 11, 6, 3, 0), (12, 12, 7, 2, 0), (12, 24, 13, 1, 0),
+                          (12, 12, 7, 2, 16)]:
         majority = n // 2 + 1
         dj = T // n
         if balanced:
@@ -122,23 +126,34 @@ def test_crossword_matches_oracle(ctx, oracle, balanced):
         else:
             policies = [rng.integers(0, 1 << T, size=n).astype(np.uint32) for _ in range(4)]
             policies.append(oracle.cw_brr_assignment(n, T, dj))
+        if K:                                                       # cycle / draw up to exactly K policies
+            while len(policies) < K:
+                policies.append(policies[len(policies) % 4] if balanced else rng.integers(0, 1 << T, size=n).astype(np.uint32))
+            policies = policies[:K]
         K = len(policies)
         N = 20011
         width = np.uint8 if n <= 8 else np.uint16
         masks = rng.integers(0, 1 << n, N).astype(width)
         pidx = rng.integers(0, K, N).astype(np.uint8)
+        bad = rng.random(N) < 0.05
+        pidx[bad] = rng.integers(K, 256, int(bad.sum()))              # out-of-range policy: never commits
         bits = ctx.tally_crossword(_t(masks), _t(pidx), [list(map(int, pol)) for pol in policies], T, d, majority, f, balanced)
         torch.cuda.synchronize()
         got = np.unpackbits(bits.cpu().numpy().view(np.uint8), bitorder="little")[:N]
-        lut = {(k, a): oracle.cw_committed(T, n, d, majority, f, a, policies[k], balanced)
-               for k in range(K) for a in range(1 << n)}
-        want = np.array([lut[(int(k), int(a))] for k, a in zip(pidx, masks)], dtype=np.uint8)
-        assert (got == want).all(), (n, T, d, f)
+        lut = np.array([[oracle.cw_committed(T, n, d, majority, f, a, policies[k], balanced) for a in range(1 << n)]
+                        for k in range(K)], dtype=np.uint8)
+        want = np.where(bad, 0, lut[np.minimum(pidx, K - 1), masks.astype(np.int64)]).astype(np.uint8)
+        assert (got == want).all(), (n, T, d, f, K)
+        assert want[~bad].any() and not got[bad].any()
 
 
-@pytest.mark.parametrize("n_rep,thr", [(7, 4), (5, 3), (3, 2), (9, 5), (5, 4), (7, 6), (2, 2), (1, 1), (5, 9)])
+@pytest.mark.parametrize("n_rep,thr", [(7, 4), (5, 3), (3, 2), (9, 5), (5, 4), (7, 6), (2, 2), (1, 1), (5, 9),
+                                       # 9..16 peers: the NP = 16 instance; thresholds 1, majority and n_rep
+                                       (10, 1), (10, 6), (10, 10), (12, 1), (12, 7), (12, 12), (13, 1), (13, 7), (13, 13),
+                                       (17, 1), (17, 9), (17, 17)])
 def test_raft_scan_matches_oracle(ctx, oracle, n_rep, thr):
-    for G, W in [(1, 64), (33, 64), (5000, 64), (777, 17), (300, 200)]:
+    # W % 4 != 0 takes the cooperative warp walk, W % 4 == 0 the vectorised one
+    for G, W in [(1, 64), (33, 64), (5000, 64), (777, 17), (300, 200), (777, 1), (777, 2), (777, 3)]:
         w = wl.cfg5_raft(G, n_rep, W, seed_extra=n_rep * 10 + thr)
         match = w["match"] if n_rep > 1 else np.zeros((0, G), dtype=np.uint32)
         if n_rep == 1:

@@ -124,7 +124,7 @@ def _t(a):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("n,f", [(5, 1), (7, 2), (3, 0), (9, 2)])
+@pytest.mark.parametrize("n,f", [(5, 1), (7, 2), (3, 0), (9, 2), (11, 2), (13, 3), (17, 4)])
 def test_craft_on_gpu(ctx, oracle, n, f):
     majority = n // 2 + 1
     G = 5003
@@ -144,6 +144,17 @@ def test_craft_on_gpu(ctx, oracle, n, f):
     allm = ctx.raft_kth_match(_t(w["match"]), n - 1)
     torch.cuda.synchronize()
     assert (allm.cpu().numpy().view(np.uint32) == w["match"].min(axis=0)).all()
+    # every k over match values from a small range, so that ties are common: k-th largest = shadow_last_commit with
+    # threshold k + 1 (craft/messages.rs:677-690)
+    P = n - 1
+    m = np.random.default_rng(n).integers(0, 4, (P, G)).astype(np.uint32)
+    desc = -np.sort(-m.astype(np.int64), axis=0)
+    for k in range(1, P + 1):
+        out = ctx.raft_kth_match(_t(m), k)
+        torch.cuda.synchronize()
+        got = out.cpu().numpy().view(np.uint32)
+        assert (got == desc[k - 1]).all(), k
+        assert all(int(got[g]) == oracle.craft_shadow_last_commit(m[:, g], k + 1) for g in range(0, G, 97)), k
 
 
 @pytest.mark.gpu
