@@ -116,7 +116,14 @@ int ss_ipc_close(ss_ctx *ctx, void *dptr);
  * M = vandermonde(d+p, d) * inverse(top d x d) -- bit-identical to the crate's.
  * Errors: d == 0 -> TOO_FEW_DATA_SHARDS, p == 0 -> TOO_FEW_PARITY_SHARDS, d+p > 256 ->
  * TOO_MANY_SHARDS (the crate's behaviour; Summerset special-cases p == 0 before touching the
- * coder, rscoding.rs:454-456,498-507).  Batched kernels need d <= 32, p <= 8, d+p <= 32. */
+ * coder, rscoding.rs:454-456,498-507).  Any such code gets a coder, but the kernels cover less:
+ *   encode (ss_rs_encode, ss_rs_verify and every batched encode / accept step) needs d <= 32 and p <= 8,
+ *     so up to 40 shards;
+ *   reconstruct (ss_rs_reconstruct, ss_rs_reconstruct_data, ss_rs_reconstruct_batch_dev and
+ *     ss_rs_reconstruct_uniform_dev) needs d + p <= 12 as well.
+ * Past those limits the calls return SS_ERR_UNSUPPORTED and write nothing, except where no work is
+ * left: a single-codeword reconstruct with every shard it would regenerate already present returns
+ * SS_OK for any code. */
 int ss_rs_coder_create(ss_ctx *ctx, int data_shards, int parity_shards, ss_rs_coder **out);
 int ss_rs_coder_destroy(ss_rs_coder *coder);
 int ss_rs_data_shard_count(const ss_rs_coder *coder);    /* rscoding.rs:428 */
@@ -133,8 +140,10 @@ int ss_rs_coder_matrix(const ss_rs_coder *coder, uint8_t *out);
  * ss_rs_verify            replaces rs.verify(&slices)            (rscoding.rs:575)
  * present[j] != 0 <=> shards[j] is Some(..); missing entries must still point at a
  * shard_len-byte buffer to fill (the crate allocates it; here the caller does).  On success
- * present[] is updated for the regenerated shards.  Fewer than d present ->
- * SS_ERR_TOO_FEW_SHARDS_PRESENT and no output is written (never partial). */
+ * present[] is updated for the regenerated shards.  ss_rs_reconstruct_data neither reads nor
+ * writes missing parity entries (they may all alias one scratch buffer) and leaves their present[]
+ * at 0.  Fewer than d present -> SS_ERR_TOO_FEW_SHARDS_PRESENT and no output is written (never
+ * partial). */
 int ss_rs_encode(ss_rs_coder *coder, uint8_t *const *shards, size_t n_shards, size_t shard_len);
 int ss_rs_reconstruct(ss_rs_coder *coder, uint8_t *const *shards, uint8_t *present,
                       size_t n_shards, size_t shard_len);

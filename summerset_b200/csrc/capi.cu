@@ -30,6 +30,9 @@ int set_error(int code, const char *fmt, ...) {
 }
 
 int cuda_error(cudaError_t e, const char *what, const char *file, int line) {
+    // A failed runtime call also leaves its error as the thread's last error.  Clear it: otherwise the next successful
+    // call reports it again from the cudaGetLastError() after its first kernel launch.
+    cudaGetLastError();
     const char *base = strrchr(file, '/');
     const int code = (e == cudaErrorNoDevice || e == cudaErrorInsufficientDriver || e == cudaErrorNoKernelImageForDevice)
                          ? SS_ERR_NO_DEVICE
@@ -616,6 +619,10 @@ static int reconstruct_one(ss_rs_coder *c, uint8_t *const *shards, uint8_t *pres
     for (int i = 0; i < t; ++i) np += present[i] ? 1 : 0;
     if (np == t) return SS_OK;                       // crate: nothing to do
     if (np < d) return set_error(SS_ERR_TOO_FEW_SHARDS_PRESENT, "too few shards present: %d < %d", np, d);
+    const int upto = data_only ? d : t;
+    int nmiss = 0;
+    for (int i = 0; i < upto; ++i) nmiss += present[i] ? 0 : 1;
+    if (nmiss == 0) return SS_OK;                    // reconstruct_data with every data shard present: nothing to regenerate
     if (!c->dec_ok)
         return set_error(SS_ERR_UNSUPPORTED, "reconstruct needs d+p <= 12 on this build (coder is %d,%d)", d, p);
     const size_t L = shard_len, ds = (L + 15) & ~size_t(15);
@@ -628,7 +635,6 @@ static int reconstruct_one(ss_rs_coder *c, uint8_t *const *shards, uint8_t *pres
     for (int i = 0; i < t; ++i)
         if (present[i]) pat |= 1u << i;
     struct Meta { uint64_t off; uint32_t len; uint32_t pat; int32_t status; } h = {0, static_cast<uint32_t>(size_t(d) * L), pat, 0};
-    const int upto = data_only ? d : t;
     const bool staged = meta + size_t(t) * ds <= kStagedCallLimit;
     uint8_t *pin = nullptr;
     if (staged) {
@@ -878,8 +884,9 @@ static int encode_uniform_host(ss_rs_coder *c, const uint8_t *data, uint64_t dat
         uint64_t *dcm = reinterpret_cast<uint64_t *>(dout + out_par);
         uint32_t *dbar = reinterpret_cast<uint32_t *>(dout + out_par + out_cm);
         if (k >= ss_ctx::kStages) SS_CUDA(cudaStreamWaitEvent(ctx->h2d_stream, ctx->ev_done[b], 0));
-        if (in_contig)
-            SS_CUDA(cudaMemcpyAsync(din, data + g0 * data_stride, nc * data_stride, cudaMemcpyHostToDevice, ctx->h2d_stream));
+        if (in_contig)      // up to the last payload's end, not its row's: the caller's buffer may stop there
+            SS_CUDA(cudaMemcpyAsync(din, data + g0 * data_stride, (nc - 1) * data_stride + data_len, cudaMemcpyHostToDevice,
+                                    ctx->h2d_stream));
         else
             SS_CUDA(cudaMemcpy2DAsync(din, in_stride_dev, data + g0 * data_stride, data_stride, data_len, nc,
                                       cudaMemcpyHostToDevice, ctx->h2d_stream));
