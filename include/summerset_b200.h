@@ -620,6 +620,92 @@ int ss_engine_raft_append(ss_engine *engine, const uint32_t *n_new);
 int ss_engine_raft_ingest(ss_engine *engine, const uint32_t *rec_group, const uint8_t *rec_peer,
                           const uint32_t *rec_end_slot, uint64_t n_records);
 
+/* ---- batched acceptor (RSPaxos / Crossword follower side of the accept path) -----------------------------------
+ * The follower half of SURVEY 3.2 step 4 for n_groups groups this replica follows: Accept frames in (rspaxos/messages.rs
+ * handle_msg_accept, crossword/messages.rs:403-470), held shards into a caller-owned store, WalEntry::AcceptData records
+ * and AcceptReply frames out (rspaxos/durability.rs:101-118, crossword/durability.rs:96-125).  Per-group state lives in
+ * HBM as a struct of arrays; per-slot arrays are rings of 64 indexed like the engine's (absolute slot s at s & 63).
+ * One stated difference from the reference: the instance log is the engine's 64-slot window [window_base,
+ * window_base + 64), not a vector that grows without bound; a frame beyond it takes no part in the call and the host
+ * re-submits it after ss_acceptor_advance. */
+typedef struct ss_acceptor ss_acceptor;
+typedef struct ss_acceptor_config {
+    uint32_t protocol;          /* SS_PROTO_RSPAXOS or SS_PROTO_CROSSWORD */
+    uint32_t population;        /* replicas, 1..32 */
+    uint32_t me;                /* this replica's id (Crossword reply size: assignment[me]) */
+    uint32_t data_shards, total_shards;   /* the code every Accept must carry: 1 <= d <= T <= 32 */
+    uint32_t accept_variant;    /* index of Accept in PeerMsg (2) */
+    uint32_t wal_variant;       /* index of AcceptData in WalEntry (1) */
+    uint32_t reply_variant;     /* index of AcceptReply in PeerMsg (3) */
+} ss_acceptor_config;
+typedef struct ss_acceptor_view {
+    uint64_t n_groups;
+    uint32_t protocol, population, me, data_shards, total_shards, pad0;
+    uint64_t *window_base;      /* [G] start_slot */
+    uint64_t *bal_max_seen;     /* [G] */
+    uint64_t *inst_bal;         /* [G*64] */
+    uint64_t *accepting;        /* [G] bit s & 63 = Status::Accepting */
+    uint64_t *shard_addr;       /* [G*64] device address of the instance's first held shard in the caller's store */
+    uint32_t *held;             /* [G*64] shard mask the instance holds */
+    uint32_t *data_len;         /* [G*64] */
+    uint32_t *assignment;       /* Crossword [G*64]: the instance's assignment row of `me`; NULL for RSPaxos */
+    uint8_t *source;            /* [G*64] peer the Accept came from (replica_bk.source) */
+} ss_acceptor_view;
+/* Configuration checks come first (SS_ERR_INVALID_ARG); a NULL ctx then gives SS_ERR_NO_DEVICE when the machine has no
+ * usable device, SS_ERR_INVALID_ARG otherwise.  All state starts at zero. */
+int ss_acceptor_create(ss_ctx *ctx, const ss_acceptor_config *cfg, uint64_t n_groups, ss_acceptor **out);
+int ss_acceptor_destroy(ss_acceptor *acceptor);
+int ss_acceptor_view_get(ss_acceptor *acceptor, ss_acceptor_view *view);
+/* *window_base = the acceptor's device array [G] of window bases; a host may install bases (a snapshot's start_slot)
+ * while the window holds no instance. */
+int ss_acceptor_window_get(ss_acceptor *acceptor, uint64_t **window_base);
+/* retires window prefixes: upto (device [G] absolute slots, required -- the acceptor keeps no commit state):
+ * k = clamp(upto[g] - window_base[g], 0, 64); the k retired ring positions leave Accepting and window_base[g] += k. */
+int ss_acceptor_advance(ss_acceptor *acceptor, const uint64_t *upto);
+/* Verdicts of ss_acceptor_accept, beside the PeerMsg variant index k (another message; 0x80000000 | k for the
+ * PeerMessage variants) and SS_FRAME_KIND_MALFORMED */
+#define SS_ACCEPT_VERDICT_ACCEPTED 0xfffffff0u
+#define SS_ACCEPT_VERDICT_STALE_SLOT 0xfffffff1u      /* slot < window_base: ignored (messages.rs `slot < start_slot`) */
+#define SS_ACCEPT_VERDICT_STALE_BALLOT 0xfffffff2u    /* ballot < bal_max_seen as it stands when the frame is reached */
+#define SS_ACCEPT_VERDICT_BEYOND_WINDOW 0xfffffff3u   /* slot >= window_base + 64: re-submit after ss_acceptor_advance */
+#define SS_ACCEPT_VERDICT_STORE_FULL 0xfffffff4u      /* its store region ends past store_capacity */
+#define SS_ACCEPT_VERDICT_WAL_FULL 0xfffffff5u        /* its WAL region ends past wal_capacity */
+/* One batch of frames (device pointers; asynchronous on the context's stream, no host synchronisation).
+ * buf holds frames as read off the leaders' connections at any byte alignment; frame i starts at frame_off[i] and came
+ * from replica frame_peer[i] for group frame_group[i] (a group >= n_groups: malformed).  verdict[i] is one of the above.
+ * Malformed: truncated or not decodable as a PeerMessage::Msg{Accept{slot, ballot, reqs_cw[, assignment]}}; a codeword
+ * whose (d, p) is not the acceptor's code; shard_len != ceil(data_len / d) (rscoding.rs:177-181); a present shard of
+ * another length; data_len >= 2^32; a body longer than 2^32 - 65 bytes; Crossword: an assignment that is not
+ * `population` bitmaps of total_shards bits.  Non-minimal varints are read as the oracle's decoder reads them (tag 251
+ * + u16 for a small value is that value) and stay as they came in the verbatim part of the record.
+ * Ballot order (check_leader, rspaxos/leadership.rs:11-17, replayed in frame order): frame i of group g is checked
+ * against max(bal_max_seen[g] before the call, the ballots of every earlier well-formed frame of g inside the window);
+ * frames of different groups are independent.  Placement follows: the frames that pass take store and WAL regions by
+ * exclusive scans in frame order; one whose region ends past store_capacity / wal_capacity is STORE_FULL / WAL_FULL
+ * (SS_DEV_STATUS_STORE_FULL / SS_DEV_STATUS_FRAME_OVERFLOW), changes nothing and does not raise bal_max_seen.  At the
+ * end bal_max_seen[g] = max(before, accepted ballots).  When several accepted frames name one (group, slot), the last in
+ * frame order defines the instance (inst.bal, source, shards, assignment); every accepted frame still gets its record.
+ * Outputs of accepted frame i (UINT64_MAX offsets and 0 lengths for the others):
+ *   store: its held shards in index order at store + store_off[i] + k*SS_CW_SLOT_PITCH(L), bytes L..round_up(L,16)
+ *          zero (the layout ss_engine_propose_ragged writes); store_off = exclusive scan of popcount(held)*pitch
+ *   wal:   WalEntry::AcceptData at wal + wal_off[i] (16-byte aligned scan), wal_len[i] bytes: 8-byte big-endian length,
+ *          wal_variant, then the frame's bytes from `slot` on, verbatim (rspaxos/mod.rs:219-228; Crossword keeps
+ *          assignment, crossword/mod.rs:288-293)
+ *   reply: PeerMessage::Msg{AcceptReply{slot, ballot[, size, reply_ts: None]}} in the 48-byte cell replies + 48*i,
+ *          reply_len[i] bytes, to be sent to replica reply_dst[i] (0xff for frames not accepted).  ballot and
+ *          destination are the instance's inst.bal and source after the whole call; Crossword size =
+ *          popcount(assignment[me]) * (data_len / d + 1), the reference's formula (crossword/durability.rs:113-119).
+ *          The host sends these cells only once the WAL records of the call are durable.
+ * totals (device u64[2], may be NULL): the store and WAL bytes the batch asked for.  store and wal 16-byte aligned.
+ * Cost: the ballot order and the placement walk each group's frames on one thread, so a batch costs its largest
+ * per-group run of frames in those two steps (a batch that is mostly one group, e.g. a follower catching up, runs that
+ * bookkeeping serially); the copy pass is a warp per frame whatever the grouping. */
+int ss_acceptor_accept(ss_acceptor *acceptor, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off,
+                       const uint32_t *frame_group, const uint8_t *frame_peer, uint64_t n_frames, uint8_t *store,
+                       uint64_t store_capacity, uint64_t *store_off, uint8_t *wal, uint64_t wal_capacity, uint64_t *wal_off,
+                       uint32_t *wal_len, uint8_t *replies, uint32_t *reply_len, uint8_t *reply_dst, uint32_t *verdict,
+                       uint64_t *totals);
+
 /* ---- tuning / introspection (bench + tests) ------------------------------------------------ */
 /* Tuning knob for experiments; 0 = the defaults.
  *   bits 0-3  kernel choice / register budget: 1 = flat one-column-per-thread RS(3,2) kernel instead of the row kernel,

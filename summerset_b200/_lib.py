@@ -115,6 +115,12 @@ SIGNATURES = {
     "ss_engine_window_get": (_i, [_vp, C.POINTER(_vp)]),
     "ss_engine_raft_append": (_i, [_vp, _vp]),
     "ss_engine_raft_ingest": (_i, [_vp, _vp, _vp, _vp, _u64]),
+    "ss_acceptor_create": (_i, [_vp, _vp, _u64, C.POINTER(_vp)]),
+    "ss_acceptor_destroy": (_i, [_vp]),
+    "ss_acceptor_view_get": (_i, [_vp, _vp]),
+    "ss_acceptor_window_get": (_i, [_vp, C.POINTER(_vp)]),
+    "ss_acceptor_advance": (_i, [_vp, _vp]),
+    "ss_acceptor_accept": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _vp, _u64, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ss_rs_set_variant": (_i, [_vp, _i]),
     "ss_rs_last_kernel": (C.c_char_p, [_vp]),
     "ss_rs_jit_status": (C.c_char_p, [_vp]),
@@ -153,6 +159,31 @@ class EngineView(C.Structure):
                 ("committed", C.c_void_p), ("commit_bar", C.c_void_p), ("shards", C.c_void_p), ("policy_idx", C.c_void_p),
                 ("match", C.c_void_p), ("next_slot", C.c_void_p), ("last_commit", C.c_void_p), ("log_end", C.c_void_p),
                 ("curr_term", C.c_void_p), ("last_snap", C.c_void_p), ("terms", C.c_void_p)]
+
+
+class AcceptorConfig(C.Structure):
+    """ss_acceptor_config"""
+    _fields_ = [("protocol", C.c_uint32), ("population", C.c_uint32), ("me", C.c_uint32), ("data_shards", C.c_uint32),
+                ("total_shards", C.c_uint32), ("accept_variant", C.c_uint32), ("wal_variant", C.c_uint32), ("reply_variant", C.c_uint32)]
+
+
+class AcceptorView(C.Structure):
+    """ss_acceptor_view"""
+    _fields_ = [("n_groups", C.c_uint64), ("protocol", C.c_uint32), ("population", C.c_uint32), ("me", C.c_uint32),
+                ("data_shards", C.c_uint32), ("total_shards", C.c_uint32), ("pad0", C.c_uint32),
+                ("window_base", C.c_void_p), ("bal_max_seen", C.c_void_p), ("inst_bal", C.c_void_p), ("accepting", C.c_void_p),
+                ("shard_addr", C.c_void_p), ("held", C.c_void_p), ("data_len", C.c_void_p), ("assignment", C.c_void_p),
+                ("source", C.c_void_p)]
+
+
+# verdicts of ss_acceptor_accept (beside PeerMsg variant indices and SS_FRAME_KIND_MALFORMED)
+SS_ACCEPT_VERDICT_ACCEPTED = 0xFFFFFFF0
+SS_ACCEPT_VERDICT_STALE_SLOT = 0xFFFFFFF1
+SS_ACCEPT_VERDICT_STALE_BALLOT = 0xFFFFFFF2
+SS_ACCEPT_VERDICT_BEYOND_WINDOW = 0xFFFFFFF3
+SS_ACCEPT_VERDICT_STORE_FULL = 0xFFFFFFF4
+SS_ACCEPT_VERDICT_WAL_FULL = 0xFFFFFFF5
+SS_FRAME_KIND_MALFORMED = 0xFFFFFFFF
 
 
 class SummersetError(RuntimeError):

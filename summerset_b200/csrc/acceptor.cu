@@ -1,0 +1,529 @@
+// acceptor.cu -- the follower side of the RSPaxos / Crossword accept path behind the C ABI (ss_acceptor_*).
+//
+// What a follower does for every Accept (SURVEY 3.2 step 4): handle_msg_accept (rspaxos/messages.rs:329-392,
+// crossword/messages.rs:403-470) with check_leader's bal_max_seen update (rspaxos/leadership.rs:11-17), the
+// WalEntry::AcceptData it logs, and the AcceptReply it sends once the record is durable (rspaxos/durability.rs:101-118,
+// crossword/durability.rs:96-125) -- for a batch of frames of many groups at once:
+//
+//   acceptor_header_kernel   a thread per frame: walks the varints, validates, keeps the fields, the held mask and the
+//                            offsets of `slot` and of the first shard tag; slot / window filters; region sizes
+//   (CUB radix sort)         frame indices stably sorted by group: each group's frames in frame order
+//   acceptor_ballot_kernel   a thread per group segment: check_leader's running maximum, replayed in frame order
+//   (engine.cu's scan)       store and WAL regions: exclusive scans in frame order
+//   acceptor_place_kernel    a thread per group segment, backwards: capacity, the final verdicts, the last accepted
+//                            frame of each (group, slot) defines the instance, bal_max_seen = max of the accepted
+//   acceptor_copy_kernel     a warp per accepted frame: the AcceptData record (length, wal_variant, the frame from `slot`
+//                            on, verbatim), the held shards into their padded store slots, the AcceptReply cell
+//
+// Frames sit in a receive buffer at any byte alignment; every 128-bit store is aligned, its 16 source bytes come from
+// the two aligned loads around them (dev::load16).
+#include <cub/device/device_radix_sort.cuh>
+
+#include <cstring>
+#include <new>
+
+#include "device_common.cuh"
+#include "ss_internal.hpp"
+#include "window_ring.cuh"
+#include "wire_common.cuh"
+
+namespace ssb {
+
+// one decoded Accept frame
+struct FrameHdr {
+    uint64_t slot, ballot;
+    uint64_t end;                   // frame bytes: 8-byte length prefix + body
+    uint32_t kind;                  // verdict so far
+    uint32_t held, dlen, L;
+    uint32_t slot_at;               // offset of the `slot` varint inside the frame
+    uint32_t tags_at;               // offset of shard 0's Option tag
+    uint32_t asg;                   // Crossword: assignment[me]
+    uint32_t pad;
+};
+
+}  // namespace ssb
+
+struct ss_acceptor {
+    ss_ctx *ctx = nullptr;
+    ss_acceptor_config cfg{};
+    uint64_t G = 0;
+    uint64_t *window_base = nullptr, *bal_max_seen = nullptr, *inst_bal = nullptr, *accepting = nullptr, *shard_addr = nullptr;
+    uint32_t *held = nullptr, *data_len = nullptr, *assignment = nullptr;
+    uint8_t *source = nullptr;
+    // per-call scratch, grow-only
+    uint64_t cap_frames = 0;
+    ssb::FrameHdr *hdr = nullptr;
+    uint32_t *keys = nullptr;       // [2][cap]: sort keys in / out
+    uint32_t *idx = nullptr;        // [2][cap]: frame indices in / out
+    uint64_t *partials = nullptr;   // [scan_tiles(cap)]
+    void *sort_tmp = nullptr;
+    size_t sort_tmp_bytes = 0;
+    uint64_t *totals = nullptr;     // [2] when the caller passes none
+};
+
+namespace ssb {
+
+constexpr int kAccThreads = 256;
+constexpr uint32_t kPending = 0xfffffffeu;          // in the window, ballot not yet checked
+constexpr uint32_t kVariantLimit = 1u << 16;        // no enum of the protocol has this many variants: malformed
+constexpr uint64_t kMaxFrameBody = 0xffffffffull - 64u;   // longer frames are malformed: every record length fits a u32
+
+struct AccArgs {
+    const uint8_t *buf;
+    uint64_t buf_len;
+    const uint64_t *frame_off;
+    const uint32_t *frame_group;
+    const uint8_t *frame_peer;
+    uint64_t n, G;
+    uint32_t d, T, population, me, accept_variant, wal_variant, reply_variant, crossword;
+    // state
+    uint64_t *window_base, *bal_max_seen, *inst_bal, *accepting, *shard_addr;
+    uint32_t *held, *data_len, *assignment;
+    uint8_t *source;
+    // scratch
+    FrameHdr *hdr;
+    uint32_t *key_in, *idx_in;
+    const uint32_t *key, *idx;      // sorted
+    // outputs
+    uint8_t *store;
+    uint64_t store_cap;
+    uint64_t *store_off;
+    uint8_t *wal;
+    uint64_t wal_cap;
+    uint64_t *wal_off;
+    uint32_t *wal_len;
+    uint8_t *replies;
+    uint32_t *reply_len;
+    uint8_t *reply_dst;
+    uint32_t *verdict;
+    uint32_t *status;
+};
+
+__device__ __forceinline__ uint64_t store_bytes(const FrameHdr &h) {
+    return static_cast<uint64_t>(__popc(h.held)) * SS_CW_SLOT_PITCH(h.L);
+}
+__device__ __forceinline__ uint64_t wal_bytes(const FrameHdr &h, uint32_t wal_variant) {
+    return 8u + static_cast<uint64_t>(wv_len(wal_variant)) + (h.end - h.slot_at);
+}
+__device__ __forceinline__ uint64_t round16(uint64_t x) { return (x + 15u) & ~15ull; }
+
+// decodes frame i as ssor_decode_accept reads it, plus the acceptor's own checks (code, shard_len, assignment shape)
+__device__ __forceinline__ FrameHdr decode_frame(const AccArgs &A, uint64_t i) {
+    FrameHdr h{};
+    h.kind = SS_FRAME_KIND_MALFORMED;
+    const uint32_t grp = A.frame_group[i];
+    const uint64_t off = A.frame_off[i];
+    if (grp >= A.G || off > A.buf_len || A.buf_len - off < 8u) return h;
+    const uint8_t *fr = A.buf + off;
+    uint64_t len = 0;
+    for (int b = 0; b < 8; ++b) len = (len << 8) | fr[b];
+    if (len > A.buf_len - off - 8u || len > kMaxFrameBody) return h;
+    const uint8_t *b = fr + 8;
+    uint64_t n = 0, v = 0;
+    uint32_t c;
+#define SS_GET(dst) do { if (!(c = wv_get(b + n, len - n, (dst)))) return h; n += c; } while (0)
+    SS_GET(v);
+    if (v != 0u) {                                                          // LeaseMsg / Leave / LeaveReply
+        if (v < kVariantLimit) h.kind = 0x80000000u | static_cast<uint32_t>(v);
+        return h;
+    }
+    SS_GET(v);
+    if (v != A.accept_variant) {                                            // another PeerMsg: the host's business
+        if (v < kVariantLimit) h.kind = static_cast<uint32_t>(v);
+        return h;
+    }
+    h.slot_at = static_cast<uint32_t>(8u + n);
+    SS_GET(h.slot);
+    SS_GET(h.ballot);
+    if (len - n < 2u || b[n] != A.d || b[n + 1] != A.T - A.d) return h;   // num_data_shards, num_parity_shards
+    n += 2;
+    uint64_t dl = 0, sl = 0;
+    SS_GET(dl);
+    SS_GET(sl);
+    SS_GET(v);
+    if (dl > 0xffffffffull || v != A.T || sl != (dl + A.d - 1u) / A.d) return h;   // rscoding.rs:177-181
+    h.tags_at = static_cast<uint32_t>(8u + n);
+    uint32_t held = 0;
+    for (uint32_t j = 0; j < A.T; ++j) {
+        if (n >= len) return h;
+        const uint8_t tag = b[n++];
+        if (tag == 0u) continue;
+        if (tag != 1u) return h;
+        SS_GET(v);
+        if (v != sl || len - n < sl) return h;
+        held |= 1u << j;
+        n += sl;
+    }
+    if (n >= len || b[n++] != 0u) return h;                                 // data_copy: None
+    if (A.crossword) {                                                      // assignment: Vec<Bitmap>, one row per replica
+        SS_GET(v);
+        if (v != A.population) return h;
+        for (uint32_t r = 0; r < A.population; ++r) {
+            uint64_t sz = 0, nb = 0, blk = 0;
+            SS_GET(sz);
+            SS_GET(nb);
+            if (sz != A.T || nb != 1u) return h;
+            SS_GET(blk);
+            if (blk >> A.T) return h;
+            if (r == A.me) h.asg = static_cast<uint32_t>(blk);
+        }
+    }
+#undef SS_GET
+    if (n != len) return h;
+    h.end = 8u + len;
+    h.held = held;
+    h.dlen = static_cast<uint32_t>(dl);
+    h.L = static_cast<uint32_t>(sl);
+    const uint64_t base = A.window_base[grp];
+    h.kind = h.slot < base ? SS_ACCEPT_VERDICT_STALE_SLOT : h.slot - base >= 64u ? SS_ACCEPT_VERDICT_BEYOND_WINDOW : kPending;
+    return h;
+}
+
+// 1. a thread per frame: decode, filter, region sizes (0 for frames that cannot be accepted), sort keys
+__global__ void __launch_bounds__(kAccThreads) acceptor_header_kernel(const __grid_constant__ AccArgs A) {
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; i < A.n; i += stride) {
+        const FrameHdr h = decode_frame(A, i);
+        A.hdr[i] = h;
+        const bool pending = h.kind == kPending;
+        A.store_off[i] = pending ? store_bytes(h) : 0ull;
+        A.wal_off[i] = pending ? round16(wal_bytes(h, A.wal_variant)) : 0ull;
+        const uint32_t grp = A.frame_group[i];
+        A.key_in[i] = grp < A.G ? grp : static_cast<uint32_t>(A.G);
+        A.idx_in[i] = static_cast<uint32_t>(i);
+    }
+}
+
+__device__ __forceinline__ bool segment_head(const AccArgs &A, uint64_t t) { return t == 0u || A.key[t] != A.key[t - 1]; }
+
+// 2. a thread per group segment (the group's frames in frame order): a frame inside the window passes when its ballot
+//    is at least the running maximum, which it then raises (check_leader); the others are stale and take no room
+__global__ void __launch_bounds__(kAccThreads) acceptor_ballot_kernel(const __grid_constant__ AccArgs A) {
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
+    for (uint64_t t = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; t < A.n; t += stride) {
+        if (!segment_head(A, t)) continue;
+        const uint32_t g = A.key[t];
+        if (g >= A.G) continue;
+        uint64_t run = A.bal_max_seen[g];
+        for (uint64_t k = t; k < A.n && A.key[k] == g; ++k) {
+            const uint32_t i = A.idx[k];
+            if (A.hdr[i].kind != kPending) continue;
+            const uint64_t bal = A.hdr[i].ballot;
+            if (bal < run) {
+                A.hdr[i].kind = SS_ACCEPT_VERDICT_STALE_BALLOT;
+                A.store_off[i] = 0ull;
+                A.wal_off[i] = 0ull;
+            } else {
+                A.hdr[i].kind = SS_ACCEPT_VERDICT_ACCEPTED;            // subject to capacity
+                run = bal;
+            }
+        }
+    }
+}
+
+// 3. a thread per group segment, last frame first: store_off / wal_off hold the scanned region starts.  A frame whose
+//    region ends past the capacity changes nothing; of the accepted frames of one slot the last defines the instance.
+__global__ void __launch_bounds__(kAccThreads) acceptor_place_kernel(const __grid_constant__ AccArgs A) {
+    bool store_full = false, wal_full = false;
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
+    for (uint64_t t = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; t < A.n; t += stride) {
+        if (!segment_head(A, t)) continue;
+        const uint32_t g = A.key[t];
+        const bool known = g < A.G;
+        uint64_t e = t + 1u;
+        while (e < A.n && A.key[e] == g) ++e;
+        uint64_t seen = 0ull, mx = known ? A.bal_max_seen[g] : 0ull;
+        for (uint64_t k = e; k-- > t;) {
+            const uint32_t i = A.idx[k];
+            const FrameHdr h = A.hdr[i];
+            uint32_t kind = h.kind;
+            if (kind == SS_ACCEPT_VERDICT_ACCEPTED) {
+                const uint64_t so = A.store_off[i], sz = store_bytes(h), wo = A.wal_off[i];
+                const uint64_t wl = wal_bytes(h, A.wal_variant);
+                if (so > A.store_cap || sz > A.store_cap - so) {
+                    kind = SS_ACCEPT_VERDICT_STORE_FULL;
+                    store_full = true;
+                } else if (wo > A.wal_cap || round16(wl) > A.wal_cap - wo) {
+                    kind = SS_ACCEPT_VERDICT_WAL_FULL;
+                    wal_full = true;
+                } else {
+                    A.wal_len[i] = static_cast<uint32_t>(wl);
+                    mx = h.ballot > mx ? h.ballot : mx;
+                    const uint32_t pos = static_cast<uint32_t>(h.slot & 63u);
+                    if (!((seen >> pos) & 1ull)) {                     // the last accepted frame of this slot
+                        seen |= 1ull << pos;
+                        const uint64_t at = static_cast<uint64_t>(g) * 64u + pos;
+                        A.inst_bal[at] = h.ballot;
+                        A.source[at] = A.frame_peer[i];
+                        A.held[at] = h.held;
+                        A.data_len[at] = h.dlen;
+                        A.shard_addr[at] = reinterpret_cast<uint64_t>(A.store + so);
+                        if (A.assignment != nullptr) A.assignment[at] = h.asg;
+                    }
+                }
+            }
+            if (kind != SS_ACCEPT_VERDICT_ACCEPTED) {
+                A.store_off[i] = ~0ull;
+                A.wal_off[i] = ~0ull;
+                A.wal_len[i] = 0u;
+                A.reply_len[i] = 0u;
+                A.reply_dst[i] = 0xffu;
+            }
+            A.verdict[i] = kind;
+        }
+        if (known) {
+            A.accepting[g] |= seen;                                     // Status::Accepting
+            A.bal_max_seen[g] = mx;
+        }
+    }
+    if (store_full) atomicOr(A.status, SS_DEV_STATUS_STORE_FULL);
+    if (wal_full) atomicOr(A.status, SS_DEV_STATUS_FRAME_OVERFLOW);
+}
+
+// 4. a warp per accepted frame: AcceptData record, held shards into the store, AcceptReply cell
+__global__ void __launch_bounds__(kAccThreads) acceptor_copy_kernel(const __grid_constant__ AccArgs A) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint64_t warp = (static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x) >> 5;
+    const uint64_t nwarps = (static_cast<uint64_t>(gridDim.x) * kAccThreads) >> 5;
+    for (uint64_t i = warp; i < A.n; i += nwarps) {
+        if (A.verdict[i] != SS_ACCEPT_VERDICT_ACCEPTED) continue;
+        const FrameHdr h = A.hdr[i];
+        const uint8_t *fr = A.buf + A.frame_off[i];
+        // WalEntry::AcceptData: length, wal_variant, then the Accept body from `slot` on as it came
+        uint8_t *rec = A.wal + A.wal_off[i];
+        const uint32_t wvl = static_cast<uint32_t>(wv_len(A.wal_variant));
+        const uint64_t tail = h.end - h.slot_at;
+        if (lane == 0u) {
+            const uint64_t body = wvl + tail;
+            for (int b = 0; b < 8; ++b) rec[b] = static_cast<uint8_t>(body >> (8 * (7 - b)));
+            wv_put(rec + 8, A.wal_variant);
+        }
+        warp_copy_unaligned(rec + 8u + wvl, fr + h.slot_at, tail, lane);
+        // held shards in index order, each in a SS_CW_SLOT_PITCH(L) slot, zero up to round_up(L, 16)
+        const uint64_t pitch = SS_CW_SLOT_PITCH(h.L);
+        const uint64_t nvec = (static_cast<uint64_t>(h.L) + 15u) >> 4;
+        uint8_t *dst = A.store + A.store_off[i];
+        uint64_t at = h.tags_at;
+        for (uint32_t j = 0; j < A.T; ++j) {
+            if (!((h.held >> j) & 1u)) { at += 1u; continue; }
+            // Some tag, then the shard length as the frame spells it: a non-minimal varint is as valid as the header
+            // pass found it, so its width comes from its own tag byte
+            const uint8_t t = fr[at + 1u];
+            const uint64_t some_len = 1u + (t < 251u ? 1u : t == 251u ? 3u : t == 252u ? 5u : 9u);
+            const uint8_t *src = fr + at + some_len;
+            for (uint64_t v = lane; v < nvec; v += 32u) {
+                const uint64_t left = h.L - v * 16u;
+                dev::stg128_cs(dst + v * 16u, dev::load16(src + v * 16u, left < 16u ? static_cast<int>(left) : 16));
+            }
+            dst += pitch;
+            at += some_len + static_cast<uint64_t>(h.L);
+        }
+        // AcceptReply of the instance as the whole call left it
+        if (lane == 0u) {
+            const uint32_t g = A.frame_group[i];
+            const uint64_t at_s = static_cast<uint64_t>(g) * 64u + (h.slot & 63u);
+            uint8_t *cell = A.replies + i * 48u;
+            uint32_t m = 8u;
+            m += wv_put(cell + m, 0u);                                   // PeerMessage::Msg
+            m += wv_put(cell + m, A.reply_variant);
+            m += wv_put(cell + m, h.slot);
+            m += wv_put(cell + m, A.inst_bal[at_s]);
+            if (A.crossword) {                                           // size, reply_ts: None
+                const uint64_t size = static_cast<uint64_t>(__popc(A.assignment[at_s])) * (static_cast<uint64_t>(A.data_len[at_s]) / A.d + 1u);
+                m += wv_put(cell + m, size);
+                cell[m++] = 0u;
+            }
+            const uint64_t body = m - 8u;
+            for (int b = 0; b < 8; ++b) cell[b] = static_cast<uint8_t>(body >> (8 * (7 - b)));
+            A.reply_len[i] = m;
+            A.reply_dst[i] = A.source[at_s];
+        }
+    }
+}
+
+// retire window prefixes: k = clamp(upto - base, 0, 64) positions leave Accepting, the base moves on
+__global__ void __launch_bounds__(kAccThreads)
+acceptor_advance_kernel(const uint64_t *__restrict__ upto, uint64_t G, uint64_t *__restrict__ window_base, uint64_t *__restrict__ accepting) {
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
+    for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; g < G; g += stride) {
+        const uint64_t base = window_base[g], u = upto[g];
+        const uint64_t k = u <= base ? 0ull : (u - base < 64u ? u - base : 64ull);
+        if (k == 0ull) continue;
+        accepting[g] &= ring_keep_after(k, base);
+        window_base[g] = base + k;
+    }
+}
+
+static inline uint32_t acc_grid(ss_ctx *ctx, uint64_t items, uint32_t per_cta) {
+    uint64_t ctas = (items + per_cta - 1) / per_cta;
+    const uint64_t cap = static_cast<uint64_t>(ctx->sm_count) * 8ull * 8ull;
+    if (ctas > cap) ctas = cap;
+    if (ctas == 0) ctas = 1;
+    return static_cast<uint32_t>(ctas);
+}
+
+template <typename T>
+static int acc_alloc(T **p, size_t count) {
+    SS_CUDA(cudaMalloc(reinterpret_cast<void **>(p), count * sizeof(T) ? count * sizeof(T) : 1));
+    SS_CUDA(cudaMemset(*p, 0, count * sizeof(T)));
+    return SS_OK;
+}
+
+static int key_bits(uint64_t G) {
+    int b = 1;
+    while (b < 32 && (G >> b) != 0u) ++b;                                    // keys run 0..G
+    return b;
+}
+
+static int ensure_scratch(ss_acceptor *a, uint64_t n) {
+    if (n <= a->cap_frames) return SS_OK;
+    ss_ctx *ctx = a->ctx;
+    SS_CUDA(cudaStreamSynchronize(ctx->stream));
+    void *old[] = {a->hdr, a->keys, a->idx, a->partials, a->sort_tmp};
+    for (void *b : old)
+        if (b) cudaFree(b);
+    a->hdr = nullptr; a->keys = nullptr; a->idx = nullptr; a->partials = nullptr; a->sort_tmp = nullptr;
+    a->cap_frames = 0;
+    SS_TRY(acc_alloc(&a->hdr, n));
+    SS_TRY(acc_alloc(&a->keys, 2 * n));
+    SS_TRY(acc_alloc(&a->idx, 2 * n));
+    SS_TRY(acc_alloc(&a->partials, scan_tiles(n)));
+    size_t bytes = 0;
+    SS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, a->keys, a->keys + n, a->idx, a->idx + n, static_cast<int>(n), 0,
+                                            key_bits(a->G), ctx->stream));
+    SS_CUDA(cudaMalloc(&a->sort_tmp, bytes ? bytes : 1));
+    a->sort_tmp_bytes = bytes;
+    a->cap_frames = n;
+    return SS_OK;
+}
+
+}  // namespace ssb
+
+using namespace ssb;
+
+extern "C" {
+
+int ss_acceptor_destroy(ss_acceptor *a) {
+    if (a == nullptr) return SS_OK;
+    if (a->ctx) {
+        cudaSetDevice(a->ctx->device);
+        cudaStreamSynchronize(a->ctx->stream);
+    }
+    void *bufs[] = {a->window_base, a->bal_max_seen, a->inst_bal, a->accepting, a->shard_addr, a->held, a->data_len, a->assignment,
+                    a->source, a->hdr, a->keys, a->idx, a->partials, a->sort_tmp, a->totals};
+    for (void *b : bufs)
+        if (b) cudaFree(b);
+    if (a->ctx) ctx_release(a->ctx);
+    delete a;
+    return SS_OK;
+}
+
+int ss_acceptor_create(ss_ctx *ctx, const ss_acceptor_config *cfg, uint64_t G, ss_acceptor **out) {
+    if (out == nullptr) return set_error(SS_ERR_INVALID_ARG, "null out pointer");
+    *out = nullptr;
+    if (cfg == nullptr || G == 0) return set_error(SS_ERR_INVALID_ARG, "null config or zero groups");
+    if (G > 0xffffffffull) return set_error(SS_ERR_INVALID_ARG, "at most 2^32 - 1 groups");
+    if (cfg->protocol != SS_PROTO_RSPAXOS && cfg->protocol != SS_PROTO_CROSSWORD)
+        return set_error(SS_ERR_INVALID_ARG, "the acceptor serves RSPaxos and Crossword, not protocol %u", cfg->protocol);
+    if (cfg->population == 0 || cfg->population > 32 || cfg->me >= cfg->population)
+        return set_error(SS_ERR_INVALID_ARG, "bad population %u / me %u", cfg->population, cfg->me);
+    if (cfg->data_shards == 0 || cfg->data_shards > cfg->total_shards || cfg->total_shards > 32)
+        return set_error(SS_ERR_INVALID_ARG, "shard counts must satisfy 1 <= d <= T <= 32 (d=%u, T=%u)", cfg->data_shards,
+                         cfg->total_shards);
+    if (ctx == nullptr) {
+        int count = 0;
+        const cudaError_t e = cudaGetDeviceCount(&count);
+        cudaGetLastError();
+        if (e != cudaSuccess || count == 0) return set_error(SS_ERR_NO_DEVICE, "no CUDA device available; this library has no CPU fallback");
+        return set_error(SS_ERR_INVALID_ARG, "null context");
+    }
+    SS_TRY(ctx_bind(ctx));
+    ss_acceptor *a = new (std::nothrow) ss_acceptor();
+    if (!a) return set_error(SS_ERR_OUT_OF_MEMORY, "host allocation failed");
+    a->ctx = ctx; a->cfg = *cfg; a->G = G;
+    ctx_retain(ctx);
+    int rc = SS_OK;
+    if ((rc = acc_alloc(&a->window_base, G)) || (rc = acc_alloc(&a->bal_max_seen, G)) || (rc = acc_alloc(&a->inst_bal, G * 64)) ||
+        (rc = acc_alloc(&a->accepting, G)) || (rc = acc_alloc(&a->shard_addr, G * 64)) || (rc = acc_alloc(&a->held, G * 64)) ||
+        (rc = acc_alloc(&a->data_len, G * 64)) || (rc = acc_alloc(&a->source, G * 64)) || (rc = acc_alloc(&a->totals, 2)) ||
+        (cfg->protocol == SS_PROTO_CROSSWORD && (rc = acc_alloc(&a->assignment, G * 64)))) {
+        ss_acceptor_destroy(a);
+        return rc;
+    }
+    *out = a;
+    return SS_OK;
+}
+
+int ss_acceptor_view_get(ss_acceptor *a, ss_acceptor_view *v) {
+    if (a == nullptr || v == nullptr) return set_error(SS_ERR_INVALID_ARG, "null argument");
+    memset(v, 0, sizeof(*v));
+    v->n_groups = a->G; v->protocol = a->cfg.protocol; v->population = a->cfg.population; v->me = a->cfg.me;
+    v->data_shards = a->cfg.data_shards; v->total_shards = a->cfg.total_shards;
+    v->window_base = a->window_base; v->bal_max_seen = a->bal_max_seen; v->inst_bal = a->inst_bal; v->accepting = a->accepting;
+    v->shard_addr = a->shard_addr; v->held = a->held; v->data_len = a->data_len; v->assignment = a->assignment; v->source = a->source;
+    return SS_OK;
+}
+
+int ss_acceptor_window_get(ss_acceptor *a, uint64_t **window_base) {
+    if (a == nullptr || window_base == nullptr) return set_error(SS_ERR_INVALID_ARG, "null argument");
+    *window_base = a->window_base;
+    return SS_OK;
+}
+
+int ss_acceptor_advance(ss_acceptor *a, const uint64_t *upto) {
+    if (a == nullptr || upto == nullptr) return set_error(SS_ERR_INVALID_ARG, "null acceptor or upto");
+    ss_ctx *ctx = a->ctx;
+    SS_TRY(ctx_bind(ctx));
+    acceptor_advance_kernel<<<acc_grid(ctx, a->G, kAccThreads), kAccThreads, 0, ctx->stream>>>(upto, a->G, a->window_base, a->accepting);
+    return launched(ctx);
+}
+
+int ss_acceptor_accept(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
+                       const uint8_t *frame_peer, uint64_t n, uint8_t *store, uint64_t store_capacity, uint64_t *store_off,
+                       uint8_t *wal, uint64_t wal_capacity, uint64_t *wal_off, uint32_t *wal_len, uint8_t *replies,
+                       uint32_t *reply_len, uint8_t *reply_dst, uint32_t *verdict, uint64_t *totals) {
+    if (a == nullptr) return set_error(SS_ERR_INVALID_ARG, "null acceptor");
+    ss_ctx *ctx = a->ctx;
+    SS_TRY(ctx_bind(ctx));
+    if (n == 0) {
+        if (totals != nullptr) SS_CUDA(cudaMemsetAsync(totals, 0, 16, ctx->stream));
+        return SS_OK;
+    }
+    if (!buf || !frame_off || !frame_group || !frame_peer || !store || !store_off || !wal || !wal_off || !wal_len || !replies ||
+        !reply_len || !reply_dst || !verdict)
+        return set_error(SS_ERR_INVALID_ARG, "null buffer");
+    if ((reinterpret_cast<uintptr_t>(store) | reinterpret_cast<uintptr_t>(wal)) & 15u)
+        return set_error(SS_ERR_INVALID_ARG, "store and wal must be 16-byte aligned");
+    if (n > 0x7fffffffull) return set_error(SS_ERR_INVALID_ARG, "at most 2^31 - 1 frames per call");
+    SS_TRY(ensure_scratch(a, n));
+    uint64_t *tot = totals != nullptr ? totals : a->totals;
+    AccArgs A{};
+    A.buf = buf; A.buf_len = buf_len; A.frame_off = frame_off; A.frame_group = frame_group; A.frame_peer = frame_peer;
+    A.n = n; A.G = a->G;
+    A.d = a->cfg.data_shards; A.T = a->cfg.total_shards; A.population = a->cfg.population; A.me = a->cfg.me;
+    A.accept_variant = a->cfg.accept_variant; A.wal_variant = a->cfg.wal_variant; A.reply_variant = a->cfg.reply_variant;
+    A.crossword = a->cfg.protocol == SS_PROTO_CROSSWORD ? 1u : 0u;
+    A.window_base = a->window_base; A.bal_max_seen = a->bal_max_seen; A.inst_bal = a->inst_bal; A.accepting = a->accepting;
+    A.shard_addr = a->shard_addr; A.held = a->held; A.data_len = a->data_len; A.assignment = a->assignment; A.source = a->source;
+    A.hdr = a->hdr; A.key_in = a->keys; A.idx_in = a->idx; A.key = a->keys + n; A.idx = a->idx + n;
+    A.store = store; A.store_cap = store_capacity; A.store_off = store_off;
+    A.wal = wal; A.wal_cap = wal_capacity; A.wal_off = wal_off; A.wal_len = wal_len;
+    A.replies = replies; A.reply_len = reply_len; A.reply_dst = reply_dst; A.verdict = verdict; A.status = ctx->dev_status;
+    const uint32_t grid_t = acc_grid(ctx, n, kAccThreads);
+    acceptor_header_kernel<<<grid_t, kAccThreads, 0, ctx->stream>>>(A);
+    SS_TRY(launched(ctx));
+    size_t bytes = a->sort_tmp_bytes;
+    SS_CUDA(cub::DeviceRadixSort::SortPairs(a->sort_tmp, bytes, a->keys, a->keys + n, a->idx, a->idx + n, static_cast<int>(n), 0,
+                                            key_bits(a->G), ctx->stream));
+    SS_TRY(launched(ctx));
+    acceptor_ballot_kernel<<<grid_t, kAccThreads, 0, ctx->stream>>>(A);
+    SS_TRY(launched(ctx));
+    SS_TRY(launch_exclusive_scan_u64(ctx, store_off, n, a->partials, tot));
+    SS_TRY(launch_exclusive_scan_u64(ctx, wal_off, n, a->partials, tot + 1));
+    acceptor_place_kernel<<<grid_t, kAccThreads, 0, ctx->stream>>>(A);
+    SS_TRY(launched(ctx));
+    acceptor_copy_kernel<<<acc_grid(ctx, n, kAccThreads / 32), kAccThreads, 0, ctx->stream>>>(A);
+    return launched(ctx);
+}
+
+}  // extern "C"

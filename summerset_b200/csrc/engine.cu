@@ -32,6 +32,7 @@
 
 #include "device_common.cuh"
 #include "ss_internal.hpp"
+#include "window_ring.cuh"
 
 struct ss_engine {
     ss_ctx *ctx = nullptr;
@@ -73,10 +74,6 @@ static inline uint32_t eng_grid(ss_ctx *ctx, uint64_t items) {
     if (ctas == 0) ctas = 1;
     return static_cast<uint32_t>(ctas);
 }
-
-// ring word (bit p = absolute slot with s & 63 == p) <-> window word (bit i = absolute slot base + i), r = base & 63
-__device__ __forceinline__ uint64_t ring_to_window(uint64_t x, uint32_t r) { return (x >> r) | (x << ((64u - r) & 63u)); }
-__device__ __forceinline__ uint64_t window_to_ring(uint64_t x, uint32_t r) { return (x << r) | (x >> ((64u - r) & 63u)); }
 
 // ---- propose bookkeeping: one new instance per group enters Accepting --------------------------------------------
 // window position of the group's first Null slot (rspaxos/mod.rs:434-442); 64 = the window is full
@@ -299,7 +296,7 @@ engine_advance_kernel(const uint64_t *__restrict__ upto, uint64_t *__restrict__ 
             k = u <= base ? 0ull : (u - base < k ? u - base : k);
         }
         if (k == 0ull) continue;
-        const uint64_t keep = window_to_ring(k == 64ull ? 0ull : ~0ull << k, r);
+        const uint64_t keep = ring_keep_after(k, base);
         committed[g] = cm & keep;
         accepting[g] &= keep;
         for (uint32_t q = 0; q < R; ++q) planes[static_cast<uint64_t>(q) * G + g] &= keep;

@@ -12,6 +12,11 @@ torch tensors (zero-copy views) so tests can read results and install state; it 
         on_accept_replies(records)          handle_msg_accept_reply filters (multipaxos/messages.rs:377-409, ...)
         tick()                              commit decision + commit_bar, one kernel
         advance([upto])                     retire committed prefixes: window_base moves on (multipaxos/snapshot.rs:121-171)
+    Acceptor(ctx, protocol, G, population, me, d, T)   protocol in {"rspaxos", "crossword"}: the follower side
+        accept(buf, frame_off, frame_group, frame_peer, store, wal)   handle_msg_accept over a batch of Accept frames
+                                            (rspaxos/messages.rs:329-392, crossword/messages.rs:403-470): store, AcceptData
+                                            records and AcceptReply cells
+        advance(upto)                       retire window prefixes
     RaftEngine(ctx, G, population[, fault_tolerance, craft])
         append(n_new) / on_append_replies(records) / tick()      raft/messages.rs:243-309, craft/messages.rs:300-308
 """
@@ -197,3 +202,72 @@ class RaftEngine(_EngineBase):
     def tick(self) -> Tuple[torch.Tensor, torch.Tensor]:
         check(self.lib.ss_engine_tick(self.h, None))
         return self.last_commit, self.last_snap
+
+
+class Acceptor:
+    """The follower side of the RSPaxos / Crossword accept path for G groups (ss_acceptor_* in include/summerset_b200.h).
+    State tensors are zero-copy views of the acceptor's device arrays; per-slot arrays are rings (slot s at s & 63)."""
+
+    REPLY_CELL = 48
+
+    def __init__(self, ctx: Context, protocol: str, n_groups: int, population: int, me: int, data_shards: int, total_shards: int,
+                 accept_variant: int = 2, wal_variant: int = 1, reply_variant: int = 3):
+        assert protocol in ("rspaxos", "crossword")
+        self.ctx, self.lib, self.G = ctx, ctx.lib, n_groups
+        self.protocol, self.n, self.me, self.d, self.T = protocol, population, me, data_shards, total_shards
+        cfg = _lib.AcceptorConfig(_PROTO[protocol], population, me, data_shards, total_shards, accept_variant, wal_variant,
+                                  reply_variant)
+        h = C.c_void_p()
+        check(self.lib.ss_acceptor_create(ctx.h, C.byref(cfg), n_groups, C.byref(h)))
+        self.h = h
+        v = self.view = _lib.AcceptorView()
+        check(self.lib.ss_acceptor_view_get(self.h, C.byref(v)))
+        self.dev = torch.device("cuda", ctx.device)
+        G = n_groups
+        t = lambda ptr, shape, ts, dt: None if not ptr else torch.as_tensor(_DevArray(ptr, shape, ts), device=self.dev).view(dt).view(shape)
+        self.window_base = t(v.window_base, (G,), "<i8", torch.int64)
+        self.bal_max_seen = t(v.bal_max_seen, (G,), "<i8", torch.int64)
+        self.inst_bal = t(v.inst_bal, (G * 64,), "<i8", torch.int64)
+        self.accepting = t(v.accepting, (G,), "<i8", torch.int64)
+        self.shard_addr = t(v.shard_addr, (G * 64,), "<i8", torch.int64)
+        self.held = t(v.held, (G * 64,), "<i4", torch.int32)
+        self.data_len = t(v.data_len, (G * 64,), "<i4", torch.int32)
+        self.assignment = t(v.assignment, (G * 64,), "<i4", torch.int32)
+        self.source = t(v.source, (G * 64,), "|u1", torch.uint8)
+
+    def accept(self, buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor, frame_peer: torch.Tensor,
+               store: torch.Tensor, wal: torch.Tensor, store_capacity: Optional[int] = None, wal_capacity: Optional[int] = None) -> dict:
+        """buf uint8 (frames at any alignment), frame_off int64 [n], frame_group int32 [n], frame_peer uint8 [n]; store / wal:
+        caller-owned uint8 buffers (16-byte aligned).  Returns the per-frame outputs as device tensors: store_off, wal_off
+        (int64, -1 = not accepted), wal_len, reply_len, verdict (int32), reply_dst (uint8), replies (uint8 [n, 48]) and
+        totals (int64 [2]: store and WAL bytes asked for)."""
+        assert buf.dtype == torch.uint8 and frame_off.dtype == torch.int64 and frame_group.dtype == torch.int32
+        assert frame_peer.dtype == torch.uint8 and store.dtype == torch.uint8 and wal.dtype == torch.uint8
+        n, dev = frame_off.numel(), buf.device
+        e = lambda dt, *shape: torch.empty(shape if shape else (n,), dtype=dt, device=dev)
+        out = dict(store_off=e(torch.int64), wal_off=e(torch.int64), wal_len=e(torch.int32),
+                   replies=torch.zeros((n, self.REPLY_CELL), dtype=torch.uint8, device=dev), reply_len=e(torch.int32),
+                   reply_dst=e(torch.uint8), verdict=e(torch.int32), totals=e(torch.int64, 2))
+        p = lambda x: x.data_ptr()
+        check(self.lib.ss_acceptor_accept(self.h, p(buf), buf.numel(), p(frame_off), p(frame_group), p(frame_peer), n, p(store),
+                                          store.numel() if store_capacity is None else store_capacity, p(out["store_off"]), p(wal),
+                                          wal.numel() if wal_capacity is None else wal_capacity, p(out["wal_off"]), p(out["wal_len"]),
+                                          p(out["replies"]), p(out["reply_len"]), p(out["reply_dst"]), p(out["verdict"]),
+                                          p(out["totals"])))
+        return out
+
+    def advance(self, upto: torch.Tensor) -> None:
+        """Retires window prefixes up to the absolute slots upto (int64 [G])."""
+        assert upto.is_cuda and upto.dtype == torch.int64 and upto.numel() == self.G
+        check(self.lib.ss_acceptor_advance(self.h, upto.data_ptr()))
+
+    def close(self) -> None:
+        if getattr(self, "h", None) is not None and self.h:
+            self.lib.ss_acceptor_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

@@ -5,6 +5,8 @@
 //   ssb::Bitmap        <- src/utils/bitmap.rs            (u8 id -> bool bitset)
 //   ssb::ReedSolomon   <- reed_solomon_erasure::galois_8::ReedSolomon as used by src/utils/rscoding.rs
 //   ssb::RSCodeword    <- src/utils/rscoding.rs          (T = an already serialised byte string)
+//   ssb::Acceptor      <- the follower side of rspaxos/messages.rs handle_msg_accept + durability.rs's AcceptReply,
+//                         batched over many groups (ss_acceptor_*, device buffers)
 // Only bookkeeping happens here.  Every shard byte is computed by the CUDA kernels behind the C ABI;
 // a failing ABI call becomes a SummersetError (src/utils/error.rs:6-14) -- there is no CPU fallback.
 #pragma once
@@ -286,6 +288,39 @@ class RSCodeword {
     }
     uint8_t d_ = 0, p_ = 0;
     size_t data_len_ = 0, shard_len_ = 0;
+};
+
+// ---------------------------------------------------------------------------------------------
+// Acceptor: RAII over ss_acceptor (follower side of the RSPaxos / Crossword accept path).  handle_msg_accept runs for a
+// whole batch of received Accept frames; the AcceptData records it returns are what the host appends to its WAL, and
+// the AcceptReply cells go out (send_msg to reply_dst[i]) only once those records are durable.
+// ---------------------------------------------------------------------------------------------
+class Acceptor {
+  public:
+    Acceptor(ss_ctx *ctx, const ss_acceptor_config &cfg, uint64_t n_groups) { check(ss_acceptor_create(ctx, &cfg, n_groups, &acc_)); }
+    ~Acceptor() { ss_acceptor_destroy(acc_); }
+    Acceptor(const Acceptor &) = delete;
+    Acceptor &operator=(const Acceptor &) = delete;
+
+    // every pointer is a device pointer; see ss_acceptor_accept for the outputs
+    void handle_msg_accept(const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
+                           const uint8_t *frame_peer, uint64_t n_frames, uint8_t *store, uint64_t store_capacity,
+                           uint64_t *store_off, uint8_t *wal, uint64_t wal_capacity, uint64_t *wal_off, uint32_t *wal_len,
+                           uint8_t *replies, uint32_t *reply_len, uint8_t *reply_dst, uint32_t *verdict, uint64_t *totals) {
+        check(ss_acceptor_accept(acc_, buf, buf_len, frame_off, frame_group, frame_peer, n_frames, store, store_capacity, store_off,
+                                 wal, wal_capacity, wal_off, wal_len, replies, reply_len, reply_dst, verdict, totals));
+    }
+    // start_slot moves to upto[g] (device [G]), at most 64 slots at a time
+    void advance_start_slot(const uint64_t *upto) { check(ss_acceptor_advance(acc_, upto)); }
+    ss_acceptor_view view() const {
+        ss_acceptor_view v;
+        check(ss_acceptor_view_get(acc_, &v));
+        return v;
+    }
+    ss_acceptor *handle() const { return acc_; }
+
+  private:
+    ss_acceptor *acc_ = nullptr;
 };
 
 }  // namespace ssb
