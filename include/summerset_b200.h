@@ -278,9 +278,12 @@ int ss_raft_kth_match_dev(ss_ctx *ctx, const uint32_t *match, uint32_t n_peers, 
 
 /* Prepare-phase shard merge + decision for n_instances recovering instances (leader fail-over;
  * rspaxos/messages.rs:182-259, crossword/messages.rs:233-312).  vote_bal[r*N+i] / vote_mask[r*N+i] = the
- * (ballot, shards carried) of replica r's PrepareReply vote for instance i; vote_mask == 0 means "no vote".
- * merged[i] = shard set inst.reqs_cw ends with (shards voted at the highest ballot; max_bal[i] that ballot;
- * order-independent because absorb_other only adds).  action[i]: bit0 USE (>= data_shards shards), bit1 NULL
+ * (ballot, shards carried) of replica r's PrepareReply vote for instance i; vote_bal == 0 means "no vote", as the
+ * reply's `voted = if inst.voted.0 > 0 { Some(..) } else { None }` (rspaxos/durability.rs, crossword/durability.rs).
+ * A vote with vote_bal > 0 and vote_mask == 0 is Some((bal, no shards)) -- a Crossword replica whose assignment row is
+ * empty still records its ballot when it accepts -- and, at a ballot above the others, discards the shards gathered
+ * at lower ballots.  merged[i] = shard set inst.reqs_cw ends with (shards voted at the highest ballot; max_bal[i] that
+ * ballot; order-independent because absorb_other only adds).  action[i]: bit0 USE (>= data_shards shards), bit1 NULL
  * request batch (fewer, but acks_cnt[i] >= population - fault_tolerance), 0 = not yet; bit2 reconstruct_data
  * needed; bit3 compute_parity needed (avail shards < POPULATION, as the reference compares).  The regeneration
  * itself is ss_rs_reconstruct_batch_dev(present = merged, data_only = 0). */

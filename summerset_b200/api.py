@@ -231,7 +231,8 @@ def _ctx_extras():
 
     def prepare_merge(self, vote_bal: torch.Tensor, vote_mask: torch.Tensor, acks_cnt: torch.Tensor, data_shards: int,
                       population: int, fault_tolerance: int):
-        """vote_bal int64 [R, N], vote_mask int32 [R, N] (0 = no vote), acks_cnt uint8 [N]."""
+        """vote_bal int64 [R, N] (0 = no vote), vote_mask int32 [R, N], acks_cnt uint8 [N].  A vote with a non-zero
+        ballot and mask 0 carries no shards but still counts: at the highest ballot it clears the merged set."""
         assert vote_bal.dtype == torch.int64 and vote_mask.dtype == torch.int32 and acks_cnt.dtype == torch.uint8
         R, N = vote_bal.shape
         dev = vote_bal.device

@@ -399,7 +399,9 @@ kth_match_kernel(const uint32_t *__restrict__ match, uint32_t n_peers, uint64_t 
 // Prepare-phase shard merge + decision, one instance per thread (rspaxos/messages.rs:182-259,
 // crossword/messages.rs:233-312): keep the shards voted at the highest ballot (the union over the replies
 // carrying that ballot is what the chain of absorb_other calls leaves in inst.reqs_cw, in any arrival order),
-// then decide use / null / wait and whether reconstruct_data and compute_parity are needed.
+// then decide use / null / wait and whether reconstruct_data and compute_parity are needed.  A reply votes iff its
+// ballot is non-zero (rspaxos/durability.rs, crossword/durability.rs: `voted = if inst.voted.0 > 0`): a vote with no
+// shards still raises the ballot and discards the shards gathered at lower ones.
 __global__ void __launch_bounds__(kTallyThreads)
 prepare_merge_kernel(const uint64_t *__restrict__ vote_bal, const uint32_t *__restrict__ vote_mask, uint32_t R, uint64_t N,
                      const uint8_t *__restrict__ acks_cnt, uint32_t d, uint32_t population, uint32_t f,
@@ -410,9 +412,9 @@ prepare_merge_kernel(const uint64_t *__restrict__ vote_bal, const uint32_t *__re
         uint64_t mb = 0;              // prepare_max_bal starts at 0
         uint32_t cw = 0;
         for (uint32_t r = 0; r < R; ++r) {
-            const uint32_t m = __ldg(vote_mask + static_cast<uint64_t>(r) * N + i);
-            if (m == 0u) continue;    // voted == None
             const uint64_t b = __ldg(vote_bal + static_cast<uint64_t>(r) * N + i);
+            if (b == 0ull) continue;  // voted == None
+            const uint32_t m = __ldg(vote_mask + static_cast<uint64_t>(r) * N + i);
             if (b > mb) { mb = b; cw = m; }
             else if (b == mb) cw |= m;
         }

@@ -158,15 +158,17 @@ def test_craft_on_gpu(ctx, oracle, n, f):
 
 
 @pytest.mark.gpu
-def test_prepare_merge_on_gpu_and_recovery_roundtrip(ctx, oracle):
+def test_prepare_merge_by_ballot_on_gpu_and_recovery_roundtrip(ctx, oracle):
     """merge + decision vs oracle, then the full fail-over data path on the GPU: reconstruct_all on the merged
-    shard sets regenerates the codewords the USE decision promises (rspaxos/messages.rs:227-259)."""
+    shard sets regenerates the codewords the USE decision promises (rspaxos/messages.rs:227-259).  A replica that
+    did not vote replies ballot 0 (rspaxos/durability.rs: `voted` is None iff its ballot is 0); a non-zero ballot
+    with no shards is a vote, which tests/test_failover.py covers."""
     from summerset_b200.api import ReedSolomon, round_up, shard_len
     rng = np.random.default_rng(2)
     R, d, p, population, f = 5, 3, 2, 5, 1
     N = 4099
     has = rng.random((R, N)) < 0.75
-    bal = rng.integers(1, 4, (R, N)).astype(np.uint64)
+    bal = np.where(has, rng.integers(1, 4, (R, N)), 0).astype(np.uint64)          # a replica with no vote replies ballot 0
     mask = np.where(has, (1 << np.arange(R))[:, None], 0).astype(np.uint32)
     acks = rng.integers(3, 6, N).astype(np.uint8)
     mb, mg, act = ctx.prepare_merge(_t(bal), _t(mask), torch.from_numpy(acks).to(DEV), d, population, f)
