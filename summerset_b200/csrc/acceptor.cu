@@ -362,10 +362,12 @@ static inline uint32_t acc_grid(ss_ctx *ctx, uint64_t items, uint32_t per_cta) {
     return static_cast<uint32_t>(ctas);
 }
 
+// zeroed on the context's stream: a cudaMemset would go to the legacy default stream, which a non-blocking context
+// stream does not wait for, so it could land after the caller's first writes (window_base) or the first accept
 template <typename T>
-static int acc_alloc(T **p, size_t count) {
+static int acc_alloc(ss_ctx *ctx, T **p, size_t count, bool zero = true) {
     SS_CUDA(cudaMalloc(reinterpret_cast<void **>(p), count * sizeof(T) ? count * sizeof(T) : 1));
-    SS_CUDA(cudaMemset(*p, 0, count * sizeof(T)));
+    if (zero) SS_CUDA(cudaMemsetAsync(*p, 0, count * sizeof(T), ctx->stream));
     return SS_OK;
 }
 
@@ -384,10 +386,11 @@ static int ensure_scratch(ss_acceptor *a, uint64_t n) {
         if (b) cudaFree(b);
     a->hdr = nullptr; a->keys = nullptr; a->idx = nullptr; a->partials = nullptr; a->sort_tmp = nullptr;
     a->cap_frames = 0;
-    SS_TRY(acc_alloc(&a->hdr, n));
-    SS_TRY(acc_alloc(&a->keys, 2 * n));
-    SS_TRY(acc_alloc(&a->idx, 2 * n));
-    SS_TRY(acc_alloc(&a->partials, scan_tiles(n)));
+    // the header pass writes hdr, key_in and idx_in of every frame, the sort the rest, the scan its partials
+    SS_TRY(acc_alloc(ctx, &a->hdr, n, false));
+    SS_TRY(acc_alloc(ctx, &a->keys, 2 * n, false));
+    SS_TRY(acc_alloc(ctx, &a->idx, 2 * n, false));
+    SS_TRY(acc_alloc(ctx, &a->partials, scan_tiles(n), false));
     size_t bytes = 0;
     SS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, a->keys, a->keys + n, a->idx, a->idx + n, static_cast<int>(n), 0,
                                             key_bits(a->G), ctx->stream));
@@ -443,10 +446,11 @@ int ss_acceptor_create(ss_ctx *ctx, const ss_acceptor_config *cfg, uint64_t G, s
     a->ctx = ctx; a->cfg = *cfg; a->G = G;
     ctx_retain(ctx);
     int rc = SS_OK;
-    if ((rc = acc_alloc(&a->window_base, G)) || (rc = acc_alloc(&a->bal_max_seen, G)) || (rc = acc_alloc(&a->inst_bal, G * 64)) ||
-        (rc = acc_alloc(&a->accepting, G)) || (rc = acc_alloc(&a->shard_addr, G * 64)) || (rc = acc_alloc(&a->held, G * 64)) ||
-        (rc = acc_alloc(&a->data_len, G * 64)) || (rc = acc_alloc(&a->source, G * 64)) || (rc = acc_alloc(&a->totals, 2)) ||
-        (cfg->protocol == SS_PROTO_CROSSWORD && (rc = acc_alloc(&a->assignment, G * 64)))) {
+    if ((rc = acc_alloc(ctx, &a->window_base, G)) || (rc = acc_alloc(ctx, &a->bal_max_seen, G)) ||
+        (rc = acc_alloc(ctx, &a->inst_bal, G * 64)) || (rc = acc_alloc(ctx, &a->accepting, G)) ||
+        (rc = acc_alloc(ctx, &a->shard_addr, G * 64)) || (rc = acc_alloc(ctx, &a->held, G * 64)) ||
+        (rc = acc_alloc(ctx, &a->data_len, G * 64)) || (rc = acc_alloc(ctx, &a->source, G * 64)) || (rc = acc_alloc(ctx, &a->totals, 2)) ||
+        (cfg->protocol == SS_PROTO_CROSSWORD && (rc = acc_alloc(ctx, &a->assignment, G * 64)))) {
         ss_acceptor_destroy(a);
         return rc;
     }

@@ -333,7 +333,8 @@ static int ctx_create_common(int device, void *stream, bool borrow, ss_ctx **out
         ctx->owns_stream = true;
     }
     e = cudaMalloc(reinterpret_cast<void **>(&ctx->dev_status), 256);
-    if (e == cudaSuccess) e = cudaMemset(ctx->dev_status, 0, 256);
+    // on the context's stream, which a non-blocking stream needs: the legacy default stream is not ordered before it
+    if (e == cudaSuccess) e = cudaMemsetAsync(ctx->dev_status, 0, 256, ctx->stream);
     if (e != cudaSuccess) {
         if (ctx->owns_stream) cudaStreamDestroy(ctx->stream);
         delete ctx;

@@ -482,10 +482,12 @@ engine_raft_snap_kernel(const uint32_t *__restrict__ match, uint32_t P, uint64_t
     }
 }
 
+// zeroed on the context's stream: a cudaMemset would go to the legacy default stream, which a non-blocking context
+// stream does not wait for, so it could land after the caller's first writes (set_prepared_ballots, window_base)
 template <typename T>
-static int dalloc(T **p, size_t count, bool zero = true) {
+static int dalloc(ss_ctx *ctx, T **p, size_t count, bool zero = true) {
     SS_CUDA(cudaMalloc(reinterpret_cast<void **>(p), count * sizeof(T) ? count * sizeof(T) : 1));
-    if (zero) SS_CUDA(cudaMemset(*p, 0, count * sizeof(T)));
+    if (zero) SS_CUDA(cudaMemsetAsync(*p, 0, count * sizeof(T), ctx->stream));
     return SS_OK;
 }
 
@@ -555,14 +557,16 @@ int ss_engine_create(ss_ctx *ctx, const ss_engine_config *cfg, uint64_t G, ss_en
         if ((e->W & (e->W - 1)) || e->W > 4096) return fail(set_error(SS_ERR_INVALID_ARG, "raft_window must be a power of two <= 4096"));
         // quorum_cnt (raft/mod.rs), or CRaft's majority + f (craft/messages.rs:300-308; full-copy mode = plain Raft)
         e->threshold = cfg->protocol == SS_PROTO_CRAFT ? majority + cfg->fault_tolerance : majority;
-        if ((rc = dalloc(&e->match, size_t(e->n_peers) * G)) || (rc = dalloc(&e->next_slot, size_t(e->n_peers) * G)) ||
-            (rc = dalloc(&e->last_commit, G)) || (rc = dalloc(&e->log_end, G)) || (rc = dalloc(&e->curr_term, G)) ||
-            (rc = dalloc(&e->terms, G * e->W)) || (rc = dalloc(&e->last_snap, G)) || (rc = dalloc(&e->touched, G)))
+        if ((rc = dalloc(ctx, &e->match, size_t(e->n_peers) * G)) || (rc = dalloc(ctx, &e->next_slot, size_t(e->n_peers) * G)) ||
+            (rc = dalloc(ctx, &e->last_commit, G)) || (rc = dalloc(ctx, &e->log_end, G)) || (rc = dalloc(ctx, &e->curr_term, G)) ||
+            (rc = dalloc(ctx, &e->terms, G * e->W)) || (rc = dalloc(ctx, &e->last_snap, G)) || (rc = dalloc(ctx, &e->touched, G)))
             return fail(rc);
         // slot 0 is the sentinel entry (raft/mod.rs: log starts with a dummy entry): next_slot = 1, log_end = 1
+        // on the context's stream, after the zeroing above; `ones` lives until the copies have completed
         std::vector<uint32_t> ones(size_t(e->n_peers) * G > G ? size_t(e->n_peers) * G : G, 1u);
-        cudaError_t ce = cudaMemcpy(e->next_slot, ones.data(), size_t(e->n_peers) * G * 4, cudaMemcpyHostToDevice);
-        if (ce == cudaSuccess) ce = cudaMemcpy(e->log_end, ones.data(), G * 4, cudaMemcpyHostToDevice);
+        cudaError_t ce = cudaMemcpyAsync(e->next_slot, ones.data(), size_t(e->n_peers) * G * 4, cudaMemcpyHostToDevice, ctx->stream);
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(e->log_end, ones.data(), G * 4, cudaMemcpyHostToDevice, ctx->stream);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(ctx->stream);
         if (ce != cudaSuccess) return fail(cuda_error(ce, "initialise Raft state", __FILE__, __LINE__));
         *out = e;
         return SS_OK;
@@ -581,9 +585,9 @@ int ss_engine_create(ss_ctx *ctx, const ss_engine_config *cfg, uint64_t G, ss_en
             e->threshold = 0;
         }
     }
-    if ((rc = dalloc(&e->planes, size_t(n) * G)) || (rc = dalloc(&e->bal_prepared, G)) || (rc = dalloc(&e->inst_bal, G * 64)) ||
-        (rc = dalloc(&e->accepting, G)) || (rc = dalloc(&e->committed, G)) || (rc = dalloc(&e->window_base, G)) ||
-        (rc = dalloc(&e->commit_bar, G)))
+    if ((rc = dalloc(ctx, &e->planes, size_t(n) * G)) || (rc = dalloc(ctx, &e->bal_prepared, G)) || (rc = dalloc(ctx, &e->inst_bal, G * 64)) ||
+        (rc = dalloc(ctx, &e->accepting, G)) || (rc = dalloc(ctx, &e->committed, G)) || (rc = dalloc(ctx, &e->window_base, G)) ||
+        (rc = dalloc(ctx, &e->commit_bar, G)))
         return fail(rc);
     if (cfg->protocol != SS_PROTO_MULTIPAXOS) {
         if (cfg->data_len == 0) return fail(set_error(SS_ERR_INVALID_ARG, "data_len must be > 0 for an RS-coded protocol"));
@@ -592,10 +596,10 @@ int ss_engine_create(ss_ctx *ctx, const ss_engine_config *cfg, uint64_t G, ss_en
         e->ds = (e->L + 15u) & ~15u;
         const uint32_t keep = cfg->keep_slots ? cfg->keep_slots : 1;
         e->cfg.keep_slots = keep;
-        if ((rc = dalloc(&e->shards, size_t(keep) * e->T * G * e->ds))) return fail(rc);
+        if ((rc = dalloc(ctx, &e->shards, size_t(keep) * e->T * G * e->ds))) return fail(rc);
     }
     if (cfg->protocol == SS_PROTO_CROSSWORD) {
-        if ((rc = dalloc(&e->policy_idx, G * 64))) return fail(rc);
+        if ((rc = dalloc(ctx, &e->policy_idx, G * 64))) return fail(rc);
     }
     *out = e;
     return SS_OK;
@@ -634,9 +638,10 @@ int ss_engine_set_policies(ss_engine *e, const uint32_t *policies_host, uint32_t
     e->lut_words = (entries + 31) / 32;
     e->n_policies = n_policies;
     e->balanced = balanced;
-    SS_TRY(dalloc(&e->policies, size_t(n_policies) * e->n, false));
-    SS_TRY(dalloc(&e->lut_bits, e->lut_words));
-    SS_CUDA(cudaMemcpy(e->policies, policies_host, size_t(n_policies) * e->n * 4, cudaMemcpyHostToDevice));
+    SS_TRY(dalloc(ctx, &e->policies, size_t(n_policies) * e->n, false));
+    SS_TRY(dalloc(ctx, &e->lut_bits, e->lut_words));
+    // stream-ordered before the table kernel; from pageable memory the call returns once the bytes are staged
+    SS_CUDA(cudaMemcpyAsync(e->policies, policies_host, size_t(n_policies) * e->n * 4, cudaMemcpyHostToDevice, ctx->stream));
     return launch_crossword_lut(ctx, e->policies, n_policies, e->n, e->T, e->d, e->majority, e->cfg.fault_tolerance, balanced,
                                 e->lut_bits);
 }
@@ -696,9 +701,9 @@ int ss_engine_propose_ragged(ss_engine *e, const uint8_t *arena, const uint64_t 
         return set_error(SS_ERR_INVALID_ARG, "ss_engine_set_policies must be called before proposing");
     ss_ctx *ctx = e->ctx;
     SS_TRY(ctx_bind(ctx));
-    if (e->rg_len == nullptr) SS_TRY(dalloc(&e->rg_len, e->G, false));
-    if (e->rg_partials == nullptr) SS_TRY(dalloc(&e->rg_partials, scan_tiles(e->G), false));
-    if (e->rg_need == nullptr) SS_TRY(dalloc(&e->rg_need, 1, false));
+    if (e->rg_len == nullptr) SS_TRY(dalloc(ctx, &e->rg_len, e->G, false));
+    if (e->rg_partials == nullptr) SS_TRY(dalloc(ctx, &e->rg_partials, scan_tiles(e->G), false));
+    if (e->rg_need == nullptr) SS_TRY(dalloc(ctx, &e->rg_need, 1, false));
     const uint32_t grid = eng_grid(ctx, e->G);
     engine_ragged_prepare_kernel<<<grid, kEngThreads, 0, ctx->stream>>>(data_len, e->G, e->d, e->window_base, e->accepting, e->committed,
                                                                       e->rg_len, shard_off, ctx->dev_status);

@@ -218,7 +218,7 @@ __global__ void __launch_bounds__(kWireThreads) accept_reply_parse_kernel(const 
         const uint32_t grp = A.frame_group[i];
         const uint64_t off = A.frame_off[i];
         do {
-            if (off + 8u > A.buf_len) break;
+            if (off > A.buf_len || A.buf_len - off < 8u) break;                       // off + 8 would wrap near 2^64
             const uint8_t *fr = A.buf + off;
             uint64_t len = 0;
             for (int b = 0; b < 8; ++b) len = (len << 8) | fr[b];

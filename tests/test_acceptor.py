@@ -171,12 +171,12 @@ def _stream(cfg, st, frames, groups, peers, store_cap, wal_cap):
     run = list(st.bmax)
     s_at = w_at = 0
     for i, (fr, g) in enumerate(zip(frames, groups)):
+        if g >= G:                                    # a group this acceptor does not hold: malformed, whatever the frame
+            verdict[i] = MALFORMED
+            continue
         f = _decode(fr, cfg)
         if isinstance(f, int):
             verdict[i] = f
-            continue
-        if g >= G:
-            verdict[i] = MALFORMED
             continue
         dec[i] = f
         if f["slot"] < st.base[g]:                    # `slot < start_slot`: ignored
@@ -221,11 +221,13 @@ def _stream(cfg, st, frames, groups, peers, store_cap, wal_cap):
 
 def _oracle_record(oracle, cfg, f):
     """WalEntry::AcceptData re-encoded from the decoded fields by the oracle's encoders; Crossword appends
-    assignment: Vec<Bitmap> (crossword/mod.rs:288-293) after the oracle's RSPaxos-shaped record body"""
+    assignment: Vec<Bitmap> (crossword/mod.rs:288-293) after the oracle's RSPaxos-shaped record body.  The oracle
+    writes the record variant as 1 (one byte): the body after it is kept, the variant is the acceptor's wal_variant."""
     rec = oracle.wal_accept_data(f["slot"], f["ballot"], cfg.d, cfg.T - cfg.d, f["dlen"], f["shards"])
-    if not cfg.cw:
-        return rec
-    body = rec[8:] + oracle.varint(len(f["asg"])) + b"".join(oracle.bitmap_encode(cfg.T, a) for a in f["asg"])
+    assert rec[8] == 1
+    body = oracle.varint(cfg.wv) + rec[9:]
+    if cfg.cw:
+        body += oracle.varint(len(f["asg"])) + b"".join(oracle.bitmap_encode(cfg.T, a) for a in f["asg"])
     return len(body).to_bytes(8, "big") + body
 
 
@@ -252,20 +254,20 @@ def _advance(st, upto):
 RS = Cfg("rspaxos", 5, 1, 3, 5)
 
 
-def _acc(oracle, slot, ballot, held=0b00010, dlen=9, d=3, p=2, asg=None, T=5):
+def _acc(oracle, slot, ballot, held=0b00010, dlen=9, d=3, p=2, asg=None, T=5, av=2):
     L = -(-dlen // d)
     shards = [bytes([(slot + j) & 255]) * L if (held >> j) & 1 else None for j in range(d + p)]
     if not any(shards):
         shards[0] = b""
-    return oracle.frame_accept(2, slot, ballot, d, p, dlen, shards, asg, T)
+    return oracle.frame_accept(av, slot, ballot, d, p, dlen, shards, asg, T)
 
 
-def _acc_wide(slot, ballot, held, dlen, d, p, asg, T):
+def _acc_wide(slot, ballot, held, dlen, d, p, asg, T, av=2):
     """an Accept whose every u64 varint uses the 9-byte form (tag 253): not minimal, but what the crate's decoder and
     the oracle's read as the same values"""
     w = lambda v: bytes([253]) + int(v).to_bytes(8, "little")
     L = -(-dlen // d)
-    body = b"\x00\x02" + w(slot) + w(ballot) + bytes([d, p]) + w(dlen) + w(L) + w(d + p)
+    body = b"\x00" + _vput(av) + w(slot) + w(ballot) + bytes([d, p]) + w(dlen) + w(L) + w(d + p)
     for j in range(d + p):
         body += (b"\x01" + w(L) + bytes([(slot + 3 * j) & 255]) * L) if (held >> j) & 1 else b"\x00"
     body += b"\x00"
@@ -427,7 +429,7 @@ def _buffer(rng, frames, odd=True):
 
 def _acceptor(ctx, cfg, G):
     from summerset_b200.engine import Acceptor
-    return Acceptor(ctx, cfg.protocol, G, cfg.n, cfg.me, cfg.d, cfg.T)
+    return Acceptor(ctx, cfg.protocol, G, cfg.n, cfg.me, cfg.d, cfg.T, cfg.av, cfg.wv, cfg.rv)
 
 
 def _install(acc, st):
@@ -549,25 +551,33 @@ def _check_state(acc, cfg, st, store_ptr):
 # GPU 1: frames from the real leader path
 # ---------------------------------------------------------------------------------------------
 LEADER_CASES = [("rspaxos", 5, 0, 0, True), ("crossword", 5, 5, 3, True), ("crossword", 5, 10, 6, True), ("crossword", 5, 5, 3, False),
-                ("crossword", 5, 10, 6, False)]
+                ("crossword", 5, 10, 6, False), ("rspaxos", 3, 0, 0, True), ("rspaxos", 12, 0, 0, True), ("crossword", 3, 6, 2, True),
+                ("crossword", 7, 14, 7, False), ("crossword", 12, 24, 16, True), ("crossword", 12, 24, 16, False)]
 
 
-def _leader_frames(ctx, oracle, rng, protocol, n, T, d, balanced, peer):
+def _leader_frames(ctx, oracle, rng, protocol, n, T, d, balanced, peer, lens=None, policies=None):
+    """Accept frames for `peer` from the real leader path (LeaderEngine.propose_ragged -> frame_accept_pack_ragged), one
+    per group, at random window bases and prepared ballots.  lens: the groups' request lengths (default: every varint
+    edge plus a workload mix); policies: a Crossword policy table to use instead of the balanced / unbalanced ones."""
     from summerset_b200 import workloads as wl
     from summerset_b200.engine import LeaderEngine
     cw = protocol == "crossword"
-    edges = [1, 2, 3, 250, 251, 750, 753, 65535, 65536, 196605, 196608, 4096, 1365, 1366]
-    lens = np.concatenate([edges, wl.cfg4_lengths(150, seed_extra=7)[0]]).astype(np.uint32)
+    if lens is None:
+        edges = [1, 2, 3, 250, 251, 750, 753, 65535, 65536, 196605, 196608, 4096, 1365, 1366]
+        lens = np.concatenate([edges, wl.cfg4_lengths(150, seed_extra=7)[0]]).astype(np.uint32)
+    lens = np.array(lens, dtype=np.uint32)
     rng.shuffle(lens)
     G = len(lens)
-    eng = LeaderEngine(ctx, protocol, G, n, 1, 1, rs_total_shards=T, rs_data_shards=d)
+    eng = LeaderEngine(ctx, protocol, G, n, min(1, n - (n // 2 + 1)), 1, rs_total_shards=T, rs_data_shards=d)
     bal = rng.integers(1, 1 << 40, G).astype(np.uint64)
     eng.set_prepared_ballots(_t(bal))
     base = rng.integers(0, 1 << 40, G).astype(np.uint64)
     eng.window_base.copy_(_t(base))
     d, p, T = eng.d, eng.T - eng.d, eng.T
     if cw:
-        if balanced:
+        if policies is not None:
+            policies = np.array(policies, dtype=np.uint32)
+        elif balanced:
             policies = np.stack([oracle.cw_brr_assignment(n, T, spr) for spr in range(T // n, d + 1, T // n)])
         else:
             full = (1 << T) - 1
@@ -634,7 +644,7 @@ def _adversarial(oracle, rng, cfg, st, nfr):
         dlen = int(rng.choice([1, 5, 40, 251, 700]))
         held = int(rng.integers(1, 1 << cfg.T))
         asg = [int(rng.integers(0, 1 << cfg.T)) for _ in range(cfg.n)] if cfg.cw else None
-        f = _acc(oracle, slot, bal, held, dlen, cfg.d, cfg.T - cfg.d, asg, cfg.T)
+        f = _acc(oracle, slot, bal, held, dlen, cfg.d, cfg.T - cfg.d, asg, cfg.T, cfg.av)
         k = rng.random()
         if k < 0.04:
             f = f[:int(rng.integers(0, len(f)))]
@@ -643,9 +653,9 @@ def _adversarial(oracle, rng, cfg, st, nfr):
         elif k < 0.08:
             f = b"\x00" * 7 + b"\x02" + b"\x01\x00"
         elif k < 0.10:
-            f = _acc(oracle, slot, bal, held, dlen, cfg.d + 1, cfg.T - cfg.d - 1, asg, cfg.T)
+            f = _acc(oracle, slot, bal, held, dlen, cfg.d + 1, cfg.T - cfg.d - 1, asg, cfg.T, cfg.av)
         elif k < 0.20:                    # every varint in its 9-byte form: the shard offsets shift by 8 per shard
-            f = _acc_wide(slot, bal, held, dlen, cfg.d, cfg.T - cfg.d, asg, cfg.T)
+            f = _acc_wide(slot, bal, held, dlen, cfg.d, cfg.T - cfg.d, asg, cfg.T, cfg.av)
         frames.append(f)
         groups.append(g)
         peers.append(int(rng.integers(0, cfg.n)))
@@ -724,19 +734,21 @@ def test_acceptor_capacity_cuts(ctx, oracle, which):
 # GPU 4: closed loop -- leader frames -> one acceptor per peer -> replies -> parse -> ingest -> tick, over windows
 # ---------------------------------------------------------------------------------------------
 @pytest.mark.gpu
-@pytest.mark.parametrize("protocol", ["rspaxos", "crossword"])
-def test_acceptor_closed_loop(ctx, oracle, protocol):
+@pytest.mark.parametrize("protocol,n,T", [pytest.param("rspaxos", 5, 0, id="rspaxos"), pytest.param("crossword", 5, 5, id="crossword")] +
+                         [pytest.param("rspaxos", n, 0, id=f"rspaxos-{n}") for n in (3, 7, 9, 12)] +
+                         [pytest.param("crossword", n, T, id=f"crossword-{n}-{T}") for n, T in ((3, 6), (7, 14), (12, 24))])
+def test_acceptor_closed_loop(ctx, oracle, protocol, n, T):
     from summerset_b200 import workloads as wl
     from summerset_b200.engine import LeaderEngine
-    n, f, G = 5, 1, 300
+    f, G = 1, 300
     cw = protocol == "crossword"
-    rng = np.random.default_rng(21 if cw else 22)
-    eng = LeaderEngine(ctx, protocol, G, n, f, 1, rs_total_shards=5 if cw else 0, rs_data_shards=3 if cw else 0)
+    rng = np.random.default_rng((21 if cw else 22) + 100 * (n != 5) * (n + T))
+    eng = LeaderEngine(ctx, protocol, G, n, f, 1, rs_total_shards=T, rs_data_shards=max(n // 2 + 1, T - 8) if cw else 0)
     bal = rng.integers(1, 1 << 30, G).astype(np.uint64)
     eng.set_prepared_ballots(_t(bal))
     d, p, T = eng.d, eng.T - eng.d, eng.T
     if cw:
-        policies = np.stack([oracle.cw_brr_assignment(n, T, spr) for spr in (1, 2, 3)])
+        policies = np.stack([oracle.cw_brr_assignment(n, T, spr) for spr in range(T // n, d + 1, T // n)])
         eng.set_policies([list(map(int, q)) for q in policies], True)
     else:
         policies = np.array([[1 << r for r in range(n)]], dtype=np.uint32)
