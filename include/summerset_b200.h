@@ -662,8 +662,9 @@ int ss_acceptor_view_get(ss_acceptor *acceptor, ss_acceptor_view *view);
 /* *window_base = the acceptor's device array [G] of window bases; a host may install bases (a snapshot's start_slot)
  * while the window holds no instance. */
 int ss_acceptor_window_get(ss_acceptor *acceptor, uint64_t **window_base);
-/* retires window prefixes: upto (device [G] absolute slots, required -- the acceptor keeps no commit state):
- * k = clamp(upto[g] - window_base[g], 0, 64); the k retired ring positions leave Accepting and window_base[g] += k. */
+/* retires window prefixes: upto (device [G] absolute slots, required -- the host decides what is retired):
+ * k = clamp(upto[g] - window_base[g], 0, 64); the k retired ring positions leave Accepting and Committed and
+ * window_base[g] += k. */
 int ss_acceptor_advance(ss_acceptor *acceptor, const uint64_t *upto);
 /* Verdicts of ss_acceptor_accept, beside the PeerMsg variant index k (another message; 0x80000000 | k for the
  * PeerMessage variants) and SS_FRAME_KIND_MALFORMED */
@@ -708,6 +709,53 @@ int ss_acceptor_accept(ss_acceptor *acceptor, const uint8_t *buf, uint64_t buf_l
                        uint64_t store_capacity, uint64_t *store_off, uint8_t *wal, uint64_t wal_capacity, uint64_t *wal_off,
                        uint32_t *wal_len, uint8_t *replies, uint32_t *reply_len, uint8_t *reply_dst, uint32_t *verdict,
                        uint64_t *totals);
+/* Commit and execute on the acceptor: the commit half of heard_heartbeat (rspaxos/leadership.rs:222-311,
+ * crossword/leadership.rs:260-359) and handle_logged_commit_slot's execution walk (rspaxos/durability.rs:125-186,
+ * crossword/durability.rs:142-206).  Three more per-group arrays, all zero at creation: committed (ring word, bit s & 63
+ * = Status::Committed), commit_bar (absolute: the first slot not yet submitted for execution) and exec_bar (absolute:
+ * installed by the host as its state machine reports results, handle_cmd_result; the heartbeat filter reads it).
+ * ss_acceptor_accept takes an accepted slot back to Accepting from Committed (rspaxos/messages.rs:363) and
+ * ss_acceptor_advance clears committed on the retired positions.  Both walks start at max(commit_bar, window_base), so a
+ * base installed by the host or moved by advance needs no fix-up.  Peer-side bookkeeping of heard_heartbeat stays on the
+ * host: the Heartbeat reply, hear timers, peer_exec_bar and snap_bar.  The `Executed` status (empty batches) is not
+ * tracked. */
+typedef struct ss_acceptor_commit_view {
+    uint64_t n_groups;
+    uint64_t *committed;        /* [G] bit s & 63 = Status::Committed */
+    uint64_t *commit_bar;       /* [G] */
+    uint64_t *exec_bar;         /* [G] */
+} ss_acceptor_commit_view;
+int ss_acceptor_commit_view_get(ss_acceptor *acceptor, ss_acceptor_commit_view *view);
+/* Heartbeat records (device arrays [n]: group, peer, ballot, commit_bar, exec_bar), replayed per group in record order
+ * as if they arrived one at a time.  For each record of group g: if peer != me, bal_max_seen rises to its ballot
+ * (check_leader); the record is skipped if ballot < bal_max_seen or its exec_bar < exec_bar[g]; otherwise slots from
+ * max(commit_bar[g], window_base[g]) up to min(record's commit_bar, window_base[g] + 64) are walked: the walk breaks at
+ * inst_bal < ballot or at a slot that is neither Accepting nor Committed, passes a committed slot, and commits the
+ * others (committed bit set, accepting bit cleared, a WalEntry::CommitSlot to log).  Slots at or beyond window_base + 64
+ * are left for a later heartbeat after ss_acceptor_advance.  Records with group >= n_groups are ignored.
+ * newly (device [G], may be NULL): bit i = instance window_base[g] + i committed by THIS call, in window order as
+ * ss_engine_tick writes it -- ss_wal_commit_pack_dev(newly, window_base, ...) packs the CommitSlot records. */
+int ss_acceptor_heartbeat(ss_acceptor *acceptor, const uint32_t *hb_group, const uint8_t *hb_peer, const uint64_t *hb_ballot,
+                          const uint64_t *hb_commit_bar, const uint64_t *hb_exec_bar, uint64_t n_records, uint64_t *newly);
+/* Execution, once the CommitSlot records of earlier heartbeat calls are durable: for every group, from
+ * max(commit_bar, window_base) while the slot is inside the window and committed, an instance holding fewer than d
+ * shards postpones the walk (RSPaxos majority = d, Crossword num_data_shards); otherwise it executes and commit_bar
+ * moves past it.  Its payload is get_data's input, the first data_len bytes of the concatenated data shards
+ * (rscoding.rs:177-199, 581-683); a data shard not held is regenerated from the first d held shards in index order, as
+ * reconstruct_data does (rscoding.rs:490-537).  The shards are read through shard_addr: the caller's acceptor stores
+ * must still hold them.
+ * Outputs, executed instances ordered by (group, slot): record k = rec_group[k], rec_slot[k] (absolute), rec_off[k],
+ * rec_len[k] (= data_len); the payload at out + rec_off[k] in a region of round_up(data_len, 16) bytes, zero past
+ * data_len (regions placed by exclusive scans; out 16-byte aligned).  totals (device u64[2], may be NULL): records and
+ * bytes the walk asked for.  An instance whose record index reaches rec_capacity or whose region ends past out_capacity
+ * does not execute and its group's walk stops there (SS_DEV_STATUS_EXEC_FULL); the offsets are monotone, so the
+ * records written are a prefix and a host drains by calling again.  A committed instance with data_len == 0 is a null
+ * codeword that get_data and reconstruct_data refuse (rscoding.rs:495-497, 581-583): it does not execute, its group's
+ * walk stops there (SS_DEV_STATUS_EXEC_NULL). */
+#define SS_DEV_STATUS_EXEC_FULL 32u
+#define SS_DEV_STATUS_EXEC_NULL 64u
+int ss_acceptor_execute(ss_acceptor *acceptor, uint8_t *out, uint64_t out_capacity, uint32_t *rec_group, uint64_t *rec_slot,
+                        uint64_t *rec_off, uint32_t *rec_len, uint64_t rec_capacity, uint64_t *totals);
 
 /* ---- tuning / introspection (bench + tests) ------------------------------------------------ */
 /* Tuning knob for experiments; 0 = the defaults.

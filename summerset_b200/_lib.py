@@ -121,6 +121,9 @@ SIGNATURES = {
     "ss_acceptor_window_get": (_i, [_vp, C.POINTER(_vp)]),
     "ss_acceptor_advance": (_i, [_vp, _vp]),
     "ss_acceptor_accept": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _vp, _u64, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "ss_acceptor_commit_view_get": (_i, [_vp, _vp]),
+    "ss_acceptor_heartbeat": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _u64, _vp]),
+    "ss_acceptor_execute": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp]),
     "ss_rs_set_variant": (_i, [_vp, _i]),
     "ss_rs_last_kernel": (C.c_char_p, [_vp]),
     "ss_rs_jit_status": (C.c_char_p, [_vp]),
@@ -175,6 +178,15 @@ class AcceptorView(C.Structure):
                 ("shard_addr", C.c_void_p), ("held", C.c_void_p), ("data_len", C.c_void_p), ("assignment", C.c_void_p),
                 ("source", C.c_void_p)]
 
+
+class AcceptorCommitView(C.Structure):
+    """ss_acceptor_commit_view"""
+    _fields_ = [("n_groups", C.c_uint64), ("committed", C.c_void_p), ("commit_bar", C.c_void_p), ("exec_bar", C.c_void_p)]
+
+
+# ss_acceptor_execute's bits of the device status word
+SS_DEV_STATUS_EXEC_FULL = 32
+SS_DEV_STATUS_EXEC_NULL = 64
 
 # verdicts of ss_acceptor_accept (beside PeerMsg variant indices and SS_FRAME_KIND_MALFORMED)
 SS_ACCEPT_VERDICT_ACCEPTED = 0xFFFFFFF0

@@ -17,12 +17,27 @@
 //
 // Frames sit in a receive buffer at any byte alignment; every 128-bit store is aligned, its 16 source bytes come from
 // the two aligned loads around them (dev::load16).
+//
+// What the follower does next: the commit half of heard_heartbeat (rspaxos/leadership.rs:222-311,
+// crossword/leadership.rs:260-359) and, once the CommitSlot records are durable, handle_logged_commit_slot's execution
+// walk (rspaxos/durability.rs:125-186, crossword/durability.rs:142-206):
+//
+//   heartbeat_keys_kernel    a thread per record: sort keys (the records are then stably sorted by group as above)
+//   heartbeat_walk_kernel    a thread per group segment: check_leader, the ballot / exec_bar filters and the commit walk
+//                            of every record of the group in record order
+//   exec_count_kernel        a thread per group: how many instances the walk executes, and their payload bytes
+//   (engine.cu's scan)       record indices and payload regions
+//   exec_place_kernel        a thread per group: capacities, the records, commit_bar
+//   exec_payload_kernel      a warp per executed instance: get_data's bytes, with reconstruct_data's regeneration of
+//                            missing data shards from the first d held shards (Gauss-Jordan on the device, then packed
+//                            GF(2^8) Horner rows on the byte stream)
 #include <cub/device/device_radix_sort.cuh>
 
 #include <cstring>
 #include <new>
 
 #include "device_common.cuh"
+#include "gf256.hpp"
 #include "ss_internal.hpp"
 #include "window_ring.cuh"
 #include "wire_common.cuh"
@@ -50,6 +65,9 @@ struct ss_acceptor {
     uint64_t *window_base = nullptr, *bal_max_seen = nullptr, *inst_bal = nullptr, *accepting = nullptr, *shard_addr = nullptr;
     uint32_t *held = nullptr, *data_len = nullptr, *assignment = nullptr;
     uint8_t *source = nullptr;
+    uint64_t *committed = nullptr, *commit_bar = nullptr, *exec_bar = nullptr;
+    uint8_t *matrix = nullptr;      // [T*d] the coder's coding matrix (gf256.hpp), row-major
+    uint64_t *ex_cnt = nullptr, *ex_bytes = nullptr, *ex_partials = nullptr, *ex_n = nullptr;   // execute scratch
     // per-call scratch, grow-only
     uint64_t cap_frames = 0;
     ssb::FrameHdr *hdr = nullptr;
@@ -77,7 +95,7 @@ struct AccArgs {
     uint64_t n, G;
     uint32_t d, T, population, me, accept_variant, wal_variant, reply_variant, crossword;
     // state
-    uint64_t *window_base, *bal_max_seen, *inst_bal, *accepting, *shard_addr;
+    uint64_t *window_base, *bal_max_seen, *inst_bal, *accepting, *shard_addr, *committed;
     uint32_t *held, *data_len, *assignment;
     uint8_t *source;
     // scratch
@@ -272,7 +290,8 @@ __global__ void __launch_bounds__(kAccThreads) acceptor_place_kernel(const __gri
             A.verdict[i] = kind;
         }
         if (known) {
-            A.accepting[g] |= seen;                                     // Status::Accepting
+            A.accepting[g] |= seen;                                     // Status::Accepting, also for a committed slot
+            A.committed[g] &= ~seen;                                    // (rspaxos/messages.rs:363)
             A.bal_max_seen[g] = mx;
         }
     }
@@ -341,16 +360,296 @@ __global__ void __launch_bounds__(kAccThreads) acceptor_copy_kernel(const __grid
     }
 }
 
-// retire window prefixes: k = clamp(upto - base, 0, 64) positions leave Accepting, the base moves on
+// retire window prefixes: k = clamp(upto - base, 0, 64) positions leave Accepting and Committed, the base moves on
 __global__ void __launch_bounds__(kAccThreads)
-acceptor_advance_kernel(const uint64_t *__restrict__ upto, uint64_t G, uint64_t *__restrict__ window_base, uint64_t *__restrict__ accepting) {
+acceptor_advance_kernel(const uint64_t *__restrict__ upto, uint64_t G, uint64_t *__restrict__ window_base, uint64_t *__restrict__ accepting,
+                        uint64_t *__restrict__ committed) {
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
     for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; g < G; g += stride) {
         const uint64_t base = window_base[g], u = upto[g];
         const uint64_t k = u <= base ? 0ull : (u - base < 64u ? u - base : 64ull);
         if (k == 0ull) continue;
-        accepting[g] &= ring_keep_after(k, base);
+        const uint64_t keep = ring_keep_after(k, base);
+        accepting[g] &= keep;
+        committed[g] &= keep;
         window_base[g] = base + k;
+    }
+}
+
+// ---- commit (heartbeat) -----------------------------------------------------------------------------------------
+struct HbArgs {
+    const uint32_t *group;
+    const uint8_t *peer;
+    const uint64_t *ballot, *hb_commit_bar, *hb_exec_bar;
+    uint64_t n, G;
+    uint32_t me;
+    const uint64_t *window_base, *inst_bal, *commit_bar, *exec_bar;
+    uint64_t *bal_max_seen, *accepting, *committed, *newly;
+    uint32_t *key_in, *idx_in;
+    const uint32_t *key, *idx;      // sorted
+};
+
+__global__ void __launch_bounds__(kAccThreads) heartbeat_keys_kernel(const __grid_constant__ HbArgs A) {
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; i < A.n; i += stride) {
+        const uint32_t grp = A.group[i];
+        A.key_in[i] = grp < A.G ? grp : static_cast<uint32_t>(A.G);
+        A.idx_in[i] = static_cast<uint32_t>(i);
+    }
+}
+
+// a thread per group segment, records in record order: heard_heartbeat's check_leader, its two filters and its commit
+// walk over [max(commit_bar, window_base), min(hb commit_bar, window_base + 64)).  commit_bar does not move here (only
+// execution moves it), so every record of the call walks from the same start.
+__global__ void __launch_bounds__(kAccThreads) heartbeat_walk_kernel(const __grid_constant__ HbArgs A) {
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
+    for (uint64_t t = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; t < A.n; t += stride) {
+        if (t != 0u && A.key[t] == A.key[t - 1]) continue;
+        const uint32_t g = A.key[t];
+        if (g >= A.G) continue;
+        const uint64_t base = A.window_base[g], cb = A.commit_bar[g], eb = A.exec_bar[g];
+        const uint64_t start = cb > base ? cb : base, wend = base + 64u;
+        const uint64_t *ib = A.inst_bal + static_cast<uint64_t>(g) * 64u;
+        uint64_t bmax = A.bal_max_seen[g], acc = A.accepting[g], com = A.committed[g], nw = 0ull;
+        for (uint64_t k = t; k < A.n && A.key[k] == g; ++k) {
+            const uint32_t i = A.idx[k];
+            const uint64_t bal = A.ballot[i];
+            if (A.peer[i] != A.me && bal > bmax) bmax = bal;           // check_leader
+            if (bal < bmax || A.hb_exec_bar[i] < eb) continue;          // outdated heartbeat; exec_bar behind ours
+            const uint64_t hcb = A.hb_commit_bar[i], stop = hcb < wend ? hcb : wend;
+            for (uint64_t s = start; s < stop; ++s) {
+                const uint64_t bit = 1ull << (s & 63u);
+                if (ib[s & 63u] < bal || !((acc | com) & bit)) break;   // inst.bal < ballot, status < Accepting
+                if (com & bit) continue;
+                com |= bit;                                            // Status::Committed, a CommitSlot record
+                acc &= ~bit;
+                nw |= bit;
+            }
+        }
+        A.bal_max_seen[g] = bmax;
+        A.accepting[g] = acc;
+        A.committed[g] = com;
+        if (A.newly != nullptr) A.newly[g] = ring_to_window(nw, static_cast<uint32_t>(base & 63u));
+    }
+}
+
+// ---- execute -----------------------------------------------------------------------------------------------------
+struct ExecArgs {
+    uint64_t G;
+    uint32_t d, T;
+    const uint64_t *window_base, *committed, *shard_addr;
+    const uint32_t *held, *data_len;
+    const uint8_t *matrix;          // [T*d]
+    uint64_t *commit_bar;
+    uint64_t *cnt, *bytes;          // [G] per group: records, payload bytes; then their exclusive scans
+    uint64_t *n_exec;               // records written (they are a prefix: the offsets are monotone)
+    uint8_t *out;
+    uint64_t out_cap;
+    uint32_t *rec_group;
+    uint64_t *rec_slot, *rec_off;
+    uint32_t *rec_len;
+    uint64_t rec_cap;
+    uint32_t *status;
+};
+
+enum : uint32_t { kExecStop = 0u, kExecRun = 1u, kExecNull = 2u };
+
+// what handle_logged_commit_slot's walk does at slot s of group g: stop (past the window, not committed, or fewer than
+// d shards: postponed), run it (*dlen = its data_len), or stop at a null codeword, which get_data and reconstruct_data
+// both refuse (rscoding.rs:495-497, 581-583)
+__device__ __forceinline__ uint32_t exec_next(const ExecArgs &A, uint64_t g, uint64_t s, uint64_t base, uint64_t com, uint32_t *dlen) {
+    if (s - base >= 64u || !((com >> (s & 63u)) & 1u)) return kExecStop;
+    const uint64_t at = g * 64u + (s & 63u);
+    if (static_cast<uint32_t>(__popc(A.held[at])) < A.d) return kExecStop;
+    *dlen = A.data_len[at];
+    return *dlen == 0u ? kExecNull : kExecRun;
+}
+
+__device__ __forceinline__ uint64_t exec_start(const ExecArgs &A, uint64_t g) {
+    const uint64_t cb = A.commit_bar[g], base = A.window_base[g];
+    return cb > base ? cb : base;
+}
+
+__global__ void __launch_bounds__(kAccThreads) exec_count_kernel(const __grid_constant__ ExecArgs A) {
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
+    for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; g < A.G; g += stride) {
+        const uint64_t base = A.window_base[g], com = A.committed[g];
+        uint64_t n = 0u, b = 0u;
+        uint32_t dl = 0u;
+        for (uint64_t s = exec_start(A, g); exec_next(A, g, s, base, com, &dl) == kExecRun; ++s, ++n) b += round16(dl);
+        A.cnt[g] = n;
+        A.bytes[g] = b;
+    }
+}
+
+__global__ void __launch_bounds__(kAccThreads) exec_place_kernel(const __grid_constant__ ExecArgs A) {
+    bool full = false, null_cw = false;
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
+    for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; g < A.G; g += stride) {
+        const uint64_t base = A.window_base[g], com = A.committed[g], s0 = exec_start(A, g);
+        uint64_t ro = A.cnt[g], bo = A.bytes[g], s = s0;
+        uint32_t dl = 0u, r;
+        while ((r = exec_next(A, g, s, base, com, &dl)) == kExecRun) {
+            const uint64_t sz = round16(dl);
+            if (ro >= A.rec_cap || bo > A.out_cap || sz > A.out_cap - bo) { full = true; break; }
+            A.rec_group[ro] = static_cast<uint32_t>(g);
+            A.rec_slot[ro] = s;
+            A.rec_off[ro] = bo;
+            A.rec_len[ro] = dl;
+            ++ro;
+            bo += sz;
+            ++s;
+        }
+        null_cw |= r == kExecNull;
+        if (s != s0) {
+            A.commit_bar[g] = s;
+            atomicMax(reinterpret_cast<unsigned long long *>(A.n_exec), static_cast<unsigned long long>(ro));
+        }
+    }
+    if (full) atomicOr(A.status, SS_DEV_STATUS_EXEC_FULL);
+    if (null_cw) atomicOr(A.status, SS_DEV_STATUS_EXEC_NULL);
+}
+
+constexpr int kExecWarps = kAccThreads / 32;
+constexpr int kChunk = 4;           // sources per Horner pass: their loads are issued together
+
+struct ExecShared {
+    uint8_t exp[512], log[256];
+    uint8_t a[kExecWarps][32][32];  // Gauss-Jordan: lane r owns row r of M[sources] ...
+    uint8_t inv[kExecWarps][32][32];   // ... and of the identity it turns into the inverse
+    uint8_t piv[kExecWarps][32];    // piv[c]: the row that took column c as its pivot
+};
+
+__device__ __forceinline__ uint32_t gmul(const ExecShared &S, uint32_t a, uint32_t b) {
+    return (a != 0u && b != 0u) ? S.exp[S.log[a] + S.log[b]] : 0u;
+}
+
+// x * 2 in GF(2^8) on 16 packed bytes
+__device__ __forceinline__ uint4 xtime16(uint4 v) {
+    return make_uint4(dev::xtime4(v.x), dev::xtime4(v.y), dev::xtime4(v.z), dev::xtime4(v.w));
+}
+
+// v moved up by k (1..15) byte positions: bytes [16-k, 32-k) of the 32-byte window {0, v}
+__device__ __forceinline__ uint4 shift_up(const uint4 &v, uint32_t k) { return dev::funnel16(make_uint4(0u, 0u, 0u, 0u), v, 16u - k); }
+
+// a warp per executed instance, output-stationary: lane v writes payload bytes [16v, 16v + 16) with one aligned 128-bit
+// store.  Data shard i is payload bytes [i*L, (i+1)*L); a held one is read from its store slot (rank k among the held
+// shards, at shard_addr + k*pitch), a missing one is the GF(2^8) combination of the first d held shards (store ranks
+// 0..d-1) with row i of inverse(M[sources]), reconstruct_data's choice of sources (rscoding.rs:490-537).
+__global__ void __launch_bounds__(kAccThreads) exec_payload_kernel(const __grid_constant__ ExecArgs A) {
+    __shared__ ExecShared S;
+    for (uint32_t i = threadIdx.x; i < 256u; i += kAccThreads) {
+        uint32_t v = 1u;
+        for (uint32_t k = 0; k < i; ++k) v = (v << 1) ^ ((v & 0x80u) ? 0x11Du : 0u);   // 2^i, i < 255
+        if (i < 255u) { S.exp[i] = static_cast<uint8_t>(v); S.exp[i + 255u] = static_cast<uint8_t>(v); S.log[v] = static_cast<uint8_t>(i); }
+    }
+    if (threadIdx.x < 2u) S.exp[510u + threadIdx.x] = S.exp[threadIdx.x];
+    __syncthreads();
+    const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+    uint8_t (*ra)[32] = S.a[w];
+    uint8_t (*ri)[32] = S.inv[w];
+    uint8_t *piv = S.piv[w];
+    const uint32_t d = A.d;
+    const uint32_t dmask = d == 32u ? 0xffffffffu : (1u << d) - 1u;
+    const uint64_t n = *A.n_exec;
+    const uint64_t nwarps = static_cast<uint64_t>(gridDim.x) * kExecWarps;
+    for (uint64_t r = static_cast<uint64_t>(blockIdx.x) * kExecWarps + w; r < n; r += nwarps) {
+        const uint64_t g = A.rec_group[r], s = A.rec_slot[r], at = g * 64u + (s & 63u);
+        const uint32_t dlen = A.rec_len[r], held = A.held[at];
+        const uint32_t L = (dlen + d - 1u) / d;
+        const uint64_t pitch = SS_CW_SLOT_PITCH(L);
+        const uint8_t *src = reinterpret_cast<const uint8_t *>(A.shard_addr[at]);
+        uint8_t *dst = A.out + A.rec_off[r];
+        const uint32_t missing = ~held & dmask;
+        if (missing != 0u) {
+            // Gauss-Jordan on M[sources] (d x d, invertible for any d distinct rows of the coder's matrix): lane k owns
+            // row k, whose source is the k-th held shard; pivots are taken in column order, rows are never swapped
+            if (lane < d) {
+                uint32_t h = held;
+                for (uint32_t q = 0; q < lane; ++q) h &= h - 1u;
+                const uint32_t row = static_cast<uint32_t>(__ffs(h)) - 1u;
+                for (uint32_t c = 0; c < d; ++c) {
+                    ra[lane][c] = A.matrix[row * d + c];
+                    ri[lane][c] = c == lane ? 1u : 0u;
+                }
+            }
+            __syncwarp();
+            uint32_t used = 0u;
+            for (uint32_t c = 0; c < d; ++c) {
+                const uint32_t f = lane < d ? ra[lane][c] : 0u;
+                const uint32_t cand = __ballot_sync(0xffffffffu, f != 0u && !((used >> lane) & 1u));
+                if (cand == 0u) break;
+                const uint32_t p = static_cast<uint32_t>(__ffs(cand)) - 1u;
+                used |= 1u << p;
+                if (lane == p) {
+                    const uint32_t sc = S.exp[255u - S.log[f]];
+                    piv[c] = static_cast<uint8_t>(p);
+                    for (uint32_t k = c; k < d; ++k) ra[p][k] = static_cast<uint8_t>(gmul(S, ra[p][k], sc));
+                    for (uint32_t k = 0; k < d; ++k) ri[p][k] = static_cast<uint8_t>(gmul(S, ri[p][k], sc));
+                }
+                __syncwarp();
+                if (lane < d && lane != p && f != 0u) {
+                    for (uint32_t k = c; k < d; ++k) ra[lane][k] ^= static_cast<uint8_t>(gmul(S, f, ra[p][k]));
+                    for (uint32_t k = 0; k < d; ++k) ri[lane][k] ^= static_cast<uint8_t>(gmul(S, f, ri[p][k]));
+                }
+                __syncwarp();
+            }
+        }
+        // bytes [o, o + c) of data shard i (c <= 16) as the low c bytes of a uint4, the rest zero
+        auto shard16 = [&](uint32_t i, uint32_t o, int c) -> uint4 {
+            if ((held >> i) & 1u) return dev::load16(src + __popc(held & ((1u << i) - 1u)) * pitch + o, c);
+            const uint8_t *coef = ri[piv[i]];
+            uint4 acc = make_uint4(0u, 0u, 0u, 0u);
+            for (uint32_t q0 = 0; q0 < d; q0 += kChunk) {
+                uint32_t cq[kChunk], top = 0u;
+                dev::Raw16 raw[kChunk];
+#pragma unroll
+                for (int q = 0; q < kChunk; ++q) {
+                    const bool in = q0 + q < d;
+                    cq[q] = in ? coef[q0 + q] : 0u;
+                    top |= cq[q];
+                    raw[q] = dev::raw16_issue(src + (q0 + q) * pitch + o, in && cq[q] != 0u ? c : 0);
+                }
+                uint4 x[kChunk];
+#pragma unroll
+                for (int q = 0; q < kChunk; ++q) x[q] = dev::raw16_finish(raw[q], c);
+                // Horner from the top coefficient bit down: part = part * 2 ^ (XOR of the x_q whose c_q has bit k)
+                uint4 part = make_uint4(0u, 0u, 0u, 0u);
+                for (int k = top == 0u ? -1 : 31 - __clz(top); k >= 0; --k) {
+                    part = xtime16(part);
+#pragma unroll
+                    for (int q = 0; q < kChunk; ++q) {
+                        const uint32_t m = 0u - ((cq[q] >> k) & 1u);
+                        part.x ^= x[q].x & m; part.y ^= x[q].y & m; part.z ^= x[q].z & m; part.w ^= x[q].w & m;
+                    }
+                }
+                acc.x ^= part.x; acc.y ^= part.y; acc.z ^= part.z; acc.w ^= part.w;
+            }
+            return acc;
+        };
+        const uint32_t ncol = (dlen + 15u) >> 4;
+        for (uint32_t v = lane; v < ncol; v += 32u) {
+            uint32_t pos = v * 16u;
+            const uint32_t end = dlen - pos < 16u ? dlen : pos + 16u;
+            const uint32_t i = pos / L, o = pos - i * L;
+            uint4 out;
+            if (o + 16u <= L) {
+                out = shard16(i, o, static_cast<int>(end - pos));           // the column lies in one shard
+            } else {                                                       // it spans shards (always for L < 16)
+                out = make_uint4(0u, 0u, 0u, 0u);
+                for (uint32_t filled = 0u; pos < end;) {
+                    const uint32_t j = pos / L, oj = pos - j * L;
+                    const uint32_t c = L - oj < end - pos ? L - oj : end - pos;
+                    uint4 piece = shard16(j, oj, static_cast<int>(c));
+                    if (filled != 0u) piece = shift_up(piece, filled);
+                    out.x |= piece.x; out.y |= piece.y; out.z |= piece.z; out.w |= piece.w;
+                    filled += c;
+                    pos += c;
+                }
+            }
+            dev::stg128_cs(dst + static_cast<uint64_t>(v) * 16u, out);
+        }
+        __syncwarp();                   // the next instance's Gauss-Jordan overwrites the rows this one read
     }
 }
 
@@ -413,7 +712,8 @@ int ss_acceptor_destroy(ss_acceptor *a) {
         cudaStreamSynchronize(a->ctx->stream);
     }
     void *bufs[] = {a->window_base, a->bal_max_seen, a->inst_bal, a->accepting, a->shard_addr, a->held, a->data_len, a->assignment,
-                    a->source, a->hdr, a->keys, a->idx, a->partials, a->sort_tmp, a->totals};
+                    a->source, a->committed, a->commit_bar, a->exec_bar, a->matrix, a->ex_cnt, a->ex_bytes, a->ex_partials,
+                    a->ex_n, a->hdr, a->keys, a->idx, a->partials, a->sort_tmp, a->totals};
     for (void *b : bufs)
         if (b) cudaFree(b);
     if (a->ctx) ctx_release(a->ctx);
@@ -450,12 +750,85 @@ int ss_acceptor_create(ss_ctx *ctx, const ss_acceptor_config *cfg, uint64_t G, s
         (rc = acc_alloc(ctx, &a->inst_bal, G * 64)) || (rc = acc_alloc(ctx, &a->accepting, G)) ||
         (rc = acc_alloc(ctx, &a->shard_addr, G * 64)) || (rc = acc_alloc(ctx, &a->held, G * 64)) ||
         (rc = acc_alloc(ctx, &a->data_len, G * 64)) || (rc = acc_alloc(ctx, &a->source, G * 64)) || (rc = acc_alloc(ctx, &a->totals, 2)) ||
-        (cfg->protocol == SS_PROTO_CROSSWORD && (rc = acc_alloc(ctx, &a->assignment, G * 64)))) {
+        (cfg->protocol == SS_PROTO_CROSSWORD && (rc = acc_alloc(ctx, &a->assignment, G * 64))) ||
+        (rc = acc_alloc(ctx, &a->committed, G)) || (rc = acc_alloc(ctx, &a->commit_bar, G)) || (rc = acc_alloc(ctx, &a->exec_bar, G)) ||
+        (rc = acc_alloc(ctx, &a->ex_cnt, G, false)) || (rc = acc_alloc(ctx, &a->ex_bytes, G, false)) ||
+        (rc = acc_alloc(ctx, &a->ex_partials, scan_tiles(G), false)) || (rc = acc_alloc(ctx, &a->ex_n, 1, false)) ||
+        (rc = acc_alloc(ctx, &a->matrix, size_t(cfg->total_shards) * cfg->data_shards, false))) {
         ss_acceptor_destroy(a);
         return rc;
     }
+    // the coder's matrix, whose rows ss_acceptor_execute inverts on the device; a pageable source is staged before the
+    // call returns
+    const gf::Matrix m = gf::coding_matrix(static_cast<int>(cfg->data_shards), static_cast<int>(cfg->total_shards - cfg->data_shards));
+    if (cudaMemcpyAsync(a->matrix, m.v.data(), m.v.size(), cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) {
+        ss_acceptor_destroy(a);
+        return set_error(SS_ERR_CUDA, "coding matrix upload failed");
+    }
     *out = a;
     return SS_OK;
+}
+
+int ss_acceptor_commit_view_get(ss_acceptor *a, ss_acceptor_commit_view *v) {
+    if (a == nullptr || v == nullptr) return set_error(SS_ERR_INVALID_ARG, "null argument");
+    memset(v, 0, sizeof(*v));
+    v->n_groups = a->G;
+    v->committed = a->committed; v->commit_bar = a->commit_bar; v->exec_bar = a->exec_bar;
+    return SS_OK;
+}
+
+int ss_acceptor_heartbeat(ss_acceptor *a, const uint32_t *hb_group, const uint8_t *hb_peer, const uint64_t *hb_ballot,
+                          const uint64_t *hb_commit_bar, const uint64_t *hb_exec_bar, uint64_t n, uint64_t *newly) {
+    if (a == nullptr) return set_error(SS_ERR_INVALID_ARG, "null acceptor");
+    ss_ctx *ctx = a->ctx;
+    SS_TRY(ctx_bind(ctx));
+    if (newly != nullptr) SS_CUDA(cudaMemsetAsync(newly, 0, a->G * 8, ctx->stream));
+    if (n == 0) return SS_OK;
+    if (!hb_group || !hb_peer || !hb_ballot || !hb_commit_bar || !hb_exec_bar) return set_error(SS_ERR_INVALID_ARG, "null buffer");
+    if (n > 0x7fffffffull) return set_error(SS_ERR_INVALID_ARG, "at most 2^31 - 1 records per call");
+    SS_TRY(ensure_scratch(a, n));
+    HbArgs H{};
+    H.group = hb_group; H.peer = hb_peer; H.ballot = hb_ballot; H.hb_commit_bar = hb_commit_bar; H.hb_exec_bar = hb_exec_bar;
+    H.n = n; H.G = a->G; H.me = a->cfg.me;
+    H.window_base = a->window_base; H.inst_bal = a->inst_bal; H.commit_bar = a->commit_bar; H.exec_bar = a->exec_bar;
+    H.bal_max_seen = a->bal_max_seen; H.accepting = a->accepting; H.committed = a->committed; H.newly = newly;
+    H.key_in = a->keys; H.idx_in = a->idx; H.key = a->keys + n; H.idx = a->idx + n;
+    const uint32_t grid = acc_grid(ctx, n, kAccThreads);
+    heartbeat_keys_kernel<<<grid, kAccThreads, 0, ctx->stream>>>(H);
+    SS_TRY(launched(ctx));
+    size_t bytes = a->sort_tmp_bytes;
+    SS_CUDA(cub::DeviceRadixSort::SortPairs(a->sort_tmp, bytes, a->keys, a->keys + n, a->idx, a->idx + n, static_cast<int>(n), 0,
+                                            key_bits(a->G), ctx->stream));
+    SS_TRY(launched(ctx));
+    heartbeat_walk_kernel<<<grid, kAccThreads, 0, ctx->stream>>>(H);
+    return launched(ctx);
+}
+
+int ss_acceptor_execute(ss_acceptor *a, uint8_t *out, uint64_t out_capacity, uint32_t *rec_group, uint64_t *rec_slot,
+                        uint64_t *rec_off, uint32_t *rec_len, uint64_t rec_capacity, uint64_t *totals) {
+    if (a == nullptr) return set_error(SS_ERR_INVALID_ARG, "null acceptor");
+    if (!out || !rec_group || !rec_slot || !rec_off || !rec_len) return set_error(SS_ERR_INVALID_ARG, "null buffer");
+    if (reinterpret_cast<uintptr_t>(out) & 15u) return set_error(SS_ERR_INVALID_ARG, "out must be 16-byte aligned");
+    ss_ctx *ctx = a->ctx;
+    SS_TRY(ctx_bind(ctx));
+    ExecArgs E{};
+    E.G = a->G; E.d = a->cfg.data_shards; E.T = a->cfg.total_shards;
+    E.window_base = a->window_base; E.committed = a->committed; E.shard_addr = a->shard_addr; E.held = a->held; E.data_len = a->data_len;
+    E.matrix = a->matrix; E.commit_bar = a->commit_bar; E.cnt = a->ex_cnt; E.bytes = a->ex_bytes; E.n_exec = a->ex_n;
+    E.out = out; E.out_cap = out_capacity; E.rec_group = rec_group; E.rec_slot = rec_slot; E.rec_off = rec_off; E.rec_len = rec_len;
+    E.rec_cap = rec_capacity; E.status = ctx->dev_status;
+    uint64_t *tot = totals != nullptr ? totals : a->totals;
+    const uint32_t grid = acc_grid(ctx, a->G, kAccThreads);
+    SS_CUDA(cudaMemsetAsync(a->ex_n, 0, 8, ctx->stream));
+    exec_count_kernel<<<grid, kAccThreads, 0, ctx->stream>>>(E);
+    SS_TRY(launched(ctx));
+    SS_TRY(launch_exclusive_scan_u64(ctx, a->ex_cnt, a->G, a->ex_partials, tot));
+    SS_TRY(launch_exclusive_scan_u64(ctx, a->ex_bytes, a->G, a->ex_partials, tot + 1));
+    exec_place_kernel<<<grid, kAccThreads, 0, ctx->stream>>>(E);
+    SS_TRY(launched(ctx));
+    // a warp per instance the window can hold, up to the grid cap; warps past the executed count return at once
+    exec_payload_kernel<<<acc_grid(ctx, a->G * 64u, kExecWarps), kAccThreads, 0, ctx->stream>>>(E);
+    return launched(ctx);
 }
 
 int ss_acceptor_view_get(ss_acceptor *a, ss_acceptor_view *v) {
@@ -478,7 +851,8 @@ int ss_acceptor_advance(ss_acceptor *a, const uint64_t *upto) {
     if (a == nullptr || upto == nullptr) return set_error(SS_ERR_INVALID_ARG, "null acceptor or upto");
     ss_ctx *ctx = a->ctx;
     SS_TRY(ctx_bind(ctx));
-    acceptor_advance_kernel<<<acc_grid(ctx, a->G, kAccThreads), kAccThreads, 0, ctx->stream>>>(upto, a->G, a->window_base, a->accepting);
+    acceptor_advance_kernel<<<acc_grid(ctx, a->G, kAccThreads), kAccThreads, 0, ctx->stream>>>(upto, a->G, a->window_base, a->accepting,
+                                                                                               a->committed);
     return launched(ctx);
 }
 
@@ -509,6 +883,7 @@ int ss_acceptor_accept(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, con
     A.crossword = a->cfg.protocol == SS_PROTO_CROSSWORD ? 1u : 0u;
     A.window_base = a->window_base; A.bal_max_seen = a->bal_max_seen; A.inst_bal = a->inst_bal; A.accepting = a->accepting;
     A.shard_addr = a->shard_addr; A.held = a->held; A.data_len = a->data_len; A.assignment = a->assignment; A.source = a->source;
+    A.committed = a->committed;
     A.hdr = a->hdr; A.key_in = a->keys; A.idx_in = a->idx; A.key = a->keys + n; A.idx = a->idx + n;
     A.store = store; A.store_cap = store_capacity; A.store_off = store_off;
     A.wal = wal; A.wal_cap = wal_capacity; A.wal_off = wal_off; A.wal_len = wal_len;

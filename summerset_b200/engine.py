@@ -17,6 +17,9 @@ torch tensors (zero-copy views) so tests can read results and install state; it 
                                             (rspaxos/messages.rs:329-392, crossword/messages.rs:403-470): store, AcceptData
                                             records and AcceptReply cells
         advance(upto)                       retire window prefixes
+        heartbeat(group, peer, ballot, commit_bar, exec_bar)   heard_heartbeat's commit walk (rspaxos/leadership.rs:222-311)
+        execute(out, rec_capacity)          handle_logged_commit_slot's execution walk (rspaxos/durability.rs:125-186):
+                                            request batches decoded from the held shards
     RaftEngine(ctx, G, population[, fault_tolerance, craft])
         append(n_new) / on_append_replies(records) / tick()      raft/messages.rs:243-309, craft/messages.rs:300-308
 """
@@ -234,6 +237,11 @@ class Acceptor:
         self.data_len = t(v.data_len, (G * 64,), "<i4", torch.int32)
         self.assignment = t(v.assignment, (G * 64,), "<i4", torch.int32)
         self.source = t(v.source, (G * 64,), "|u1", torch.uint8)
+        cv = self.commit_view = _lib.AcceptorCommitView()
+        check(self.lib.ss_acceptor_commit_view_get(self.h, C.byref(cv)))
+        self.committed = t(cv.committed, (G,), "<i8", torch.int64)
+        self.commit_bar = t(cv.commit_bar, (G,), "<i8", torch.int64)
+        self.exec_bar = t(cv.exec_bar, (G,), "<i8", torch.int64)
 
     def accept(self, buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor, frame_peer: torch.Tensor,
                store: torch.Tensor, wal: torch.Tensor, store_capacity: Optional[int] = None, wal_capacity: Optional[int] = None) -> dict:
@@ -260,6 +268,36 @@ class Acceptor:
         """Retires window prefixes up to the absolute slots upto (int64 [G])."""
         assert upto.is_cuda and upto.dtype == torch.int64 and upto.numel() == self.G
         check(self.lib.ss_acceptor_advance(self.h, upto.data_ptr()))
+
+    def heartbeat(self, group: torch.Tensor, peer: torch.Tensor, ballot: torch.Tensor, commit_bar: torch.Tensor,
+                  exec_bar: torch.Tensor) -> torch.Tensor:
+        """Heartbeat records group int32 [n], peer uint8 [n], ballot / commit_bar / exec_bar int64 [n] (heard_heartbeat's
+        commit half, per group in record order).  Returns newly (int64 [G], window order): the instances this call
+        committed, which ss_wal_commit_pack_dev packs as CommitSlot records with window_base."""
+        assert group.dtype == torch.int32 and peer.dtype == torch.uint8
+        assert ballot.dtype == commit_bar.dtype == exec_bar.dtype == torch.int64
+        n = group.numel()
+        assert peer.numel() == ballot.numel() == commit_bar.numel() == exec_bar.numel() == n
+        newly = torch.empty(self.G, dtype=torch.int64, device=self.dev)
+        check(self.lib.ss_acceptor_heartbeat(self.h, group.data_ptr(), peer.data_ptr(), ballot.data_ptr(), commit_bar.data_ptr(),
+                                             exec_bar.data_ptr(), n, newly.data_ptr()))
+        return newly
+
+    def execute(self, out: torch.Tensor, rec_capacity: int, out_capacity: Optional[int] = None) -> dict:
+        """Executes the committed instances handle_logged_commit_slot would: payloads into out (uint8, 16-byte aligned,
+        one round_up(data_len, 16) region each).  Returns device tensors rec_group (int32), rec_slot, rec_off (int64),
+        rec_len (int32), each [rec_capacity], and totals (int64 [2]: records and bytes asked for)."""
+        assert out.dtype == torch.uint8 and out.is_contiguous()
+        dev = out.device
+        res = dict(rec_group=torch.empty(rec_capacity, dtype=torch.int32, device=dev),
+                   rec_slot=torch.empty(rec_capacity, dtype=torch.int64, device=dev),
+                   rec_off=torch.empty(rec_capacity, dtype=torch.int64, device=dev),
+                   rec_len=torch.empty(rec_capacity, dtype=torch.int32, device=dev),
+                   totals=torch.empty(2, dtype=torch.int64, device=dev))
+        p = lambda x: x.data_ptr()
+        check(self.lib.ss_acceptor_execute(self.h, p(out), out.numel() if out_capacity is None else out_capacity, p(res["rec_group"]),
+                                           p(res["rec_slot"]), p(res["rec_off"]), p(res["rec_len"]), rec_capacity, p(res["totals"])))
+        return res
 
     def close(self) -> None:
         if getattr(self, "h", None) is not None and self.h:

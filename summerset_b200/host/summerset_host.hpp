@@ -312,9 +312,24 @@ class Acceptor {
     }
     // start_slot moves to upto[g] (device [G]), at most 64 slots at a time
     void advance_start_slot(const uint64_t *upto) { check(ss_acceptor_advance(acc_, upto)); }
+    // heard_heartbeat's commit walk; newly[g] (may be NULL) = the instances to log as CommitSlot (ss_wal_commit_pack_dev)
+    void heard_heartbeat(const uint32_t *group, const uint8_t *peer, const uint64_t *ballot, const uint64_t *commit_bar,
+                         const uint64_t *exec_bar, uint64_t n_records, uint64_t *newly) {
+        check(ss_acceptor_heartbeat(acc_, group, peer, ballot, commit_bar, exec_bar, n_records, newly));
+    }
+    // once those CommitSlot records are durable: handle_logged_commit_slot's walk, request batches into out
+    void execute(uint8_t *out, uint64_t out_capacity, uint32_t *rec_group, uint64_t *rec_slot, uint64_t *rec_off, uint32_t *rec_len,
+                 uint64_t rec_capacity, uint64_t *totals) {
+        check(ss_acceptor_execute(acc_, out, out_capacity, rec_group, rec_slot, rec_off, rec_len, rec_capacity, totals));
+    }
     ss_acceptor_view view() const {
         ss_acceptor_view v;
         check(ss_acceptor_view_get(acc_, &v));
+        return v;
+    }
+    ss_acceptor_commit_view commit_view() const {
+        ss_acceptor_commit_view v;
+        check(ss_acceptor_commit_view_get(acc_, &v));
         return v;
     }
     ss_acceptor *handle() const { return acc_; }
