@@ -756,6 +756,77 @@ int ss_acceptor_heartbeat(ss_acceptor *acceptor, const uint32_t *hb_group, const
 #define SS_DEV_STATUS_EXEC_NULL 64u
 int ss_acceptor_execute(ss_acceptor *acceptor, uint8_t *out, uint64_t out_capacity, uint32_t *rec_group, uint64_t *rec_slot,
                         uint64_t *rec_off, uint32_t *rec_len, uint64_t rec_capacity, uint64_t *totals);
+/* Reconstruct reads on the acceptor: handle_msg_reconstruct (rspaxos/messages.rs:468-516, crossword/messages.rs:577-632)
+ * serves Reconstruct frames from the held shards, handle_msg_reconstruct_reply (rspaxos/messages.rs:519-594,
+ * crossword/messages.rs:635-722) absorbs ReconstructReply shards into the store; ss_acceptor_execute then runs the
+ * instances that now hold d shards.  Neither call writes a WAL record, as in the reference.  Frames are taken as by
+ * ss_acceptor_accept: buf at any byte alignment, frame i at frame_off[i], of group frame_group[i] (>= n_groups:
+ * malformed), from replica frame_peer[i] (the reply goes back to it).  The variant indices are arguments: Reconstruct is
+ * PeerMsg 4 and ReconstructReply 5 in both protocols (rspaxos/mod.rs:249-310, crossword/mod.rs:324-398).  Verdicts:
+ * SS_ACCEPT_VERDICT_ACCEPTED (handled), another message's variant index (0x80000000 | k for the PeerMessage variants),
+ * SS_FRAME_KIND_MALFORMED (not decodable as the requested message), and the ones below.
+ * Stated differences from the reference:
+ *   1. absorb ignores entries beyond the 64-slot window (the reference indexes past its vector; its debug_assert says
+ *      this does not happen);
+ *   2. absorb ignores entries for instances that are neither Accepting nor Committed, and for null instances
+ *      (data_len == 0): the reference debug_asserts status >= Committed, and absorb_other would adopt the entry's
+ *      lengths while keeping zero-length shards, a codeword it cannot decode;
+ *   3. an entry that fails absorb_other's checks (data_len / shard_len) is rejected alone; in the reference the error
+ *      aborts the rest of that message, in HashMap iteration order, which is not deterministic;
+ *   4. a present shard of the wrong length makes the frame malformed, as in ss_acceptor_accept; the reference would
+ *      absorb it;
+ *   5. served codewords carry the held shards and data_len, always with data_copy None; a reference replica that has
+ *      executed an instance also sends the data shards reconstruct_data regenerated and, in RSPaxos, data_copy.
+ *      Receivers ignore data_copy, and gossip only asks a peer for shards of its own assignment row, which it holds. */
+#define SS_RECON_VERDICT_NULL_CODEWORD 0xfffffff6u    /* Crossword serve: a listed instance is a null codeword */
+#define SS_RECON_VERDICT_SHARD_RANGE 0xfffffff7u      /* Crossword serve: flip(exclusion) selects a shard index >= T */
+#define SS_RECON_VERDICT_OUT_FULL 0xfffffff8u         /* serve: the reply's region ends past out_capacity */
+/* Serve: frame i is PeerMessage::Msg{Reconstruct{slots: Vec<usize>}} (RSPaxos) or {slots_excl: Vec<(usize, Bitmap)>}
+ * (Crossword; a Bitmap is size, block count and u64 blocks as ssor_bitmap_encode writes it, read as Bitmap::decode
+ * does: any number of blocks, padded with zeros or cut to the size).  The listed slots are walked in order: a slot
+ * below window_base, at or beyond window_base + 64, or of an instance neither Accepting nor Committed is skipped.  The
+ * entry is the held set (RSPaxos, skipped when empty) or held & flip(exclusion) (Crossword, skipped when empty), where
+ * subset_copy walks the bits [0, size mod 256): its iterator stops at Bitmap::size(), a u8 (bitmap.rs:103-105,
+ * 258-270).  Crossword subset_copy fails, and the reference sends nothing for the whole message, when a listed instance
+ * is a null codeword (data_len == 0) or flip selects an index >= T (a bit of [T, size mod 256) left clear): the frame
+ * gets SS_RECON_VERDICT_NULL_CODEWORD / _SHARD_RANGE and no reply.  A slot listed twice
+ * is one entry, with the value of its last occurrence (Crossword: the last with a non-empty subset).
+ * The reply is PeerMessage::Msg{ReconstructReply{slots_data}}, framed with the 8-byte big-endian length: the map length,
+ * then per entry slot, inst.bal and the RSCodeword (d, p, data_len, shard_len, T shard Options, data_copy None) whose
+ * shards are read through shard_addr.  Map order is unspecified in the reference; entries here follow the order of
+ * their defining occurrences.  A frame whose map is empty gets reply_len 0 (the reference sends nothing).
+ * Outputs: reply i at out + reply_off[i], reply_len[i] bytes; regions of round_up(reply_len, 16) bytes packed in frame
+ * order by an exclusive scan (out 16-byte aligned; bytes past reply_len are not written); reply_off UINT64_MAX for
+ * frames without a reply.  A reply whose region ends past out_capacity is not written: SS_RECON_VERDICT_OUT_FULL and
+ * SS_DEV_STATUS_FRAME_OVERFLOW; the offsets are monotone, so the written replies are a prefix.  *total (device u64, may
+ * be NULL) = the bytes the batch asked for.  Acceptor state is not changed.
+ * Cost: the walk and the copy take a warp per frame; the copy writes the entries of a frame one after another. */
+int ss_acceptor_reconstruct_serve(ss_acceptor *acceptor, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off,
+                                  const uint32_t *frame_group, const uint8_t *frame_peer, uint64_t n_frames,
+                                  uint32_t reconstruct_variant, uint32_t reply_variant, uint8_t *out, uint64_t out_capacity,
+                                  uint64_t *reply_off, uint64_t *reply_len, uint32_t *verdict, uint64_t *total);
+/* Absorb: frame i is PeerMessage::Msg{ReconstructReply{slots_data: HashMap<usize, (Ballot, RSCodeword)>}}.  Every
+ * codeword must carry the acceptor's d and p, shard_len = ceil(data_len / d) and exactly T shard Options, each present
+ * shard shard_len bytes; data_copy is None or Some followed by exactly data_len bytes (a reference RSPaxos replica
+ * that has executed the instance sends its cached batch, rscoding.rs:593-602).  A frame that does not decode so is
+ * malformed and absorbs nothing.  A key repeated inside one frame counts once, with its last value (a HashMap decode
+ * keeps the last insert).  Entries are taken in frame order, then wire order; an entry (slot, ballot, codeword) of
+ * group g is ignored when the slot is outside [window_base, window_base + 64), the instance is neither Accepting nor
+ * Committed, slot < exec_bar[g] (Executed), ballot < inst_bal, the instance is null, or data_len differs from the
+ * instance's (absorb_other); otherwise it adds the shards the instance does not hold yet, so of two entries carrying
+ * one shard index the first wins.  Every instance whose held mask grows gets a new region of
+ * popcount(new held) * SS_CW_SLOT_PITCH(L) bytes in `store`, placed by an exclusive scan in (group, slot) order: the old
+ * shards (copied from the old shard_addr) and the new ones in index order, in the padded layout ss_acceptor_accept
+ * writes; held and shard_addr then name it.  An instance whose region would end past store_capacity is left unchanged
+ * and its frames get SS_ACCEPT_VERDICT_STORE_FULL (SS_DEV_STATUS_STORE_FULL); the placed instances are a prefix, and
+ * submitting the same frames again absorbs what was left.  absorbed[i] = the entries of frame i that added shards to a
+ * placed instance; *total (device u64, may be NULL) = the store bytes the batch asked for.  store 16-byte aligned, not
+ * overlapping the shards the instances hold.
+ * Cost: a group's frames are walked by one warp (once to plan, twice to copy), so a batch costs its largest per-group
+ * run of entries; the copies take the whole warp. */
+int ss_acceptor_absorb(ss_acceptor *acceptor, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off,
+                       const uint32_t *frame_group, const uint8_t *frame_peer, uint64_t n_frames, uint32_t reply_variant,
+                       uint8_t *store, uint64_t store_capacity, uint32_t *absorbed, uint32_t *verdict, uint64_t *total);
 
 /* ---- tuning / introspection (bench + tests) ------------------------------------------------ */
 /* Tuning knob for experiments; 0 = the defaults.

@@ -124,6 +124,8 @@ SIGNATURES = {
     "ss_acceptor_commit_view_get": (_i, [_vp, _vp]),
     "ss_acceptor_heartbeat": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _u64, _vp]),
     "ss_acceptor_execute": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp]),
+    "ss_acceptor_reconstruct_serve": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _u32, _vp, _u64, _vp, _vp, _vp, _vp]),
+    "ss_acceptor_absorb": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _vp, _u64, _vp, _vp, _vp]),
     "ss_rs_set_variant": (_i, [_vp, _i]),
     "ss_rs_last_kernel": (C.c_char_p, [_vp]),
     "ss_rs_jit_status": (C.c_char_p, [_vp]),
@@ -196,6 +198,10 @@ SS_ACCEPT_VERDICT_BEYOND_WINDOW = 0xFFFFFFF3
 SS_ACCEPT_VERDICT_STORE_FULL = 0xFFFFFFF4
 SS_ACCEPT_VERDICT_WAL_FULL = 0xFFFFFFF5
 SS_FRAME_KIND_MALFORMED = 0xFFFFFFFF
+# verdicts of ss_acceptor_reconstruct_serve beside those above
+SS_RECON_VERDICT_NULL_CODEWORD = 0xFFFFFFF6
+SS_RECON_VERDICT_SHARD_RANGE = 0xFFFFFFF7
+SS_RECON_VERDICT_OUT_FULL = 0xFFFFFFF8
 
 
 class SummersetError(RuntimeError):

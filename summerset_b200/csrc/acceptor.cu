@@ -31,6 +31,22 @@
 //   exec_payload_kernel      a warp per executed instance: get_data's bytes, with reconstruct_data's regeneration of
 //                            missing data shards from the first d held shards (Gauss-Jordan on the device, then packed
 //                            GF(2^8) Horner rows on the byte stream)
+//
+// Reconstruct reads, for the instances the follower cannot execute from its own shards: handle_msg_reconstruct
+// (rspaxos/messages.rs:468-516, crossword/messages.rs:577-632) and handle_msg_reconstruct_reply
+// (rspaxos/messages.rs:519-594, crossword/messages.rs:635-722):
+//
+//   serve_count_kernel       a warp per Reconstruct frame: filters, refusals, one entry per slot, reply bytes
+//   (engine.cu's scan)       reply regions
+//   serve_copy_kernel        a warp per frame: capacity, the ReconstructReply with entries in the order of their defining
+//                            occurrences, shards from the store slots
+//   absorb_decode_kernel     a thread per ReconstructReply frame: validates, notes a slot repeated in the window
+//   (CUB radix sort)         frames by group, as above
+//   absorb_plan_kernel       a warp per group segment: the entries in frame, then wire order; bytes of the growing regions
+//   (engine.cu's scan)       group region offsets
+//   absorb_copy_kernel       a warp per group segment: capacity, old and new shards into the new regions, held /
+//                            shard_addr, per-frame counts and verdicts
+// Stated differences from the reference: include/summerset_b200.h at ss_acceptor_reconstruct_serve.
 #include <cub/device/device_radix_sort.cuh>
 
 #include <cstring>
@@ -44,7 +60,7 @@
 
 namespace ssb {
 
-// one decoded Accept frame
+// one decoded Accept frame (ss_acceptor_accept)
 struct FrameHdr {
     uint64_t slot, ballot;
     uint64_t end;                   // frame bytes: 8-byte length prefix + body
@@ -55,6 +71,16 @@ struct FrameHdr {
     uint32_t asg;                   // Crossword: assignment[me]
     uint32_t pad;
 };
+
+// one decoded ReconstructReply frame (ss_acceptor_absorb); it lives in the FrameHdr scratch, which is at least as large
+struct ReplyHdr {
+    uint64_t count;                 // map entries
+    uint64_t entries_at;            // offset of the first entry inside the body
+    uint64_t body_len;              // bytes after the 8-byte length prefix
+    uint32_t kind;                  // verdict so far
+    uint32_t repeated;              // a slot inside the window appears twice: its last value counts
+};
+static_assert(sizeof(ReplyHdr) <= sizeof(FrameHdr) && alignof(ReplyHdr) <= alignof(FrameHdr), "ReplyHdr reuses FrameHdr scratch");
 
 }  // namespace ssb
 
@@ -124,6 +150,38 @@ __device__ __forceinline__ uint64_t wal_bytes(const FrameHdr &h, uint32_t wal_va
     return 8u + static_cast<uint64_t>(wv_len(wal_variant)) + (h.end - h.slot_at);
 }
 __device__ __forceinline__ uint64_t round16(uint64_t x) { return (x + 15u) & ~15ull; }
+
+// one shard of L bytes at src (any alignment) into its padded store slot at dst (16-byte aligned): aligned 128-bit
+// stores, each fed by dev::load16, bytes L..round_up(L, 16) zero
+__device__ __forceinline__ void warp_fill_slot(uint8_t *dst, const uint8_t *src, uint64_t L, uint32_t lane) {
+    const uint64_t nvec = (L + 15u) >> 4;
+    for (uint64_t v = lane; v < nvec; v += 32u) {
+        const uint64_t left = L - v * 16u;
+        dev::stg128_cs(dst + v * 16u, dev::load16(src + v * 16u, left < 16u ? static_cast<int>(left) : 16));
+    }
+}
+
+// the T shard Options of a bincode RSCodeword starting at tags (Option tag, length varint, bytes): the shards of `take`
+// (a subset of the present ones, `present`) go to their padded slots of the region at dst: one after the other, or with
+// a dst_mask, shard j at its rank among the shards of dst_mask
+__device__ __forceinline__ void warp_fill_shards(uint8_t *dst, const uint8_t *tags, uint32_t T, uint32_t present, uint32_t take,
+                                                 uint32_t L, uint32_t lane, uint64_t dst_mask = ~0ull) {
+    const uint64_t pitch = SS_CW_SLOT_PITCH(L);
+    uint64_t at = 0;
+    uint32_t k = 0;
+    for (uint32_t j = 0; j < T; ++j) {
+        if (!((present >> j) & 1u)) { at += 1u; continue; }
+        // Some tag, then the shard length as the frame spells it: a non-minimal varint is as valid as the header pass
+        // found it, so its width comes from its own tag byte
+        const uint8_t t = tags[at + 1u];
+        const uint64_t some_len = 1u + (t < 251u ? 1u : t == 251u ? 3u : t == 252u ? 5u : 9u);
+        if ((take >> j) & 1u) {
+            const uint64_t slot = dst_mask == ~0ull ? k++ : static_cast<uint64_t>(__popc(static_cast<uint32_t>(dst_mask) & ((1u << j) - 1u)));
+            warp_fill_slot(dst + slot * pitch, tags + at + some_len, L, lane);
+        }
+        at += some_len + static_cast<uint64_t>(L);
+    }
+}
 
 // decodes frame i as ssor_decode_accept reads it, plus the acceptor's own checks (code, shard_len, assignment shape)
 __device__ __forceinline__ FrameHdr decode_frame(const AccArgs &A, uint64_t i) {
@@ -319,24 +377,7 @@ __global__ void __launch_bounds__(kAccThreads) acceptor_copy_kernel(const __grid
         }
         warp_copy_unaligned(rec + 8u + wvl, fr + h.slot_at, tail, lane);
         // held shards in index order, each in a SS_CW_SLOT_PITCH(L) slot, zero up to round_up(L, 16)
-        const uint64_t pitch = SS_CW_SLOT_PITCH(h.L);
-        const uint64_t nvec = (static_cast<uint64_t>(h.L) + 15u) >> 4;
-        uint8_t *dst = A.store + A.store_off[i];
-        uint64_t at = h.tags_at;
-        for (uint32_t j = 0; j < A.T; ++j) {
-            if (!((h.held >> j) & 1u)) { at += 1u; continue; }
-            // Some tag, then the shard length as the frame spells it: a non-minimal varint is as valid as the header
-            // pass found it, so its width comes from its own tag byte
-            const uint8_t t = fr[at + 1u];
-            const uint64_t some_len = 1u + (t < 251u ? 1u : t == 251u ? 3u : t == 252u ? 5u : 9u);
-            const uint8_t *src = fr + at + some_len;
-            for (uint64_t v = lane; v < nvec; v += 32u) {
-                const uint64_t left = h.L - v * 16u;
-                dev::stg128_cs(dst + v * 16u, dev::load16(src + v * 16u, left < 16u ? static_cast<int>(left) : 16));
-            }
-            dst += pitch;
-            at += some_len + static_cast<uint64_t>(h.L);
-        }
+        warp_fill_shards(A.store + A.store_off[i], fr + h.tags_at, A.T, h.held, h.held, h.L, lane);
         // AcceptReply of the instance as the whole call left it
         if (lane == 0u) {
             const uint32_t g = A.frame_group[i];
@@ -653,6 +694,507 @@ __global__ void __launch_bounds__(kAccThreads) exec_payload_kernel(const __grid_
     }
 }
 
+// ---- reconstruct reads ---------------------------------------------------------------------------------------------
+struct RecArgs {
+    const uint8_t *buf;
+    uint64_t buf_len;
+    const uint64_t *frame_off;
+    const uint32_t *frame_group;
+    uint64_t n, G;
+    uint32_t d, T, variant, reply_variant, crossword;
+    // state
+    const uint64_t *window_base, *inst_bal, *accepting, *committed, *exec_bar;
+    const uint32_t *data_len;
+    uint64_t *shard_addr;
+    uint32_t *held;
+    // serve
+    uint8_t *out;
+    uint64_t out_cap;
+    uint64_t *reply_off, *reply_len;
+    // absorb
+    ReplyHdr *rhdr;
+    uint32_t *key_in, *idx_in;
+    const uint32_t *key, *idx;      // sorted
+    uint64_t *grp_bytes;            // [G] region bytes per group, then their exclusive scan
+    uint8_t *store;
+    uint64_t store_cap;
+    uint32_t *absorbed;
+    uint32_t *verdict;
+    uint32_t *status;
+};
+
+// Per-warp scratch of the walks below.  Every lane of a warp runs the same walk over the same frame bytes (the loads
+// broadcast), so the warp stays converged and copies the shards of an entry together; lane 0 writes the arrays and
+// __syncwarp publishes them.
+struct RecWarp {
+    uint32_t mask[64];              // serve: the defining entry's shards; absorb: the instance's mask as the walk goes
+    uint32_t last[64];              // occurrence index of the defining (last) entry of each ring position
+    uint32_t fin[64];               // absorb: the instance's final mask
+    uint64_t off[64];               // serve: entry offsets in the reply; absorb: new region offsets (~0: unchanged)
+};
+
+#define SS_GETV(dst) do { if (!(c = wv_get(b + n, len - n, (dst)))) return SS_FRAME_KIND_MALFORMED; n += c; } while (0)
+
+// the 8-byte length, PeerMessage::Msg and the PeerMsg variant of frame i; kPending with b / len / n past the entry count
+// (cnt) when it is `variant`
+__device__ __forceinline__ uint32_t rec_head(const RecArgs &A, uint64_t i, const uint8_t *&b, uint64_t &len, uint64_t &n, uint64_t &cnt) {
+    const uint32_t grp = A.frame_group[i];
+    const uint64_t off = A.frame_off[i];
+    if (grp >= A.G || off > A.buf_len || A.buf_len - off < 8u) return SS_FRAME_KIND_MALFORMED;
+    const uint8_t *fr = A.buf + off;
+    len = 0;
+    for (int k = 0; k < 8; ++k) len = (len << 8) | fr[k];
+    if (len > A.buf_len - off - 8u || len > kMaxFrameBody) return SS_FRAME_KIND_MALFORMED;
+    b = fr + 8;
+    n = 0;
+    uint64_t v = 0;
+    uint32_t c;
+    SS_GETV(v);
+    if (v != 0u) return v < kVariantLimit ? 0x80000000u | static_cast<uint32_t>(v) : SS_FRAME_KIND_MALFORMED;
+    SS_GETV(v);
+    if (v != A.variant) return v < kVariantLimit ? static_cast<uint32_t>(v) : SS_FRAME_KIND_MALFORMED;
+    SS_GETV(cnt);
+    return kPending;
+}
+
+__device__ __forceinline__ uint64_t ring_slot(uint64_t base, uint32_t pos) { return base + ((pos - base) & 63u); }
+
+// Reconstruct{slots} (RSPaxos) or Reconstruct{slots_excl} (Crossword) of frame i, walked as handle_msg_reconstruct
+// walks it (rspaxos/messages.rs:468-516, crossword/messages.rs:577-632).  Returns kPending when the frame is well formed
+// and refused nothing, and *nz = the ring positions with an entry: W.mask the defining entry's shards, W.last its
+// occurrence index (HashMap::insert keeps the last value).  Warp-uniform.
+__device__ uint32_t serve_walk(const RecArgs &A, uint64_t i, RecWarp &W, uint32_t lane, uint64_t *nz) {
+    *nz = 0ull;
+    const uint8_t *b;
+    uint64_t len, n, cnt;
+    const uint32_t kind = rec_head(A, i, b, len, n, cnt);
+    if (kind != kPending) return kind;
+    const uint32_t g = A.frame_group[i];
+    const uint64_t base = A.window_base[g], live = A.accepting[g] | A.committed[g];
+    const uint64_t T = A.T;
+    uint32_t err = 0u, c;
+    for (uint64_t e = 0; e < cnt; ++e) {
+        uint64_t slot = 0;
+        SS_GETV(slot);
+        uint32_t sel = 0xffffffffu;
+        bool range_bad = false;
+        if (A.crossword) {
+            // Bitmap::decode: size, then any number of u64 blocks, padded with zeros or cut to the size (bitmap.rs:32-40).
+            // subset_copy walks subset.iter() (rscoding.rs:264-275), which stops at Bitmap::size() = size as u8
+            // (bitmap.rs:103-105, 258-270), so only bits [0, size mod 256) take part.  flip() selects the ones the
+            // exclusion leaves clear, and one at index >= T makes subset_copy fail: every bit of [T, size mod 256) must
+            // be set.
+            uint64_t sz = 0, nb = 0, blk = 0, lo = 0;
+            SS_GETV(sz);
+            SS_GETV(nb);
+            const uint64_t walk = sz & 255u;
+            for (uint64_t k = 0; k < nb; ++k) {
+                SS_GETV(blk);
+                if (k == 0u) lo = blk;
+                const uint64_t b0 = 64u * k, from = T > b0 ? T : b0, to = walk < b0 + 64u ? walk : b0 + 64u;
+                if (from < to) {
+                    const uint64_t w = to - from, m = (w == 64u ? ~0ull : (1ull << w) - 1u) << (from - b0);
+                    if ((blk & m) != m) range_bad = true;
+                }
+            }
+            const uint64_t pad_from = T > 64u * nb ? T : 64u * nb;
+            if (walk > pad_from) range_bad = true;                              // zero-padded blocks
+            const uint64_t w = walk < T ? walk : T;
+            sel = ~static_cast<uint32_t>(lo) & (w >= 32u ? 0xffffffffu : (1u << w) - 1u);
+        }
+        if (err != 0u || slot < base || slot - base >= 64u) continue;           // below start_slot; a padded null instance
+        const uint32_t pos = static_cast<uint32_t>(slot & 63u);
+        if (!((live >> pos) & 1u)) continue;                                    // status < Accepting
+        const uint64_t at = static_cast<uint64_t>(g) * 64u + pos;
+        if (A.crossword) {
+            if (A.data_len[at] == 0u) { err = SS_RECON_VERDICT_NULL_CODEWORD; continue; }
+            if (range_bad) { err = SS_RECON_VERDICT_SHARD_RANGE; continue; }
+        }
+        const uint32_t m = A.held[at] & sel;                                    // RSPaxos: reqs_cw.clone()
+        if (m == 0u) continue;
+        if (lane == 0u) { W.mask[pos] = m; W.last[pos] = static_cast<uint32_t>(e); }
+        *nz |= 1ull << pos;
+    }
+    __syncwarp();
+    if (n != len) return SS_FRAME_KIND_MALFORMED;
+    return err != 0u ? err : kPending;
+}
+
+// bytes of one (slot, (inst.bal, RSCodeword)) map entry carrying the shards m of instance `at`
+__device__ __forceinline__ uint64_t serve_entry_bytes(const RecArgs &A, uint64_t slot, uint64_t at, uint32_t m) {
+    const uint64_t dl = A.data_len[at], L = (dl + A.d - 1u) / A.d, k = static_cast<uint64_t>(__popc(m));
+    return wv_len(slot) + wv_len(A.inst_bal[at]) + 2u + wv_len(dl) + wv_len(L) + wv_len(A.T) + (A.T - k) +
+           k * (1u + wv_len(L) + L) + 1u;
+}
+
+__device__ __forceinline__ uint64_t warp_sum(uint64_t x) {
+    for (int s = 16; s > 0; s >>= 1) x += __shfl_xor_sync(0xffffffffu, x, s);
+    return x;
+}
+
+// 1. a warp per frame: verdict, reply bytes (8-byte length, Msg, variant, map length, entries)
+__global__ void __launch_bounds__(kAccThreads) serve_count_kernel(const __grid_constant__ RecArgs A) {
+    __shared__ RecWarp Ws[kExecWarps];
+    const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+    RecWarp &W = Ws[w];
+    const uint64_t nwarps = static_cast<uint64_t>(gridDim.x) * kExecWarps;
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kExecWarps + w; i < A.n; i += nwarps) {
+        uint64_t nz;
+        uint32_t kind = serve_walk(A, i, W, lane, &nz);
+        uint64_t bytes = 0;
+        if (kind == kPending) {
+            kind = SS_ACCEPT_VERDICT_ACCEPTED;
+            if (nz != 0u) {
+                const uint32_t g = A.frame_group[i];
+                const uint64_t base = A.window_base[g];
+                for (uint32_t p = lane; p < 64u; p += 32u)
+                    if ((nz >> p) & 1u) bytes += serve_entry_bytes(A, ring_slot(base, p), static_cast<uint64_t>(g) * 64u + p, W.mask[p]);
+                bytes = warp_sum(bytes) + 9u + wv_len(A.reply_variant) + wv_len(__popcll(nz));
+            }
+        }
+        if (lane == 0u) {
+            A.verdict[i] = kind;
+            A.reply_len[i] = bytes;
+            A.reply_off[i] = round16(bytes);
+        }
+        __syncwarp();                   // the next frame's walk overwrites W
+    }
+}
+
+// 2. a warp per frame with a reply: capacity, then the ReconstructReply, entries in the order of their defining
+//    occurrences; every shard is copied from its 16-byte aligned store slot
+__global__ void __launch_bounds__(kAccThreads) serve_copy_kernel(const __grid_constant__ RecArgs A) {
+    __shared__ RecWarp Ws[kExecWarps];
+    const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+    RecWarp &W = Ws[w];
+    bool full = false;
+    const uint64_t nwarps = static_cast<uint64_t>(gridDim.x) * kExecWarps;
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kExecWarps + w; i < A.n; i += nwarps) {
+        const uint64_t len = A.reply_len[i], off = A.reply_off[i];
+        if (A.verdict[i] != SS_ACCEPT_VERDICT_ACCEPTED || len == 0u || off > A.out_cap || round16(len) > A.out_cap - off) {
+            if (lane == 0u) {
+                if (len != 0u) {
+                    A.verdict[i] = SS_RECON_VERDICT_OUT_FULL;
+                    A.reply_len[i] = 0u;
+                }
+                A.reply_off[i] = ~0ull;
+            }
+            full |= len != 0u;
+            continue;
+        }
+        uint64_t nz;
+        serve_walk(A, i, W, lane, &nz);
+        const uint32_t g = A.frame_group[i];
+        const uint64_t base = A.window_base[g];
+        const uint64_t cnt = static_cast<uint64_t>(__popcll(nz)), head = 9u + wv_len(A.reply_variant) + wv_len(cnt);
+        uint64_t mine[2] = {0u, 0u};
+        for (uint32_t r = 0; r < 2u; ++r) {
+            const uint32_t p = lane + 32u * r;
+            if ((nz >> p) & 1u) mine[r] = serve_entry_bytes(A, ring_slot(base, p), static_cast<uint64_t>(g) * 64u + p, W.mask[p]);
+        }
+        if (lane == 0u) for (uint32_t p = 0; p < 64u; ++p) W.off[p] = 0u;
+        __syncwarp();
+        for (uint32_t r = 0; r < 2u; ++r) if (mine[r]) W.off[lane + 32u * r] = mine[r];
+        __syncwarp();
+        for (uint32_t r = 0; r < 2u; ++r) {                                      // offsets: sizes of the earlier entries
+            const uint32_t p = lane + 32u * r;
+            if (!((nz >> p) & 1u)) continue;
+            uint64_t o = head;
+            for (uint32_t q = 0; q < 64u; ++q)
+                if (((nz >> q) & 1u) && W.last[q] < W.last[p]) o += W.off[q];
+            mine[r] = o;
+        }
+        __syncwarp();
+        for (uint32_t r = 0; r < 2u; ++r) if ((nz >> (lane + 32u * r)) & 1u) W.off[lane + 32u * r] = mine[r];
+        __syncwarp();
+        uint8_t *dst = A.out + off;
+        if (lane == 0u) {
+            const uint64_t body = len - 8u;
+            for (int k = 0; k < 8; ++k) dst[k] = static_cast<uint8_t>(body >> (8 * (7 - k)));
+            uint32_t m = 8u;
+            m += wv_put(dst + m, 0u);                                            // PeerMessage::Msg
+            m += wv_put(dst + m, A.reply_variant);
+            wv_put(dst + m, cnt);
+        }
+        for (uint64_t rest = nz; rest != 0u; rest &= rest - 1u) {
+            const uint32_t p = static_cast<uint32_t>(__ffsll(static_cast<long long>(rest))) - 1u;
+            const uint64_t at = static_cast<uint64_t>(g) * 64u + p, slot = ring_slot(base, p);
+            const uint32_t m = W.mask[p], held = A.held[at];
+            const uint64_t dl = A.data_len[at], L = (dl + A.d - 1u) / A.d, pitch = SS_CW_SLOT_PITCH(L), bal = A.inst_bal[at];
+            const uint8_t *src = reinterpret_cast<const uint8_t *>(A.shard_addr[at]);
+            uint8_t *e = dst + W.off[p];
+            const uint64_t h0 = wv_len(slot) + wv_len(bal) + 2u + wv_len(dl) + wv_len(L) + wv_len(A.T), some = 1u + wv_len(L);
+            if (lane == 0u) {                                                    // (slot, (bal, RSCodeword)) around the shards
+                uint64_t q = 0;
+                q += wv_put(e + q, slot);
+                q += wv_put(e + q, bal);
+                e[q++] = static_cast<uint8_t>(A.d);
+                e[q++] = static_cast<uint8_t>(A.T - A.d);
+                q += wv_put(e + q, dl);
+                q += wv_put(e + q, L);
+                q += wv_put(e + q, A.T);
+                for (uint32_t j = 0; j < A.T; ++j) {
+                    if ((m >> j) & 1u) {
+                        e[q] = 1u;
+                        wv_put(e + q + 1u, L);
+                        q += some + L;
+                    } else {
+                        e[q++] = 0u;
+                    }
+                }
+                e[q] = 0u;                                                       // data_copy: None
+            }
+            for (uint32_t rest_j = m; rest_j != 0u; rest_j &= rest_j - 1u) {
+                const uint32_t j = static_cast<uint32_t>(__ffs(rest_j)) - 1u;
+                const uint32_t below = (1u << j) - 1u;
+                const uint64_t sel_before = static_cast<uint64_t>(__popc(m & below));
+                const uint64_t at_j = h0 + (j - sel_before) + sel_before * (some + L) + some;
+                warp_copy_unaligned(e + at_j, src + static_cast<uint64_t>(__popc(held & below)) * pitch, L, lane);
+            }
+        }
+        __syncwarp();
+    }
+    if (full && lane == 0u) atomicOr(A.status, SS_DEV_STATUS_FRAME_OVERFLOW);
+}
+
+// one (slot, (ballot, RSCodeword)) of a ReconstructReply at b + n: the codeword must carry the acceptor's code,
+// shard_len = ceil(data_len / d), T shard Options of shard_len bytes each, and data_copy None or Some(data_len bytes)
+struct RecEntry {
+    uint64_t slot, bal, tags_at;
+    uint32_t dlen, L, mask;
+};
+__device__ __forceinline__ bool absorb_entry(const RecArgs &A, const uint8_t *b, uint64_t len, uint64_t &n, RecEntry &E) {
+    uint64_t v = 0, dl = 0, sl = 0;
+    uint32_t c;
+#define SS_GETB(dst) do { if (!(c = wv_get(b + n, len - n, (dst)))) return false; n += c; } while (0)
+    SS_GETB(E.slot);
+    SS_GETB(E.bal);
+    if (len - n < 2u || b[n] != A.d || b[n + 1] != A.T - A.d) return false;
+    n += 2;
+    SS_GETB(dl);
+    SS_GETB(sl);
+    SS_GETB(v);
+    if (dl > 0xffffffffull || v != A.T || sl != (dl + A.d - 1u) / A.d) return false;
+    E.tags_at = n;
+    uint32_t mask = 0;
+    for (uint32_t j = 0; j < A.T; ++j) {
+        if (n >= len) return false;
+        const uint8_t tag = b[n++];
+        if (tag == 0u) continue;
+        if (tag != 1u) return false;
+        SS_GETB(v);
+        if (v != sl || len - n < sl) return false;
+        mask |= 1u << j;
+        n += sl;
+    }
+    if (n >= len) return false;
+    const uint8_t tag = b[n++];                                                  // data_copy
+    if (tag == 1u) {
+        if (len - n < dl) return false;
+        n += dl;
+    } else if (tag != 0u) {
+        return false;
+    }
+#undef SS_GETB
+    E.dlen = static_cast<uint32_t>(dl);
+    E.L = static_cast<uint32_t>(sl);
+    E.mask = mask;
+    return true;
+}
+
+// 1. a thread per frame: decode the whole ReconstructReply, note a slot repeated in the window, sort keys
+__global__ void __launch_bounds__(kAccThreads) absorb_decode_kernel(const __grid_constant__ RecArgs A) {
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; i < A.n; i += stride) {
+        const uint8_t *b = nullptr;
+        uint64_t len = 0, n = 0, cnt = 0;
+        uint32_t kind = rec_head(A, i, b, len, n, cnt);
+        ReplyHdr h{};
+        if (kind == kPending) {
+            const uint64_t base = A.window_base[A.frame_group[i]];
+            h.entries_at = n;
+            h.count = cnt;
+            uint64_t seen = 0;
+            RecEntry E;
+            kind = SS_ACCEPT_VERDICT_ACCEPTED;
+            for (uint64_t e = 0; e < cnt; ++e) {
+                if (!absorb_entry(A, b, len, n, E)) { kind = SS_FRAME_KIND_MALFORMED; break; }
+                if (E.slot < base || E.slot - base >= 64u) continue;
+                const uint64_t bit = 1ull << (E.slot & 63u);
+                h.repeated |= (seen & bit) ? 1u : 0u;
+                seen |= bit;
+            }
+            if (n != len) kind = SS_FRAME_KIND_MALFORMED;
+            h.body_len = len;
+        }
+        h.kind = kind;
+        A.rhdr[i] = h;
+        A.verdict[i] = kind;
+        A.absorbed[i] = 0u;
+        A.key_in[i] = kind == SS_ACCEPT_VERDICT_ACCEPTED ? A.frame_group[i] : static_cast<uint32_t>(A.G);
+        A.idx_in[i] = static_cast<uint32_t>(i);
+    }
+}
+
+// The entries of group g's frames (sorted positions [t, e)) in frame order, then wire order, through
+// handle_msg_reconstruct_reply's filters (rspaxos/messages.rs:519-594, crossword/messages.rs:635-722); a slot repeated
+// inside one frame counts once, with its last value (a HashMap decode keeps the last insert).  W.mask starts at the held
+// masks; an entry that passes adds the shards the instance does not hold yet (absorb_other, rscoding.rs:337-343), and
+// on_entry(b, E, pos, contribution) runs for each entry that adds any; on_frame(i) runs after each frame.  Warp-uniform.
+template <typename FE, typename FF>
+__device__ void absorb_replay(const RecArgs &A, uint64_t t, uint64_t e, uint32_t g, RecWarp &W, uint32_t lane, FE &&on_entry,
+                              FF &&on_frame) {
+    const uint64_t base = A.window_base[g], live = A.accepting[g] | A.committed[g], eb = A.exec_bar[g];
+    const uint64_t row = static_cast<uint64_t>(g) * 64u;
+    W.mask[lane] = A.held[row + lane];
+    W.mask[lane + 32u] = A.held[row + lane + 32u];
+    __syncwarp();
+    for (uint64_t k = t; k < e; ++k) {
+        const uint32_t i = A.idx[k];
+        const ReplyHdr h = A.rhdr[i];
+        const uint8_t *b = A.buf + A.frame_off[i] + 8u;
+        RecEntry E;
+        uint64_t n = h.entries_at;
+        if (h.repeated) {                                                             // a repeated slot: find its last value
+            __syncwarp();
+            for (uint64_t q = 0; q < h.count; ++q) {
+                absorb_entry(A, b, h.body_len, n, E);
+                if (E.slot >= base && E.slot - base < 64u && lane == 0u) W.last[E.slot & 63u] = static_cast<uint32_t>(q);
+            }
+            __syncwarp();
+            n = h.entries_at;
+        }
+        for (uint64_t q = 0; q < h.count; ++q) {
+            absorb_entry(A, b, h.body_len, n, E);
+            if (E.slot < base || E.slot - base >= 64u) continue;                 // outdated; beyond the window
+            const uint32_t pos = static_cast<uint32_t>(E.slot & 63u);
+            if (h.repeated && W.last[pos] != q) continue;
+            const uint64_t at = row + pos;
+            if (!((live >> pos) & 1u) || E.slot < eb || E.bal < A.inst_bal[at]) continue;   // status, Executed, ballot
+            const uint32_t dl = A.data_len[at];
+            if (dl == 0u || E.dlen != dl) continue;                              // null instance; absorb_other's checks
+            const uint32_t cur = W.mask[pos], add = E.mask & ~cur;
+            if (add == 0u) continue;
+            __syncwarp();
+            if (lane == 0u) W.mask[pos] = cur | add;
+            __syncwarp();
+            on_entry(b, E, pos, add);
+        }
+        on_frame(i);
+    }
+}
+
+__device__ __forceinline__ uint64_t segment_end(const RecArgs &A, uint64_t t) {
+    uint64_t e = t + 1u;
+    while (e < A.n && A.key[e] == A.key[t]) ++e;
+    return e;
+}
+
+// 2. a warp per group segment: the final masks, and the bytes of the regions of the instances that grow
+__global__ void __launch_bounds__(kAccThreads) absorb_plan_kernel(const __grid_constant__ RecArgs A) {
+    __shared__ RecWarp Ws[kExecWarps];
+    const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+    RecWarp &W = Ws[w];
+    const uint64_t nwarps = static_cast<uint64_t>(gridDim.x) * kExecWarps;
+    for (uint64_t t = static_cast<uint64_t>(blockIdx.x) * kExecWarps + w; t < A.n; t += nwarps) {
+        if (t != 0u && A.key[t] == A.key[t - 1]) continue;
+        const uint32_t g = A.key[t];
+        if (g >= A.G) continue;
+        absorb_replay(A, t, segment_end(A, t), g, W, lane, [](const uint8_t *, const RecEntry &, uint32_t, uint32_t) {}, [](uint32_t) {});
+        uint64_t bytes = 0;
+        for (uint32_t p = lane; p < 64u; p += 32u) {
+            const uint64_t at = static_cast<uint64_t>(g) * 64u + p;
+            if (W.mask[p] != A.held[at]) bytes += static_cast<uint64_t>(__popc(W.mask[p])) * SS_CW_SLOT_PITCH((A.data_len[at] + A.d - 1u) / A.d);
+        }
+        bytes = warp_sum(bytes);
+        if (lane == 0u) A.grp_bytes[g] = bytes;
+        __syncwarp();
+    }
+}
+
+// 3. a warp per group segment: regions in slot order from the group's scanned offset, capacity, the old shards and
+//    then the new ones into the new regions, held / shard_addr, per-frame counts and verdicts
+__global__ void __launch_bounds__(kAccThreads) absorb_copy_kernel(const __grid_constant__ RecArgs A) {
+    __shared__ RecWarp Ws[kExecWarps];
+    const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+    RecWarp &W = Ws[w];
+    bool full = false;
+    const uint64_t nwarps = static_cast<uint64_t>(gridDim.x) * kExecWarps;
+    for (uint64_t t = static_cast<uint64_t>(blockIdx.x) * kExecWarps + w; t < A.n; t += nwarps) {
+        if (t != 0u && A.key[t] == A.key[t - 1]) continue;
+        const uint32_t g = A.key[t];
+        if (g >= A.G) continue;
+        const uint64_t e = segment_end(A, t), row = static_cast<uint64_t>(g) * 64u, base = A.window_base[g];
+        absorb_replay(A, t, e, g, W, lane, [](const uint8_t *, const RecEntry &, uint32_t, uint32_t) {}, [](uint32_t) {});
+        W.fin[lane] = W.mask[lane];
+        W.fin[lane + 32u] = W.mask[lane + 32u];
+        __syncwarp();
+        // region offsets in window order: lane r takes positions base + r and base + 32 + r
+        uint64_t sz[2], pre[2];
+        for (uint32_t h = 0; h < 2u; ++h) {
+            const uint32_t p = static_cast<uint32_t>((base + 32u * h + lane) & 63u);
+            const uint32_t old = A.held[row + p], nw = W.fin[p];
+            sz[h] = nw != old ? static_cast<uint64_t>(__popc(nw)) * SS_CW_SLOT_PITCH((A.data_len[row + p] + A.d - 1u) / A.d) : 0u;
+            uint64_t x = sz[h];
+            for (int s = 1; s < 32; s <<= 1) {
+                const uint64_t y = __shfl_up_sync(0xffffffffu, x, s);
+                if (lane >= static_cast<uint32_t>(s)) x += y;
+            }
+            pre[h] = x - sz[h];
+        }
+        pre[1] += __shfl_sync(0xffffffffu, pre[0] + sz[0], 31);
+        const uint64_t goff = A.grp_bytes[g];
+        for (uint32_t h = 0; h < 2u; ++h) {
+            const uint32_t p = static_cast<uint32_t>((base + 32u * h + lane) & 63u);
+            const uint32_t old = A.held[row + p];
+            const uint64_t o = goff + pre[h];
+            const bool grows = W.fin[p] != old, placed = o <= A.store_cap && sz[h] <= A.store_cap - o;
+            W.off[p] = grows && placed ? o : ~0ull;
+            full |= grows && !placed;
+        }
+        __syncwarp();
+        // the shards the instance held, into their ranks of the new mask
+        for (uint32_t p = 0; p < 64u; ++p) {
+            if (W.off[p] == ~0ull) continue;
+            const uint32_t old = A.held[row + p], nw = W.fin[p];
+            const uint64_t L = (A.data_len[row + p] + A.d - 1u) / A.d, pitch = SS_CW_SLOT_PITCH(L);
+            const uint8_t *src = reinterpret_cast<const uint8_t *>(A.shard_addr[row + p]);
+            uint8_t *dst = A.store + W.off[p];
+            uint32_t k = 0;
+            for (uint32_t rest = old; rest != 0u; rest &= rest - 1u, ++k) {
+                const uint32_t j = static_cast<uint32_t>(__ffs(rest)) - 1u;
+                warp_fill_slot(dst + static_cast<uint64_t>(__popc(nw & ((1u << j) - 1u))) * pitch, src + k * pitch, L, lane);
+            }
+        }
+        // the new shards, each from the first entry that carries it
+        uint32_t taken = 0u;
+        bool frame_full = false;
+        absorb_replay(
+            A, t, e, g, W, lane,
+            [&](const uint8_t *b, const RecEntry &E, uint32_t pos, uint32_t add) {
+                if (W.off[pos] == ~0ull) { frame_full = true; return; }
+                warp_fill_shards(A.store + W.off[pos], b + E.tags_at, A.T, E.mask, add, E.L, lane, W.fin[pos]);
+                ++taken;
+            },
+            [&](uint32_t i) {
+                if (lane == 0u) {
+                    A.absorbed[i] = taken;
+                    if (frame_full) A.verdict[i] = SS_ACCEPT_VERDICT_STORE_FULL;
+                }
+                taken = 0u;
+                frame_full = false;
+            });
+        for (uint32_t p = lane; p < 64u; p += 32u) {
+            if (W.off[p] == ~0ull) continue;
+            A.held[row + p] = W.fin[p];
+            A.shard_addr[row + p] = reinterpret_cast<uint64_t>(A.store + W.off[p]);
+        }
+        __syncwarp();
+    }
+    if (full) atomicOr(A.status, SS_DEV_STATUS_STORE_FULL);
+}
+#undef SS_GETV
+
 static inline uint32_t acc_grid(ss_ctx *ctx, uint64_t items, uint32_t per_cta) {
     uint64_t ctas = (items + per_cta - 1) / per_cta;
     const uint64_t cap = static_cast<uint64_t>(ctx->sm_count) * 8ull * 8ull;
@@ -902,6 +1444,79 @@ int ss_acceptor_accept(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, con
     acceptor_place_kernel<<<grid_t, kAccThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     acceptor_copy_kernel<<<acc_grid(ctx, n, kAccThreads / 32), kAccThreads, 0, ctx->stream>>>(A);
+    return launched(ctx);
+}
+
+static RecArgs rec_args(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
+                        uint64_t n, uint32_t variant) {
+    RecArgs R{};
+    R.buf = buf; R.buf_len = buf_len; R.frame_off = frame_off; R.frame_group = frame_group; R.n = n; R.G = a->G;
+    R.d = a->cfg.data_shards; R.T = a->cfg.total_shards; R.variant = variant;
+    R.crossword = a->cfg.protocol == SS_PROTO_CROSSWORD ? 1u : 0u;
+    R.window_base = a->window_base; R.inst_bal = a->inst_bal; R.accepting = a->accepting; R.committed = a->committed;
+    R.exec_bar = a->exec_bar; R.data_len = a->data_len; R.shard_addr = a->shard_addr; R.held = a->held;
+    R.status = a->ctx->dev_status;
+    return R;
+}
+
+int ss_acceptor_reconstruct_serve(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off,
+                                  const uint32_t *frame_group, const uint8_t *frame_peer, uint64_t n, uint32_t reconstruct_variant,
+                                  uint32_t reply_variant, uint8_t *out, uint64_t out_capacity, uint64_t *reply_off,
+                                  uint64_t *reply_len, uint32_t *verdict, uint64_t *total) {
+    if (a == nullptr) return set_error(SS_ERR_INVALID_ARG, "null acceptor");
+    ss_ctx *ctx = a->ctx;
+    SS_TRY(ctx_bind(ctx));
+    if (n == 0) {
+        if (total != nullptr) SS_CUDA(cudaMemsetAsync(total, 0, 8, ctx->stream));
+        return SS_OK;
+    }
+    if (!buf || !frame_off || !frame_group || !frame_peer || !out || !reply_off || !reply_len || !verdict)
+        return set_error(SS_ERR_INVALID_ARG, "null buffer");
+    if (reinterpret_cast<uintptr_t>(out) & 15u) return set_error(SS_ERR_INVALID_ARG, "out must be 16-byte aligned");
+    if (n > 0x7fffffffull) return set_error(SS_ERR_INVALID_ARG, "at most 2^31 - 1 frames per call");
+    SS_TRY(ensure_scratch(a, n));
+    RecArgs R = rec_args(a, buf, buf_len, frame_off, frame_group, n, reconstruct_variant);
+    R.reply_variant = reply_variant; R.out = out; R.out_cap = out_capacity; R.reply_off = reply_off; R.reply_len = reply_len;
+    R.verdict = verdict;
+    const uint32_t grid_w = acc_grid(ctx, n, kExecWarps);
+    serve_count_kernel<<<grid_w, kAccThreads, 0, ctx->stream>>>(R);
+    SS_TRY(launched(ctx));
+    SS_TRY(launch_exclusive_scan_u64(ctx, reply_off, n, a->partials, total != nullptr ? total : a->totals));
+    serve_copy_kernel<<<grid_w, kAccThreads, 0, ctx->stream>>>(R);
+    return launched(ctx);
+}
+
+int ss_acceptor_absorb(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
+                       const uint8_t *frame_peer, uint64_t n, uint32_t reply_variant, uint8_t *store, uint64_t store_capacity,
+                       uint32_t *absorbed, uint32_t *verdict, uint64_t *total) {
+    if (a == nullptr) return set_error(SS_ERR_INVALID_ARG, "null acceptor");
+    ss_ctx *ctx = a->ctx;
+    SS_TRY(ctx_bind(ctx));
+    if (n == 0) {
+        if (total != nullptr) SS_CUDA(cudaMemsetAsync(total, 0, 8, ctx->stream));
+        return SS_OK;
+    }
+    if (!buf || !frame_off || !frame_group || !frame_peer || !store || !absorbed || !verdict) return set_error(SS_ERR_INVALID_ARG, "null buffer");
+    if (reinterpret_cast<uintptr_t>(store) & 15u) return set_error(SS_ERR_INVALID_ARG, "store must be 16-byte aligned");
+    if (n > 0x7fffffffull) return set_error(SS_ERR_INVALID_ARG, "at most 2^31 - 1 frames per call");
+    SS_TRY(ensure_scratch(a, n));
+    RecArgs R = rec_args(a, buf, buf_len, frame_off, frame_group, n, reply_variant);
+    R.rhdr = reinterpret_cast<ReplyHdr *>(a->hdr);   // the accept pass's per-frame header scratch, reused
+    R.key_in = a->keys; R.idx_in = a->idx; R.key = a->keys + n; R.idx = a->idx + n;
+    R.grp_bytes = a->ex_bytes;      // execute's per-group scratch: both calls are ordered on the context's stream
+    R.store = store; R.store_cap = store_capacity; R.absorbed = absorbed; R.verdict = verdict;
+    absorb_decode_kernel<<<acc_grid(ctx, n, kAccThreads), kAccThreads, 0, ctx->stream>>>(R);
+    SS_TRY(launched(ctx));
+    size_t bytes = a->sort_tmp_bytes;
+    SS_CUDA(cub::DeviceRadixSort::SortPairs(a->sort_tmp, bytes, a->keys, a->keys + n, a->idx, a->idx + n, static_cast<int>(n), 0,
+                                            key_bits(a->G), ctx->stream));
+    SS_TRY(launched(ctx));
+    SS_CUDA(cudaMemsetAsync(a->ex_bytes, 0, a->G * 8, ctx->stream));
+    const uint32_t grid_w = acc_grid(ctx, n, kExecWarps);
+    absorb_plan_kernel<<<grid_w, kAccThreads, 0, ctx->stream>>>(R);
+    SS_TRY(launched(ctx));
+    SS_TRY(launch_exclusive_scan_u64(ctx, a->ex_bytes, a->G, a->ex_partials, total != nullptr ? total : a->totals));
+    absorb_copy_kernel<<<grid_w, kAccThreads, 0, ctx->stream>>>(R);
     return launched(ctx);
 }
 

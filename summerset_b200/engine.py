@@ -299,6 +299,42 @@ class Acceptor:
                                            p(res["rec_slot"]), p(res["rec_off"]), p(res["rec_len"]), rec_capacity, p(res["totals"])))
         return res
 
+    def reconstruct_serve(self, buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor, frame_peer: torch.Tensor,
+                          out: torch.Tensor, out_capacity: Optional[int] = None, reconstruct_variant: int = 4,
+                          reply_variant: int = 5) -> dict:
+        """Serves Reconstruct frames (handle_msg_reconstruct) from the held shards: ReconstructReply frames into out
+        (uint8, 16-byte aligned, one round_up(reply_len, 16) region per frame with a reply, packed in frame order).
+        Returns device tensors reply_off (int64, -1 = no reply), reply_len (int64, 0 = nothing to send), verdict (int32)
+        and total (int64 [1]: the bytes the batch asked for); reply i goes to frame_peer[i]."""
+        assert buf.dtype == torch.uint8 and frame_off.dtype == torch.int64 and frame_group.dtype == torch.int32
+        assert frame_peer.dtype == torch.uint8 and out.dtype == torch.uint8
+        n, dev = frame_off.numel(), buf.device
+        res = dict(reply_off=torch.empty(n, dtype=torch.int64, device=dev), reply_len=torch.empty(n, dtype=torch.int64, device=dev),
+                   verdict=torch.empty(n, dtype=torch.int32, device=dev), total=torch.empty(1, dtype=torch.int64, device=dev))
+        p = lambda x: x.data_ptr()
+        check(self.lib.ss_acceptor_reconstruct_serve(self.h, p(buf), buf.numel(), p(frame_off), p(frame_group), p(frame_peer), n,
+                                                     reconstruct_variant, reply_variant, p(out),
+                                                     out.numel() if out_capacity is None else out_capacity, p(res["reply_off"]),
+                                                     p(res["reply_len"]), p(res["verdict"]), p(res["total"])))
+        return res
+
+    def absorb(self, buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor, frame_peer: torch.Tensor,
+               store: torch.Tensor, store_capacity: Optional[int] = None, reply_variant: int = 5) -> dict:
+        """Absorbs ReconstructReply frames (handle_msg_reconstruct_reply): every instance that gains shards moves to a new
+        region of store (uint8, 16-byte aligned, caller-owned; keep it alive while the instances hold it).  Returns
+        device tensors absorbed (int32: entries of each frame that added shards), verdict (int32) and total (int64 [1]:
+        the store bytes the batch asked for).  ss_acceptor_execute then runs what now holds d shards."""
+        assert buf.dtype == torch.uint8 and frame_off.dtype == torch.int64 and frame_group.dtype == torch.int32
+        assert frame_peer.dtype == torch.uint8 and store.dtype == torch.uint8
+        n, dev = frame_off.numel(), buf.device
+        res = dict(absorbed=torch.empty(n, dtype=torch.int32, device=dev), verdict=torch.empty(n, dtype=torch.int32, device=dev),
+                   total=torch.empty(1, dtype=torch.int64, device=dev))
+        p = lambda x: x.data_ptr()
+        check(self.lib.ss_acceptor_absorb(self.h, p(buf), buf.numel(), p(frame_off), p(frame_group), p(frame_peer), n, reply_variant,
+                                          p(store), store.numel() if store_capacity is None else store_capacity, p(res["absorbed"]),
+                                          p(res["verdict"]), p(res["total"])))
+        return res
+
     def close(self) -> None:
         if getattr(self, "h", None) is not None and self.h:
             self.lib.ss_acceptor_destroy(self.h)

@@ -322,6 +322,23 @@ class Acceptor {
                  uint64_t rec_capacity, uint64_t *totals) {
         check(ss_acceptor_execute(acc_, out, out_capacity, rec_group, rec_slot, rec_off, rec_len, rec_capacity, totals));
     }
+    // handle_msg_reconstruct: Reconstruct frames (PeerMsg variant 4) in, ReconstructReply frames (variant 5) into out;
+    // reply i goes to frame_peer[i]
+    void reconstruct_serve(const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
+                           const uint8_t *frame_peer, uint64_t n_frames, uint8_t *out, uint64_t out_capacity, uint64_t *reply_off,
+                           uint64_t *reply_len, uint32_t *verdict, uint64_t *total, uint32_t reconstruct_variant = 4,
+                           uint32_t reply_variant = 5) {
+        check(ss_acceptor_reconstruct_serve(acc_, buf, buf_len, frame_off, frame_group, frame_peer, n_frames, reconstruct_variant,
+                                            reply_variant, out, out_capacity, reply_off, reply_len, verdict, total));
+    }
+    // handle_msg_reconstruct_reply: the shards of ReconstructReply frames into new regions of store; execute() then runs
+    // what now holds d shards
+    void absorb(const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group, const uint8_t *frame_peer,
+                uint64_t n_frames, uint8_t *store, uint64_t store_capacity, uint32_t *absorbed, uint32_t *verdict, uint64_t *total,
+                uint32_t reply_variant = 5) {
+        check(ss_acceptor_absorb(acc_, buf, buf_len, frame_off, frame_group, frame_peer, n_frames, reply_variant, store, store_capacity,
+                                 absorbed, verdict, total));
+    }
     ss_acceptor_view view() const {
         ss_acceptor_view v;
         check(ss_acceptor_view_get(acc_, &v));
