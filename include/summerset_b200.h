@@ -827,6 +827,98 @@ int ss_acceptor_reconstruct_serve(ss_acceptor *acceptor, const uint8_t *buf, uin
 int ss_acceptor_absorb(ss_acceptor *acceptor, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off,
                        const uint32_t *frame_group, const uint8_t *frame_peer, uint64_t n_frames, uint32_t reply_variant,
                        uint8_t *store, uint64_t store_capacity, uint32_t *absorbed, uint32_t *verdict, uint64_t *total);
+/* Prepare on the acceptor, the follower half of leader fail-over: handle_msg_prepare (rspaxos/messages.rs:13-84,
+ * crossword/messages.rs:63-136) and, once its PrepareBal records are durable, the follower branch of
+ * handle_logged_prepare_bal (rspaxos/durability.rs:10-79, crossword/durability.rs:9-79).  Five more arrays, all zero at
+ * creation: preparing (ring word, bit s & 63 = Status::Preparing), inst.voted = (voted_bal, voted_mask) kept apart from
+ * inst_bal and held, and replica_bk's trigger_slot and endprep_slot - trigger_slot (always < 64).  An accepted Accept
+ * sets voted = (ballot, the frame's shards), clears preparing and sets trigger and span to 0 (replica_bk = {source, 0,
+ * 0}, rspaxos/messages.rs:365-372); ss_acceptor_advance clears preparing on the retired positions; absorb leaves the vote
+ * alone, and shard j of the vote sits at rank popcount(held & ((1 << j) - 1)) of the instance's store region, since the
+ * vote stays a subset of held.  A Preparing instance is neither Accepting nor Committed: it stops the heartbeat commit
+ * walk and the execution walk, and serve and absorb skip it, as the reference's `status < Accepting` checks do. */
+typedef struct ss_acceptor_prepare_view {
+    uint64_t n_groups;
+    uint64_t *preparing;        /* [G] bit s & 63 = Status::Preparing */
+    uint64_t *voted_bal;        /* [G*64] ballot of inst.voted; 0 = voted None */
+    uint32_t *voted_mask;       /* [G*64] shard set of inst.voted */
+    uint64_t *prep_trigger;     /* [G*64] replica_bk.trigger_slot */
+    uint8_t *prep_span;         /* [G*64] replica_bk.endprep_slot - trigger_slot */
+} ss_acceptor_prepare_view;
+int ss_acceptor_prepare_view_get(ss_acceptor *acceptor, ss_acceptor_prepare_view *view);
+/* Prepare frames, taken as by ss_acceptor_accept: buf at any byte alignment, frame i at frame_off[i], of group
+ * frame_group[i] (>= n_groups: malformed), from replica frame_peer[i].  Frame i is PeerMessage::Msg{Prepare{trigger_slot,
+ * ballot}}; prepare_variant (PeerMsg::Prepare, 0) and wal_variant (WalEntry::PrepareBal, 0; below 2^16) are arguments.
+ * verdict[i]: SS_ACCEPT_VERDICT_ACCEPTED; SS_ACCEPT_VERDICT_STALE_SLOT (trigger_slot < window_base, ignored);
+ * SS_ACCEPT_VERDICT_STALE_BALLOT (ballot < bal_max_seen as it stands when the frame is reached);
+ * SS_ACCEPT_VERDICT_BEYOND_WINDOW (trigger_slot >= window_base + 64: re-submit after ss_acceptor_advance);
+ * SS_ACCEPT_VERDICT_WAL_FULL (below); another message's variant index (0x80000000 | k for the PeerMessage variants);
+ * SS_FRAME_KIND_MALFORMED: truncated, trailing bytes, a variant >= 2^16, or a Prepare whose frame_peer is `me`.
+ * Each group's frames are replayed in frame order as if they arrived one at a time.  A frame that passes raises
+ * bal_max_seen to its ballot; endprep_slot = max(window_base + the last window position that is Preparing, Accepting or
+ * Committed, trigger_slot), with the positions earlier frames of the call made Preparing counted as such; every slot of
+ * [trigger_slot, endprep_slot] gets inst_bal = ballot, Status::Preparing (also over Committed), source = frame_peer and
+ * the frame's trigger and span; a slot that was null (neither Preparing, Accepting nor Committed) also gets voted None
+ * (voted_bal = voted_mask = 0), as a fresh null_instance() has it, so a retired position leaks no earlier vote.  Of
+ * several frames covering one slot the last applied defines it.
+ * Records: one WalEntry::PrepareBal{slot, ballot} per slot of each applied frame's range, numbered by an exclusive scan
+ * of the per-frame counts in frame order; record k is the 32-byte cell wal + 32k (8-byte big-endian length + bincode
+ * body, at most 29 bytes, zero to the end of the cell), with rec_group[k], rec_slot[k] (absolute) and rec_frame[k]
+ * beside it.  totals (device u64[2], may be NULL): the records and the WAL bytes (32 per record) the batch asked for.
+ * Capacity: the first frame in frame order whose records end past rec_capacity or past wal_capacity / 32 cells gets
+ * SS_ACCEPT_VERDICT_WAL_FULL and changes nothing, and so does every later frame whose verdict came from the replay
+ * (ACCEPTED or STALE_BALLOT); SS_DEV_STATUS_FRAME_OVERFLOW.  The applied frames are then a prefix in frame order, and
+ * within each group a prefix of its frames, so the ranges computed for them stay exact; the host re-submits the rest.
+ * Unlike ss_acceptor_accept's per-frame cut this cut is a suffix, because a Prepare's range depends on the Prepares before
+ * it in its group.  wal 16-byte aligned.
+ * Stated differences from the reference: the window (a trigger beyond it is re-submitted; the reference grows its log
+ * with null instances instead, and endprep_slot never reaches past the window); the capacity suffix above; a Prepare
+ * from `me` is malformed, where check_leader debug-asserts peer != me.  Peer-side bookkeeping of check_leader (leader
+ * change, hear timers) stays on the host.
+ * Cost: the walk and the apply pass take a thread per group segment, so a batch costs its largest per-group run of
+ * frames there; the record cells and per-slot writes take a warp per applied frame. */
+int ss_acceptor_prepare(ss_acceptor *acceptor, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off,
+                        const uint32_t *frame_group, const uint8_t *frame_peer, uint64_t n_frames, uint32_t prepare_variant,
+                        uint32_t wal_variant, uint8_t *wal, uint64_t wal_capacity, uint32_t *rec_group, uint64_t *rec_slot,
+                        uint32_t *rec_frame, uint64_t rec_capacity, uint32_t *verdict, uint64_t *totals);
+/* PrepareReply frames for PrepareBal records that became durable (device arrays [n_records], normally rec_group /
+ * rec_slot of ss_acceptor_prepare).  The instance's state is read when this call runs, as the reference reads inst.bal,
+ * replica_bk and inst.voted when the log result arrives.  Record k produces nothing (reply_len 0, reply_off UINT64_MAX,
+ * reply_dst 0xff) when its group is >= n_groups, its slot is outside [window_base, window_base + 64), or the instance is
+ * null (no replica_bk).  Otherwise it produces PeerMessage::Msg{PrepareReply{slot, trigger_slot, endprep_slot, ballot:
+ * inst_bal, voted}}, framed with the 8-byte big-endian length, for replica reply_dst[k] = source; reply_variant is
+ * PeerMsg::PrepareReply (1).  voted = Some((voted_bal, RSCodeword)) when voted_bal > 0, else None; the codeword carries
+ * d, p, data_len, shard_len, T shard Options with the voted_mask shards read through shard_addr at their rank in held,
+ * and data_copy None.  An instance accepted after the Prepare replies with trigger and endprep 0, as the reference does.
+ * Regions of round_up(reply_len, 16) bytes are placed by an exclusive scan in record order at out + reply_off[k] (out
+ * 16-byte aligned; bytes past reply_len are not written).  A reply whose region ends past out_capacity is not written:
+ * reply_off UINT64_MAX with reply_len kept, reply_dst 0xff, SS_DEV_STATUS_FRAME_OVERFLOW; the offsets are monotone, so
+ * the written replies are a prefix and a host drains by calling again with the rest.  *total (device u64, may be NULL)
+ * = the bytes the batch asked for.  Acceptor state is not changed.
+ * Cost: a thread per record sizes, a warp per record writes. */
+int ss_acceptor_prepare_reply(ss_acceptor *acceptor, const uint32_t *rec_group, const uint64_t *rec_slot, uint64_t n_records,
+                              uint32_t reply_variant, uint8_t *out, uint64_t out_capacity, uint64_t *reply_off,
+                              uint64_t *reply_len, uint8_t *reply_dst, uint64_t *total);
+/* PrepareReply frames -> one record per frame for the new leader (a thread per frame, no copies; the PrepareReply
+ * counterpart of ss_accept_reply_parse_dev).  Frame i at buf + frame_off[i] (any alignment) must be
+ * PeerMessage::Msg{PrepareReply{slot, trigger_slot, endprep_slot, ballot, voted}} whose codeword, when voted is Some,
+ * carries this d and p, shard_len = ceil(data_len / d) with data_len < 2^32, exactly T shard Options each present one
+ * shard_len bytes, and data_copy None or Some followed by exactly data_len bytes -- the rules ss_acceptor_absorb applies.
+ * kind = reply_variant for such a frame; another message's variant index (0x80000000 | k for the PeerMessage variants);
+ * SS_FRAME_KIND_MALFORMED otherwise (including trailing bytes and variants >= 2^16).  The other fields are zero and
+ * shards_at UINT64_MAX unless kind = reply_variant.  Group, peer and instance indexing stay the caller's: it scatters
+ * vote_bal / vote_mask into the [r*N + i] arrays ss_prepare_merge_dev takes. */
+typedef struct ss_prepare_reply_rec {
+    uint64_t slot, trigger_slot, endprep_slot, ballot;
+    uint64_t vote_bal;          /* 0 for voted None */
+    uint64_t shards_at;         /* offset in buf of the codeword's first shard Option tag; UINT64_MAX for None */
+    uint32_t vote_mask;         /* shards present */
+    uint32_t data_len;
+    uint32_t kind;
+    uint32_t pad;
+} ss_prepare_reply_rec;
+int ss_prepare_reply_parse_dev(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, uint64_t n_frames,
+                               uint32_t data_shards, uint32_t total_shards, uint32_t reply_variant, ss_prepare_reply_rec *rec);
 
 /* ---- tuning / introspection (bench + tests) ------------------------------------------------ */
 /* Tuning knob for experiments; 0 = the defaults.

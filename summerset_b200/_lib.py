@@ -126,6 +126,10 @@ SIGNATURES = {
     "ss_acceptor_execute": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp]),
     "ss_acceptor_reconstruct_serve": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _u32, _vp, _u64, _vp, _vp, _vp, _vp]),
     "ss_acceptor_absorb": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _vp, _u64, _vp, _vp, _vp]),
+    "ss_acceptor_prepare_view_get": (_i, [_vp, _vp]),
+    "ss_acceptor_prepare": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _u32, _vp, _u64, _vp, _vp, _vp, _u64, _vp, _vp]),
+    "ss_acceptor_prepare_reply": (_i, [_vp, _vp, _vp, _u64, _u32, _vp, _u64, _vp, _vp, _vp, _vp]),
+    "ss_prepare_reply_parse_dev": (_i, [_vp, _vp, _u64, _vp, _u64, _u32, _u32, _u32, _vp]),
     "ss_rs_set_variant": (_i, [_vp, _i]),
     "ss_rs_last_kernel": (C.c_char_p, [_vp]),
     "ss_rs_jit_status": (C.c_char_p, [_vp]),
@@ -184,6 +188,19 @@ class AcceptorView(C.Structure):
 class AcceptorCommitView(C.Structure):
     """ss_acceptor_commit_view"""
     _fields_ = [("n_groups", C.c_uint64), ("committed", C.c_void_p), ("commit_bar", C.c_void_p), ("exec_bar", C.c_void_p)]
+
+
+class AcceptorPrepareView(C.Structure):
+    """ss_acceptor_prepare_view"""
+    _fields_ = [("n_groups", C.c_uint64), ("preparing", C.c_void_p), ("voted_bal", C.c_void_p), ("voted_mask", C.c_void_p),
+                ("prep_trigger", C.c_void_p), ("prep_span", C.c_void_p)]
+
+
+class PrepareReplyRec(C.Structure):
+    """ss_prepare_reply_rec (64 bytes)"""
+    _fields_ = [("slot", C.c_uint64), ("trigger_slot", C.c_uint64), ("endprep_slot", C.c_uint64), ("ballot", C.c_uint64),
+                ("vote_bal", C.c_uint64), ("shards_at", C.c_uint64), ("vote_mask", C.c_uint32), ("data_len", C.c_uint32),
+                ("kind", C.c_uint32), ("pad", C.c_uint32)]
 
 
 # ss_acceptor_execute's bits of the device status word

@@ -47,6 +47,23 @@
 //   absorb_copy_kernel       a warp per group segment: capacity, old and new shards into the new regions, held /
 //                            shard_addr, per-frame counts and verdicts
 // Stated differences from the reference: include/summerset_b200.h at ss_acceptor_reconstruct_serve.
+//
+// The follower half of leader fail-over: handle_msg_prepare (rspaxos/messages.rs:13-84, crossword/messages.rs:63-136)
+// and, once the PrepareBal records are durable, the follower branch of handle_logged_prepare_bal
+// (rspaxos/durability.rs:10-79, crossword/durability.rs:9-79):
+//
+//   prepare_header_kernel    a thread per Prepare frame: decode, window filters, sort keys
+//   (CUB radix sort)         frames by group, as above
+//   prepare_walk_kernel      a thread per group segment: check_leader and each frame's [trigger_slot, endprep_slot],
+//                            replayed in frame order over the group's state words held in registers; writes no state
+//   (engine.cu's scan)       record numbers: exclusive scan of the per-frame counts in frame order
+//   prepare_apply_kernel     a thread per group segment, last frame first: the capacity suffix, verdicts, state words,
+//                            bal_max_seen, and the positions each applied frame defines
+//   prepare_write_kernel     a warp per applied frame: the PrepareBal cells, the per-slot arrays of the defined positions
+//   prep_reply_size_kernel   a thread per record: PrepareReply bytes
+//   (engine.cu's scan)       reply regions
+//   prep_reply_copy_kernel   a warp per record: capacity, the PrepareReply with the voted shards (the RSCodeword writer
+//                            serve_copy_kernel uses)
 #include <cub/device/device_radix_sort.cuh>
 
 #include <cstring>
@@ -82,6 +99,17 @@ struct ReplyHdr {
 };
 static_assert(sizeof(ReplyHdr) <= sizeof(FrameHdr) && alignof(ReplyHdr) <= alignof(FrameHdr), "ReplyHdr reuses FrameHdr scratch");
 
+// one decoded Prepare frame (ss_acceptor_prepare), also in the FrameHdr scratch
+struct PrepHdr {
+    uint64_t trigger, ballot;
+    uint64_t endprep;               // the walk's endprep_slot, for the frames that pass
+    uint64_t define;                // ring positions for which this frame is the last applied frame covering them
+    uint64_t fresh;                 // of those, the ones null before the call: their vote becomes None
+    uint32_t kind;                  // verdict so far
+    uint32_t pad;
+};
+static_assert(sizeof(PrepHdr) <= sizeof(FrameHdr) && alignof(PrepHdr) <= alignof(FrameHdr), "PrepHdr reuses FrameHdr scratch");
+
 }  // namespace ssb
 
 struct ss_acceptor {
@@ -92,6 +120,11 @@ struct ss_acceptor {
     uint32_t *held = nullptr, *data_len = nullptr, *assignment = nullptr;
     uint8_t *source = nullptr;
     uint64_t *committed = nullptr, *commit_bar = nullptr, *exec_bar = nullptr;
+    // Prepare: Status::Preparing (ring word), inst.voted = (voted_bal, voted_mask), replica_bk's trigger_slot and
+    // endprep_slot - trigger_slot
+    uint64_t *preparing = nullptr, *voted_bal = nullptr, *prep_trigger = nullptr;
+    uint32_t *voted_mask = nullptr;
+    uint8_t *prep_span = nullptr;
     uint8_t *matrix = nullptr;      // [T*d] the coder's coding matrix (gf256.hpp), row-major
     uint64_t *ex_cnt = nullptr, *ex_bytes = nullptr, *ex_partials = nullptr, *ex_n = nullptr;   // execute scratch
     // per-call scratch, grow-only
@@ -100,6 +133,7 @@ struct ss_acceptor {
     uint32_t *keys = nullptr;       // [2][cap]: sort keys in / out
     uint32_t *idx = nullptr;        // [2][cap]: frame indices in / out
     uint64_t *partials = nullptr;   // [scan_tiles(cap)]
+    uint64_t *fcnt = nullptr;       // [cap]: ss_acceptor_prepare's per-frame record counts, then their scan
     void *sort_tmp = nullptr;
     size_t sort_tmp_bytes = 0;
     uint64_t *totals = nullptr;     // [2] when the caller passes none
@@ -124,6 +158,9 @@ struct AccArgs {
     uint64_t *window_base, *bal_max_seen, *inst_bal, *accepting, *shard_addr, *committed;
     uint32_t *held, *data_len, *assignment;
     uint8_t *source;
+    uint64_t *preparing, *voted_bal, *prep_trigger;
+    uint32_t *voted_mask;
+    uint8_t *prep_span;
     // scratch
     FrameHdr *hdr;
     uint32_t *key_in, *idx_in;
@@ -335,6 +372,10 @@ __global__ void __launch_bounds__(kAccThreads) acceptor_place_kernel(const __gri
                         A.data_len[at] = h.dlen;
                         A.shard_addr[at] = reinterpret_cast<uint64_t>(A.store + so);
                         if (A.assignment != nullptr) A.assignment[at] = h.asg;
+                        A.voted_bal[at] = h.ballot;                     // inst.voted = (ballot, reqs_cw as accepted)
+                        A.voted_mask[at] = h.held;
+                        A.prep_trigger[at] = 0u;                        // replica_bk = {source, 0, 0}
+                        A.prep_span[at] = 0u;
                     }
                 }
             }
@@ -350,6 +391,7 @@ __global__ void __launch_bounds__(kAccThreads) acceptor_place_kernel(const __gri
         if (known) {
             A.accepting[g] |= seen;                                     // Status::Accepting, also for a committed slot
             A.committed[g] &= ~seen;                                    // (rspaxos/messages.rs:363)
+            A.preparing[g] &= ~seen;
             A.bal_max_seen[g] = mx;
         }
     }
@@ -401,10 +443,11 @@ __global__ void __launch_bounds__(kAccThreads) acceptor_copy_kernel(const __grid
     }
 }
 
-// retire window prefixes: k = clamp(upto - base, 0, 64) positions leave Accepting and Committed, the base moves on
+// retire window prefixes: k = clamp(upto - base, 0, 64) positions leave Preparing, Accepting and Committed, the base
+// moves on
 __global__ void __launch_bounds__(kAccThreads)
 acceptor_advance_kernel(const uint64_t *__restrict__ upto, uint64_t G, uint64_t *__restrict__ window_base, uint64_t *__restrict__ accepting,
-                        uint64_t *__restrict__ committed) {
+                        uint64_t *__restrict__ committed, uint64_t *__restrict__ preparing) {
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
     for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; g < G; g += stride) {
         const uint64_t base = window_base[g], u = upto[g];
@@ -413,6 +456,7 @@ acceptor_advance_kernel(const uint64_t *__restrict__ upto, uint64_t G, uint64_t 
         const uint64_t keep = ring_keep_after(k, base);
         accepting[g] &= keep;
         committed[g] &= keep;
+        preparing[g] &= keep;
         window_base[g] = base + k;
     }
 }
@@ -820,11 +864,49 @@ __device__ uint32_t serve_walk(const RecArgs &A, uint64_t i, RecWarp &W, uint32_
     return err != 0u ? err : kPending;
 }
 
+// bytes of a bincode RSCodeword carrying the shards m: d, p, data_len, shard_len, T shard Options, data_copy None
+__device__ __forceinline__ uint64_t codeword_bytes(uint32_t d, uint32_t T, uint64_t dl, uint32_t m) {
+    const uint64_t L = (dl + d - 1u) / d, k = static_cast<uint64_t>(__popc(m));
+    return 2u + wv_len(dl) + wv_len(L) + wv_len(T) + (T - k) + k * (1u + wv_len(L) + L) + 1u;
+}
+
+// that codeword at e (any alignment): lane 0 writes the header, the Option tags and the shard lengths; the warp copies
+// shard j of m from its padded slot in the instance's store region at src, rank popcount(held & below j).  Not inlined:
+// inlined into serve_copy_kernel it made that kernel spill; the call costs one per entry.
+__device__ __noinline__ void warp_put_codeword(uint8_t *e, uint32_t d, uint32_t T, uint64_t dl, uint32_t m, uint32_t held, const uint8_t *src,
+                                  uint32_t lane) {
+    const uint64_t L = (dl + d - 1u) / d, pitch = SS_CW_SLOT_PITCH(L);
+    const uint64_t h0 = 2u + wv_len(dl) + wv_len(L) + wv_len(T), some = 1u + wv_len(L);
+    if (lane == 0u) {
+        uint64_t q = 0;
+        e[q++] = static_cast<uint8_t>(d);
+        e[q++] = static_cast<uint8_t>(T - d);
+        q += wv_put(e + q, dl);
+        q += wv_put(e + q, L);
+        q += wv_put(e + q, T);
+        for (uint32_t j = 0; j < T; ++j) {
+            if ((m >> j) & 1u) {
+                e[q] = 1u;
+                wv_put(e + q + 1u, L);
+                q += some + L;
+            } else {
+                e[q++] = 0u;
+            }
+        }
+        e[q] = 0u;                                                           // data_copy: None
+    }
+    for (uint32_t rest_j = m; rest_j != 0u; rest_j &= rest_j - 1u) {
+        const uint32_t j = static_cast<uint32_t>(__ffs(rest_j)) - 1u;
+        const uint32_t below = (1u << j) - 1u;
+        const uint64_t sel_before = static_cast<uint64_t>(__popc(m & below));
+        const uint64_t at_j = h0 + (j - sel_before) + sel_before * (some + L) + some;
+        warp_copy_unaligned(e + at_j, src + static_cast<uint64_t>(__popc(held & below)) * pitch, L, lane);
+    }
+}
+
 // bytes of one (slot, (inst.bal, RSCodeword)) map entry carrying the shards m of instance `at`
 __device__ __forceinline__ uint64_t serve_entry_bytes(const RecArgs &A, uint64_t slot, uint64_t at, uint32_t m) {
-    const uint64_t dl = A.data_len[at], L = (dl + A.d - 1u) / A.d, k = static_cast<uint64_t>(__popc(m));
-    return wv_len(slot) + wv_len(A.inst_bal[at]) + 2u + wv_len(dl) + wv_len(L) + wv_len(A.T) + (A.T - k) +
-           k * (1u + wv_len(L) + L) + 1u;
+    return wv_len(slot) + wv_len(A.inst_bal[at]) + codeword_bytes(A.d, A.T, A.data_len[at], m);
 }
 
 __device__ __forceinline__ uint64_t warp_sum(uint64_t x) {
@@ -919,38 +1001,11 @@ __global__ void __launch_bounds__(kAccThreads) serve_copy_kernel(const __grid_co
         for (uint64_t rest = nz; rest != 0u; rest &= rest - 1u) {
             const uint32_t p = static_cast<uint32_t>(__ffsll(static_cast<long long>(rest))) - 1u;
             const uint64_t at = static_cast<uint64_t>(g) * 64u + p, slot = ring_slot(base, p);
-            const uint32_t m = W.mask[p], held = A.held[at];
-            const uint64_t dl = A.data_len[at], L = (dl + A.d - 1u) / A.d, pitch = SS_CW_SLOT_PITCH(L), bal = A.inst_bal[at];
-            const uint8_t *src = reinterpret_cast<const uint8_t *>(A.shard_addr[at]);
+            const uint64_t bal = A.inst_bal[at];
             uint8_t *e = dst + W.off[p];
-            const uint64_t h0 = wv_len(slot) + wv_len(bal) + 2u + wv_len(dl) + wv_len(L) + wv_len(A.T), some = 1u + wv_len(L);
-            if (lane == 0u) {                                                    // (slot, (bal, RSCodeword)) around the shards
-                uint64_t q = 0;
-                q += wv_put(e + q, slot);
-                q += wv_put(e + q, bal);
-                e[q++] = static_cast<uint8_t>(A.d);
-                e[q++] = static_cast<uint8_t>(A.T - A.d);
-                q += wv_put(e + q, dl);
-                q += wv_put(e + q, L);
-                q += wv_put(e + q, A.T);
-                for (uint32_t j = 0; j < A.T; ++j) {
-                    if ((m >> j) & 1u) {
-                        e[q] = 1u;
-                        wv_put(e + q + 1u, L);
-                        q += some + L;
-                    } else {
-                        e[q++] = 0u;
-                    }
-                }
-                e[q] = 0u;                                                       // data_copy: None
-            }
-            for (uint32_t rest_j = m; rest_j != 0u; rest_j &= rest_j - 1u) {
-                const uint32_t j = static_cast<uint32_t>(__ffs(rest_j)) - 1u;
-                const uint32_t below = (1u << j) - 1u;
-                const uint64_t sel_before = static_cast<uint64_t>(__popc(m & below));
-                const uint64_t at_j = h0 + (j - sel_before) + sel_before * (some + L) + some;
-                warp_copy_unaligned(e + at_j, src + static_cast<uint64_t>(__popc(held & below)) * pitch, L, lane);
-            }
+            if (lane == 0u) wv_put(e + wv_put(e, slot), bal);                 // (slot, (bal, RSCodeword))
+            warp_put_codeword(e + wv_len(slot) + wv_len(bal), A.d, A.T, A.data_len[at], W.mask[p], A.held[at],
+                              reinterpret_cast<const uint8_t *>(A.shard_addr[at]), lane);
         }
         __syncwarp();
     }
@@ -1195,6 +1250,313 @@ __global__ void __launch_bounds__(kAccThreads) absorb_copy_kernel(const __grid_c
 }
 #undef SS_GETV
 
+// ---- prepare -----------------------------------------------------------------------------------------------------
+struct PrepArgs {
+    const uint8_t *buf;
+    uint64_t buf_len;
+    const uint64_t *frame_off;
+    const uint32_t *frame_group;
+    const uint8_t *frame_peer;
+    uint64_t n, G;
+    uint32_t me, variant, wal_variant;
+    // state
+    const uint64_t *window_base;
+    uint64_t *bal_max_seen, *inst_bal, *accepting, *committed, *preparing, *voted_bal, *prep_trigger;
+    uint32_t *voted_mask;
+    uint8_t *source, *prep_span;
+    // scratch
+    PrepHdr *hdr;
+    uint32_t *key_in, *idx_in;
+    const uint32_t *key, *idx;      // sorted
+    uint64_t *cnt;                  // [n] records per frame, then their exclusive scan (the first record's number)
+    uint64_t *totals;               // [2]: [0] the scan's total, [1] its WAL bytes
+    uint64_t cap;                   // min(rec_capacity, wal_capacity / 32)
+    // outputs
+    uint8_t *wal;
+    uint32_t *rec_group;
+    uint64_t *rec_slot;
+    uint32_t *rec_frame;
+    uint32_t *verdict;
+    uint32_t *status;
+};
+
+// PeerMessage::Msg{Prepare{trigger_slot, ballot}}, then the window filters; a Prepare from `me` is malformed
+// (check_leader debug-asserts peer != me)
+__device__ __forceinline__ PrepHdr decode_prepare(const PrepArgs &A, uint64_t i) {
+    PrepHdr h{};
+    h.kind = SS_FRAME_KIND_MALFORMED;
+    const uint32_t grp = A.frame_group[i];
+    const uint64_t off = A.frame_off[i];
+    if (grp >= A.G || off > A.buf_len || A.buf_len - off < 8u) return h;
+    const uint8_t *fr = A.buf + off;
+    uint64_t len = 0;
+    for (int k = 0; k < 8; ++k) len = (len << 8) | fr[k];
+    if (len > A.buf_len - off - 8u || len > kMaxFrameBody) return h;
+    const uint8_t *b = fr + 8;
+    uint64_t n = 0, v = 0, trig = 0, bal = 0;
+    uint32_t c;
+#define SS_GETP(dst) do { if (!(c = wv_get(b + n, len - n, (dst)))) return h; n += c; } while (0)
+    SS_GETP(v);
+    if (v != 0u) {
+        if (v < kVariantLimit) h.kind = 0x80000000u | static_cast<uint32_t>(v);
+        return h;
+    }
+    SS_GETP(v);
+    if (v != A.variant) {
+        if (v < kVariantLimit) h.kind = static_cast<uint32_t>(v);
+        return h;
+    }
+    SS_GETP(trig);
+    SS_GETP(bal);
+#undef SS_GETP
+    if (n != len || A.frame_peer[i] == A.me) return h;
+    h.trigger = trig;
+    h.ballot = bal;
+    const uint64_t base = A.window_base[grp];
+    h.kind = trig < base ? SS_ACCEPT_VERDICT_STALE_SLOT : trig - base >= 64u ? SS_ACCEPT_VERDICT_BEYOND_WINDOW : kPending;
+    return h;
+}
+
+// 1. a thread per frame
+__global__ void __launch_bounds__(kAccThreads) prepare_header_kernel(const __grid_constant__ PrepArgs A) {
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; i < A.n; i += stride) {
+        A.hdr[i] = decode_prepare(A, i);
+        A.cnt[i] = 0u;
+        const uint32_t grp = A.frame_group[i];
+        A.key_in[i] = grp < A.G ? grp : static_cast<uint32_t>(A.G);
+        A.idx_in[i] = static_cast<uint32_t>(i);
+    }
+}
+
+// window positions [lo, hi] (0 <= lo <= hi < 64) as a ring word of a window at base
+__device__ __forceinline__ uint64_t window_range_ring(uint64_t lo, uint64_t hi, uint64_t base) {
+    const uint64_t w = hi - lo + 1u;
+    return window_to_ring((w == 64u ? ~0ull : (1ull << w) - 1u) << lo, static_cast<uint32_t>(base & 63u));
+}
+
+// 2. a thread per group segment, frames in frame order: check_leader, then endprep_slot = max(the last window position
+//    that is not null, trigger_slot) over the state as the earlier frames of the call left it; [trigger, endprep]
+//    becomes Preparing.  Only the per-frame verdict, endprep and record count are written.
+__global__ void __launch_bounds__(kAccThreads) prepare_walk_kernel(const __grid_constant__ PrepArgs A) {
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
+    for (uint64_t t = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; t < A.n; t += stride) {
+        if (t != 0u && A.key[t] == A.key[t - 1]) continue;
+        const uint32_t g = A.key[t];
+        if (g >= A.G) continue;
+        const uint64_t base = A.window_base[g];
+        const uint32_t r = static_cast<uint32_t>(base & 63u);
+        uint64_t bmax = A.bal_max_seen[g], prep = A.preparing[g], acc = A.accepting[g], com = A.committed[g];
+        for (uint64_t k = t; k < A.n && A.key[k] == g; ++k) {
+            const uint32_t i = A.idx[k];
+            if (A.hdr[i].kind != kPending) continue;
+            const uint64_t bal = A.hdr[i].ballot, tw = A.hdr[i].trigger - base;
+            if (bal < bmax) {
+                A.hdr[i].kind = SS_ACCEPT_VERDICT_STALE_BALLOT;
+                continue;
+            }
+            bmax = bal;
+            const uint64_t live = ring_to_window(prep | acc | com, r);       // rposition(status > Null)
+            const uint64_t hi = live != 0u ? 63u - static_cast<uint64_t>(__clzll(static_cast<long long>(live))) : 0u;
+            const uint64_t ew = hi > tw ? hi : tw;
+            const uint64_t m = window_range_ring(tw, ew, base);
+            prep |= m;
+            acc &= ~m;
+            com &= ~m;
+            A.hdr[i].kind = SS_ACCEPT_VERDICT_ACCEPTED;                       // subject to capacity
+            A.hdr[i].endprep = base + ew;
+            A.cnt[i] = ew - tw + 1u;
+        }
+    }
+}
+
+// 3. a thread per group segment, last frame first.  cnt holds the scanned record numbers, so frame j's records end at
+//    cnt[j + 1] (the total for the last frame), monotone in frame order: the first frame whose records end past the
+//    capacity is found by bisection, and it and every later frame whose verdict came from the replay get WAL_FULL.
+//    The applied frames are then a prefix in frame order, so each group's applied frames are a prefix of its frames and
+//    the ranges the walk computed for them stay exact.
+__global__ void __launch_bounds__(kAccThreads) prepare_apply_kernel(const __grid_constant__ PrepArgs A) {
+    const uint64_t total = A.totals[0];
+    if (blockIdx.x == 0u && threadIdx.x == 0u) A.totals[1] = total * 32u;
+    uint64_t cut = A.n;
+    if (total > A.cap) {
+        uint64_t lo = 0, hi = A.n;
+        while (lo < hi) {
+            const uint64_t mid = (lo + hi) >> 1, end = mid + 1u < A.n ? A.cnt[mid + 1u] : total;
+            if (end > A.cap) hi = mid; else lo = mid + 1u;
+        }
+        cut = lo;
+    }
+    bool full = false;
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
+    for (uint64_t t = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; t < A.n; t += stride) {
+        if (t != 0u && A.key[t] == A.key[t - 1]) continue;
+        const uint32_t g = A.key[t];
+        const bool known = g < A.G;
+        uint64_t e = t + 1u;
+        while (e < A.n && A.key[e] == g) ++e;
+        const uint64_t base = known ? A.window_base[g] : 0u;
+        const uint64_t null0 = known ? ~(A.preparing[g] | A.accepting[g] | A.committed[g]) : 0u;
+        uint64_t seen = 0u, mx = known ? A.bal_max_seen[g] : 0u;
+        for (uint64_t k = e; k-- > t;) {
+            const uint32_t i = A.idx[k];
+            uint32_t kind = A.hdr[i].kind;
+            if ((kind == SS_ACCEPT_VERDICT_ACCEPTED || kind == SS_ACCEPT_VERDICT_STALE_BALLOT) && i >= cut) {
+                kind = SS_ACCEPT_VERDICT_WAL_FULL;
+                full = true;
+            }
+            if (kind == SS_ACCEPT_VERDICT_ACCEPTED) {
+                const PrepHdr h = A.hdr[i];
+                mx = h.ballot > mx ? h.ballot : mx;
+                const uint64_t m = window_range_ring(h.trigger - base, h.endprep - base, base), def = m & ~seen;
+                seen |= m;
+                A.hdr[i].define = def;
+                A.hdr[i].fresh = def & null0;
+            }
+            A.verdict[i] = kind;
+        }
+        if (known) {
+            A.preparing[g] |= seen;                                           // Status::Preparing, also over Committed
+            A.accepting[g] &= ~seen;
+            A.committed[g] &= ~seen;
+            A.bal_max_seen[g] = mx;
+        }
+    }
+    if (full) atomicOr(A.status, SS_DEV_STATUS_FRAME_OVERFLOW);
+}
+
+// 4. a warp per applied frame: its WalEntry::PrepareBal{slot, ballot} cells (8-byte big-endian length + bincode, zero to
+//    32 bytes) and, at the positions it defines, inst.bal, replica_bk and -- for a position that was null -- voted None
+__global__ void __launch_bounds__(kAccThreads) prepare_write_kernel(const __grid_constant__ PrepArgs A) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint64_t warp = (static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x) >> 5;
+    const uint64_t nwarps = (static_cast<uint64_t>(gridDim.x) * kAccThreads) >> 5;
+    for (uint64_t i = warp; i < A.n; i += nwarps) {
+        if (A.verdict[i] != SS_ACCEPT_VERDICT_ACCEPTED) continue;
+        const PrepHdr h = A.hdr[i];
+        const uint32_t g = A.frame_group[i];
+        const uint64_t first = A.cnt[i], count = h.endprep - h.trigger + 1u;
+        for (uint64_t q = lane; q < count; q += 32u) {
+            const uint64_t k = first + q, slot = h.trigger + q;
+            uint8_t cell[32];
+#pragma unroll
+            for (int b = 0; b < 32; ++b) cell[b] = 0u;
+            uint32_t m = 8u;
+            m += wv_put(cell + m, A.wal_variant);
+            m += wv_put(cell + m, slot);
+            m += wv_put(cell + m, h.ballot);
+            cell[7] = static_cast<uint8_t>(m - 8u);                          // the body is < 256 bytes
+            uint4 lo, hi;
+            memcpy(&lo, cell, 16);
+            memcpy(&hi, cell + 16, 16);
+            uint4 *dst = reinterpret_cast<uint4 *>(A.wal + k * 32u);
+            dst[0] = lo;
+            dst[1] = hi;
+            A.rec_group[k] = g;
+            A.rec_slot[k] = slot;
+            A.rec_frame[k] = static_cast<uint32_t>(i);
+        }
+        for (uint32_t p = lane; p < 64u; p += 32u) {
+            if (!((h.define >> p) & 1u)) continue;
+            const uint64_t at = static_cast<uint64_t>(g) * 64u + p;
+            A.inst_bal[at] = h.ballot;
+            A.source[at] = A.frame_peer[i];
+            A.prep_trigger[at] = h.trigger;
+            A.prep_span[at] = static_cast<uint8_t>(h.endprep - h.trigger);
+            if ((h.fresh >> p) & 1u) {                                        // a fresh null_instance(): voted (0, null)
+                A.voted_bal[at] = 0u;
+                A.voted_mask[at] = 0u;
+            }
+        }
+    }
+}
+
+// ---- prepare replies ----------------------------------------------------------------------------------------------
+struct PrepReplyArgs {
+    const uint32_t *rec_group;
+    const uint64_t *rec_slot;
+    uint64_t n, G;
+    uint32_t d, T, variant;
+    const uint64_t *window_base, *preparing, *accepting, *committed, *inst_bal, *voted_bal, *prep_trigger, *shard_addr;
+    const uint32_t *voted_mask, *held, *data_len;
+    const uint8_t *source, *prep_span;
+    uint8_t *out;
+    uint64_t out_cap;
+    uint64_t *reply_off, *reply_len;
+    uint8_t *reply_dst;
+    uint32_t *status;
+};
+
+// PrepareReply bytes of record k (0: no reply), *at its instance
+__device__ __forceinline__ uint64_t prep_reply_bytes(const PrepReplyArgs &A, uint64_t k, uint64_t *at) {
+    const uint32_t g = A.rec_group[k];
+    if (g >= A.G) return 0u;
+    const uint64_t s = A.rec_slot[k], base = A.window_base[g];
+    if (s < base || s - base >= 64u) return 0u;
+    const uint32_t p = static_cast<uint32_t>(s & 63u);
+    if (!(((A.preparing[g] | A.accepting[g] | A.committed[g]) >> p) & 1u)) return 0u;   // null: no replica_bk
+    *at = static_cast<uint64_t>(g) * 64u + p;
+    const uint64_t trig = A.prep_trigger[*at], vb = A.voted_bal[*at];
+    uint64_t len = 9u + wv_len(A.variant) + wv_len(s) + wv_len(trig) + wv_len(trig + A.prep_span[*at]) + wv_len(A.inst_bal[*at]) + 1u;
+    if (vb > 0u) len += wv_len(vb) + codeword_bytes(A.d, A.T, A.data_len[*at], A.voted_mask[*at]);
+    return len;
+}
+
+// 1. a thread per record: the reply's bytes and its 16-byte region
+__global__ void __launch_bounds__(kAccThreads) prep_reply_size_kernel(const __grid_constant__ PrepReplyArgs A) {
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
+    for (uint64_t k = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; k < A.n; k += stride) {
+        uint64_t at = 0;
+        const uint64_t len = prep_reply_bytes(A, k, &at);
+        A.reply_len[k] = len;
+        A.reply_off[k] = round16(len);
+    }
+}
+
+// 2. a warp per record: capacity, then PeerMessage::Msg{PrepareReply{slot, trigger_slot, endprep_slot, ballot, voted}}
+__global__ void __launch_bounds__(kAccThreads) prep_reply_copy_kernel(const __grid_constant__ PrepReplyArgs A) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint64_t warp = (static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x) >> 5;
+    const uint64_t nwarps = (static_cast<uint64_t>(gridDim.x) * kAccThreads) >> 5;
+    bool full = false;
+    for (uint64_t k = warp; k < A.n; k += nwarps) {
+        const uint64_t len = A.reply_len[k], off = A.reply_off[k];
+        if (len == 0u || off > A.out_cap || round16(len) > A.out_cap - off) {
+            full |= len != 0u;
+            if (lane == 0u) {
+                A.reply_off[k] = ~0ull;
+                A.reply_dst[k] = 0xffu;
+            }
+            continue;
+        }
+        uint64_t at = 0;
+        prep_reply_bytes(A, k, &at);
+        const uint64_t s = A.rec_slot[k], trig = A.prep_trigger[at], vb = A.voted_bal[at];
+        uint8_t *dst = A.out + off;
+        uint64_t q = 8u;
+        q += wv_len(0u) + wv_len(A.variant) + wv_len(s) + wv_len(trig) + wv_len(trig + A.prep_span[at]) + wv_len(A.inst_bal[at]) + 1u;
+        if (vb > 0u) q += wv_len(vb);
+        if (lane == 0u) {
+            const uint64_t body = len - 8u;
+            for (int b = 0; b < 8; ++b) dst[b] = static_cast<uint8_t>(body >> (8 * (7 - b)));
+            uint64_t m = 8u;
+            m += wv_put(dst + m, 0u);                                           // PeerMessage::Msg
+            m += wv_put(dst + m, A.variant);
+            m += wv_put(dst + m, s);
+            m += wv_put(dst + m, trig);
+            m += wv_put(dst + m, trig + A.prep_span[at]);
+            m += wv_put(dst + m, A.inst_bal[at]);
+            dst[m++] = vb > 0u ? 1u : 0u;                                       // voted: Option
+            if (vb > 0u) wv_put(dst + m, vb);
+            A.reply_dst[k] = A.source[at];
+        }
+        if (vb > 0u)
+            warp_put_codeword(dst + q, A.d, A.T, A.data_len[at], A.voted_mask[at], A.held[at],
+                              reinterpret_cast<const uint8_t *>(A.shard_addr[at]), lane);
+    }
+    if (full && lane == 0u) atomicOr(A.status, SS_DEV_STATUS_FRAME_OVERFLOW);
+}
+
 static inline uint32_t acc_grid(ss_ctx *ctx, uint64_t items, uint32_t per_cta) {
     uint64_t ctas = (items + per_cta - 1) / per_cta;
     const uint64_t cap = static_cast<uint64_t>(ctx->sm_count) * 8ull * 8ull;
@@ -1222,16 +1584,17 @@ static int ensure_scratch(ss_acceptor *a, uint64_t n) {
     if (n <= a->cap_frames) return SS_OK;
     ss_ctx *ctx = a->ctx;
     SS_CUDA(cudaStreamSynchronize(ctx->stream));
-    void *old[] = {a->hdr, a->keys, a->idx, a->partials, a->sort_tmp};
+    void *old[] = {a->hdr, a->keys, a->idx, a->partials, a->fcnt, a->sort_tmp};
     for (void *b : old)
         if (b) cudaFree(b);
-    a->hdr = nullptr; a->keys = nullptr; a->idx = nullptr; a->partials = nullptr; a->sort_tmp = nullptr;
+    a->hdr = nullptr; a->keys = nullptr; a->idx = nullptr; a->partials = nullptr; a->fcnt = nullptr; a->sort_tmp = nullptr;
     a->cap_frames = 0;
-    // the header pass writes hdr, key_in and idx_in of every frame, the sort the rest, the scan its partials
+    // the header pass writes hdr, key_in and idx_in (and fcnt) of every frame, the sort the rest, the scan its partials
     SS_TRY(acc_alloc(ctx, &a->hdr, n, false));
     SS_TRY(acc_alloc(ctx, &a->keys, 2 * n, false));
     SS_TRY(acc_alloc(ctx, &a->idx, 2 * n, false));
     SS_TRY(acc_alloc(ctx, &a->partials, scan_tiles(n), false));
+    SS_TRY(acc_alloc(ctx, &a->fcnt, n, false));
     size_t bytes = 0;
     SS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, a->keys, a->keys + n, a->idx, a->idx + n, static_cast<int>(n), 0,
                                             key_bits(a->G), ctx->stream));
@@ -1254,8 +1617,9 @@ int ss_acceptor_destroy(ss_acceptor *a) {
         cudaStreamSynchronize(a->ctx->stream);
     }
     void *bufs[] = {a->window_base, a->bal_max_seen, a->inst_bal, a->accepting, a->shard_addr, a->held, a->data_len, a->assignment,
-                    a->source, a->committed, a->commit_bar, a->exec_bar, a->matrix, a->ex_cnt, a->ex_bytes, a->ex_partials,
-                    a->ex_n, a->hdr, a->keys, a->idx, a->partials, a->sort_tmp, a->totals};
+                    a->source, a->committed, a->commit_bar, a->exec_bar, a->preparing, a->voted_bal, a->voted_mask,
+                    a->prep_trigger, a->prep_span, a->matrix, a->ex_cnt, a->ex_bytes, a->ex_partials, a->ex_n, a->hdr,
+                    a->keys, a->idx, a->partials, a->fcnt, a->sort_tmp, a->totals};
     for (void *b : bufs)
         if (b) cudaFree(b);
     if (a->ctx) ctx_release(a->ctx);
@@ -1294,6 +1658,9 @@ int ss_acceptor_create(ss_ctx *ctx, const ss_acceptor_config *cfg, uint64_t G, s
         (rc = acc_alloc(ctx, &a->data_len, G * 64)) || (rc = acc_alloc(ctx, &a->source, G * 64)) || (rc = acc_alloc(ctx, &a->totals, 2)) ||
         (cfg->protocol == SS_PROTO_CROSSWORD && (rc = acc_alloc(ctx, &a->assignment, G * 64))) ||
         (rc = acc_alloc(ctx, &a->committed, G)) || (rc = acc_alloc(ctx, &a->commit_bar, G)) || (rc = acc_alloc(ctx, &a->exec_bar, G)) ||
+        (rc = acc_alloc(ctx, &a->preparing, G)) || (rc = acc_alloc(ctx, &a->voted_bal, G * 64)) ||
+        (rc = acc_alloc(ctx, &a->voted_mask, G * 64)) || (rc = acc_alloc(ctx, &a->prep_trigger, G * 64)) ||
+        (rc = acc_alloc(ctx, &a->prep_span, G * 64)) ||
         (rc = acc_alloc(ctx, &a->ex_cnt, G, false)) || (rc = acc_alloc(ctx, &a->ex_bytes, G, false)) ||
         (rc = acc_alloc(ctx, &a->ex_partials, scan_tiles(G), false)) || (rc = acc_alloc(ctx, &a->ex_n, 1, false)) ||
         (rc = acc_alloc(ctx, &a->matrix, size_t(cfg->total_shards) * cfg->data_shards, false))) {
@@ -1394,7 +1761,7 @@ int ss_acceptor_advance(ss_acceptor *a, const uint64_t *upto) {
     ss_ctx *ctx = a->ctx;
     SS_TRY(ctx_bind(ctx));
     acceptor_advance_kernel<<<acc_grid(ctx, a->G, kAccThreads), kAccThreads, 0, ctx->stream>>>(upto, a->G, a->window_base, a->accepting,
-                                                                                               a->committed);
+                                                                                               a->committed, a->preparing);
     return launched(ctx);
 }
 
@@ -1426,6 +1793,8 @@ int ss_acceptor_accept(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, con
     A.window_base = a->window_base; A.bal_max_seen = a->bal_max_seen; A.inst_bal = a->inst_bal; A.accepting = a->accepting;
     A.shard_addr = a->shard_addr; A.held = a->held; A.data_len = a->data_len; A.assignment = a->assignment; A.source = a->source;
     A.committed = a->committed;
+    A.preparing = a->preparing; A.voted_bal = a->voted_bal; A.voted_mask = a->voted_mask; A.prep_trigger = a->prep_trigger;
+    A.prep_span = a->prep_span;
     A.hdr = a->hdr; A.key_in = a->keys; A.idx_in = a->idx; A.key = a->keys + n; A.idx = a->idx + n;
     A.store = store; A.store_cap = store_capacity; A.store_off = store_off;
     A.wal = wal; A.wal_cap = wal_capacity; A.wal_off = wal_off; A.wal_len = wal_len;
@@ -1517,6 +1886,90 @@ int ss_acceptor_absorb(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, con
     SS_TRY(launched(ctx));
     SS_TRY(launch_exclusive_scan_u64(ctx, a->ex_bytes, a->G, a->ex_partials, total != nullptr ? total : a->totals));
     absorb_copy_kernel<<<grid_w, kAccThreads, 0, ctx->stream>>>(R);
+    return launched(ctx);
+}
+
+int ss_acceptor_prepare_view_get(ss_acceptor *a, ss_acceptor_prepare_view *v) {
+    if (a == nullptr || v == nullptr) return set_error(SS_ERR_INVALID_ARG, "null argument");
+    memset(v, 0, sizeof(*v));
+    v->n_groups = a->G;
+    v->preparing = a->preparing; v->voted_bal = a->voted_bal; v->voted_mask = a->voted_mask;
+    v->prep_trigger = a->prep_trigger; v->prep_span = a->prep_span;
+    return SS_OK;
+}
+
+int ss_acceptor_prepare(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
+                        const uint8_t *frame_peer, uint64_t n, uint32_t prepare_variant, uint32_t wal_variant, uint8_t *wal,
+                        uint64_t wal_capacity, uint32_t *rec_group, uint64_t *rec_slot, uint32_t *rec_frame, uint64_t rec_capacity,
+                        uint32_t *verdict, uint64_t *totals) {
+    if (a == nullptr) return set_error(SS_ERR_INVALID_ARG, "null acceptor");
+    if (wal_variant >= kVariantLimit) return set_error(SS_ERR_INVALID_ARG, "wal_variant must be below 2^16");
+    ss_ctx *ctx = a->ctx;
+    SS_TRY(ctx_bind(ctx));
+    if (n == 0) {
+        if (totals != nullptr) SS_CUDA(cudaMemsetAsync(totals, 0, 16, ctx->stream));
+        return SS_OK;
+    }
+    if (!buf || !frame_off || !frame_group || !frame_peer || !wal || !rec_group || !rec_slot || !rec_frame || !verdict)
+        return set_error(SS_ERR_INVALID_ARG, "null buffer");
+    if (reinterpret_cast<uintptr_t>(wal) & 15u) return set_error(SS_ERR_INVALID_ARG, "wal must be 16-byte aligned");
+    if (n > 0x7fffffffull) return set_error(SS_ERR_INVALID_ARG, "at most 2^31 - 1 frames per call");
+    SS_TRY(ensure_scratch(a, n));
+    PrepArgs P{};
+    P.buf = buf; P.buf_len = buf_len; P.frame_off = frame_off; P.frame_group = frame_group; P.frame_peer = frame_peer;
+    P.n = n; P.G = a->G; P.me = a->cfg.me; P.variant = prepare_variant; P.wal_variant = wal_variant;
+    P.window_base = a->window_base; P.bal_max_seen = a->bal_max_seen; P.inst_bal = a->inst_bal; P.accepting = a->accepting;
+    P.committed = a->committed; P.preparing = a->preparing; P.voted_bal = a->voted_bal; P.prep_trigger = a->prep_trigger;
+    P.voted_mask = a->voted_mask; P.source = a->source; P.prep_span = a->prep_span;
+    P.hdr = reinterpret_cast<PrepHdr *>(a->hdr);
+    P.key_in = a->keys; P.idx_in = a->idx; P.key = a->keys + n; P.idx = a->idx + n;
+    P.cnt = a->fcnt; P.totals = totals != nullptr ? totals : a->totals;
+    const uint64_t wal_cells = wal_capacity / 32u;
+    P.cap = rec_capacity < wal_cells ? rec_capacity : wal_cells;
+    P.wal = wal; P.rec_group = rec_group; P.rec_slot = rec_slot; P.rec_frame = rec_frame; P.verdict = verdict;
+    P.status = ctx->dev_status;
+    const uint32_t grid_t = acc_grid(ctx, n, kAccThreads);
+    prepare_header_kernel<<<grid_t, kAccThreads, 0, ctx->stream>>>(P);
+    SS_TRY(launched(ctx));
+    size_t bytes = a->sort_tmp_bytes;
+    SS_CUDA(cub::DeviceRadixSort::SortPairs(a->sort_tmp, bytes, a->keys, a->keys + n, a->idx, a->idx + n, static_cast<int>(n), 0,
+                                            key_bits(a->G), ctx->stream));
+    SS_TRY(launched(ctx));
+    prepare_walk_kernel<<<grid_t, kAccThreads, 0, ctx->stream>>>(P);
+    SS_TRY(launched(ctx));
+    SS_TRY(launch_exclusive_scan_u64(ctx, a->fcnt, n, a->partials, P.totals));
+    prepare_apply_kernel<<<grid_t, kAccThreads, 0, ctx->stream>>>(P);
+    SS_TRY(launched(ctx));
+    prepare_write_kernel<<<acc_grid(ctx, n, kAccThreads / 32), kAccThreads, 0, ctx->stream>>>(P);
+    return launched(ctx);
+}
+
+int ss_acceptor_prepare_reply(ss_acceptor *a, const uint32_t *rec_group, const uint64_t *rec_slot, uint64_t n, uint32_t reply_variant,
+                              uint8_t *out, uint64_t out_capacity, uint64_t *reply_off, uint64_t *reply_len, uint8_t *reply_dst,
+                              uint64_t *total) {
+    if (a == nullptr) return set_error(SS_ERR_INVALID_ARG, "null acceptor");
+    ss_ctx *ctx = a->ctx;
+    SS_TRY(ctx_bind(ctx));
+    if (n == 0) {
+        if (total != nullptr) SS_CUDA(cudaMemsetAsync(total, 0, 8, ctx->stream));
+        return SS_OK;
+    }
+    if (!rec_group || !rec_slot || !out || !reply_off || !reply_len || !reply_dst) return set_error(SS_ERR_INVALID_ARG, "null buffer");
+    if (reinterpret_cast<uintptr_t>(out) & 15u) return set_error(SS_ERR_INVALID_ARG, "out must be 16-byte aligned");
+    if (n > 0x7fffffffull) return set_error(SS_ERR_INVALID_ARG, "at most 2^31 - 1 records per call");
+    SS_TRY(ensure_scratch(a, n));
+    PrepReplyArgs R{};
+    R.rec_group = rec_group; R.rec_slot = rec_slot; R.n = n; R.G = a->G;
+    R.d = a->cfg.data_shards; R.T = a->cfg.total_shards; R.variant = reply_variant;
+    R.window_base = a->window_base; R.preparing = a->preparing; R.accepting = a->accepting; R.committed = a->committed;
+    R.inst_bal = a->inst_bal; R.voted_bal = a->voted_bal; R.prep_trigger = a->prep_trigger; R.shard_addr = a->shard_addr;
+    R.voted_mask = a->voted_mask; R.held = a->held; R.data_len = a->data_len; R.source = a->source; R.prep_span = a->prep_span;
+    R.out = out; R.out_cap = out_capacity; R.reply_off = reply_off; R.reply_len = reply_len; R.reply_dst = reply_dst;
+    R.status = ctx->dev_status;
+    prep_reply_size_kernel<<<acc_grid(ctx, n, kAccThreads), kAccThreads, 0, ctx->stream>>>(R);
+    SS_TRY(launched(ctx));
+    SS_TRY(launch_exclusive_scan_u64(ctx, reply_off, n, a->partials, total != nullptr ? total : a->totals));
+    prep_reply_copy_kernel<<<acc_grid(ctx, n, kExecWarps), kAccThreads, 0, ctx->stream>>>(R);
     return launched(ctx);
 }
 

@@ -12,6 +12,8 @@
 //                               both share frame_layout / frame_write with frame_pack_kernel
 //   accept_reply_parse_kernel   AcceptReply frames -> (group, window slot, peer, ballot) records for ss_ack_ingest_dev /
 //                               ss_engine_ingest (rspaxos/mod.rs:290-291, crossword/mod.rs:365-373)
+//   prepare_reply_parse_kernel  PrepareReply frames -> (slot, trigger, endprep, ballot, vote ballot / shards) records for
+//                               the new leader's ss_prepare_merge_dev (rspaxos/messages.rs:88-196)
 //   wal_commit_pack_kernel      newly committed instances -> WalEntry::CommitSlot{slot} records (rspaxos/mod.rs:231)
 //   reconstruct_serve_kernel    Reconstruct serving: reply shards = held & flip(exclude) per requested instance, packed
 //                               (crossword/messages.rs:577-632, rspaxos/messages.rs:468-517)
@@ -264,6 +266,86 @@ __global__ void __launch_bounds__(kWireThreads) accept_reply_parse_kernel(const 
     }
 }
 
+struct PrepParseArgs {
+    const uint8_t *buf;
+    uint64_t buf_len;
+    const uint64_t *frame_off;
+    uint64_t n_frames;
+    uint32_t d, T, reply_variant;
+    ss_prepare_reply_rec *rec;
+};
+
+// a thread per frame: PrepareReply{slot, trigger_slot, endprep_slot, ballot, voted} with the codeword checked as
+// ss_acceptor_absorb checks one; the shards stay where they are (shards_at)
+__global__ void __launch_bounds__(kWireThreads) prepare_reply_parse_kernel(const __grid_constant__ PrepParseArgs A) {
+    constexpr uint64_t kVariantLimit = 1u << 16;
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kWireThreads;
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kWireThreads + threadIdx.x; i < A.n_frames; i += stride) {
+        ss_prepare_reply_rec r{};
+        r.kind = SS_FRAME_KIND_MALFORMED;
+        r.shards_at = ~0ull;
+        const uint64_t off = A.frame_off[i];
+        do {
+            if (off > A.buf_len || A.buf_len - off < 8u) break;
+            const uint8_t *fr = A.buf + off;
+            uint64_t len = 0;
+            for (int b = 0; b < 8; ++b) len = (len << 8) | fr[b];
+            if (len > A.buf_len - off - 8u) break;
+            const uint8_t *b = fr + 8;
+            uint64_t n = 0, v = 0, f[4], vb = 0, dl = 0, sl = 0, at = ~0ull;
+            uint32_t c, mask = 0;
+            bool ok = true;
+#define SS_GETR(dst) if (!(c = wv_get(b + n, len - n, (dst)))) break; n += c
+            SS_GETR(v);
+            if (v != 0u) { if (v < kVariantLimit) r.kind = 0x80000000u | static_cast<uint32_t>(v); break; }
+            SS_GETR(v);
+            if (v != A.reply_variant) { if (v < kVariantLimit) r.kind = static_cast<uint32_t>(v); break; }
+            SS_GETR(f[0]);
+            SS_GETR(f[1]);
+            SS_GETR(f[2]);
+            SS_GETR(f[3]);
+            if (n >= len) break;
+            const uint8_t tag = b[n++];
+            if (tag == 1u) {
+                SS_GETR(vb);
+                if (len - n < 2u || b[n] != A.d || b[n + 1] != A.T - A.d) break;
+                n += 2;
+                SS_GETR(dl);
+                SS_GETR(sl);
+                SS_GETR(v);
+                if (dl > 0xffffffffull || v != A.T || sl != (dl + A.d - 1u) / A.d) break;
+                at = off + 8u + n;
+                for (uint32_t j = 0; j < A.T && ok; ++j) {
+                    if (n >= len) { ok = false; break; }
+                    const uint8_t t = b[n++];
+                    if (t == 0u) continue;
+                    if (t != 1u || !(c = wv_get(b + n, len - n, v))) { ok = false; break; }
+                    n += c;
+                    if (v != sl || len - n < sl) { ok = false; break; }
+                    mask |= 1u << j;
+                    n += sl;
+                }
+                if (!ok || n >= len) break;
+                const uint8_t dc = b[n++];                                            // data_copy
+                if (dc == 1u) {
+                    if (len - n < dl) break;
+                    n += dl;
+                } else if (dc != 0u) {
+                    break;
+                }
+            } else if (tag != 0u) {
+                break;
+            }
+#undef SS_GETR
+            if (n != len) break;
+            r.slot = f[0]; r.trigger_slot = f[1]; r.endprep_slot = f[2]; r.ballot = f[3];
+            r.vote_bal = vb; r.vote_mask = mask; r.data_len = static_cast<uint32_t>(dl); r.shards_at = at;
+            r.kind = A.reply_variant;
+        } while (false);
+        A.rec[i] = r;
+    }
+}
+
 // newly committed instances -> CommitSlot records (24-byte cells: the record is at most 8 + 1 + 9 bytes)
 __global__ void __launch_bounds__(kWireThreads)
 wal_commit_pack_kernel(const uint64_t *__restrict__ newly, const uint64_t *__restrict__ window_base, uint64_t G, uint32_t variant,
@@ -435,6 +517,21 @@ int ss_accept_reply_parse_dev(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len,
     A.window_base = window_base; A.n_frames = n_frames; A.G = n_groups; A.reply_variant = reply_variant; A.with_size = with_size ? 1u : 0u;
     A.rec_group = rec_group; A.rec_slot = rec_slot; A.rec_peer = rec_peer; A.rec_ballot = rec_ballot; A.rec_kind = rec_kind;
     accept_reply_parse_kernel<<<wire_grid(ctx, n_frames, kWireThreads), kWireThreads, 0, ctx->stream>>>(A);
+    return launched(ctx);
+}
+
+int ss_prepare_reply_parse_dev(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, uint64_t n_frames,
+                               uint32_t data_shards, uint32_t total_shards, uint32_t reply_variant, ss_prepare_reply_rec *rec) {
+    if (ctx == nullptr) return set_error(SS_ERR_INVALID_ARG, "null context");
+    if (data_shards == 0 || data_shards > total_shards || total_shards > 32)
+        return set_error(SS_ERR_INVALID_ARG, "shard counts must satisfy 1 <= d <= T <= 32 (d=%u, T=%u)", data_shards, total_shards);
+    SS_TRY(ctx_bind(ctx));
+    if (n_frames == 0) return SS_OK;
+    if (!buf || !frame_off || !rec) return set_error(SS_ERR_INVALID_ARG, "null buffer");
+    PrepParseArgs A;
+    A.buf = buf; A.buf_len = buf_len; A.frame_off = frame_off; A.n_frames = n_frames;
+    A.d = data_shards; A.T = total_shards; A.reply_variant = reply_variant; A.rec = rec;
+    prepare_reply_parse_kernel<<<wire_grid(ctx, n_frames, kWireThreads), kWireThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
 }
 

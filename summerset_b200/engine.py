@@ -20,6 +20,9 @@ torch tensors (zero-copy views) so tests can read results and install state; it 
         heartbeat(group, peer, ballot, commit_bar, exec_bar)   heard_heartbeat's commit walk (rspaxos/leadership.rs:222-311)
         execute(out, rec_capacity)          handle_logged_commit_slot's execution walk (rspaxos/durability.rs:125-186):
                                             request batches decoded from the held shards
+        prepare(buf, ..., wal, rec_capacity)   handle_msg_prepare (rspaxos/messages.rs:13-84): PrepareBal records
+        prepare_reply(rec_group, rec_slot, out)   handle_logged_prepare_bal's follower branch: PrepareReply frames
+    prepare_reply_parse(ctx, buf, frame_off, d, T)   the new leader's side: PrepareReply frames -> vote records
     RaftEngine(ctx, G, population[, fault_tolerance, craft])
         append(n_new) / on_append_replies(records) / tick()      raft/messages.rs:243-309, craft/messages.rs:300-308
 """
@@ -242,6 +245,13 @@ class Acceptor:
         self.committed = t(cv.committed, (G,), "<i8", torch.int64)
         self.commit_bar = t(cv.commit_bar, (G,), "<i8", torch.int64)
         self.exec_bar = t(cv.exec_bar, (G,), "<i8", torch.int64)
+        pv = self.prepare_view = _lib.AcceptorPrepareView()
+        check(self.lib.ss_acceptor_prepare_view_get(self.h, C.byref(pv)))
+        self.preparing = t(pv.preparing, (G,), "<i8", torch.int64)
+        self.voted_bal = t(pv.voted_bal, (G * 64,), "<i8", torch.int64)
+        self.voted_mask = t(pv.voted_mask, (G * 64,), "<i4", torch.int32)
+        self.prep_trigger = t(pv.prep_trigger, (G * 64,), "<i8", torch.int64)
+        self.prep_span = t(pv.prep_span, (G * 64,), "|u1", torch.uint8)
 
     def accept(self, buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor, frame_peer: torch.Tensor,
                store: torch.Tensor, wal: torch.Tensor, store_capacity: Optional[int] = None, wal_capacity: Optional[int] = None) -> dict:
@@ -335,6 +345,41 @@ class Acceptor:
                                           p(res["verdict"]), p(res["total"])))
         return res
 
+    def prepare(self, buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor, frame_peer: torch.Tensor,
+                wal: torch.Tensor, rec_capacity: int, wal_capacity: Optional[int] = None, prepare_variant: int = 0,
+                wal_variant: int = 0) -> dict:
+        """Takes Prepare frames (handle_msg_prepare): the covered slots become Preparing at the frame's ballot.  wal: uint8,
+        16-byte aligned, one 32-byte PrepareBal cell per record.  Returns device tensors rec_group (int32), rec_slot (int64),
+        rec_frame (int32), each [rec_capacity], verdict (int32 [n]) and totals (int64 [2]: records and WAL bytes asked for)."""
+        assert buf.dtype == torch.uint8 and frame_off.dtype == torch.int64 and frame_group.dtype == torch.int32
+        assert frame_peer.dtype == torch.uint8 and wal.dtype == torch.uint8
+        n, dev = frame_off.numel(), buf.device
+        cap = max(rec_capacity, 1)
+        res = dict(rec_group=torch.empty(cap, dtype=torch.int32, device=dev), rec_slot=torch.empty(cap, dtype=torch.int64, device=dev),
+                   rec_frame=torch.empty(cap, dtype=torch.int32, device=dev), verdict=torch.empty(n, dtype=torch.int32, device=dev),
+                   totals=torch.empty(2, dtype=torch.int64, device=dev))
+        p = lambda x: x.data_ptr()
+        check(self.lib.ss_acceptor_prepare(self.h, p(buf), buf.numel(), p(frame_off), p(frame_group), p(frame_peer), n, prepare_variant,
+                                           wal_variant, p(wal), wal.numel() if wal_capacity is None else wal_capacity, p(res["rec_group"]),
+                                           p(res["rec_slot"]), p(res["rec_frame"]), rec_capacity, p(res["verdict"]), p(res["totals"])))
+        return res
+
+    def prepare_reply(self, rec_group: torch.Tensor, rec_slot: torch.Tensor, out: torch.Tensor, out_capacity: Optional[int] = None,
+                      reply_variant: int = 1) -> dict:
+        """PrepareReply frames for durable PrepareBal records (handle_logged_prepare_bal, follower branch), read from the
+        instances' state now: into out (uint8, 16-byte aligned, round_up(reply_len, 16) regions packed in record order).
+        Returns device tensors reply_off (int64, -1 = not written), reply_len (int64, 0 = no reply), reply_dst (uint8) and
+        total (int64 [1]: the bytes the batch asked for)."""
+        assert rec_group.dtype == torch.int32 and rec_slot.dtype == torch.int64 and out.dtype == torch.uint8
+        n, dev = rec_group.numel(), out.device
+        res = dict(reply_off=torch.empty(n, dtype=torch.int64, device=dev), reply_len=torch.empty(n, dtype=torch.int64, device=dev),
+                   reply_dst=torch.empty(n, dtype=torch.uint8, device=dev), total=torch.empty(1, dtype=torch.int64, device=dev))
+        p = lambda x: x.data_ptr()
+        check(self.lib.ss_acceptor_prepare_reply(self.h, p(rec_group), p(rec_slot), n, reply_variant, p(out),
+                                                 out.numel() if out_capacity is None else out_capacity, p(res["reply_off"]),
+                                                 p(res["reply_len"]), p(res["reply_dst"]), p(res["total"])))
+        return res
+
     def close(self) -> None:
         if getattr(self, "h", None) is not None and self.h:
             self.lib.ss_acceptor_destroy(self.h)
@@ -345,3 +390,23 @@ class Acceptor:
             self.close()
         except Exception:
             pass
+
+
+PREPARE_REPLY_REC = 64      # sizeof(ss_prepare_reply_rec)
+
+
+def prepare_reply_parse(ctx: Context, buf: torch.Tensor, frame_off: torch.Tensor, data_shards: int, total_shards: int,
+                        reply_variant: int = 1) -> dict:
+    """PrepareReply frames (buf uint8 at any alignment, frame_off int64 [n]) -> one ss_prepare_reply_rec per frame, as
+    device tensors: slot, trigger_slot, endprep_slot, ballot, vote_bal, shards_at (int64; -1 = voted None), vote_mask,
+    data_len, kind (int32).  The new leader scatters vote_bal / vote_mask into ss_prepare_merge_dev's [r*N + i] arrays."""
+    assert buf.dtype == torch.uint8 and frame_off.dtype == torch.int64
+    n = frame_off.numel()
+    rec = torch.empty((n, PREPARE_REPLY_REC), dtype=torch.uint8, device=buf.device)
+    check(ctx.lib.ss_prepare_reply_parse_dev(ctx.h, buf.data_ptr(), buf.numel(), frame_off.data_ptr(), n, data_shards, total_shards,
+                                             reply_variant, rec.data_ptr()))
+    q, w = rec.view(torch.int64), rec.view(torch.int32)
+    names = ("slot", "trigger_slot", "endprep_slot", "ballot", "vote_bal", "shards_at")
+    out = {k: q[:, j] for j, k in enumerate(names)}
+    out.update(vote_mask=w[:, 12], data_len=w[:, 13], kind=w[:, 14])
+    return out

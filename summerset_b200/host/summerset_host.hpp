@@ -339,6 +339,20 @@ class Acceptor {
         check(ss_acceptor_absorb(acc_, buf, buf_len, frame_off, frame_group, frame_peer, n_frames, reply_variant, store, store_capacity,
                                  absorbed, verdict, total));
     }
+    // handle_msg_prepare: Prepare frames (PeerMsg variant 0) in, one 32-byte WalEntry::PrepareBal cell (variant 0) per
+    // covered slot out; a capacity cut leaves a prefix of the frames applied (see the header)
+    void prepare(const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group, const uint8_t *frame_peer,
+                 uint64_t n_frames, uint8_t *wal, uint64_t wal_capacity, uint32_t *rec_group, uint64_t *rec_slot, uint32_t *rec_frame,
+                 uint64_t rec_capacity, uint32_t *verdict, uint64_t *totals, uint32_t prepare_variant = 0, uint32_t wal_variant = 0) {
+        check(ss_acceptor_prepare(acc_, buf, buf_len, frame_off, frame_group, frame_peer, n_frames, prepare_variant, wal_variant, wal,
+                                  wal_capacity, rec_group, rec_slot, rec_frame, rec_capacity, verdict, totals));
+    }
+    // once those PrepareBal records are durable: PrepareReply frames (variant 1) into out; reply k goes to reply_dst[k]
+    void prepare_reply(const uint32_t *rec_group, const uint64_t *rec_slot, uint64_t n_records, uint8_t *out, uint64_t out_capacity,
+                       uint64_t *reply_off, uint64_t *reply_len, uint8_t *reply_dst, uint64_t *total, uint32_t reply_variant = 1) {
+        check(ss_acceptor_prepare_reply(acc_, rec_group, rec_slot, n_records, reply_variant, out, out_capacity, reply_off, reply_len,
+                                        reply_dst, total));
+    }
     ss_acceptor_view view() const {
         ss_acceptor_view v;
         check(ss_acceptor_view_get(acc_, &v));
@@ -347,6 +361,11 @@ class Acceptor {
     ss_acceptor_commit_view commit_view() const {
         ss_acceptor_commit_view v;
         check(ss_acceptor_commit_view_get(acc_, &v));
+        return v;
+    }
+    ss_acceptor_prepare_view prepare_view() const {
+        ss_acceptor_prepare_view v;
+        check(ss_acceptor_prepare_view_get(acc_, &v));
         return v;
     }
     ss_acceptor *handle() const { return acc_; }
