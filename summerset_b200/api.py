@@ -44,6 +44,13 @@ def shard_len(data_len: int, d: int) -> int:
     return data_len // d if data_len % d == 0 else data_len // d + 1
 
 
+def frame_accept_room(L, total_shards: int, population: int, with_assignment: bool):
+    """ss_frame_accept_max_len(spec, total_shards) for shard length L (an int or a numpy array of them): the room
+    Context.frame_accept_pack_ragged leaves per codeword when it sizes the output itself."""
+    n = 8 + 44 + total_shards + total_shards * (5 + L) + 1 + (5 + population * 19 if with_assignment else 0)
+    return (n + 15 + 15) // 16 * 16
+
+
 class Context:
     """A device context bound to torch's CURRENT stream on `device` at creation time."""
 
@@ -307,8 +314,7 @@ def _ctx_extras():
         spec = _lib.FrameSpec(kind, msg_variant, d, p, 0, pol.shape[1], 1 if with_assignment else 0, T)
         if out_capacity is None:
             L = (data_len.cpu().numpy().astype(np.int64) + d - 1) // d
-            per = 8 + 44 + T + T * (5 + L) + 1 + (5 + pol.shape[1] * 19 if with_assignment else 0) + 15
-            out_capacity = max(16, int(((per + 15) // 16 * 16).sum()))
+            out_capacity = max(16, int(frame_accept_room(L, T, pol.shape[1], with_assignment).sum()))
         out = torch.full((out_capacity,), 0xA5, dtype=torch.uint8, device=dev)      # the C ABI does not require a zeroed buffer
         off = torch.empty(n, dtype=torch.int64, device=dev)
         ln = torch.empty(n, dtype=torch.int32, device=dev)
