@@ -899,6 +899,70 @@ int ss_acceptor_prepare(ss_acceptor *acceptor, const uint8_t *buf, uint64_t buf_
 int ss_acceptor_prepare_reply(ss_acceptor *acceptor, const uint32_t *rec_group, const uint64_t *rec_slot, uint64_t n_records,
                               uint32_t reply_variant, uint8_t *out, uint64_t out_capacity, uint64_t *reply_off,
                               uint64_t *reply_len, uint8_t *reply_dst, uint64_t *total);
+/* Reconstruct requests from the acceptor, for the committed instances it cannot execute from its own shards: Crossword
+ * follower gossip (trigger_gossiping with gossip_targets_excl, crossword/gossiping.rs:35-192; the reference runs it on
+ * the gossip timer in the groups this replica does not lead, crossword/mod.rs:1150) and the reconstruct half of a new
+ * leader's become_a_leader (recon_slots, rspaxos/leadership.rs:99-172, crossword/leadership.rs:105-190).  The peers
+ * serve them with ss_acceptor_reconstruct_serve, this acceptor absorbs the replies with ss_acceptor_absorb and
+ * ss_acceptor_execute runs what now holds d shards, all without the window state leaving the device.
+ * Two more arrays: assign_rows (Crossword only, [G*64*population] u32, population * 256 bytes per group: row r of the
+ * instance at ring position p of group g at (g*64 + p)*population + r, the instance's whole `assignment: Vec<Bitmap>`,
+ * written by ss_acceptor_accept from the frame that defines the instance, beside assignment[me]) and gossip_bar ([G],
+ * zero at creation; ss_acceptor_advance leaves it alone).  assign_rows is NULL for RSPaxos. */
+typedef struct ss_acceptor_gossip_view {
+    uint64_t n_groups;
+    uint32_t population, pad0;
+    uint32_t *assign_rows;      /* Crossword [G*64*population]; NULL for RSPaxos */
+    uint64_t *gossip_bar;       /* [G] absolute */
+} ss_acceptor_gossip_view;
+int ss_acceptor_gossip_view_get(ss_acceptor *acceptor, ss_acceptor_gossip_view *view);
+/* Gossip (Crossword only; RSPaxos: SS_ERR_INVALID_ARG).  groups (device u32 [n_listed]) lists the groups to walk, in
+ * the order their frames come out (the host leaves out the groups it leads); NULL walks every group in index order.  A
+ * listed group >= n_groups is ignored; a group listed twice is planned twice from the state before the call.
+ * peer_alive (device [G] u32 peer masks) may be NULL: every peer alive.  batch_size >= 1 (the host resolves
+ * gossip_batch_size == 0 to msg_chunk_size); reconstruct_variant is PeerMsg::Reconstruct (4).
+ * Per listed group g, trigger_gossiping: log_end = window_base + 1 + the last window position that is Preparing,
+ * Accepting or Committed (window_base when none is); until = log_end - tail_ignores (0 below); slot_up_to = gossip_bar;
+ * every slot of [max(gossip_bar, window_base), until) in order sets slot_up_to = slot, then: slot < exec_bar is Executed
+ * and passed; a slot that is not Committed stops the walk; a Committed instance holding fewer than d shards is planned by
+ * gossip_targets_excl (src_peer = source, avail = held, the instance's assign_rows, peer_alive[g]; the walk of
+ * ss_gossip_plan_dev), and every selected peer gets the entry (slot, Bitmap{size T, avail at that moment}).  A null
+ * instance (data_len 0) is planned like any other.  Then gossip_bar = max(gossip_bar, slot_up_to): the last slot
+ * visited is walked again next time, as in the reference.
+ * Frames: each peer's entries in slot order, cut into frames of batch_size entries (the last one partial); frame =
+ * 8-byte big-endian length + PeerMessage::Msg{Reconstruct{slots_excl: Vec<(usize, Bitmap)>}}, the Bitmap as
+ * ssor_bitmap_encode writes it (size, one block, the block) -- what ss_acceptor_reconstruct_serve parses.  Frames are
+ * ordered by (listed group, peer, chunk): frame f is frame_group[f], for replica frame_dst[f], at out + frame_off[f]
+ * (16-byte aligned regions of round_up(frame_len, 16) bytes placed by exclusive scans of the per-group frames and bytes;
+ * out 16-byte aligned; bytes past frame_len are not written).  totals (device u64[2], may be NULL): the frames and bytes
+ * the call asked for.
+ * Capacity is per group: a listed group whose frames end past frame_capacity or whose region ends past out_capacity
+ * writes no frame and keeps its gossip_bar; its frame records below frame_capacity get frame_off UINT64_MAX, frame_len 0
+ * and frame_dst 0xff; SS_DEV_STATUS_FRAME_OVERFLOW.  The ends are monotone, so the written groups are a prefix of the
+ * list, and calling again with the same arguments plans the rest as this call would have.
+ * Stated differences from the reference:
+ *   1. log_end is the window, not start_slot + insts.len(): the reference also counts trailing null instances that a
+ *      Prepare or a step-up appended to its vector;
+ *   2. Executed is slot < exec_bar (the host installs exec_bar), as in ss_acceptor_absorb;
+ *   3. the per-group capacity cut above (the reference sends every frame);
+ *   4. assign_rows costs population * 256 bytes per group of device memory on a Crossword acceptor.
+ * Cost: a warp per listed group, each lane two window positions; gossip_targets_excl runs once per instance and once
+ * more per selected peer, so a group costs O(population^2) per position in the worst case. */
+int ss_acceptor_gossip(ss_acceptor *acceptor, const uint32_t *groups, uint64_t n_listed, const uint32_t *peer_alive,
+                       uint64_t tail_ignores, uint64_t batch_size, uint32_t reconstruct_variant, uint8_t *out,
+                       uint64_t out_capacity, uint32_t *frame_group, uint8_t *frame_dst, uint64_t *frame_off,
+                       uint32_t *frame_len, uint64_t frame_capacity, uint64_t *totals);
+/* Step-up reads (RSPaxos and Crossword): the reconstruct half of become_a_leader.  groups, outputs and capacity as for
+ * ss_acceptor_gossip; chunk_size (msg_chunk_size) >= 1.  Per listed group every slot of
+ * [max(exec_bar, window_base), window_base + 64) is walked with no stop, and each Committed instance holding fewer than
+ * d shards (RSPaxos: majority, the acceptor's d) is listed; the list is cut into frames of chunk_size entries,
+ * PeerMessage::Msg{Reconstruct{slots}} (RSPaxos) or {slots_excl} with the exclusion = held as a size-T Bitmap
+ * (Crossword), each with frame_dst 0xff: the host broadcasts it.  No state changes; the Prepare, PrepareBal and ballot
+ * parts of become_a_leader stay with the host. */
+int ss_acceptor_step_up_reads(ss_acceptor *acceptor, const uint32_t *groups, uint64_t n_listed, uint64_t chunk_size,
+                              uint32_t reconstruct_variant, uint8_t *out, uint64_t out_capacity, uint32_t *frame_group,
+                              uint8_t *frame_dst, uint64_t *frame_off, uint32_t *frame_len, uint64_t frame_capacity,
+                              uint64_t *totals);
 /* PrepareReply frames -> one record per frame for the new leader (a thread per frame, no copies; the PrepareReply
  * counterpart of ss_accept_reply_parse_dev).  Frame i at buf + frame_off[i] (any alignment) must be
  * PeerMessage::Msg{PrepareReply{slot, trigger_slot, endprep_slot, ballot, voted}} whose codeword, when voted is Some,

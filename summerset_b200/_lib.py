@@ -129,6 +129,9 @@ SIGNATURES = {
     "ss_acceptor_prepare_view_get": (_i, [_vp, _vp]),
     "ss_acceptor_prepare": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _u32, _vp, _u64, _vp, _vp, _vp, _u64, _vp, _vp]),
     "ss_acceptor_prepare_reply": (_i, [_vp, _vp, _vp, _u64, _u32, _vp, _u64, _vp, _vp, _vp, _vp]),
+    "ss_acceptor_gossip_view_get": (_i, [_vp, _vp]),
+    "ss_acceptor_gossip": (_i, [_vp, _vp, _u64, _vp, _u64, _u64, _u32, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp]),
+    "ss_acceptor_step_up_reads": (_i, [_vp, _vp, _u64, _u64, _u32, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp]),
     "ss_prepare_reply_parse_dev": (_i, [_vp, _vp, _u64, _vp, _u64, _u32, _u32, _u32, _vp]),
     "ss_rs_set_variant": (_i, [_vp, _i]),
     "ss_rs_last_kernel": (C.c_char_p, [_vp]),
@@ -194,6 +197,12 @@ class AcceptorPrepareView(C.Structure):
     """ss_acceptor_prepare_view"""
     _fields_ = [("n_groups", C.c_uint64), ("preparing", C.c_void_p), ("voted_bal", C.c_void_p), ("voted_mask", C.c_void_p),
                 ("prep_trigger", C.c_void_p), ("prep_span", C.c_void_p)]
+
+
+class AcceptorGossipView(C.Structure):
+    """ss_acceptor_gossip_view"""
+    _fields_ = [("n_groups", C.c_uint64), ("population", C.c_uint32), ("pad0", C.c_uint32), ("assign_rows", C.c_void_p),
+                ("gossip_bar", C.c_void_p)]
 
 
 class PrepareReplyRec(C.Structure):

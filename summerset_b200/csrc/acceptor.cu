@@ -64,6 +64,16 @@
 //   (engine.cu's scan)       reply regions
 //   prep_reply_copy_kernel   a warp per record: capacity, the PrepareReply with the voted shards (the RSCodeword writer
 //                            serve_copy_kernel uses)
+//
+// Reconstruct requests for the instances this follower cannot execute: Crossword's trigger_gossiping with
+// gossip_targets_excl (crossword/gossiping.rs:35-192) and become_a_leader's recon_slots (rspaxos/leadership.rs:99-172,
+// crossword/leadership.rs:105-190):
+//
+//   request_size_kernel      a warp per listed group: the walk, each lane's two instances planned (gossip_walk.cuh),
+//                            per destination the entries' bytes, frames and region bytes
+//   (engine.cu's scan)       frame numbers and regions per listed group
+//   request_write_kernel     a warp per listed group: the per-group capacity cut, the same plan again, frame headers and
+//                            entries, gossip_bar
 #include <cub/device/device_radix_sort.cuh>
 
 #include <cstring>
@@ -72,6 +82,7 @@
 #include "device_common.cuh"
 #include "gf256.hpp"
 #include "ss_internal.hpp"
+#include "gossip_walk.cuh"
 #include "window_ring.cuh"
 #include "wire_common.cuh"
 
@@ -86,7 +97,7 @@ struct FrameHdr {
     uint32_t slot_at;               // offset of the `slot` varint inside the frame
     uint32_t tags_at;               // offset of shard 0's Option tag
     uint32_t asg;                   // Crossword: assignment[me]
-    uint32_t pad;
+    uint32_t asg_at;                // Crossword: offset of assignment[0] inside the frame
 };
 
 // one decoded ReconstructReply frame (ss_acceptor_absorb); it lives in the FrameHdr scratch, which is at least as large
@@ -125,6 +136,9 @@ struct ss_acceptor {
     uint64_t *preparing = nullptr, *voted_bal = nullptr, *prep_trigger = nullptr;
     uint32_t *voted_mask = nullptr;
     uint8_t *prep_span = nullptr;
+    // Crossword follower gossip: the instance's whole assignment ([G*64][population] rows) and gossip_bar ([G])
+    uint32_t *assign_rows = nullptr;
+    uint64_t *gossip_bar = nullptr;
     uint8_t *matrix = nullptr;      // [T*d] the coder's coding matrix (gf256.hpp), row-major
     uint64_t *ex_cnt = nullptr, *ex_bytes = nullptr, *ex_partials = nullptr, *ex_n = nullptr;   // execute scratch
     // per-call scratch, grow-only
@@ -156,7 +170,7 @@ struct AccArgs {
     uint32_t d, T, population, me, accept_variant, wal_variant, reply_variant, crossword;
     // state
     uint64_t *window_base, *bal_max_seen, *inst_bal, *accepting, *shard_addr, *committed;
-    uint32_t *held, *data_len, *assignment;
+    uint32_t *held, *data_len, *assignment, *assign_rows;
     uint8_t *source;
     uint64_t *preparing, *voted_bal, *prep_trigger;
     uint32_t *voted_mask;
@@ -271,6 +285,7 @@ __device__ __forceinline__ FrameHdr decode_frame(const AccArgs &A, uint64_t i) {
     if (A.crossword) {                                                      // assignment: Vec<Bitmap>, one row per replica
         SS_GET(v);
         if (v != A.population) return h;
+        h.asg_at = static_cast<uint32_t>(8u + n);
         for (uint32_t r = 0; r < A.population; ++r) {
             uint64_t sz = 0, nb = 0, blk = 0;
             SS_GET(sz);
@@ -371,7 +386,18 @@ __global__ void __launch_bounds__(kAccThreads) acceptor_place_kernel(const __gri
                         A.held[at] = h.held;
                         A.data_len[at] = h.dlen;
                         A.shard_addr[at] = reinterpret_cast<uint64_t>(A.store + so);
-                        if (A.assignment != nullptr) A.assignment[at] = h.asg;
+                        if (A.assignment != nullptr) {
+                            A.assignment[at] = h.asg;
+                            // the whole assignment, re-read from the rows the header pass validated
+                            const uint8_t *rb = A.buf + A.frame_off[i] + h.asg_at;
+                            uint64_t q = 0, sz = 0, nb = 0, blk = 0;
+                            for (uint32_t r = 0; r < A.population; ++r) {
+                                q += wv_get(rb + q, h.end - h.asg_at - q, sz);
+                                q += wv_get(rb + q, h.end - h.asg_at - q, nb);
+                                q += wv_get(rb + q, h.end - h.asg_at - q, blk);
+                                A.assign_rows[at * A.population + r] = static_cast<uint32_t>(blk);
+                            }
+                        }
                         A.voted_bal[at] = h.ballot;                     // inst.voted = (ballot, reqs_cw as accepted)
                         A.voted_mask[at] = h.held;
                         A.prep_trigger[at] = 0u;                        // replica_bk = {source, 0, 0}
@@ -1557,6 +1583,247 @@ __global__ void __launch_bounds__(kAccThreads) prep_reply_copy_kernel(const __gr
     if (full && lane == 0u) atomicOr(A.status, SS_DEV_STATUS_FRAME_OVERFLOW);
 }
 
+// ---- reconstruct requests ----------------------------------------------------------------------------------------
+struct ReqArgs {
+    const uint32_t *groups;         // the listed groups; nullptr: entry i is group i
+    const uint32_t *peer_alive;     // [G] peer masks; nullptr: every peer is alive
+    uint64_t n, G, tail, batch;     // batch <= 64: no destination gets more than 64 entries of one group
+    uint32_t me, population, d, T, variant, crossword, step_up;
+    const uint64_t *window_base, *accepting, *committed, *preparing, *exec_bar;
+    const uint32_t *held, *assign_rows;
+    const uint8_t *source;
+    uint64_t *gossip_bar;
+    uint64_t *bar0;                 // [n] gossip_bar of entry i's group as the size pass read it
+    uint64_t *cnt, *bytes;          // [n] frames and region bytes of entry i, then their exclusive scans
+    const uint64_t *totals;         // [2] the two scans' totals
+    uint8_t *out;
+    uint64_t out_cap;
+    uint32_t *frame_group;
+    uint8_t *frame_dst;
+    uint64_t *frame_off;
+    uint32_t *frame_len;
+    uint64_t frame_cap;
+    uint32_t *status;
+};
+
+// per-warp scratch of one destination's entries
+struct ReqWarp {
+    uint32_t pre[65];               // pre[k]: bytes of the destination's first k entries
+    uint64_t off[64];               // write pass: the frame offset of each chunk
+};
+
+__device__ __forceinline__ uint64_t warp_incl_scan(uint64_t x, uint32_t lane) {
+    for (int s = 1; s < 32; s <<= 1) {
+        const uint64_t y = __shfl_up_sync(0xffffffffu, x, s);
+        if (lane >= static_cast<uint32_t>(s)) x += y;
+    }
+    return x;
+}
+
+// The walk of group g from gossip_bar = bar0, warp-uniform.  Returns the window positions with an entry (bit w: slot
+// base + w, committed with fewer than d shards held); *bar = gossip_bar after the walk.
+//   gossip (trigger_gossiping, crossword/gossiping.rs:88-192): slots [max(bar0, base), until), until = log_end minus
+//     tail_ignores, log_end = base + 1 + the last window position that is Preparing, Accepting or Committed; a slot
+//     below exec_bar is Executed and passed, the first other slot that is not committed stops the walk; the last slot
+//     visited (the stop included) is slot_up_to, and the bar moves to max(bar0, slot_up_to)
+//   step-up (become_a_leader's recon_slots, rspaxos/leadership.rs:99-172, crossword/leadership.rs:105-190): every slot
+//     of [max(exec_bar, base), base + 64), no stop
+__device__ __forceinline__ uint64_t request_walk(const ReqArgs &A, uint32_t g, uint64_t bar0, uint32_t lane, uint64_t *bar) {
+    const uint64_t base = A.window_base[g], eb = A.exec_bar[g];
+    const uint32_t r = static_cast<uint32_t>(base & 63u);
+    const uint64_t com = ring_to_window(A.committed[g], r);
+    const uint64_t exec_w = eb <= base ? 0ull : eb - base >= 64u ? ~0ull : (1ull << (eb - base)) - 1u;
+    uint64_t walk = 0u;
+    *bar = bar0;
+    if (A.step_up) {
+        walk = com & ~exec_w;
+    } else {
+        const uint64_t live = ring_to_window(A.preparing[g] | A.accepting[g] | A.committed[g], r);
+        const uint64_t log_end = base + (live == 0u ? 0u : 64u - static_cast<uint64_t>(__clzll(static_cast<long long>(live))));
+        const uint64_t until = log_end > A.tail ? log_end - A.tail : 0u;
+        const uint64_t start = bar0 > base ? bar0 : base;
+        if (start < until) {                                                    // lo < hi <= 64
+            const uint64_t lo = start - base, hi = until - base;
+            const uint64_t range = (hi == 64u ? ~0ull : (1ull << hi) - 1u) & ~((1ull << lo) - 1u);
+            const uint64_t stop = range & ~exec_w & ~com;
+            const uint64_t first = stop != 0u ? static_cast<uint64_t>(__ffsll(static_cast<long long>(stop))) - 1u : 64u;
+            walk = range & ~exec_w & com & (first == 64u ? ~0ull : (1ull << first) - 1u);
+            const uint64_t up_to = base + (first != 64u ? first : hi - 1u);
+            *bar = up_to > bar0 ? up_to : bar0;
+        }
+    }
+    const uint64_t row = static_cast<uint64_t>(g) * 64u;
+    bool need[2];
+    for (uint32_t h = 0; h < 2u; ++h) {
+        const uint32_t w = lane + 32u * h;
+        need[h] = ((walk >> w) & 1u) && static_cast<uint32_t>(__popc(A.held[row + ((r + w) & 63u)])) < A.d;
+    }
+    return static_cast<uint64_t>(__ballot_sync(0xffffffffu, need[0])) | static_cast<uint64_t>(__ballot_sync(0xffffffffu, need[1])) << 32;
+}
+
+// gossip_targets_excl for the instance at `at`: the selected peers; *excl = the exclusion of peer q when it is selected
+__device__ __forceinline__ uint32_t request_targets(const ReqArgs &A, uint64_t at, uint32_t alive, uint32_t q, uint32_t *excl) {
+    const uint32_t *rows = A.assign_rows + at * A.population;
+    return gossip_walk(A.me, A.population, A.d, A.source[at], A.held[at], alive, [&](uint32_t p) { return rows[p]; },
+                       [&](uint32_t p, uint32_t avail) { if (p == q) *excl = avail; });
+}
+
+// one entry: slot (RSPaxos), or (slot, Bitmap{size T, one block: excl}) as ssor_bitmap_encode writes it (Crossword)
+__device__ __forceinline__ uint32_t request_entry_bytes(const ReqArgs &A, uint64_t slot, uint32_t excl) {
+    return static_cast<uint32_t>(wv_len(slot)) + (A.crossword ? static_cast<uint32_t>(wv_len(A.T) + 1 + wv_len(excl)) : 0u);
+}
+
+// frame c of a destination with cnt entries: 8-byte length, PeerMessage::Msg, the variant, the entry count, the entries
+__device__ __forceinline__ uint64_t request_frame_len(const ReqArgs &A, const ReqWarp &W, uint32_t c, uint32_t cnt) {
+    const uint32_t b = static_cast<uint32_t>(A.batch), k0 = c * b, m = cnt - k0 < b ? cnt - k0 : b;
+    return 9u + wv_len(A.variant) + wv_len(m) + (W.pre[k0 + m] - W.pre[k0]);
+}
+
+// The destinations of group g in order (gossip: peers 0..population-1, step-up: one broadcast list), each with its
+// entries in slot order.  For each destination with entries: W.pre holds the entry byte prefix, and
+// per_dst(q, cnt, sel, k, excl) runs on the whole warp (this lane's positions: sel[h], entry index k[h], exclusion).
+template <typename F>
+__device__ void request_plan(const ReqArgs &A, uint32_t g, uint64_t need, uint32_t lane, ReqWarp &W, F &&per_dst) {
+    const uint64_t base = A.window_base[g];
+    const uint32_t alive = A.peer_alive != nullptr ? A.peer_alive[g] : 0xffffffffu;
+    uint64_t at[2];
+    uint32_t t[2] = {0u, 0u};
+    for (uint32_t h = 0; h < 2u; ++h) {
+        const uint32_t w = lane + 32u * h;
+        at[h] = static_cast<uint64_t>(g) * 64u + ((base + w) & 63u);
+        if ((need >> w) & 1u) t[h] = A.step_up ? 1u : request_targets(A, at[h], alive, 32u, nullptr);
+    }
+    const uint32_t ndst = A.step_up ? 1u : A.population;
+    const uint32_t below = (1u << lane) - 1u;
+    for (uint32_t q = 0; q < ndst; ++q) {
+        bool sel[2];
+        uint32_t b[2];
+        for (uint32_t h = 0; h < 2u; ++h) {
+            sel[h] = (t[h] >> q) & 1u;
+            b[h] = __ballot_sync(0xffffffffu, sel[h]);
+        }
+        const uint32_t cnt = static_cast<uint32_t>(__popc(b[0]) + __popc(b[1]));
+        if (cnt == 0u) continue;
+        const uint32_t k[2] = {static_cast<uint32_t>(__popc(b[0] & below)), static_cast<uint32_t>(__popc(b[0]) + __popc(b[1] & below))};
+        uint32_t ex[2] = {0u, 0u}, e[2] = {0u, 0u};
+        for (uint32_t h = 0; h < 2u; ++h) {
+            if (!sel[h]) continue;
+            if (A.step_up) ex[h] = A.held[at[h]];
+            else request_targets(A, at[h], alive, q, &ex[h]);
+            e[h] = request_entry_bytes(A, base + lane + 32u * h, ex[h]);
+        }
+        const uint64_t s0 = warp_incl_scan(e[0], lane), s1 = warp_incl_scan(e[1], lane) + __shfl_sync(0xffffffffu, s0, 31);
+        __syncwarp();                   // the previous destination's readers of W are done
+        if (lane == 0u) W.pre[0] = 0u;
+        if (sel[0]) W.pre[k[0] + 1u] = static_cast<uint32_t>(s0);
+        if (sel[1]) W.pre[k[1] + 1u] = static_cast<uint32_t>(s1);
+        __syncwarp();
+        per_dst(q, cnt, sel, k, ex);
+    }
+    __syncwarp();
+}
+
+__device__ __forceinline__ uint32_t request_group(const ReqArgs &A, uint64_t i) { return A.groups != nullptr ? A.groups[i] : static_cast<uint32_t>(i); }
+
+// 1. a warp per listed group: the walk, the plan, the frames and region bytes it asks for
+__global__ void __launch_bounds__(kAccThreads) request_size_kernel(const __grid_constant__ ReqArgs A) {
+    __shared__ ReqWarp Ws[kExecWarps];
+    const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+    ReqWarp &W = Ws[w];
+    const uint64_t nwarps = static_cast<uint64_t>(gridDim.x) * kExecWarps;
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kExecWarps + w; i < A.n; i += nwarps) {
+        const uint32_t g = request_group(A, i);
+        uint64_t frames = 0u, bytes = 0u;
+        if (g < A.G) {
+            const uint64_t bar0 = A.gossip_bar[g];
+            uint64_t bar;
+            const uint64_t need = request_walk(A, g, bar0, lane, &bar);
+            request_plan(A, g, need, lane, W, [&](uint32_t, uint32_t cnt, const bool *, const uint32_t *, const uint32_t *) {
+                const uint32_t nc = (cnt + static_cast<uint32_t>(A.batch) - 1u) / static_cast<uint32_t>(A.batch);
+                uint64_t b = 0u;
+                for (uint32_t c = lane; c < nc; c += 32u) b += round16(request_frame_len(A, W, c, cnt));
+                frames += nc;
+                bytes += warp_sum(b);
+            });
+            if (lane == 0u) A.bar0[i] = bar0;
+        }
+        if (lane == 0u) {
+            A.cnt[i] = frames;
+            A.bytes[i] = bytes;
+        }
+    }
+}
+
+// 2. a warp per listed group: capacity, then the same plan again from the same bar, written: frame headers by the lane
+//    of each chunk, entries by the lane of their slot; gossip_bar of the placed groups
+__global__ void __launch_bounds__(kAccThreads) request_write_kernel(const __grid_constant__ ReqArgs A) {
+    __shared__ ReqWarp Ws[kExecWarps];
+    const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+    ReqWarp &W = Ws[w];
+    bool full = false;
+    const uint64_t nwarps = static_cast<uint64_t>(gridDim.x) * kExecWarps;
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kExecWarps + w; i < A.n; i += nwarps) {
+        const uint32_t g = request_group(A, i);
+        if (g >= A.G) continue;
+        const uint64_t f0 = A.cnt[i], o0 = A.bytes[i];
+        const uint64_t f1 = i + 1u < A.n ? A.cnt[i + 1u] : A.totals[0], o1 = i + 1u < A.n ? A.bytes[i + 1u] : A.totals[1];
+        if (f1 > A.frame_cap || o1 > A.out_cap) {                              // the ends are monotone: a suffix is cut
+            full = true;
+            for (uint64_t f = f0 + lane; f < f1 && f < A.frame_cap; f += 32u) {
+                A.frame_group[f] = g;
+                A.frame_dst[f] = 0xffu;
+                A.frame_off[f] = ~0ull;
+                A.frame_len[f] = 0u;
+            }
+            continue;
+        }
+        const uint64_t bar0 = A.bar0[i], base = A.window_base[g];
+        uint64_t bar;
+        const uint64_t need = request_walk(A, g, bar0, lane, &bar);
+        uint64_t fr = f0, ob = o0;
+        const uint32_t B = static_cast<uint32_t>(A.batch), vl = static_cast<uint32_t>(wv_len(A.variant));
+        request_plan(A, g, need, lane, W, [&](uint32_t q, uint32_t cnt, const bool *sel, const uint32_t *k, const uint32_t *ex) {
+            const uint32_t nc = (cnt + B - 1u) / B;
+            for (uint32_t c0 = 0; c0 < nc; c0 += 32u) {
+                const uint32_t c = c0 + lane;
+                const uint64_t len = c < nc ? request_frame_len(A, W, c, cnt) : 0u, reg = round16(len);
+                const uint64_t incl = warp_incl_scan(reg, lane), o = ob + incl - reg;
+                if (c < nc) {
+                    W.off[c] = o;
+                    const uint64_t f = fr + c;
+                    A.frame_group[f] = g;
+                    A.frame_dst[f] = A.step_up ? 0xffu : static_cast<uint8_t>(q);
+                    A.frame_off[f] = o;
+                    A.frame_len[f] = static_cast<uint32_t>(len);
+                    uint8_t *dst = A.out + o;
+                    const uint64_t body = len - 8u;
+                    for (int b = 0; b < 8; ++b) dst[b] = static_cast<uint8_t>(body >> (8 * (7 - b)));
+                    uint32_t m = 8u;
+                    m += wv_put(dst + m, 0u);                                   // PeerMessage::Msg
+                    m += wv_put(dst + m, A.variant);
+                    wv_put(dst + m, cnt - c * B < B ? cnt - c * B : B);
+                }
+                ob += __shfl_sync(0xffffffffu, incl, 31);
+            }
+            fr += nc;
+            __syncwarp();
+            for (uint32_t h = 0; h < 2u; ++h) {
+                if (!sel[h]) continue;
+                const uint32_t c = k[h] / B, m = cnt - c * B < B ? cnt - c * B : B;
+                uint8_t *e = A.out + W.off[c] + 9u + vl + wv_len(m) + (W.pre[k[h]] - W.pre[c * B]);
+                e += wv_put(e, base + lane + 32u * h);
+                if (A.crossword) {                                              // Bitmap: size, one block
+                    e += wv_put(e, A.T);
+                    e += wv_put(e, 1u);
+                    wv_put(e, ex[h]);
+                }
+            }
+        });
+        if (!A.step_up && lane == 0u) A.gossip_bar[g] = bar;
+    }
+    if (full && lane == 0u) atomicOr(A.status, SS_DEV_STATUS_FRAME_OVERFLOW);
+}
+
 static inline uint32_t acc_grid(ss_ctx *ctx, uint64_t items, uint32_t per_cta) {
     uint64_t ctas = (items + per_cta - 1) / per_cta;
     const uint64_t cap = static_cast<uint64_t>(ctx->sm_count) * 8ull * 8ull;
@@ -1618,7 +1885,8 @@ int ss_acceptor_destroy(ss_acceptor *a) {
     }
     void *bufs[] = {a->window_base, a->bal_max_seen, a->inst_bal, a->accepting, a->shard_addr, a->held, a->data_len, a->assignment,
                     a->source, a->committed, a->commit_bar, a->exec_bar, a->preparing, a->voted_bal, a->voted_mask,
-                    a->prep_trigger, a->prep_span, a->matrix, a->ex_cnt, a->ex_bytes, a->ex_partials, a->ex_n, a->hdr,
+                    a->prep_trigger, a->prep_span, a->assign_rows, a->gossip_bar, a->matrix, a->ex_cnt, a->ex_bytes,
+                    a->ex_partials, a->ex_n, a->hdr,
                     a->keys, a->idx, a->partials, a->fcnt, a->sort_tmp, a->totals};
     for (void *b : bufs)
         if (b) cudaFree(b);
@@ -1657,6 +1925,8 @@ int ss_acceptor_create(ss_ctx *ctx, const ss_acceptor_config *cfg, uint64_t G, s
         (rc = acc_alloc(ctx, &a->shard_addr, G * 64)) || (rc = acc_alloc(ctx, &a->held, G * 64)) ||
         (rc = acc_alloc(ctx, &a->data_len, G * 64)) || (rc = acc_alloc(ctx, &a->source, G * 64)) || (rc = acc_alloc(ctx, &a->totals, 2)) ||
         (cfg->protocol == SS_PROTO_CROSSWORD && (rc = acc_alloc(ctx, &a->assignment, G * 64))) ||
+        (cfg->protocol == SS_PROTO_CROSSWORD && (rc = acc_alloc(ctx, &a->assign_rows, G * 64 * cfg->population))) ||
+        (rc = acc_alloc(ctx, &a->gossip_bar, G)) ||
         (rc = acc_alloc(ctx, &a->committed, G)) || (rc = acc_alloc(ctx, &a->commit_bar, G)) || (rc = acc_alloc(ctx, &a->exec_bar, G)) ||
         (rc = acc_alloc(ctx, &a->preparing, G)) || (rc = acc_alloc(ctx, &a->voted_bal, G * 64)) ||
         (rc = acc_alloc(ctx, &a->voted_mask, G * 64)) || (rc = acc_alloc(ctx, &a->prep_trigger, G * 64)) ||
@@ -1792,7 +2062,7 @@ int ss_acceptor_accept(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, con
     A.crossword = a->cfg.protocol == SS_PROTO_CROSSWORD ? 1u : 0u;
     A.window_base = a->window_base; A.bal_max_seen = a->bal_max_seen; A.inst_bal = a->inst_bal; A.accepting = a->accepting;
     A.shard_addr = a->shard_addr; A.held = a->held; A.data_len = a->data_len; A.assignment = a->assignment; A.source = a->source;
-    A.committed = a->committed;
+    A.assign_rows = a->assign_rows; A.committed = a->committed;
     A.preparing = a->preparing; A.voted_bal = a->voted_bal; A.voted_mask = a->voted_mask; A.prep_trigger = a->prep_trigger;
     A.prep_span = a->prep_span;
     A.hdr = a->hdr; A.key_in = a->keys; A.idx_in = a->idx; A.key = a->keys + n; A.idx = a->idx + n;
@@ -1971,6 +2241,73 @@ int ss_acceptor_prepare_reply(ss_acceptor *a, const uint32_t *rec_group, const u
     SS_TRY(launch_exclusive_scan_u64(ctx, reply_off, n, a->partials, total != nullptr ? total : a->totals));
     prep_reply_copy_kernel<<<acc_grid(ctx, n, kExecWarps), kAccThreads, 0, ctx->stream>>>(R);
     return launched(ctx);
+}
+
+int ss_acceptor_gossip_view_get(ss_acceptor *a, ss_acceptor_gossip_view *v) {
+    if (a == nullptr || v == nullptr) return set_error(SS_ERR_INVALID_ARG, "null argument");
+    memset(v, 0, sizeof(*v));
+    v->n_groups = a->G; v->population = a->cfg.population;
+    v->assign_rows = a->assign_rows; v->gossip_bar = a->gossip_bar;
+    return SS_OK;
+}
+
+}  // extern "C"
+
+// the two request calls: size pass, scans of frames and bytes over the listed groups, write pass
+static int acceptor_requests(ss_acceptor *a, bool step_up, const uint32_t *groups, uint64_t n_listed, const uint32_t *peer_alive,
+                             uint64_t tail_ignores, uint64_t batch, uint32_t variant, uint8_t *out, uint64_t out_capacity,
+                             uint32_t *frame_group, uint8_t *frame_dst, uint64_t *frame_off, uint32_t *frame_len,
+                             uint64_t frame_capacity, uint64_t *totals) {
+    if (a == nullptr) return set_error(SS_ERR_INVALID_ARG, "null acceptor");
+    if (!step_up && a->cfg.protocol != SS_PROTO_CROSSWORD) return set_error(SS_ERR_INVALID_ARG, "gossip is Crossword's");
+    if (batch == 0) return set_error(SS_ERR_INVALID_ARG, "batch / chunk size must be at least 1");
+    ss_ctx *ctx = a->ctx;
+    SS_TRY(ctx_bind(ctx));
+    const uint64_t n = groups != nullptr ? n_listed : a->G;
+    if (n == 0) {
+        if (totals != nullptr) SS_CUDA(cudaMemsetAsync(totals, 0, 16, ctx->stream));
+        return SS_OK;
+    }
+    if (!out || !frame_group || !frame_dst || !frame_off || !frame_len) return set_error(SS_ERR_INVALID_ARG, "null buffer");
+    if (reinterpret_cast<uintptr_t>(out) & 15u) return set_error(SS_ERR_INVALID_ARG, "out must be 16-byte aligned");
+    if (n > 0x7fffffffull) return set_error(SS_ERR_INVALID_ARG, "at most 2^31 - 1 listed groups per call");
+    SS_TRY(ensure_scratch(a, n));
+    ReqArgs R{};
+    R.groups = groups; R.peer_alive = peer_alive; R.n = n; R.G = a->G; R.tail = tail_ignores; R.batch = batch < 64u ? batch : 64u;
+    R.me = a->cfg.me; R.population = a->cfg.population; R.d = a->cfg.data_shards; R.T = a->cfg.total_shards; R.variant = variant;
+    R.crossword = a->cfg.protocol == SS_PROTO_CROSSWORD ? 1u : 0u; R.step_up = step_up ? 1u : 0u;
+    R.window_base = a->window_base; R.accepting = a->accepting; R.committed = a->committed; R.preparing = a->preparing;
+    R.exec_bar = a->exec_bar; R.held = a->held; R.assign_rows = a->assign_rows; R.source = a->source; R.gossip_bar = a->gossip_bar;
+    // per-entry scratch: the header pass's FrameHdr cells (6 words each) hold bytes and bar0, fcnt the frame counts
+    uint64_t *words = reinterpret_cast<uint64_t *>(a->hdr);
+    R.bytes = words; R.bar0 = words + n; R.cnt = a->fcnt;
+    uint64_t *tot = totals != nullptr ? totals : a->totals;
+    R.totals = tot;
+    R.out = out; R.out_cap = out_capacity; R.frame_group = frame_group; R.frame_dst = frame_dst; R.frame_off = frame_off;
+    R.frame_len = frame_len; R.frame_cap = frame_capacity; R.status = ctx->dev_status;
+    const uint32_t grid_w = acc_grid(ctx, n, kExecWarps);
+    request_size_kernel<<<grid_w, kAccThreads, 0, ctx->stream>>>(R);
+    SS_TRY(launched(ctx));
+    SS_TRY(launch_exclusive_scan_u64(ctx, R.cnt, n, a->partials, tot));
+    SS_TRY(launch_exclusive_scan_u64(ctx, R.bytes, n, a->partials, tot + 1));
+    request_write_kernel<<<grid_w, kAccThreads, 0, ctx->stream>>>(R);
+    return launched(ctx);
+}
+
+extern "C" {
+
+int ss_acceptor_gossip(ss_acceptor *a, const uint32_t *groups, uint64_t n_listed, const uint32_t *peer_alive, uint64_t tail_ignores,
+                       uint64_t batch_size, uint32_t reconstruct_variant, uint8_t *out, uint64_t out_capacity, uint32_t *frame_group,
+                       uint8_t *frame_dst, uint64_t *frame_off, uint32_t *frame_len, uint64_t frame_capacity, uint64_t *totals) {
+    return acceptor_requests(a, false, groups, n_listed, peer_alive, tail_ignores, batch_size, reconstruct_variant, out, out_capacity,
+                             frame_group, frame_dst, frame_off, frame_len, frame_capacity, totals);
+}
+
+int ss_acceptor_step_up_reads(ss_acceptor *a, const uint32_t *groups, uint64_t n_listed, uint64_t chunk_size,
+                              uint32_t reconstruct_variant, uint8_t *out, uint64_t out_capacity, uint32_t *frame_group,
+                              uint8_t *frame_dst, uint64_t *frame_off, uint32_t *frame_len, uint64_t frame_capacity, uint64_t *totals) {
+    return acceptor_requests(a, true, groups, n_listed, nullptr, 0u, chunk_size, reconstruct_variant, out, out_capacity, frame_group,
+                             frame_dst, frame_off, frame_len, frame_capacity, totals);
 }
 
 }  // extern "C"

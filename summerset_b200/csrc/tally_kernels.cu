@@ -10,6 +10,7 @@
 // All of it is HBM-bound integer/bit work: coalesced 64/128-bit loads, no shared-memory staging
 // needed except for the Crossword look-up table.
 #include "device_common.cuh"
+#include "gossip_walk.cuh"
 #include "ss_internal.hpp"
 
 namespace ssb {
@@ -522,24 +523,12 @@ gossip_plan_kernel(uint32_t me, uint32_t population, uint32_t d, const uint8_t *
                    uint32_t *__restrict__ targets, uint32_t *__restrict__ excl /* [population][N] */) {
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kTallyThreads;
     for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kTallyThreads + threadIdx.x; i < N; i += stride) {
-        uint32_t avail = __ldg(avail_in + i);
-        const uint32_t src = src_peer[i];
         uint32_t k = policy_idx[i];
         if (k >= n_policies) k = 0;
         const uint32_t *asg = policies + k * population;
-        uint32_t t = 0;
-        for (uint32_t pp = me + 1u; pp < me + population; ++pp) {
-            const uint32_t peer = pp % population;
-            if (peer == src || !((peer_alive >> peer) & 1u)) continue;
-            const uint32_t useful = __ldg(asg + peer) & ~avail;
-            if (useful != 0u) {
-                excl[static_cast<uint64_t>(peer) * N + i] = avail;
-                t |= 1u << peer;
-                avail |= useful;
-            }
-            if (static_cast<uint32_t>(__popc(avail)) >= d) break;
-        }
-        targets[i] = t;
+        targets[i] = gossip_walk(me, population, d, src_peer[i], __ldg(avail_in + i), peer_alive,
+                                 [&](uint32_t peer) { return __ldg(asg + peer); },
+                                 [&](uint32_t peer, uint32_t avail) { excl[static_cast<uint64_t>(peer) * N + i] = avail; });
     }
 }
 

@@ -22,6 +22,10 @@ torch tensors (zero-copy views) so tests can read results and install state; it 
                                             request batches decoded from the held shards
         prepare(buf, ..., wal, rec_capacity)   handle_msg_prepare (rspaxos/messages.rs:13-84): PrepareBal records
         prepare_reply(rec_group, rec_slot, out)   handle_logged_prepare_bal's follower branch: PrepareReply frames
+        gossip(out, frame_capacity, batch_size)   Crossword trigger_gossiping (crossword/gossiping.rs:88-192): Reconstruct
+                                            frames for the committed instances missing shards, to the peers gossip_targets_excl picks
+        step_up_reads(out, frame_capacity, chunk_size)   become_a_leader's recon_slots (rspaxos/leadership.rs:99-172):
+                                            Reconstruct frames to broadcast
     prepare_reply_parse(ctx, buf, frame_off, d, T)   the new leader's side: PrepareReply frames -> vote records
     RaftEngine(ctx, G, population[, fault_tolerance, craft])
         append(n_new) / on_append_replies(records) / tick()      raft/messages.rs:243-309, craft/messages.rs:300-308
@@ -252,6 +256,10 @@ class Acceptor:
         self.voted_mask = t(pv.voted_mask, (G * 64,), "<i4", torch.int32)
         self.prep_trigger = t(pv.prep_trigger, (G * 64,), "<i8", torch.int64)
         self.prep_span = t(pv.prep_span, (G * 64,), "|u1", torch.uint8)
+        gv = self.gossip_view = _lib.AcceptorGossipView()
+        check(self.lib.ss_acceptor_gossip_view_get(self.h, C.byref(gv)))
+        self.assign_rows = t(gv.assign_rows, (G * 64 * population,), "<i4", torch.int32)
+        self.gossip_bar = t(gv.gossip_bar, (G,), "<i8", torch.int64)
 
     def accept(self, buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor, frame_peer: torch.Tensor,
                store: torch.Tensor, wal: torch.Tensor, store_capacity: Optional[int] = None, wal_capacity: Optional[int] = None) -> dict:
@@ -379,6 +387,47 @@ class Acceptor:
                                                  out.numel() if out_capacity is None else out_capacity, p(res["reply_off"]),
                                                  p(res["reply_len"]), p(res["reply_dst"]), p(res["total"])))
         return res
+
+    def _requests(self, step_up: bool, out: torch.Tensor, frame_capacity: int, groups: Optional[torch.Tensor], batch: int,
+                  out_capacity: Optional[int], reconstruct_variant: int, peer_alive: Optional[torch.Tensor] = None,
+                  tail_ignores: int = 0) -> dict:
+        assert out.dtype == torch.uint8
+        assert groups is None or groups.dtype == torch.int32
+        assert peer_alive is None or (peer_alive.dtype == torch.int32 and peer_alive.numel() == self.G)
+        dev = out.device
+        cap = max(frame_capacity, 1)
+        res = dict(frame_group=torch.empty(cap, dtype=torch.int32, device=dev), frame_dst=torch.empty(cap, dtype=torch.uint8, device=dev),
+                   frame_off=torch.empty(cap, dtype=torch.int64, device=dev), frame_len=torch.empty(cap, dtype=torch.int32, device=dev),
+                   totals=torch.empty(2, dtype=torch.int64, device=dev))
+        p = lambda x: None if x is None else x.data_ptr()
+        oc = out.numel() if out_capacity is None else out_capacity
+        gp, n = p(groups), 0 if groups is None else groups.numel()
+        if step_up:
+            check(self.lib.ss_acceptor_step_up_reads(self.h, gp, n, batch, reconstruct_variant, p(out), oc, p(res["frame_group"]),
+                                                     p(res["frame_dst"]), p(res["frame_off"]), p(res["frame_len"]), frame_capacity,
+                                                     p(res["totals"])))
+        else:
+            check(self.lib.ss_acceptor_gossip(self.h, gp, n, p(peer_alive), tail_ignores, batch, reconstruct_variant, p(out), oc,
+                                              p(res["frame_group"]), p(res["frame_dst"]), p(res["frame_off"]), p(res["frame_len"]),
+                                              frame_capacity, p(res["totals"])))
+        return res
+
+    def gossip(self, out: torch.Tensor, frame_capacity: int, batch_size: int, groups: Optional[torch.Tensor] = None,
+               peer_alive: Optional[torch.Tensor] = None, tail_ignores: int = 0, out_capacity: Optional[int] = None,
+               reconstruct_variant: int = 4) -> dict:
+        """Crossword follower gossip (trigger_gossiping) over the listed groups (int32, None = all): Reconstruct{slots_excl}
+        frames into out (uint8, 16-byte aligned), ordered by (listed group, peer, chunk); gossip_bar moves for the groups
+        placed.  peer_alive: int32 [G] peer masks (None = all alive).  Returns device tensors frame_group (int32),
+        frame_dst (uint8), frame_off (int64, -1 = not written), frame_len (int32), each [frame_capacity], and totals
+        (int64 [2]: frames and bytes asked for)."""
+        return self._requests(False, out, frame_capacity, groups, batch_size, out_capacity, reconstruct_variant, peer_alive, tail_ignores)
+
+    def step_up_reads(self, out: torch.Tensor, frame_capacity: int, chunk_size: int, groups: Optional[torch.Tensor] = None,
+                      out_capacity: Optional[int] = None, reconstruct_variant: int = 4) -> dict:
+        """The reconstruct reads of become_a_leader over the listed groups: Reconstruct frames of chunk_size entries for
+        every committed instance holding fewer than d shards, each to be broadcast (frame_dst 0xff).  Outputs as gossip();
+        no state changes."""
+        return self._requests(True, out, frame_capacity, groups, chunk_size, out_capacity, reconstruct_variant)
 
     def close(self) -> None:
         if getattr(self, "h", None) is not None and self.h:

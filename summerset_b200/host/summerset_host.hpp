@@ -353,6 +353,26 @@ class Acceptor {
         check(ss_acceptor_prepare_reply(acc_, rec_group, rec_slot, n_records, reply_variant, out, out_capacity, reply_off, reply_len,
                                         reply_dst, total));
     }
+    // Crossword trigger_gossiping over the listed groups (NULL: all; leave out the groups this replica leads):
+    // Reconstruct frames (variant 4) for peer frame_dst[f]; a capacity cut leaves a prefix of the groups written
+    void gossip(const uint32_t *groups, uint64_t n_listed, const uint32_t *peer_alive, uint64_t tail_ignores, uint64_t batch_size,
+                uint8_t *out, uint64_t out_capacity, uint32_t *frame_group, uint8_t *frame_dst, uint64_t *frame_off, uint32_t *frame_len,
+                uint64_t frame_capacity, uint64_t *totals, uint32_t reconstruct_variant = 4) {
+        check(ss_acceptor_gossip(acc_, groups, n_listed, peer_alive, tail_ignores, batch_size, reconstruct_variant, out, out_capacity,
+                                 frame_group, frame_dst, frame_off, frame_len, frame_capacity, totals));
+    }
+    // become_a_leader's reconstruct reads: Reconstruct frames (variant 4) to broadcast, chunk_size = msg_chunk_size
+    void step_up_reads(const uint32_t *groups, uint64_t n_listed, uint64_t chunk_size, uint8_t *out, uint64_t out_capacity,
+                       uint32_t *frame_group, uint8_t *frame_dst, uint64_t *frame_off, uint32_t *frame_len, uint64_t frame_capacity,
+                       uint64_t *totals, uint32_t reconstruct_variant = 4) {
+        check(ss_acceptor_step_up_reads(acc_, groups, n_listed, chunk_size, reconstruct_variant, out, out_capacity, frame_group, frame_dst,
+                                        frame_off, frame_len, frame_capacity, totals));
+    }
+    ss_acceptor_gossip_view gossip_view() const {
+        ss_acceptor_gossip_view v;
+        check(ss_acceptor_gossip_view_get(acc_, &v));
+        return v;
+    }
     ss_acceptor_view view() const {
         ss_acceptor_view v;
         check(ss_acceptor_view_get(acc_, &v));
