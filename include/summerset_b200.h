@@ -188,7 +188,7 @@ int ss_rs_encode_uniform_dev(ss_rs_coder *coder, const uint8_t *data, uint64_t d
 /* Batched reconstruct (rscoding.rs:490-537 over n codewords; callers rspaxos/durability.rs:146-159,
  * crossword/durability.rs:163-179).  Shard j of codeword g lives at
  * shards[j*plane_stride + off[g] .. +L_g), L_g = ceil(data_len[g]/d).  present[g] bit j =
- * shard j available.  Missing DATA shards are regenerated in place (and missing parity too when
+ * shard j available; bits d+p and above are ignored.  Missing DATA shards are regenerated in place (and missing parity too when
  * data_only == 0).  status[g] = 0, SS_ERR_TOO_FEW_SHARDS_PRESENT (nothing written for g), or
  * SS_ERR_INVALID_ARG for a null codeword (data_len == 0; rscoding.rs:495-497). */
 int ss_rs_reconstruct_batch_dev(ss_rs_coder *coder, uint8_t *shards, uint64_t plane_stride,
@@ -200,7 +200,7 @@ int ss_rs_reconstruct_batch_dev(ss_rs_coder *coder, uint8_t *shards, uint64_t pl
  * (16-byte aligned slots of capacity round_up(L,16), the layout ss_rs_encode_uniform_dev writes with
  * SS_RS_OUT_PADDED16; regenerated shards get zero padding).  For RS(3,2) -- every 5-replica deployment -- this runs
  * the pattern-specialised row kernel (compile-time decode rows per present mask); other codes go through the kernels of
- * the ragged call.  status as above. */
+ * the ragged call.  present[g] and status as above (present bits d+p and above are ignored). */
 int ss_rs_reconstruct_uniform_dev(ss_rs_coder *coder, uint8_t *shards, uint64_t plane_stride, uint64_t shard_stride,
                                   uint32_t data_len, const uint32_t *present, uint64_t n, int data_only,
                                   int32_t *status);
@@ -990,7 +990,8 @@ int ss_prepare_reply_parse_dev(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len
  *             5 = bit-plane generic kernels instead of the Horner ones, 8 = global-table Horner reconstruct instead of the
  *             shared-memory small-code kernel; 3 / 6 / 7 = 32 / 64 / 56-register builds of the row kernel (default 40)
  *   bit 4     row kernel: contiguous chunk of codewords per CTA instead of grid-stride
- *   bits 5-7  row kernel waves of CTAs per resident set: {64 (default), 1, 32, 4, 16, 256, 128, 8}
+ *   bits 5-7  row kernel waves of CTAs per resident set: {64 (default), 1, 32, 4, 16, 256, 128, 8}; the RS(3,2) row kernel
+ *             of ss_rs_reconstruct_uniform_dev reads the same bits with its own table {16 (default), 1, 32, 4, 64, 256, 128, 8}
  *   bits 8-9  cache operator of the plane stores in replicate mode: .cs (default), write-back, .cg, .wt
  *   bit 10    row kernel: fixed instead of rotating warp -> column-block assignment
  *   bit 18    the accept step (parity to local planes, up to 256 columns) on the bulk-copy kernel instead of the row kernel;
