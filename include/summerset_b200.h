@@ -984,6 +984,130 @@ typedef struct ss_prepare_reply_rec {
 int ss_prepare_reply_parse_dev(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, uint64_t n_frames,
                                uint32_t data_shards, uint32_t total_shards, uint32_t reply_variant, ss_prepare_reply_rec *rec);
 
+/* ---- batched CRaft follower (the Raft-family counterpart of the acceptor) ----------------------------------------
+ * For n_groups CRaft groups this replica follows: AppendEntries frames in (handle_msg_append_entries,
+ * craft/messages.rs:14-252, with check_term, craft/leadership.rs:16-75), the entries' shards into a caller-owned store,
+ * DurEntry::LogEntry and DurEntry::Metadata records and AppendEntriesReply frames out (craft/durability.rs:129-160).
+ * The code is derived from the population: d = majority, p = population - majority (craft/mod.rs:527-536).
+ * State lives in HBM as a struct of arrays.  Per group: start_slot, log_end, curr_term, leader (0xff = None),
+ * last_commit, last_snap.  Per log position, a ring of `window` entries (slot s at s & (window - 1)): term, data_len,
+ * held (shard mask) and shard_addr (device address of the first held shard in the caller's store, shards in index order
+ * at SS_CW_SLOT_PITCH(shard_len) apart, the layout ss_acceptor_accept writes).  At creation every group holds the slot-0
+ * null entry recovery pushes (craft/recovery.rs:99-125): start_slot 0, log_end 1, term 0, no shards.
+ * Stated differences from the reference:
+ *   1. the log is a ring of `window` entries, not a vector: a frame with an entry at or past start_slot + window takes no
+ *      part in the call (SS_FOLLOWER_VERDICT_BEYOND_WINDOW) and is re-submitted after ss_follower_advance;
+ *   2. a non-empty frame whose entries are all present with matching terms appends nothing and gets the immediate reply
+ *      {curr_term, prev_slot + n, None}; the reference, with first_new left at prev_slot + 1, would push every entry
+ *      again at the end of its log (messages.rs:102-182).  The reply's bytes are the same; no record is written;
+ *   3. role is not tracked: the host submits frames only for the groups it follows; the candidate same-term hack,
+ *      heard_heartbeat and the timers stay on the host;
+ *   4. the capacity cut is a suffix in frame order (below);
+ *   5. absorbed entries (messages.rs:143-154) take a region after every frame's region, placed in the order the group
+ *      walks reach them; one that does not fit keeps the shards it held (SS_DEV_STATUS_STORE_FULL). */
+typedef struct ss_follower ss_follower;
+typedef struct ss_follower_config {
+    uint32_t protocol;          /* SS_PROTO_CRAFT (the field leaves room for plain Raft without an ABI change) */
+    uint32_t population;        /* replicas, 1..32 */
+    uint32_t me;                /* this replica's id: a frame from `me` is malformed */
+    uint32_t window;            /* ring entries per group, power of two <= 4096 (0 = 64) */
+    uint32_t append_variant;    /* index of AppendEntries in PeerMsg (0), < 2^16 */
+    uint32_t reply_variant;     /* index of AppendEntriesReply in PeerMsg (1), < 251: a reply fills at most 47 bytes of
+                                   its 48-byte cell */
+    uint32_t meta_variant;      /* index of Metadata in DurEntry (0), < 2^16 */
+    uint32_t log_variant;       /* index of LogEntry in DurEntry (1), < 2^16 */
+} ss_follower_config;
+typedef struct ss_follower_view {
+    uint64_t n_groups;
+    uint32_t protocol, population, me, data_shards, total_shards, window;
+    uint64_t *start_slot, *log_end, *curr_term, *last_commit, *last_snap;   /* [G] */
+    uint8_t *leader;            /* [G] 0xff = None */
+    uint64_t *term;             /* [G*window] */
+    uint64_t *shard_addr;       /* [G*window] */
+    uint32_t *held;             /* [G*window] */
+    uint32_t *data_len;         /* [G*window] */
+} ss_follower_view;
+/* Configuration checks first (SS_ERR_INVALID_ARG, including protocol != SS_PROTO_CRAFT); a NULL ctx then gives
+ * SS_ERR_NO_DEVICE when the machine has no usable device, SS_ERR_INVALID_ARG otherwise. */
+int ss_follower_create(ss_ctx *ctx, const ss_follower_config *cfg, uint64_t n_groups, ss_follower **out);
+int ss_follower_destroy(ss_follower *follower);
+int ss_follower_view_get(ss_follower *follower, ss_follower_view *view);
+/* the snapshot's start_slot move (craft/snapshot.rs:130-198): upto (device [G] absolute slots) -- start_slot moves by
+ * k = clamp(upto - start_slot, 0, last_commit - start_slot), so never past last_commit */
+int ss_follower_advance(ss_follower *follower, const uint64_t *upto);
+/* Verdicts of ss_follower_append, beside the PeerMsg variant index k (another message; 0x80000000 | k for the
+ * PeerMessage variants) and SS_FRAME_KIND_MALFORMED */
+#define SS_FOLLOWER_VERDICT_ACCEPTED 0xfffffff0u      /* log matched: appended, absorbed or found its entries present */
+#define SS_FOLLOWER_VERDICT_REJECTED 0xfffffff1u      /* conflict reply sent, nothing appended */
+#define SS_FOLLOWER_VERDICT_BEYOND_WINDOW 0xfffffff3u /* an entry at or past start_slot + window: re-submit after advance */
+#define SS_FOLLOWER_VERDICT_STORE_FULL 0xfffffff4u    /* cut by the store capacity (below) */
+#define SS_FOLLOWER_VERDICT_WAL_FULL 0xfffffff5u      /* cut by the WAL capacity (below) */
+/* One batch of frames, taken as ss_acceptor_accept takes them: buf at any byte alignment, frame i at frame_off[i], of
+ * group frame_group[i] (>= n_groups: malformed), from replica frame_peer[i].  Frame i is PeerMessage::Msg{AppendEntries
+ * {term, prev_slot, prev_term, entries: Vec<LogEntry{term, reqs_cw, external, log_offset}>, leader_commit, last_snap}}.
+ * Malformed: truncated, trailing bytes, a variant >= 2^16, a codeword that is not this code, shard_len !=
+ * ceil(data_len / d), data_len >= 2^32, a present shard of another length, data_copy other than None, external not 0/1,
+ * a body over 2^32 - 65 bytes, or a frame from `me` or from a peer >= population.
+ * Each group's frames are replayed in frame order as if they arrived one at a time:
+ *   term check: term > curr_term raises curr_term (voted_for None) and sets leader; that frame gets
+ *     DurEntry::Metadata{curr_term, voted_for: 255} in the 32-byte cell meta + 32*i (meta_len[i] bytes: 8-byte
+ *     big-endian length, meta_variant, curr_term, 0xff; zero to the end of the cell; 0 = no record), which the host makes
+ *     durable before any other action of the frame.  A frame with term >= curr_term sets leader = frame_peer.
+ *   rejection: term < curr_term, prev_slot outside [start_slot, log_end) or term[prev_slot] != prev_term (also for an
+ *     empty frame): reply {curr_term, prev_slot + n, Some((conflict_term, conflict_slot))} with messages.rs:52-69's walk
+ *     back over the ring, to frame_peer, sent at once.
+ *   acceptance: entry k at slot prev_slot + 1 + k appends when it is at or past log_end; one whose term differs from
+ *     the held one truncates the log at its slot (trunc_slot[i] = that slot, else UINT64_MAX: the host applies
+ *     LogAction::Truncate at the slot's file offset before the frame's records) and appends from there; a matching one
+ *     absorbs the frame's shards when the held entry has fewer than d data shards, the same data_len and another shard
+ *     map.  Appended entries get DurEntry::LogEntry records one after the other from wal + wal_off[i], each at a 16-byte
+ *     aligned offset: 8-byte big-endian length, log_variant, the entry's bytes from term through external verbatim,
+ *     log_offset as varint 0; wal_len[i] = the bytes from wal_off[i] to the end of the last one's 16-byte slot.  Their
+ *     shards go one entry after the other from store + store_off[i].  A frame that appended anything gets the reply
+ *     {curr_term, prev_slot + n, None} for reply_dst[i] = leader as the whole call left it, sent once its records are
+ *     durable; a frame that appended nothing (wal_len 0, store_off and wal_off UINT64_MAX) gets the same bytes for
+ *     frame_peer at once.  Then leader_commit > last_commit walks last_commit + 1 ..= min(leader_commit,
+ *     first_new - 1, log_end - 1) and stops at an entry holding fewer than d shards, first_new being the first slot
+ *     the frame appended, or prev_slot + 1 when it appended nothing: the reference's cap prev_slot + entries.len()
+ *     is taken after its append loop drained entries[first_new - prev_slot - 1 ..] (messages.rs:160-203), so a frame
+ *     never commits the entries it appends itself.  last_snap = max(last_snap, the frame's).  A rejected frame also
+ *     raises last_snap.
+ * Replies: PeerMessage::Msg{AppendEntriesReply} in the 48-byte cell replies + 48*i, reply_len[i] bytes (0 = none),
+ * reply_dst[i] (0xff = none).  commit_lo (device [G], may be NULL): each group's last_commit before the call.
+ * Capacity: every frame that reaches the replay reserves, before it, a store region of the popcount(held) *
+ * SS_CW_SLOT_PITCH(shard_len) of all its entries and a WAL region of all its entries' 16-byte record slots, placed by
+ * exclusive scans in frame order.  The first frame in frame order whose region ends past store_capacity or
+ * wal_capacity, and every later frame that would reach the replay, is cut: STORE_FULL or WAL_FULL (the first frame's
+ * reason), nothing changes, SS_DEV_STATUS_STORE_FULL / SS_DEV_STATUS_FRAME_OVERFLOW.  The handled frames are then a
+ * prefix in frame order and, within each group, a prefix of its frames; the host re-submits the rest.
+ * totals (device u64[2], may be NULL): the store bytes (regions and absorbs) and WAL bytes the batch asked for.
+ * Non-handled frames get UINT64_MAX offsets and zero lengths.  store and wal 16-byte aligned.
+ * Cost: the replay walks each group's frames on one thread, so a batch costs its largest per-group run of frames there
+ * (a follower catching up on one group replays serially); absorbs are copied by that thread too.  The records and
+ * shards take a warp per frame. */
+int ss_follower_append(ss_follower *follower, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off,
+                       const uint32_t *frame_group, const uint8_t *frame_peer, uint64_t n_frames, uint8_t *store,
+                       uint64_t store_capacity, uint64_t *store_off, uint8_t *wal, uint64_t wal_capacity, uint64_t *wal_off,
+                       uint64_t *wal_len, uint8_t *meta, uint32_t *meta_len, uint8_t *replies, uint32_t *reply_len,
+                       uint8_t *reply_dst, uint64_t *trunc_slot, uint32_t *verdict, uint64_t *commit_lo, uint64_t *totals);
+/* The leader's side: AppendEntriesReply frames (buf, frame_off, frame_group, frame_peer as above; frame_peer is the
+ * peer index ss_engine_raft_ingest takes) -> records in its layout: rec_group, rec_peer, rec_end_slot.  curr_term is the
+ * CRaft engine's [G] array (ss_engine_view.curr_term).  rec_kind: SS_APPEND_REPLY_INGEST for a success reply whose term
+ * is at most curr_term[g] and end_slot < 2^32; SS_APPEND_REPLY_HIGHER_TERM (check_term makes the leader step down and
+ * drop the reply, messages.rs:272-274), _CONFLICT (the next_slot back-off stays with the host), _END_RANGE; another
+ * message's variant index (0x80000000 | k for PeerMessage variants) or SS_FRAME_KIND_MALFORMED (also a group >=
+ * n_groups).  Every record but INGEST gets rec_group UINT32_MAX, which the ingest drops.  rec_term, rec_conflict_term and
+ * rec_conflict_slot hold the decoded fields of a frame of one of the four kinds above (the conflict ones 0 for a
+ * success reply); every field is 0 for another message or a malformed frame. */
+#define SS_APPEND_REPLY_INGEST 0xfffffff0u
+#define SS_APPEND_REPLY_CONFLICT 0xfffffff1u
+#define SS_APPEND_REPLY_HIGHER_TERM 0xfffffff2u
+#define SS_APPEND_REPLY_END_RANGE 0xfffffff3u
+int ss_append_reply_parse_dev(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
+                              const uint8_t *frame_peer, const uint32_t *curr_term, uint64_t n_frames, uint64_t n_groups,
+                              uint32_t reply_variant, uint32_t *rec_group, uint8_t *rec_peer, uint32_t *rec_end_slot,
+                              uint64_t *rec_term, uint64_t *rec_conflict_term, uint64_t *rec_conflict_slot, uint32_t *rec_kind);
+
 /* ---- tuning / introspection (bench + tests) ------------------------------------------------ */
 /* Tuning knob for experiments; 0 = the defaults.
  *   bits 0-3  kernel choice / register budget: 1 = flat one-column-per-thread RS(3,2) kernel instead of the row kernel,

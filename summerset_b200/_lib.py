@@ -133,6 +133,13 @@ SIGNATURES = {
     "ss_acceptor_gossip": (_i, [_vp, _vp, _u64, _vp, _u64, _u64, _u32, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp]),
     "ss_acceptor_step_up_reads": (_i, [_vp, _vp, _u64, _u64, _u32, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp]),
     "ss_prepare_reply_parse_dev": (_i, [_vp, _vp, _u64, _vp, _u64, _u32, _u32, _u32, _vp]),
+    "ss_follower_create": (_i, [_vp, _vp, _u64, C.POINTER(_vp)]),
+    "ss_follower_destroy": (_i, [_vp]),
+    "ss_follower_view_get": (_i, [_vp, _vp]),
+    "ss_follower_advance": (_i, [_vp, _vp]),
+    "ss_follower_append": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _vp, _u64, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                _vp, _vp, _vp, _vp]),
+    "ss_append_reply_parse_dev": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _u64, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ss_rs_set_variant": (_i, [_vp, _i]),
     "ss_rs_last_kernel": (C.c_char_p, [_vp]),
     "ss_rs_jit_status": (C.c_char_p, [_vp]),
@@ -205,6 +212,22 @@ class AcceptorGossipView(C.Structure):
                 ("gossip_bar", C.c_void_p)]
 
 
+class FollowerConfig(C.Structure):
+    """ss_follower_config"""
+    _fields_ = [("protocol", C.c_uint32), ("population", C.c_uint32), ("me", C.c_uint32), ("window", C.c_uint32),
+                ("append_variant", C.c_uint32), ("reply_variant", C.c_uint32), ("meta_variant", C.c_uint32),
+                ("log_variant", C.c_uint32)]
+
+
+class FollowerView(C.Structure):
+    """ss_follower_view"""
+    _fields_ = [("n_groups", C.c_uint64), ("protocol", C.c_uint32), ("population", C.c_uint32), ("me", C.c_uint32),
+                ("data_shards", C.c_uint32), ("total_shards", C.c_uint32), ("window", C.c_uint32),
+                ("start_slot", C.c_void_p), ("log_end", C.c_void_p), ("curr_term", C.c_void_p), ("last_commit", C.c_void_p),
+                ("last_snap", C.c_void_p), ("leader", C.c_void_p), ("term", C.c_void_p), ("shard_addr", C.c_void_p),
+                ("held", C.c_void_p), ("data_len", C.c_void_p)]
+
+
 class PrepareReplyRec(C.Structure):
     """ss_prepare_reply_rec (64 bytes)"""
     _fields_ = [("slot", C.c_uint64), ("trigger_slot", C.c_uint64), ("endprep_slot", C.c_uint64), ("ballot", C.c_uint64),
@@ -228,6 +251,17 @@ SS_FRAME_KIND_MALFORMED = 0xFFFFFFFF
 SS_RECON_VERDICT_NULL_CODEWORD = 0xFFFFFFF6
 SS_RECON_VERDICT_SHARD_RANGE = 0xFFFFFFF7
 SS_RECON_VERDICT_OUT_FULL = 0xFFFFFFF8
+# verdicts of ss_follower_append (beside PeerMsg variant indices and SS_FRAME_KIND_MALFORMED)
+SS_FOLLOWER_VERDICT_ACCEPTED = 0xFFFFFFF0
+SS_FOLLOWER_VERDICT_REJECTED = 0xFFFFFFF1
+SS_FOLLOWER_VERDICT_BEYOND_WINDOW = 0xFFFFFFF3
+SS_FOLLOWER_VERDICT_STORE_FULL = 0xFFFFFFF4
+SS_FOLLOWER_VERDICT_WAL_FULL = 0xFFFFFFF5
+# record kinds of ss_append_reply_parse_dev
+SS_APPEND_REPLY_INGEST = 0xFFFFFFF0
+SS_APPEND_REPLY_CONFLICT = 0xFFFFFFF1
+SS_APPEND_REPLY_HIGHER_TERM = 0xFFFFFFF2
+SS_APPEND_REPLY_END_RANGE = 0xFFFFFFF3
 
 
 class SummersetError(RuntimeError):

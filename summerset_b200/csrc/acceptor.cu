@@ -79,6 +79,7 @@
 #include <cstring>
 #include <new>
 
+#include "codeword_wire.cuh"
 #include "device_common.cuh"
 #include "gf256.hpp"
 #include "ss_internal.hpp"
@@ -201,38 +202,6 @@ __device__ __forceinline__ uint64_t wal_bytes(const FrameHdr &h, uint32_t wal_va
     return 8u + static_cast<uint64_t>(wv_len(wal_variant)) + (h.end - h.slot_at);
 }
 __device__ __forceinline__ uint64_t round16(uint64_t x) { return (x + 15u) & ~15ull; }
-
-// one shard of L bytes at src (any alignment) into its padded store slot at dst (16-byte aligned): aligned 128-bit
-// stores, each fed by dev::load16, bytes L..round_up(L, 16) zero
-__device__ __forceinline__ void warp_fill_slot(uint8_t *dst, const uint8_t *src, uint64_t L, uint32_t lane) {
-    const uint64_t nvec = (L + 15u) >> 4;
-    for (uint64_t v = lane; v < nvec; v += 32u) {
-        const uint64_t left = L - v * 16u;
-        dev::stg128_cs(dst + v * 16u, dev::load16(src + v * 16u, left < 16u ? static_cast<int>(left) : 16));
-    }
-}
-
-// the T shard Options of a bincode RSCodeword starting at tags (Option tag, length varint, bytes): the shards of `take`
-// (a subset of the present ones, `present`) go to their padded slots of the region at dst: one after the other, or with
-// a dst_mask, shard j at its rank among the shards of dst_mask
-__device__ __forceinline__ void warp_fill_shards(uint8_t *dst, const uint8_t *tags, uint32_t T, uint32_t present, uint32_t take,
-                                                 uint32_t L, uint32_t lane, uint64_t dst_mask = ~0ull) {
-    const uint64_t pitch = SS_CW_SLOT_PITCH(L);
-    uint64_t at = 0;
-    uint32_t k = 0;
-    for (uint32_t j = 0; j < T; ++j) {
-        if (!((present >> j) & 1u)) { at += 1u; continue; }
-        // Some tag, then the shard length as the frame spells it: a non-minimal varint is as valid as the header pass
-        // found it, so its width comes from its own tag byte
-        const uint8_t t = tags[at + 1u];
-        const uint64_t some_len = 1u + (t < 251u ? 1u : t == 251u ? 3u : t == 252u ? 5u : 9u);
-        if ((take >> j) & 1u) {
-            const uint64_t slot = dst_mask == ~0ull ? k++ : static_cast<uint64_t>(__popc(static_cast<uint32_t>(dst_mask) & ((1u << j) - 1u)));
-            warp_fill_slot(dst + slot * pitch, tags + at + some_len, L, lane);
-        }
-        at += some_len + static_cast<uint64_t>(L);
-    }
-}
 
 // decodes frame i as ssor_decode_accept reads it, plus the acceptor's own checks (code, shard_len, assignment shape)
 __device__ __forceinline__ FrameHdr decode_frame(const AccArgs &A, uint64_t i) {

@@ -29,6 +29,12 @@ torch tensors (zero-copy views) so tests can read results and install state; it 
     prepare_reply_parse(ctx, buf, frame_off, d, T)   the new leader's side: PrepareReply frames -> vote records
     RaftEngine(ctx, G, population[, fault_tolerance, craft])
         append(n_new) / on_append_replies(records) / tick()      raft/messages.rs:243-309, craft/messages.rs:300-308
+    Follower(ctx, G, population, me[, window])   the CRaft follower
+        append(buf, frame_off, frame_group, frame_peer, store, wal)   handle_msg_append_entries (craft/messages.rs:14-252):
+                                            store, LogEntry / Metadata records, AppendEntriesReply cells
+        advance(upto)                       the snapshot's start_slot move
+    append_reply_parse(ctx, buf, frame_off, frame_group, frame_peer, curr_term, G)   the leader's side: AppendEntriesReply
+                                            frames -> RaftEngine.on_append_replies records
 """
 from __future__ import annotations
 
@@ -458,4 +464,95 @@ def prepare_reply_parse(ctx: Context, buf: torch.Tensor, frame_off: torch.Tensor
     names = ("slot", "trigger_slot", "endprep_slot", "ballot", "vote_bal", "shards_at")
     out = {k: q[:, j] for j, k in enumerate(names)}
     out.update(vote_mask=w[:, 12], data_len=w[:, 13], kind=w[:, 14])
+    return out
+
+
+class Follower:
+    """The CRaft follower for G groups (ss_follower_* in include/summerset_b200.h): AppendEntries frames in, LogEntry and
+    Metadata records and AppendEntriesReply cells out.  State tensors are zero-copy views of the follower's device arrays;
+    per-position arrays are rings of `window` entries (slot s at s & (window - 1))."""
+
+    REPLY_CELL = 48
+    META_CELL = 32
+
+    def __init__(self, ctx: Context, n_groups: int, population: int, me: int, window: int = 0, append_variant: int = 0,
+                 reply_variant: int = 1, meta_variant: int = 0, log_variant: int = 1):
+        self.ctx, self.lib, self.G = ctx, ctx.lib, n_groups
+        cfg = _lib.FollowerConfig(_PROTO["craft"], population, me, window, append_variant, reply_variant, meta_variant, log_variant)
+        h = C.c_void_p()
+        check(self.lib.ss_follower_create(ctx.h, C.byref(cfg), n_groups, C.byref(h)))
+        self.h = h
+        v = self.view = _lib.FollowerView()
+        check(self.lib.ss_follower_view_get(self.h, C.byref(v)))
+        self.dev = torch.device("cuda", ctx.device)
+        self.n, self.me, self.d, self.T, self.W = population, me, v.data_shards, v.total_shards, v.window
+        G, W = n_groups, v.window
+        t = lambda ptr, shape, ts, dt: torch.as_tensor(_DevArray(ptr, shape, ts), device=self.dev).view(dt).view(shape)
+        self.start_slot = t(v.start_slot, (G,), "<i8", torch.int64)
+        self.log_end = t(v.log_end, (G,), "<i8", torch.int64)
+        self.curr_term = t(v.curr_term, (G,), "<i8", torch.int64)
+        self.last_commit = t(v.last_commit, (G,), "<i8", torch.int64)
+        self.last_snap = t(v.last_snap, (G,), "<i8", torch.int64)
+        self.leader = t(v.leader, (G,), "|u1", torch.uint8)
+        self.term = t(v.term, (G, W), "<i8", torch.int64)
+        self.shard_addr = t(v.shard_addr, (G, W), "<i8", torch.int64)
+        self.held = t(v.held, (G, W), "<i4", torch.int32)
+        self.data_len = t(v.data_len, (G, W), "<i4", torch.int32)
+
+    def append(self, buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor, frame_peer: torch.Tensor,
+               store: torch.Tensor, wal: torch.Tensor, store_capacity: Optional[int] = None,
+               wal_capacity: Optional[int] = None) -> dict:
+        """buf uint8 (frames at any alignment), frame_off int64 [n], frame_group int32 [n], frame_peer uint8 [n]; store / wal:
+        caller-owned uint8 buffers (16-byte aligned).  Returns the per-frame outputs as device tensors: store_off, wal_off,
+        wal_len, trunc_slot (int64, -1 = none), meta (uint8 [n, 32]) and meta_len, replies (uint8 [n, 48]) and reply_len,
+        reply_dst (uint8), verdict (int32), commit_lo (int64 [G]) and totals (int64 [2])."""
+        assert buf.dtype == torch.uint8 and frame_off.dtype == torch.int64 and frame_group.dtype == torch.int32
+        assert frame_peer.dtype == torch.uint8 and store.dtype == torch.uint8 and wal.dtype == torch.uint8
+        n, dev = frame_off.numel(), buf.device
+        e = lambda dt, *shape: torch.empty(shape if shape else (n,), dtype=dt, device=dev)
+        out = dict(store_off=e(torch.int64), wal_off=e(torch.int64), wal_len=e(torch.int64),
+                   meta=torch.zeros((n, self.META_CELL), dtype=torch.uint8, device=dev), meta_len=e(torch.int32),
+                   replies=torch.zeros((n, self.REPLY_CELL), dtype=torch.uint8, device=dev), reply_len=e(torch.int32),
+                   reply_dst=e(torch.uint8), trunc_slot=e(torch.int64), verdict=e(torch.int32), commit_lo=e(torch.int64, self.G),
+                   totals=e(torch.int64, 2))
+        p = lambda x: x.data_ptr()
+        check(self.lib.ss_follower_append(self.h, p(buf), buf.numel(), p(frame_off), p(frame_group), p(frame_peer), n, p(store),
+                                          store.numel() if store_capacity is None else store_capacity, p(out["store_off"]), p(wal),
+                                          wal.numel() if wal_capacity is None else wal_capacity, p(out["wal_off"]), p(out["wal_len"]),
+                                          p(out["meta"]), p(out["meta_len"]), p(out["replies"]), p(out["reply_len"]),
+                                          p(out["reply_dst"]), p(out["trunc_slot"]), p(out["verdict"]), p(out["commit_lo"]),
+                                          p(out["totals"])))
+        return out
+
+    def advance(self, upto: torch.Tensor) -> None:
+        """The snapshot's start_slot move, never past last_commit (upto int64 [G], absolute slots)."""
+        assert upto.is_cuda and upto.dtype == torch.int64 and upto.numel() == self.G
+        check(self.lib.ss_follower_advance(self.h, upto.data_ptr()))
+
+    def close(self) -> None:
+        if getattr(self, "h", None) is not None and self.h:
+            self.lib.ss_follower_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def append_reply_parse(ctx: Context, buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor,
+                       frame_peer: torch.Tensor, curr_term: torch.Tensor, n_groups: int, reply_variant: int = 1) -> dict:
+    """AppendEntriesReply frames -> the records RaftEngine.on_append_replies takes (rec_group, rec_peer, rec_end_slot) plus
+    rec_term, rec_conflict_term, rec_conflict_slot and rec_kind (ss_append_reply_parse_dev).  curr_term: the CRaft
+    engine's int32 [G] view."""
+    n, dev = frame_off.numel(), buf.device
+    e = lambda dt: torch.empty(n, dtype=dt, device=dev)
+    out = dict(rec_group=e(torch.int32), rec_peer=e(torch.uint8), rec_end_slot=e(torch.int32), rec_term=e(torch.int64),
+               rec_conflict_term=e(torch.int64), rec_conflict_slot=e(torch.int64), rec_kind=e(torch.int32))
+    p = lambda x: x.data_ptr()
+    check(ctx.lib.ss_append_reply_parse_dev(ctx.h, p(buf), buf.numel(), p(frame_off), p(frame_group), p(frame_peer), p(curr_term), n,
+                                            n_groups, reply_variant, p(out["rec_group"]), p(out["rec_peer"]), p(out["rec_end_slot"]),
+                                            p(out["rec_term"]), p(out["rec_conflict_term"]), p(out["rec_conflict_slot"]),
+                                            p(out["rec_kind"])))
     return out

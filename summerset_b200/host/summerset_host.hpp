@@ -394,4 +394,43 @@ class Acceptor {
     ss_acceptor *acc_ = nullptr;
 };
 
+// the CRaft follower (ss_follower_*): AppendEntries frames in, LogEntry / Metadata records and AppendEntriesReply cells out
+class Follower {
+  public:
+    Follower(ss_ctx *ctx, const ss_follower_config &cfg, uint64_t n_groups) { check(ss_follower_create(ctx, &cfg, n_groups, &fol_)); }
+    ~Follower() { ss_follower_destroy(fol_); }
+    Follower(const Follower &) = delete;
+    Follower &operator=(const Follower &) = delete;
+
+    // every pointer is a device pointer; see ss_follower_append for the outputs
+    void handle_msg_append_entries(const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
+                                   const uint8_t *frame_peer, uint64_t n_frames, uint8_t *store, uint64_t store_capacity,
+                                   uint64_t *store_off, uint8_t *wal, uint64_t wal_capacity, uint64_t *wal_off, uint64_t *wal_len,
+                                   uint8_t *meta, uint32_t *meta_len, uint8_t *replies, uint32_t *reply_len, uint8_t *reply_dst,
+                                   uint64_t *trunc_slot, uint32_t *verdict, uint64_t *commit_lo, uint64_t *totals) {
+        check(ss_follower_append(fol_, buf, buf_len, frame_off, frame_group, frame_peer, n_frames, store, store_capacity, store_off,
+                                 wal, wal_capacity, wal_off, wal_len, meta, meta_len, replies, reply_len, reply_dst, trunc_slot,
+                                 verdict, commit_lo, totals));
+    }
+    // the snapshot's start_slot move, never past last_commit
+    void advance_start_slot(const uint64_t *upto) { check(ss_follower_advance(fol_, upto)); }
+    ss_follower_view view() const {
+        ss_follower_view v{};
+        check(ss_follower_view_get(fol_, &v));
+        return v;
+    }
+
+  private:
+    ss_follower *fol_ = nullptr;
+};
+
+// the leader's side: AppendEntriesReply frames -> the records ss_engine_raft_ingest takes (rec_group UINT32_MAX: dropped)
+inline void append_reply_parse(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
+                               const uint8_t *frame_peer, const uint32_t *curr_term, uint64_t n_frames, uint64_t n_groups,
+                               uint32_t *rec_group, uint8_t *rec_peer, uint32_t *rec_end_slot, uint64_t *rec_term,
+                               uint64_t *rec_conflict_term, uint64_t *rec_conflict_slot, uint32_t *rec_kind, uint32_t reply_variant = 1) {
+    check(ss_append_reply_parse_dev(ctx, buf, buf_len, frame_off, frame_group, frame_peer, curr_term, n_frames, n_groups, reply_variant,
+                                    rec_group, rec_peer, rec_end_slot, rec_term, rec_conflict_term, rec_conflict_slot, rec_kind));
+}
+
 }  // namespace ssb
