@@ -1108,6 +1108,117 @@ int ss_append_reply_parse_dev(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len,
                               uint32_t reply_variant, uint32_t *rec_group, uint8_t *rec_peer, uint32_t *rec_end_slot,
                               uint64_t *rec_term, uint64_t *rec_conflict_term, uint64_t *rec_conflict_slot, uint32_t *rec_kind);
 
+/* ---- the CRaft leader's log (SS_PROTO_CRAFT engines; every other protocol gets SS_ERR_INVALID_ARG) ----------------
+ * The leader half of the loop the follower above closes: request batches coded into the leader's log
+ * (handle_req_batch, craft/request.rs:70-116), AppendEntries frames out (handle_logged_leader_append,
+ * craft/durability.rs:12-127, and bcast_heartbeats, craft/leadership.rs:249-279), conflict replies backed off on the device
+ * (handle_msg_append_entries_reply's conflict branch, craft/messages.rs:386-406).  The code is (d, p) = (majority,
+ * population - majority) (craft/mod.rs:527-536), so population >= 3.
+ * Peer indexing: the engine's match / next_slot / try_next rows are the population - 1 peers with `me` excluded
+ * (raft/mod.rs:560-562): peer index q <-> replica q < me ? q : q + 1.  The same index is the frame_peer of
+ * ss_append_reply_parse_dev and the rec_peer of ss_engine_raft_ingest.
+ * State, allocated when the log is first used: log_start [G]; try_next [P][G]; per position of the engine's raft_window
+ * ring (slot s at s & (W - 1)): data_len, shard_addr (shard j of the entry at shard_addr + j * plane_stride, 16-byte
+ * aligned) and log_offset.  Entry terms are the engine's `terms` ring: while the log is in use every slot of
+ * [log_start, log_end) stays in the ring.  Slot 0 is the null entry (data_len 0, term 0).
+ * Taking the log into use: ss_engine_craft_log_view_get or any call below.  From then on ss_engine_raft_append returns
+ * SS_ERR_INVALID_ARG (an entry without a codeword cannot be sent); once ss_engine_raft_append has run, the calls below
+ * return SS_ERR_INVALID_ARG.  An engine that never uses the log behaves as before.
+ * Stated differences from the reference:
+ *   1. try_next is kept apart from the success-reply ingest: every pack first takes try = max(try_next, next_slot), which
+ *      is the reference's try_next_slot = max(try_next_slot, end_slot + 1) of messages.rs:281-283 applied lazily;
+ *   2. within one batch of replies, success replies (ss_engine_raft_ingest) are applied before conflicts, and a pair's
+ *      several conflicts are walked in frame order but answered by one resend, [next_slot, the last one's end_slot];
+ *      when the last one finds next_slot == 1 the pair gets no resend at all (want_end UINT64_MAX), where the reference
+ *      would already have resent for the earlier ones -- the next pack from try_next = 1 sends the log from slot 1;
+ *   3. the log is a ring of raft_window entries: a proposal that would hold more than raft_window slots of
+ *      [log_start, log_end] is refused (SS_DEV_STATUS_RAFT_WINDOW_FULL);
+ *   4. a prev_slot below log_start is not an error but pair status SS_APPEND_PAIR_SNAPSHOTTED;
+ *   5. the full_copy flag only chooses which shards a frame or record carries: the commit threshold stays
+ *      majority + fault_tolerance. */
+typedef struct ss_engine_craft_log_view {
+    uint64_t n_groups;
+    uint32_t population, raft_window, data_shards, total_shards;
+    uint64_t plane_stride;      /* of every ss_engine_craft_propose so far (0: none yet) */
+    uint64_t *log_start;        /* [G] the reference's start_slot */
+    uint32_t *try_next;         /* [P][G] try_next_slot */
+    uint32_t *data_len;         /* [G][raft_window] */
+    uint64_t *shard_addr;       /* [G][raft_window] device address of shard 0's slot */
+    uint64_t *log_offset;       /* [G][raft_window] the entry's offset in the leader's log file: the host may rewrite it
+                                   once the entry's write has landed (durability.rs:181-186); the packer sends what is there */
+} ss_engine_craft_log_view;
+int ss_engine_craft_log_view_get(ss_engine *engine, ss_engine_craft_log_view *view);
+/* handle_req_batch for every group g with data_len[g] > 0: one entry at log_end[g] in curr_term[g] (terms ring and log_end
+ * written as ss_engine_raft_append does).  The batch arena[data_off[g] .. + data_len[g]) is coded with d = majority,
+ * p = population - majority by one launch of the ragged encoder (SS_RS_OUT_PADDED16 | SS_RS_EMIT_DATA): shard j goes to
+ * the caller-owned plane shards + j * plane_stride at shard_off[g], SS_CW_SLOT_PITCH(ceil(data_len / d)) bytes per group,
+ * placed by an exclusive scan in group order; *need (device, may be NULL) = the total pitch.  The entry records
+ * shard_addr = shards + shard_off[g] and log_offset[g] (device [G], NULL = 0).  plane_stride: a multiple of 32, the same
+ * on every call; shards and wal 16-byte aligned.  The caller may rotate several stores: a store must outlive its entries
+ * until ss_engine_craft_advance retires them.
+ * The leader's own DurEntry::LogEntry record{term, reqs_cw: shard `me` (shards 0..majority when full_copy), external:
+ * true, log_offset: 0} (request.rs:79-104) goes to wal + wal_off[g], its 16-byte-aligned region placed by an exclusive
+ * scan in group order: 8-byte big-endian length, DurEntry variant 1, the entry; wal_len[g] = its length.
+ * Refusals leave the group unchanged: slot_out, shard_off and wal_off UINT64_MAX, wal_len 0:
+ *   log_end + 1 - log_start > raft_window   SS_DEV_STATUS_RAFT_WINDOW_FULL (no room taken)
+ *   a slot past plane_stride               SS_DEV_STATUS_STORE_FULL
+ *   a record region past wal_capacity      SS_DEV_STATUS_FRAME_OVERFLOW
+ * The offsets are monotone, so the groups that propose are a prefix of those that fit the window.  Groups with
+ * data_len 0 get the same UINT64_MAX outputs and no status bit.  No host synchronisation. */
+int ss_engine_craft_propose(ss_engine *engine, uint32_t me, const uint8_t *arena, const uint64_t *data_off, const uint32_t *data_len,
+                            uint8_t *shards, uint64_t plane_stride, uint64_t *shard_off, uint64_t *slot_out, uint64_t *need,
+                            const uint64_t *log_offset, uint8_t *wal, uint64_t wal_capacity, uint64_t *wal_off, uint64_t *wal_len,
+                            int full_copy);
+/* the snapshot's start_slot move (craft/snapshot.rs:142,184): log_start moves by clamp(upto - log_start, 0,
+ * min(last_snap, last_commit) - log_start); upto is device [G].  A host that executes behind last_commit passes its
+ * last_exec through upto. */
+int ss_engine_craft_advance(ss_engine *engine, const uint64_t *upto);
+typedef struct ss_append_pack_spec {
+    uint32_t me;                /* the leader's replica id, < population */
+    uint32_t append_variant;    /* index of AppendEntries in PeerMsg (0), < 2^16 */
+    uint32_t msg_chunk_size;    /* entries per frame, >= 1 (the reference's default is 10, mod.rs:101) */
+    uint32_t full_copy;         /* non-zero: every entry carries shards 0..majority instead of the peer's own */
+    uint32_t heartbeat;         /* non-zero: one empty frame per pair (bcast_heartbeats) */
+    uint32_t pad0;
+} ss_append_pack_spec;
+/* pair_status[q * G + g] */
+#define SS_APPEND_PAIR_SENT 0u          /* frames written */
+#define SS_APPEND_PAIR_NOTHING 1u       /* nothing to send */
+#define SS_APPEND_PAIR_SNAPSHOTTED 2u   /* prev_slot < log_start: the reference errs ("snapshotted slot queried") */
+#define SS_APPEND_PAIR_OVERFLOW 3u      /* cut by out_capacity or max_frames: nothing written, try_next unchanged */
+/* AppendEntries frames for every (peer q, group g), after try = max(try_next, next_slot):
+ *   entries (heartbeat == 0): end = want_end ? min(want_end[q*G + g], log_end - 1) : log_end - 1 (want_end device
+ *     [P][G], may be NULL; UINT64_MAX: NOTHING for that pair).  try < 1 or prev_slot = try - 1 >= log_end: NOTHING;
+ *     prev_slot < log_start: SNAPSHOTTED; end >= try: the entries [try, end] go out in frames of msg_chunk_size entries
+ *     and try_next = end + 1 (durability.rs:60-125); otherwise NOTHING.
+ *   heartbeat: one empty frame with prev_slot = min(try - 1, log_end - 1) (SNAPSHOTTED below log_start); want_end is
+ *     not read.
+ * Every pair not cut leaves try_next = try or, when entries went out, end + 1.
+ * Frame bytes: PeerMessage::Msg{AppendEntries{term: curr_term, prev_slot, prev_term: term of prev_slot, entries,
+ * leader_commit: last_commit, last_snap}} behind its 8-byte big-endian length; each entry LogEntry{term, reqs_cw:
+ * RSCodeword holding replica(q)'s shard (shards 0..majority when full_copy), data_copy None, external: false,
+ * log_offset} -- the bytes ss_follower_append takes.
+ * Placement: frame k at out + frame_off[k], frame_len[k] bytes, in its own 16-byte-aligned region (the bytes from
+ * frame_len to the region's end are not written), regions back to back in (peer, group, chunk) order, so each peer's
+ * frames are contiguous; frame_group[k] = g, frame_peer[k] = q.  A pair whose region ends past out_capacity or whose
+ * frames end past max_frames is not written: OVERFLOW, SS_DEV_STATUS_FRAME_OVERFLOW.  The offsets are monotone, so the
+ * written pairs are a prefix of those with frames.  *n_frames (device) = the frames written; entries from there on are
+ * not written.  *total (device, may be NULL) = the bytes every pair with frames asked for.  out 16-byte aligned.
+ * Cost: a warp per pair plans and places (lanes over its frames), a warp per frame writes it. */
+int ss_frame_append_pack_dev(ss_engine *engine, const ss_append_pack_spec *spec, const uint64_t *want_end, uint8_t *out,
+                             uint64_t out_capacity, uint64_t *frame_off, uint64_t *frame_len, uint32_t *frame_group, uint8_t *frame_peer,
+                             uint64_t max_frames, uint64_t *n_frames, uint32_t *pair_status, uint64_t *total);
+/* The conflict branch for the reply frames of one ss_append_reply_parse_dev call (the same buf, frame_off, frame_group,
+ * frame_peer, its rec_kind and reply_variant): each SS_APPEND_REPLY_CONFLICT frame's end_slot and (conflict_term,
+ * conflict_slot) are decoded again, and each pair's conflicts are applied in frame order: next_slot == 1 -> try_next = 1,
+ * no resend; otherwise next_slot - 1, then down while next_slot > log_start, term[next_slot] == conflict_term,
+ * next_slot >= conflict_slot and next_slot > 1; try_next = next_slot; want_end[q*G + g] = end_slot.  Pairs without a
+ * conflict get want_end UINT64_MAX.  The resend is ss_frame_append_pack_dev(..., want_end, ...); a walk that stops at
+ * log_start makes that pack report SNAPSHOTTED for the pair.  (population - 1) * n_groups < 2^32 - 1. */
+int ss_engine_craft_backoff(ss_engine *engine, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off,
+                            const uint32_t *frame_group, const uint8_t *frame_peer, const uint32_t *rec_kind, uint64_t n_frames,
+                            uint32_t reply_variant, uint64_t *want_end);
+
 /* ---- tuning / introspection (bench + tests) ------------------------------------------------ */
 /* Tuning knob for experiments; 0 = the defaults.
  *   bits 0-3  kernel choice / register budget: 1 = flat one-column-per-thread RS(3,2) kernel instead of the row kernel,

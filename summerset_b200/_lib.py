@@ -140,6 +140,11 @@ SIGNATURES = {
     "ss_follower_append": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _vp, _u64, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                 _vp, _vp, _vp, _vp]),
     "ss_append_reply_parse_dev": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _u64, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "ss_engine_craft_log_view_get": (_i, [_vp, _vp]),
+    "ss_engine_craft_propose": (_i, [_vp, _u32, _vp, _vp, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _vp, _u64, _vp, _vp, _i]),
+    "ss_engine_craft_advance": (_i, [_vp, _vp]),
+    "ss_frame_append_pack_dev": (_i, [_vp, _vp, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp, _vp, _vp]),
+    "ss_engine_craft_backoff": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _u32, _vp]),
     "ss_rs_set_variant": (_i, [_vp, _i]),
     "ss_rs_last_kernel": (C.c_char_p, [_vp]),
     "ss_rs_jit_status": (C.c_char_p, [_vp]),
@@ -228,6 +233,19 @@ class FollowerView(C.Structure):
                 ("held", C.c_void_p), ("data_len", C.c_void_p)]
 
 
+class CraftLogView(C.Structure):
+    """ss_engine_craft_log_view"""
+    _fields_ = [("n_groups", C.c_uint64), ("population", C.c_uint32), ("raft_window", C.c_uint32), ("data_shards", C.c_uint32),
+                ("total_shards", C.c_uint32), ("plane_stride", C.c_uint64), ("log_start", C.c_void_p), ("try_next", C.c_void_p),
+                ("data_len", C.c_void_p), ("shard_addr", C.c_void_p), ("log_offset", C.c_void_p)]
+
+
+class AppendPackSpec(C.Structure):
+    """ss_append_pack_spec"""
+    _fields_ = [("me", C.c_uint32), ("append_variant", C.c_uint32), ("msg_chunk_size", C.c_uint32), ("full_copy", C.c_uint32),
+                ("heartbeat", C.c_uint32), ("pad0", C.c_uint32)]
+
+
 class PrepareReplyRec(C.Structure):
     """ss_prepare_reply_rec (64 bytes)"""
     _fields_ = [("slot", C.c_uint64), ("trigger_slot", C.c_uint64), ("endprep_slot", C.c_uint64), ("ballot", C.c_uint64),
@@ -262,6 +280,8 @@ SS_APPEND_REPLY_INGEST = 0xFFFFFFF0
 SS_APPEND_REPLY_CONFLICT = 0xFFFFFFF1
 SS_APPEND_REPLY_HIGHER_TERM = 0xFFFFFFF2
 SS_APPEND_REPLY_END_RANGE = 0xFFFFFFF3
+# pair statuses of ss_frame_append_pack_dev
+SS_APPEND_PAIR_SENT, SS_APPEND_PAIR_NOTHING, SS_APPEND_PAIR_SNAPSHOTTED, SS_APPEND_PAIR_OVERFLOW = range(4)
 
 
 class SummersetError(RuntimeError):

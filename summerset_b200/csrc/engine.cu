@@ -31,37 +31,9 @@
 #include <new>
 
 #include "device_common.cuh"
+#include "engine_state.hpp"
 #include "ss_internal.hpp"
 #include "window_ring.cuh"
-
-struct ss_engine {
-    ss_ctx *ctx = nullptr;
-    ss_rs_coder *coder = nullptr;
-    ss_engine_config cfg{};
-    uint64_t G = 0;
-    uint32_t n = 0, majority = 0, threshold = 0, d = 0, T = 0;
-    uint32_t L = 0, ds = 0;
-    // Paxos family
-    uint64_t *planes = nullptr, *bal_prepared = nullptr, *inst_bal = nullptr, *accepting = nullptr, *committed = nullptr;
-    uint64_t *window_base = nullptr;        // [G] absolute slot of window position 0
-    bool windowed = false;                  // a base may be non-zero: set by ss_engine_advance / ss_engine_window_get
-    uint32_t *commit_bar = nullptr;
-    uint8_t *shards = nullptr;
-    // ragged proposals: allocated on the first ss_engine_propose_ragged call
-    uint32_t *rg_len = nullptr;             // [G] effective length (0 = the group does not propose)
-    uint64_t *rg_partials = nullptr;        // [scan_tiles(G)] tile sums of the pitch scan
-    uint64_t *rg_need = nullptr;            // [1] total pitch, when the caller does not ask for it
-    // Crossword
-    uint8_t *policy_idx = nullptr;          // [G*64]
-    uint32_t *policies = nullptr, *lut_bits = nullptr;
-    uint32_t n_policies = 0, lut_words = 0;
-    int balanced = 1;
-    // Raft
-    uint32_t *match = nullptr, *next_slot = nullptr, *last_commit = nullptr, *log_end = nullptr, *curr_term = nullptr,
-             *terms = nullptr, *last_snap = nullptr;
-    uint8_t *touched = nullptr;
-    uint32_t W = 0, n_peers = 0;
-};
 
 namespace ssb {
 
@@ -526,6 +498,7 @@ int ss_engine_destroy(ss_engine *e) {
                     e->last_snap, e->touched, e->rg_len, e->rg_partials, e->rg_need};
     for (void *b : bufs)
         if (b) cudaFree(b);
+    craft_log_free(e);
     if (e->coder) ss_rs_coder_destroy(e->coder);
     if (e->ctx) ctx_release(e->ctx);
     delete e;
@@ -794,8 +767,10 @@ int ss_engine_tick(ss_engine *e, uint64_t *newly) {
 int ss_engine_raft_append(ss_engine *e, const uint32_t *n_new) {
     if (e == nullptr || n_new == nullptr) return set_error(SS_ERR_INVALID_ARG, "null argument");
     if (e->match == nullptr) return set_error(SS_ERR_INVALID_ARG, "not a Raft engine");
+    if (e->log_in_use) return set_error(SS_ERR_INVALID_ARG, "the CRaft log is in use: an entry without a codeword cannot be sent");
     ss_ctx *ctx = e->ctx;
     SS_TRY(ctx_bind(ctx));
+    e->raft_appended = true;
     engine_raft_append_kernel<<<eng_grid(ctx, e->G), kEngThreads, 0, ctx->stream>>>(n_new, e->G, e->W, e->curr_term, e->last_commit,
                                                                                  e->log_end, e->terms, ctx->dev_status);
     return launched(ctx);

@@ -29,6 +29,10 @@ torch tensors (zero-copy views) so tests can read results and install state; it 
     prepare_reply_parse(ctx, buf, frame_off, d, T)   the new leader's side: PrepareReply frames -> vote records
     RaftEngine(ctx, G, population[, fault_tolerance, craft])
         append(n_new) / on_append_replies(records) / tick()      raft/messages.rs:243-309, craft/messages.rs:300-308
+        CRaft leader's log: propose(me, arena, data_off, data_len, store, wal)   handle_req_batch (craft/request.rs:70-116)
+        pack_append(me, out, max_frames[, want_end, heartbeat])   AppendEntries frames (craft/durability.rs:12-127)
+        backoff(buf, frame_off, frame_group, frame_peer, rec_kind)   the conflict branch (craft/messages.rs:386-406)
+        advance_log(upto) / log_view()      the snapshot's start_slot move; log_start, try_next and the entry rings
     Follower(ctx, G, population, me[, window])   the CRaft follower
         append(buf, frame_off, frame_group, frame_peer, store, wal)   handle_msg_append_entries (craft/messages.rs:14-252):
                                             store, LogEntry / Metadata records, AppendEntriesReply cells
@@ -218,6 +222,74 @@ class RaftEngine(_EngineBase):
     def tick(self) -> Tuple[torch.Tensor, torch.Tensor]:
         check(self.lib.ss_engine_tick(self.h, None))
         return self.last_commit, self.last_snap
+
+    # ---- the CRaft leader's log (ss_engine_craft_*): using it refuses append() from then on, and vice versa ----
+    def log_view(self) -> dict:
+        """Takes the log into use and returns zero-copy views: log_start int64 [G], try_next int32 [P, G], and per ring
+        position data_len int32, shard_addr and log_offset int64 [G, W]."""
+        v = _lib.CraftLogView()
+        check(self.lib.ss_engine_craft_log_view_get(self.h, C.byref(v)))
+        G, W = self.G, self.W
+        return dict(log_start=self._tensor(v.log_start, (G,), "<i8", torch.int64),
+                    try_next=self._tensor(v.try_next, (self.P, G), "<i4", torch.int32),
+                    data_len=self._tensor(v.data_len, (G, W), "<i4", torch.int32),
+                    shard_addr=self._tensor(v.shard_addr, (G, W), "<i8", torch.int64),
+                    log_offset=self._tensor(v.log_offset, (G, W), "<i8", torch.int64), plane_stride=v.plane_stride)
+
+    def propose(self, me: int, arena: torch.Tensor, data_off: torch.Tensor, data_len: torch.Tensor, store: torch.Tensor,
+                wal: torch.Tensor, log_offset: Optional[torch.Tensor] = None, wal_capacity: Optional[int] = None,
+                full_copy: bool = False) -> dict:
+        """One entry per group with a batch (data_len int32 [G] > 0), coded into store (uint8 [T, plane_stride], caller-owned,
+        alive until advance_log retires its entries) and the leader's LogEntry record into wal (uint8, 16-byte aligned).
+        Returns device tensors slot_out, shard_off, wal_off (int64 [G], -1 = not proposed), wal_len (int64 [G]) and
+        need (int64 [1])."""
+        assert arena.dtype == torch.uint8 and data_off.dtype == torch.int64 and data_len.dtype == torch.int32
+        assert store.dtype == torch.uint8 and store.dim() == 2 and store.is_contiguous() and wal.dtype == torch.uint8
+        assert log_offset is None or (log_offset.dtype == torch.int64 and log_offset.numel() == self.G)
+        e = lambda n=self.G: torch.empty(n, dtype=torch.int64, device=self.dev)
+        out = dict(slot_out=e(), shard_off=e(), wal_off=e(), wal_len=e(), need=e(1))
+        p = lambda x: None if x is None else x.data_ptr()
+        check(self.lib.ss_engine_craft_propose(self.h, me, p(arena), p(data_off), p(data_len), p(store), store.shape[1],
+                                               p(out["shard_off"]), p(out["slot_out"]), p(out["need"]), p(log_offset), p(wal),
+                                               wal.numel() if wal_capacity is None else wal_capacity, p(out["wal_off"]),
+                                               p(out["wal_len"]), 1 if full_copy else 0))
+        return out
+
+    def pack_append(self, me: int, out: torch.Tensor, max_frames: int, want_end: Optional[torch.Tensor] = None,
+                    heartbeat: bool = False, full_copy: bool = False, msg_chunk_size: int = 10, append_variant: int = 0,
+                    out_capacity: Optional[int] = None) -> dict:
+        """AppendEntries frames for every (peer, group) into out (uint8, 16-byte aligned).  Returns device tensors
+        frame_off, frame_len (int64 [max_frames]), frame_group (int32), frame_peer (uint8: the peer index), n_frames and
+        total (int64 [1]) and pair_status (int32 [P, G])."""
+        assert out.dtype == torch.uint8 and (want_end is None or (want_end.dtype == torch.int64 and want_end.numel() == self.P * self.G))
+        dev, cap = out.device, max(max_frames, 1)
+        res = dict(frame_off=torch.empty(cap, dtype=torch.int64, device=dev), frame_len=torch.empty(cap, dtype=torch.int64, device=dev),
+                   frame_group=torch.empty(cap, dtype=torch.int32, device=dev), frame_peer=torch.empty(cap, dtype=torch.uint8, device=dev),
+                   n_frames=torch.empty(1, dtype=torch.int64, device=dev), total=torch.empty(1, dtype=torch.int64, device=dev),
+                   pair_status=torch.empty((self.P, self.G), dtype=torch.int32, device=dev))
+        spec = _lib.AppendPackSpec(me, append_variant, msg_chunk_size, 1 if full_copy else 0, 1 if heartbeat else 0, 0)
+        p = lambda x: None if x is None else x.data_ptr()
+        check(self.lib.ss_frame_append_pack_dev(self.h, C.byref(spec), p(want_end), p(out), out.numel() if out_capacity is None else out_capacity,
+                                                p(res["frame_off"]), p(res["frame_len"]), p(res["frame_group"]), p(res["frame_peer"]),
+                                                max_frames, p(res["n_frames"]), p(res["pair_status"]), p(res["total"])))
+        return res
+
+    def backoff(self, buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor, frame_peer: torch.Tensor,
+                rec_kind: torch.Tensor, reply_variant: int = 1) -> torch.Tensor:
+        """The conflict replies among the frames append_reply_parse took (with its rec_kind): next_slot and try_next walk
+        back.  Returns want_end (int64 [P, G], -1 = no resend), which pack_append(want_end=...) takes."""
+        assert buf.dtype == torch.uint8 and frame_off.dtype == torch.int64 and frame_group.dtype == torch.int32
+        assert frame_peer.dtype == torch.uint8 and rec_kind.dtype == torch.int32
+        want_end = torch.empty((self.P, self.G), dtype=torch.int64, device=self.dev)
+        check(self.lib.ss_engine_craft_backoff(self.h, buf.data_ptr(), buf.numel(), frame_off.data_ptr(), frame_group.data_ptr(),
+                                               frame_peer.data_ptr(), rec_kind.data_ptr(), frame_off.numel(), reply_variant,
+                                               want_end.data_ptr()))
+        return want_end
+
+    def advance_log(self, upto: torch.Tensor) -> None:
+        """log_start moves towards upto (int64 [G]), never past min(last_snap, last_commit)."""
+        assert upto.is_cuda and upto.dtype == torch.int64 and upto.numel() == self.G
+        check(self.lib.ss_engine_craft_advance(self.h, upto.data_ptr()))
 
 
 class Acceptor:

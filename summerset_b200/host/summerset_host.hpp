@@ -433,4 +433,30 @@ inline void append_reply_parse(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len
                                     rec_group, rec_peer, rec_end_slot, rec_term, rec_conflict_term, rec_conflict_slot, rec_kind));
 }
 
+// the CRaft leader's log on a CRaft engine; every pointer is a device pointer (see the header's ss_engine_craft_* block)
+inline ss_engine_craft_log_view craft_log_view(ss_engine *e) {
+    ss_engine_craft_log_view v{};
+    check(ss_engine_craft_log_view_get(e, &v));
+    return v;
+}
+inline void craft_propose(ss_engine *e, uint32_t me, const uint8_t *arena, const uint64_t *data_off, const uint32_t *data_len,
+                          uint8_t *shards, uint64_t plane_stride, uint64_t *shard_off, uint64_t *slot_out, uint8_t *wal,
+                          uint64_t wal_capacity, uint64_t *wal_off, uint64_t *wal_len, const uint64_t *log_offset = nullptr,
+                          uint64_t *need = nullptr, bool full_copy = false) {
+    check(ss_engine_craft_propose(e, me, arena, data_off, data_len, shards, plane_stride, shard_off, slot_out, need, log_offset, wal,
+                                  wal_capacity, wal_off, wal_len, full_copy ? 1 : 0));
+}
+inline void append_pack(ss_engine *e, const ss_append_pack_spec &spec, const uint64_t *want_end, uint8_t *out, uint64_t out_capacity,
+                        uint64_t *frame_off, uint64_t *frame_len, uint32_t *frame_group, uint8_t *frame_peer, uint64_t max_frames,
+                        uint64_t *n_frames, uint32_t *pair_status, uint64_t *total = nullptr) {
+    check(ss_frame_append_pack_dev(e, &spec, want_end, out, out_capacity, frame_off, frame_len, frame_group, frame_peer, max_frames,
+                                   n_frames, pair_status, total));
+}
+inline void craft_backoff(ss_engine *e, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
+                          const uint8_t *frame_peer, const uint32_t *rec_kind, uint64_t n_frames, uint64_t *want_end,
+                          uint32_t reply_variant = 1) {
+    check(ss_engine_craft_backoff(e, buf, buf_len, frame_off, frame_group, frame_peer, rec_kind, n_frames, reply_variant, want_end));
+}
+inline void craft_advance(ss_engine *e, const uint64_t *upto) { check(ss_engine_craft_advance(e, upto)); }
+
 }  // namespace ssb
