@@ -1033,8 +1033,31 @@ int ss_follower_create(ss_ctx *ctx, const ss_follower_config *cfg, uint64_t n_gr
 int ss_follower_destroy(ss_follower *follower);
 int ss_follower_view_get(ss_follower *follower, ss_follower_view *view);
 /* the snapshot's start_slot move (craft/snapshot.rs:130-198): upto (device [G] absolute slots) -- start_slot moves by
- * k = clamp(upto - start_slot, 0, last_commit - start_slot), so never past last_commit */
+ * k = clamp(upto - start_slot, 0, last_commit - start_slot), so never past last_commit.  A host that executes behind
+ * last_commit passes last_exec (ss_follower_exec_view) through upto, so that no entry leaves before it executes. */
 int ss_follower_advance(ss_follower *follower, const uint64_t *upto);
+typedef struct ss_follower_exec_view {
+    uint64_t n_groups;
+    uint64_t *last_exec;        /* [G] the last executed slot; 0 at creation (the slot-0 null entry) */
+} ss_follower_exec_view;
+int ss_follower_exec_view_get(ss_follower *follower, ss_follower_exec_view *view);
+/* Execution of the committed entries, the walk of handle_msg_append_entries (craft/messages.rs:198-240): for every
+ * group, from max(last_exec + 1, start_slot) while the slot is at most last_commit, an entry holding fewer than d shards
+ * stops the walk (the commit walk never passes one, but state installed through the view may hold one); an entry with
+ * data_len == 0 is a null codeword get_data refuses (rscoding.rs:581-583): it does not execute and its group's walk
+ * stops there (SS_DEV_STATUS_EXEC_NULL); any other executes and last_exec moves to it.  Its payload is get_data's
+ * output, the first data_len bytes of data shards 0..d-1 concatenated (rscoding.rs:581-683): a held data shard is read
+ * at shard_addr + rank * SS_CW_SLOT_PITCH(shard_len) (rank among the held shards, the store layout of
+ * ss_follower_append), a missing one is regenerated from the first d held shards in index order, as reconstruct_data
+ * chooses them (rscoding.rs:490-537).  The caller's stores must still hold the shards.
+ * Outputs, records, capacities, totals and status bits are those of ss_acceptor_execute: executed entries ordered by
+ * (group, slot), record k = rec_group[k], rec_slot[k] (absolute), rec_off[k], rec_len[k] (= data_len); the payload at
+ * out + rec_off[k] in a region of round_up(data_len, 16) bytes, zero past data_len, placed by exclusive scans (out
+ * 16-byte aligned); totals (device u64[2], may be NULL): records and bytes the walk asked for; an entry whose record
+ * index reaches rec_capacity or whose region ends past out_capacity does not execute and its group's walk stops there
+ * (SS_DEV_STATUS_EXEC_FULL).  The records written are a prefix; a host drains by calling again. */
+int ss_follower_execute(ss_follower *follower, uint8_t *out, uint64_t out_capacity, uint32_t *rec_group, uint64_t *rec_slot,
+                        uint64_t *rec_off, uint32_t *rec_len, uint64_t rec_capacity, uint64_t *totals);
 /* Verdicts of ss_follower_append, beside the PeerMsg variant index k (another message; 0x80000000 | k for the
  * PeerMessage variants) and SS_FRAME_KIND_MALFORMED */
 #define SS_FOLLOWER_VERDICT_ACCEPTED 0xfffffff0u      /* log matched: appended, absorbed or found its entries present */
@@ -1134,8 +1157,11 @@ int ss_append_reply_parse_dev(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len,
  *   3. the log is a ring of raft_window entries: a proposal that would hold more than raft_window slots of
  *      [log_start, log_end] is refused (SS_DEV_STATUS_RAFT_WINDOW_FULL);
  *   4. a prev_slot below log_start is not an error but pair status SS_APPEND_PAIR_SNAPSHOTTED;
- *   5. the full_copy flag only chooses which shards a frame or record carries: the commit threshold stays
- *      majority + fault_tolerance. */
+ *   5. switch_assignment_mode (craft/leadership.rs:282-288) is split: the full_copy flag of ss_engine_craft_propose and
+ *      ss_frame_append_pack_dev chooses which shards a record or frame carries, ss_engine_craft_set_full_copy the commit
+ *      threshold; the detection (population - alive >= fault_tolerance) and the resend of the entries already sent
+ *      with one shard (left commented out at leadership.rs:100-135; a host rewinds try_next through the log view) stay
+ *      with the host. */
 typedef struct ss_engine_craft_log_view {
     uint64_t n_groups;
     uint32_t population, raft_window, data_shards, total_shards;
@@ -1171,8 +1197,30 @@ int ss_engine_craft_propose(ss_engine *engine, uint32_t me, const uint8_t *arena
                             int full_copy);
 /* the snapshot's start_slot move (craft/snapshot.rs:142,184): log_start moves by clamp(upto - log_start, 0,
  * min(last_snap, last_commit) - log_start); upto is device [G].  A host that executes behind last_commit passes its
- * last_exec through upto. */
+ * last_exec (ss_engine_craft_exec_view) through upto, so that no entry leaves before it executes. */
 int ss_engine_craft_advance(ss_engine *engine, const uint64_t *upto);
+/* The commit threshold of ss_engine_tick, the commit half of switch_assignment_mode (craft/leadership.rs:282-288):
+ * non-zero sets it to majority, as a leader in full-copy mode commits (craft/messages.rs:300-310), zero restores
+ * majority + fault_tolerance.  ss_engine_view.threshold reports it; the next tick uses it.  SS_PROTO_CRAFT engines only
+ * (SS_ERR_INVALID_ARG otherwise), whether or not the log is in use; it writes no device state. */
+int ss_engine_craft_set_full_copy(ss_engine *engine, int full_copy);
+typedef struct ss_engine_craft_exec_view {
+    uint64_t n_groups;
+    uint64_t *last_exec;        /* [G] the last executed slot; 0 when the log is taken into use (the slot-0 null entry) */
+} ss_engine_craft_exec_view;
+int ss_engine_craft_exec_view_get(ss_engine *engine, ss_engine_craft_exec_view *view);
+/* Execution on the leader, the execution half of handle_msg_append_entries_reply's success branch
+ * (craft/messages.rs:316-359): for every group, from max(last_exec + 1, log_start) while the slot is at most
+ * last_commit, an entry with data_len == 0 is a null codeword get_data refuses (rscoding.rs:581-583): it does not
+ * execute and its group's walk stops there (SS_DEV_STATUS_EXEC_NULL); any other executes and last_exec moves to it.
+ * The leader's last_commit is the reference's new_commit: the leader holds every shard of its own entries, so none is
+ * postponed and no Reconstruct is needed, and the reference's last_commit equals new_commit on every path the device
+ * reaches.  The payload is get_data's output, the first data_len bytes of data shards 0..d-1 concatenated
+ * (rscoding.rs:581-683), read at shard_addr + j * plane_stride: the stores of ss_engine_craft_propose must still hold
+ * the entries.  Outputs, records, capacities, totals and status bits are those of ss_acceptor_execute (see
+ * ss_follower_execute).  Takes the log into use, and is refused once ss_engine_raft_append has run. */
+int ss_engine_craft_execute(ss_engine *engine, uint8_t *out, uint64_t out_capacity, uint32_t *rec_group, uint64_t *rec_slot,
+                            uint64_t *rec_off, uint32_t *rec_len, uint64_t rec_capacity, uint64_t *totals);
 typedef struct ss_append_pack_spec {
     uint32_t me;                /* the leader's replica id, < population */
     uint32_t append_variant;    /* index of AppendEntries in PeerMsg (0), < 2^16 */

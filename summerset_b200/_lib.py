@@ -145,6 +145,11 @@ SIGNATURES = {
     "ss_engine_craft_advance": (_i, [_vp, _vp]),
     "ss_frame_append_pack_dev": (_i, [_vp, _vp, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp, _vp, _vp]),
     "ss_engine_craft_backoff": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _u32, _vp]),
+    "ss_engine_craft_set_full_copy": (_i, [_vp, _i]),
+    "ss_engine_craft_exec_view_get": (_i, [_vp, _vp]),
+    "ss_engine_craft_execute": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp]),
+    "ss_follower_exec_view_get": (_i, [_vp, _vp]),
+    "ss_follower_execute": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp]),
     "ss_rs_set_variant": (_i, [_vp, _i]),
     "ss_rs_last_kernel": (C.c_char_p, [_vp]),
     "ss_rs_jit_status": (C.c_char_p, [_vp]),
@@ -240,6 +245,16 @@ class CraftLogView(C.Structure):
                 ("data_len", C.c_void_p), ("shard_addr", C.c_void_p), ("log_offset", C.c_void_p)]
 
 
+class CraftExecView(C.Structure):
+    """ss_engine_craft_exec_view"""
+    _fields_ = [("n_groups", C.c_uint64), ("last_exec", C.c_void_p)]
+
+
+class FollowerExecView(C.Structure):
+    """ss_follower_exec_view"""
+    _fields_ = [("n_groups", C.c_uint64), ("last_exec", C.c_void_p)]
+
+
 class AppendPackSpec(C.Structure):
     """ss_append_pack_spec"""
     _fields_ = [("me", C.c_uint32), ("append_variant", C.c_uint32), ("msg_chunk_size", C.c_uint32), ("full_copy", C.c_uint32),
@@ -253,7 +268,7 @@ class PrepareReplyRec(C.Structure):
                 ("kind", C.c_uint32), ("pad", C.c_uint32)]
 
 
-# ss_acceptor_execute's bits of the device status word
+# the execution walks' bits of the device status word (ss_acceptor_execute, ss_follower_execute, ss_engine_craft_execute)
 SS_DEV_STATUS_EXEC_FULL = 32
 SS_DEV_STATUS_EXEC_NULL = 64
 

@@ -18,6 +18,11 @@
 //     backoff_key_kernel            a thread per reply frame: conflicts keyed by (group, peer)
 //     (CUB radix sort)              stable: each pair's conflicts in frame order
 //     backoff_walk_kernel           a thread per pair: the walk-back over the terms ring, try_next and want_end
+//   ss_engine_craft_execute   the execution half of handle_msg_append_entries_reply's success branch (craft/messages.rs:316-359):
+//     craft_exec_count_kernel       a thread per group: the entries the walk executes, and their payload bytes
+//     (engine.cu's scan)            record indices and payload regions
+//     craft_exec_place_kernel       a thread per group: capacities, the records, last_exec
+//     craft_exec_payload_kernel     a warp per record: get_data's bytes gathered from the planes (exec_payload.cuh)
 //   ss_engine_craft_advance   the snapshot's start_slot move (craft/snapshot.rs:142,184)
 #include <cub/device/device_radix_sort.cuh>
 
@@ -26,6 +31,7 @@
 
 #include "device_common.cuh"
 #include "engine_state.hpp"
+#include "exec_payload.cuh"
 #include "ss_internal.hpp"
 #include "wire_common.cuh"
 
@@ -517,6 +523,91 @@ __global__ void __launch_bounds__(kClThreads) backoff_walk_kernel(const __grid_c
     }
 }
 
+// ---- execution -----------------------------------------------------------------------------------------------------
+struct CraftExecArgs {
+    uint64_t G;
+    uint32_t W, d;
+    uint64_t plane_stride;
+    const uint32_t *last_commit, *ent_len;
+    const uint64_t *log_start, *ent_addr;
+    uint64_t *last_exec;
+    uint64_t *cnt, *bytes;          // [G] per group: records, payload bytes; then their exclusive scans
+    uint64_t *n_exec;               // records written (a prefix: the offsets are monotone)
+    uint8_t *out;
+    uint64_t out_cap;
+    uint32_t *rec_group;
+    uint64_t *rec_slot, *rec_off;
+    uint32_t *rec_len;
+    uint64_t rec_cap;
+    uint32_t *status;
+};
+
+__device__ __forceinline__ uint64_t craft_exec_start(const CraftExecArgs &A, uint64_t g) {
+    const uint64_t s = A.last_exec[g] + 1u, ls = A.log_start[g];
+    return s > ls ? s : ls;
+}
+
+// the data_len of the entry at slot s, or 0 past last_commit (a stop) or at a null entry
+__device__ __forceinline__ uint32_t craft_exec_len(const CraftExecArgs &A, uint64_t g, uint64_t s) {
+    return s <= A.last_commit[g] ? A.ent_len[g * A.W + (s & (A.W - 1u))] : 0u;
+}
+
+__global__ void __launch_bounds__(kClThreads) craft_exec_count_kernel(const __grid_constant__ CraftExecArgs A) {
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kClThreads;
+    for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kClThreads + threadIdx.x; g < A.G; g += stride) {
+        uint64_t n = 0u, b = 0u;
+        uint32_t dl;
+        for (uint64_t s = craft_exec_start(A, g); (dl = craft_exec_len(A, g, s)) != 0u; ++s, ++n) b += cl_round16(dl);
+        A.cnt[g] = n;
+        A.bytes[g] = b;
+    }
+}
+
+__global__ void __launch_bounds__(kClThreads) craft_exec_place_kernel(const __grid_constant__ CraftExecArgs A) {
+    bool full = false, null_ent = false;
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kClThreads;
+    for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kClThreads + threadIdx.x; g < A.G; g += stride) {
+        const uint64_t s0 = craft_exec_start(A, g), lc = A.last_commit[g];
+        uint64_t ro = A.cnt[g], bo = A.bytes[g], s = s0;
+        uint32_t dl;
+        bool cut = false;
+        while ((dl = craft_exec_len(A, g, s)) != 0u) {
+            const uint64_t sz = cl_round16(dl);
+            if (ro >= A.rec_cap || bo > A.out_cap || sz > A.out_cap - bo) { cut = true; break; }
+            A.rec_group[ro] = static_cast<uint32_t>(g);
+            A.rec_slot[ro] = s;
+            A.rec_off[ro] = bo;
+            A.rec_len[ro] = dl;
+            ++ro;
+            bo += sz;
+            ++s;
+        }
+        full |= cut;
+        null_ent |= !cut && s <= lc;                                        // stopped inside the committed prefix
+        if (s != s0) {
+            A.last_exec[g] = s - 1u;
+            atomicMax(reinterpret_cast<unsigned long long *>(A.n_exec), static_cast<unsigned long long>(ro));
+        }
+    }
+    if (full) atomicOr(A.status, SS_DEV_STATUS_EXEC_FULL);
+    if (null_ent) atomicOr(A.status, SS_DEV_STATUS_EXEC_NULL);
+}
+
+// a warp per record: the leader holds every shard of its entries, shard j at shard_addr + j * plane_stride, so the
+// gather never regenerates one and needs neither the coder's matrix nor the GF(2^8) tables
+__global__ void __launch_bounds__(kExecThreads) craft_exec_payload_kernel(const __grid_constant__ CraftExecArgs A) {
+    __shared__ ExecShared S;
+    const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+    const uint32_t all = (1u << A.d) - 1u;
+    const uint64_t n = *A.n_exec;
+    const uint64_t nwarps = static_cast<uint64_t>(gridDim.x) * kExecWarps;
+    for (uint64_t r = static_cast<uint64_t>(blockIdx.x) * kExecWarps + w; r < n; r += nwarps) {
+        const uint64_t g = A.rec_group[r], pos = g * A.W + (A.rec_slot[r] & (A.W - 1u));
+        warp_exec_payload(S, w, lane, A.d, all, A.rec_len[r], nullptr, reinterpret_cast<const uint8_t *>(A.ent_addr[pos]), A.plane_stride,
+                          A.out + A.rec_off[r]);
+    }
+}
+
 // start_slot moves by clamp(upto - log_start, 0, min(last_snap, last_commit) - log_start)
 __global__ void __launch_bounds__(kClThreads)
 craft_advance_kernel(const uint64_t *__restrict__ upto, uint64_t G, uint64_t *__restrict__ log_start,
@@ -539,7 +630,8 @@ static int cl_alloc(ss_ctx *ctx, T **p, size_t count, bool zero) {
 
 void craft_log_free(ss_engine *e) {
     void *bufs[] = {e->log_start, e->try_next, e->ent_len, e->ent_addr, e->ent_log_offset, e->cl_partials, e->cl_words, e->cl_eff,
-                    e->cl_wal, e->pk_frames, e->pk_bytes, e->pk_range, e->bo_keys, e->bo_idx, e->bo_sort_tmp};
+                    e->cl_wal, e->pk_frames, e->pk_bytes, e->pk_range, e->last_exec, e->ex_cnt, e->ex_bytes, e->ex_words, e->bo_keys,
+                    e->bo_idx, e->bo_sort_tmp};
     for (void *b : bufs)
         if (b) cudaFree(b);
 }
@@ -566,13 +658,16 @@ static int craft_log_init(ss_engine *e) {
         (rc = cl_alloc(ctx, &e->cl_partials, scan_tiles(PG > G ? PG : G), false)) || (rc = cl_alloc(ctx, &e->cl_words, 4, false)) ||
         (rc = cl_alloc(ctx, &e->cl_eff, G, false)) || (rc = cl_alloc(ctx, &e->cl_wal, G, false)) ||
         (rc = cl_alloc(ctx, &e->pk_frames, PG, false)) || (rc = cl_alloc(ctx, &e->pk_bytes, PG, false)) ||
-        (rc = cl_alloc(ctx, &e->pk_range, PG, false)) || (rc = cl_alloc(ctx, &e->log_start, G, true))) {
+        (rc = cl_alloc(ctx, &e->pk_range, PG, false)) || (rc = cl_alloc(ctx, &e->log_start, G, true)) ||
+        (rc = cl_alloc(ctx, &e->last_exec, G, true)) || (rc = cl_alloc(ctx, &e->ex_cnt, G, false)) ||
+        (rc = cl_alloc(ctx, &e->ex_bytes, G, false)) || (rc = cl_alloc(ctx, &e->ex_words, 3, false))) {
         // nothing half-built stays behind: a later call starts over, and raft_append stays allowed
         cudaStreamSynchronize(ctx->stream);
         craft_log_free(e);
         e->log_start = nullptr; e->try_next = nullptr; e->ent_len = nullptr; e->ent_addr = nullptr; e->ent_log_offset = nullptr;
         e->cl_partials = nullptr; e->cl_words = nullptr; e->cl_eff = nullptr; e->cl_wal = nullptr;
         e->pk_frames = nullptr; e->pk_bytes = nullptr; e->pk_range = nullptr;
+        e->last_exec = nullptr; e->ex_cnt = nullptr; e->ex_bytes = nullptr; e->ex_words = nullptr;
         e->bo_keys = nullptr; e->bo_idx = nullptr; e->bo_sort_tmp = nullptr; e->bo_cap = 0;
         return rc;
     }
@@ -729,6 +824,51 @@ int ss_engine_craft_backoff(ss_engine *e, const uint8_t *buf, uint64_t buf_len, 
     SS_TRY(launched(ctx));
     backoff_walk_kernel<<<grid, kClThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
+}
+
+int ss_engine_craft_exec_view_get(ss_engine *e, ss_engine_craft_exec_view *v) {
+    if (v == nullptr) return set_error(SS_ERR_INVALID_ARG, "null view");
+    SS_TRY(craft_check(e));
+    SS_TRY(craft_log_init(e));
+    memset(v, 0, sizeof(*v));
+    v->n_groups = e->G;
+    v->last_exec = e->last_exec;
+    return SS_OK;
+}
+
+int ss_engine_craft_execute(ss_engine *e, uint8_t *out, uint64_t out_capacity, uint32_t *rec_group, uint64_t *rec_slot,
+                            uint64_t *rec_off, uint32_t *rec_len, uint64_t rec_capacity, uint64_t *totals) {
+    if (!out || !rec_group || !rec_slot || !rec_off || !rec_len) return set_error(SS_ERR_INVALID_ARG, "null buffer");
+    if (reinterpret_cast<uintptr_t>(out) & 15u) return set_error(SS_ERR_INVALID_ARG, "out must be 16-byte aligned");
+    SS_TRY(craft_check(e));
+    SS_TRY(craft_log_init(e));
+    ss_ctx *ctx = e->ctx;
+    CraftExecArgs A{};
+    A.G = e->G; A.W = e->W; A.d = e->majority; A.plane_stride = e->log_plane_stride;
+    A.last_commit = e->last_commit; A.ent_len = e->ent_len; A.log_start = e->log_start; A.ent_addr = e->ent_addr;
+    A.last_exec = e->last_exec; A.cnt = e->ex_cnt; A.bytes = e->ex_bytes; A.n_exec = e->ex_words;
+    A.out = out; A.out_cap = out_capacity; A.rec_group = rec_group; A.rec_slot = rec_slot; A.rec_off = rec_off; A.rec_len = rec_len;
+    A.rec_cap = rec_capacity; A.status = ctx->dev_status;
+    uint64_t *tot = totals != nullptr ? totals : e->ex_words + 1;
+    const uint32_t grid = cl_grid(ctx, e->G, kClThreads);
+    SS_CUDA(cudaMemsetAsync(e->ex_words, 0, 8, ctx->stream));
+    craft_exec_count_kernel<<<grid, kClThreads, 0, ctx->stream>>>(A);
+    SS_TRY(launched(ctx));
+    SS_TRY(launch_exclusive_scan_u64(ctx, e->ex_cnt, e->G, e->cl_partials, tot));
+    SS_TRY(launch_exclusive_scan_u64(ctx, e->ex_bytes, e->G, e->cl_partials, tot + 1));
+    craft_exec_place_kernel<<<grid, kClThreads, 0, ctx->stream>>>(A);
+    SS_TRY(launched(ctx));
+    // a warp per entry the ring can hold, up to the grid cap; warps past the executed count return at once
+    craft_exec_payload_kernel<<<cl_grid(ctx, e->G * e->W, kExecWarps), kExecThreads, 0, ctx->stream>>>(A);
+    return launched(ctx);
+}
+
+int ss_engine_craft_set_full_copy(ss_engine *e, int full_copy) {
+    if (e == nullptr) return set_error(SS_ERR_INVALID_ARG, "null engine");
+    if (e->cfg.protocol != SS_PROTO_CRAFT) return set_error(SS_ERR_INVALID_ARG, "the full-copy threshold serves CRaft engines only");
+    // craft/messages.rs:300-310: majority in full-copy mode, majority + fault_tolerance otherwise
+    e->threshold = full_copy ? e->majority : e->majority + e->cfg.fault_tolerance;
+    return SS_OK;
 }
 
 int ss_engine_craft_advance(ss_engine *e, const uint64_t *upto) {

@@ -43,6 +43,9 @@ struct ss_engine {
     uint32_t *cl_eff = nullptr;             // [G] effective propose length
     uint64_t *cl_wal = nullptr;             // [G] propose: WAL record lengths
     uint64_t *pk_frames = nullptr, *pk_bytes = nullptr, *pk_range = nullptr;   // [P*G] pack scratch
+    uint64_t *last_exec = nullptr;          // [G] last executed slot (ss_engine_craft_execute)
+    uint64_t *ex_cnt = nullptr, *ex_bytes = nullptr;   // [G] execute scratch: records and payload bytes, then their scans
+    uint64_t *ex_words = nullptr;           // [3] records written, and the totals when the caller passes none
     uint64_t bo_cap = 0;                    // backoff scratch, grow-only
     uint32_t *bo_keys = nullptr, *bo_idx = nullptr;
     void *bo_sort_tmp = nullptr;

@@ -1,0 +1,154 @@
+// exec_payload.cuh -- get_data's bytes of one executed entry, written by one warp (rscoding.rs:490-537, 581-683).
+//
+// Shared by the three execution walks: the acceptor's (acceptor.cu), the CRaft follower's (follower.cu) and the CRaft
+// leader's (craft_leader.cu).  Each calls warp_exec_payload once per record with the entry's held mask and the address
+// rule of its shards: held shard j of rank k (k-th set bit of held) is at src + k * stride.  The acceptor and the
+// follower keep only their held shards in padded store slots (stride SS_CW_SLOT_PITCH(L)); the leader holds every shard
+// of its entries in planes (stride plane_stride, rank = shard index) and so never regenerates one.
+#pragma once
+#include <cstdint>
+
+#include "device_common.cuh"
+#include "ss_internal.hpp"
+
+namespace ssb {
+
+constexpr int kExecThreads = 256;
+constexpr int kExecWarps = kExecThreads / 32;
+constexpr int kChunk = 4;           // sources per Horner pass: their loads are issued together
+
+struct ExecShared {
+    uint8_t exp[512], log[256];
+    uint8_t a[kExecWarps][32][32];  // Gauss-Jordan: lane r owns row r of M[sources] ...
+    uint8_t inv[kExecWarps][32][32];   // ... and of the identity it turns into the inverse
+    uint8_t piv[kExecWarps][32];    // piv[c]: the row that took column c as its pivot
+};
+
+__device__ __forceinline__ uint32_t gmul(const ExecShared &S, uint32_t a, uint32_t b) {
+    return (a != 0u && b != 0u) ? S.exp[S.log[a] + S.log[b]] : 0u;
+}
+
+// x * 2 in GF(2^8) on 16 packed bytes
+__device__ __forceinline__ uint4 xtime16(uint4 v) {
+    return make_uint4(dev::xtime4(v.x), dev::xtime4(v.y), dev::xtime4(v.z), dev::xtime4(v.w));
+}
+
+// v moved up by k (1..15) byte positions: bytes [16-k, 32-k) of the 32-byte window {0, v}
+__device__ __forceinline__ uint4 shift_up(const uint4 &v, uint32_t k) { return dev::funnel16(make_uint4(0u, 0u, 0u, 0u), v, 16u - k); }
+
+// the GF(2^8) exp / log tables of the CTA (blockDim.x == kExecThreads); ends with __syncthreads
+__device__ __forceinline__ void exec_tables_init(ExecShared &S) {
+    for (uint32_t i = threadIdx.x; i < 256u; i += kExecThreads) {
+        uint32_t v = 1u;
+        for (uint32_t k = 0; k < i; ++k) v = (v << 1) ^ ((v & 0x80u) ? 0x11Du : 0u);   // 2^i, i < 255
+        if (i < 255u) { S.exp[i] = static_cast<uint8_t>(v); S.exp[i + 255u] = static_cast<uint8_t>(v); S.log[v] = static_cast<uint8_t>(i); }
+    }
+    if (threadIdx.x < 2u) S.exp[510u + threadIdx.x] = S.exp[threadIdx.x];
+    __syncthreads();
+}
+
+// Output-stationary: lane v writes payload bytes [16v, 16v + 16) of dst with one aligned 128-bit store (zero past dlen).
+// Data shard i is payload bytes [i*L, (i+1)*L); a held one is read at src + rank(i)*stride, a missing one is the
+// GF(2^8) combination of the first d held shards (ranks 0..d-1) with row i of inverse(M[sources]), reconstruct_data's
+// choice of sources (rscoding.rs:490-537).  matrix: the coder's [T*d] coding matrix; held has at least d bits below T.
+// Ends with __syncwarp: the warp's next record may overwrite the rows this one read.
+__device__ __forceinline__ void warp_exec_payload(ExecShared &S, uint32_t w, uint32_t lane, uint32_t d, uint32_t held, uint32_t dlen,
+                                                  const uint8_t *matrix, const uint8_t *src, uint64_t stride, uint8_t *dst) {
+    uint8_t (*ra)[32] = S.a[w];
+    uint8_t (*ri)[32] = S.inv[w];
+    uint8_t *piv = S.piv[w];
+    const uint32_t L = (dlen + d - 1u) / d;
+    const uint32_t dmask = d == 32u ? 0xffffffffu : (1u << d) - 1u;
+    const uint32_t missing = ~held & dmask;
+    if (missing != 0u) {
+        // Gauss-Jordan on M[sources] (d x d, invertible for any d distinct rows of the coder's matrix): lane k owns
+        // row k, whose source is the k-th held shard; pivots are taken in column order, rows are never swapped
+        if (lane < d) {
+            uint32_t h = held;
+            for (uint32_t q = 0; q < lane; ++q) h &= h - 1u;
+            const uint32_t row = static_cast<uint32_t>(__ffs(h)) - 1u;
+            for (uint32_t c = 0; c < d; ++c) {
+                ra[lane][c] = matrix[row * d + c];
+                ri[lane][c] = c == lane ? 1u : 0u;
+            }
+        }
+        __syncwarp();
+        uint32_t used = 0u;
+        for (uint32_t c = 0; c < d; ++c) {
+            const uint32_t f = lane < d ? ra[lane][c] : 0u;
+            const uint32_t cand = __ballot_sync(0xffffffffu, f != 0u && !((used >> lane) & 1u));
+            if (cand == 0u) break;
+            const uint32_t p = static_cast<uint32_t>(__ffs(cand)) - 1u;
+            used |= 1u << p;
+            if (lane == p) {
+                const uint32_t sc = S.exp[255u - S.log[f]];
+                piv[c] = static_cast<uint8_t>(p);
+                for (uint32_t k = c; k < d; ++k) ra[p][k] = static_cast<uint8_t>(gmul(S, ra[p][k], sc));
+                for (uint32_t k = 0; k < d; ++k) ri[p][k] = static_cast<uint8_t>(gmul(S, ri[p][k], sc));
+            }
+            __syncwarp();
+            if (lane < d && lane != p && f != 0u) {
+                for (uint32_t k = c; k < d; ++k) ra[lane][k] ^= static_cast<uint8_t>(gmul(S, f, ra[p][k]));
+                for (uint32_t k = 0; k < d; ++k) ri[lane][k] ^= static_cast<uint8_t>(gmul(S, f, ri[p][k]));
+            }
+            __syncwarp();
+        }
+    }
+    // bytes [o, o + c) of data shard i (c <= 16) as the low c bytes of a uint4, the rest zero
+    auto shard16 = [&](uint32_t i, uint32_t o, int c) -> uint4 {
+        if ((held >> i) & 1u) return dev::load16(src + __popc(held & ((1u << i) - 1u)) * stride + o, c);
+        const uint8_t *coef = ri[piv[i]];
+        uint4 acc = make_uint4(0u, 0u, 0u, 0u);
+        for (uint32_t q0 = 0; q0 < d; q0 += kChunk) {
+            uint32_t cq[kChunk], top = 0u;
+            dev::Raw16 raw[kChunk];
+#pragma unroll
+            for (int q = 0; q < kChunk; ++q) {
+                const bool in = q0 + q < d;
+                cq[q] = in ? coef[q0 + q] : 0u;
+                top |= cq[q];
+                raw[q] = dev::raw16_issue(src + (q0 + q) * stride + o, in && cq[q] != 0u ? c : 0);
+            }
+            uint4 x[kChunk];
+#pragma unroll
+            for (int q = 0; q < kChunk; ++q) x[q] = dev::raw16_finish(raw[q], c);
+            // Horner from the top coefficient bit down: part = part * 2 ^ (XOR of the x_q whose c_q has bit k)
+            uint4 part = make_uint4(0u, 0u, 0u, 0u);
+            for (int k = top == 0u ? -1 : 31 - __clz(top); k >= 0; --k) {
+                part = xtime16(part);
+#pragma unroll
+                for (int q = 0; q < kChunk; ++q) {
+                    const uint32_t m = 0u - ((cq[q] >> k) & 1u);
+                    part.x ^= x[q].x & m; part.y ^= x[q].y & m; part.z ^= x[q].z & m; part.w ^= x[q].w & m;
+                }
+            }
+            acc.x ^= part.x; acc.y ^= part.y; acc.z ^= part.z; acc.w ^= part.w;
+        }
+        return acc;
+    };
+    const uint32_t ncol = (dlen + 15u) >> 4;
+    for (uint32_t v = lane; v < ncol; v += 32u) {
+        uint32_t pos = v * 16u;
+        const uint32_t end = dlen - pos < 16u ? dlen : pos + 16u;
+        const uint32_t i = pos / L, o = pos - i * L;
+        uint4 out;
+        if (o + 16u <= L) {
+            out = shard16(i, o, static_cast<int>(end - pos));           // the column lies in one shard
+        } else {                                                       // it spans shards (always for L < 16)
+            out = make_uint4(0u, 0u, 0u, 0u);
+            for (uint32_t filled = 0u; pos < end;) {
+                const uint32_t j = pos / L, oj = pos - j * L;
+                const uint32_t c = L - oj < end - pos ? L - oj : end - pos;
+                uint4 piece = shard16(j, oj, static_cast<int>(c));
+                if (filled != 0u) piece = shift_up(piece, filled);
+                out.x |= piece.x; out.y |= piece.y; out.z |= piece.z; out.w |= piece.w;
+                filled += c;
+                pos += c;
+            }
+        }
+        dev::stg128_cs(dst + static_cast<uint64_t>(v) * 16u, out);
+    }
+    __syncwarp();                       // the next record's Gauss-Jordan overwrites the rows this one read
+}
+
+}  // namespace ssb

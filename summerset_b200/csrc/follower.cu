@@ -19,6 +19,14 @@
 // group's frames serially on one thread); the copies take a warp per frame whatever the grouping.
 //
 //   append_reply_parse_kernel  a thread per AppendEntriesReply frame: the records ss_engine_raft_ingest takes
+//
+// Execution of the committed entries (the walk in handle_msg_append_entries, craft/messages.rs:198-240):
+//
+//   fol_exec_count_kernel    a thread per group: the entries the walk executes, and their payload bytes
+//   (engine.cu's scan)       record indices and payload regions
+//   fol_exec_place_kernel    a thread per group: capacities, the records, last_exec
+//   fol_exec_payload_kernel  a warp per record: get_data's bytes from the held shards, a missing data shard regenerated
+//                            from the first d held ones (exec_payload.cuh)
 #include <cub/device/device_radix_sort.cuh>
 
 #include <cstring>
@@ -26,6 +34,8 @@
 
 #include "codeword_wire.cuh"
 #include "device_common.cuh"
+#include "exec_payload.cuh"
+#include "gf256.hpp"
 #include "ss_internal.hpp"
 #include "wire_common.cuh"
 
@@ -57,6 +67,9 @@ struct ss_follower {
     uint8_t *leader = nullptr;
     uint64_t *term = nullptr, *shard_addr = nullptr;
     uint32_t *held = nullptr, *data_len = nullptr;
+    uint64_t *last_exec = nullptr;  // [G] last executed slot (ss_follower_execute)
+    uint8_t *matrix = nullptr;      // [T*d] the coder's coding matrix (gf256.hpp), row-major
+    uint64_t *ex_cnt = nullptr, *ex_bytes = nullptr, *ex_partials = nullptr, *ex_words = nullptr;   // execute scratch
     // per-call scratch, grow-only
     uint64_t cap_frames = 0;
     ssb::FolHdr *hdr = nullptr;
@@ -475,6 +488,98 @@ follower_advance_kernel(const uint64_t *__restrict__ upto, uint64_t G, uint64_t 
     }
 }
 
+// ---- execution -----------------------------------------------------------------------------------------------------
+struct FolExecArgs {
+    uint64_t G;
+    uint32_t W, d;
+    const uint64_t *start_slot, *last_commit, *shard_addr;
+    const uint32_t *held, *data_len;
+    const uint8_t *matrix;          // [T*d]
+    uint64_t *last_exec;
+    uint64_t *cnt, *bytes;          // [G] per group: records, payload bytes; then their exclusive scans
+    uint64_t *n_exec;               // records written (a prefix: the offsets are monotone)
+    uint8_t *out;
+    uint64_t out_cap;
+    uint32_t *rec_group;
+    uint64_t *rec_slot, *rec_off;
+    uint32_t *rec_len;
+    uint64_t rec_cap;
+    uint32_t *status;
+};
+
+enum : uint32_t { kFolExecStop = 0u, kFolExecRun = 1u, kFolExecNull = 2u };
+
+__device__ __forceinline__ uint64_t fol_exec_start(const FolExecArgs &A, uint64_t g) {
+    const uint64_t s = A.last_exec[g] + 1u, st = A.start_slot[g];
+    return s > st ? s : st;
+}
+
+// what the walk does at slot s of group g: stop (past last_commit, or fewer than d shards held, which the commit walk
+// already excludes but state a host installed may hold), run it (*dlen = its data_len), or stop at a null entry, which
+// get_data refuses (rscoding.rs:581-583)
+__device__ __forceinline__ uint32_t fol_exec_next(const FolExecArgs &A, uint64_t g, uint64_t s, uint32_t *dlen) {
+    if (s > A.last_commit[g]) return kFolExecStop;
+    const uint64_t pos = g * A.W + (s & (A.W - 1u));
+    if (static_cast<uint32_t>(__popc(A.held[pos])) < A.d) return kFolExecStop;
+    *dlen = A.data_len[pos];
+    return *dlen == 0u ? kFolExecNull : kFolExecRun;
+}
+
+__global__ void __launch_bounds__(kFolThreads) fol_exec_count_kernel(const __grid_constant__ FolExecArgs A) {
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kFolThreads;
+    for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kFolThreads + threadIdx.x; g < A.G; g += stride) {
+        uint64_t n = 0u, b = 0u;
+        uint32_t dl = 0u;
+        for (uint64_t s = fol_exec_start(A, g); fol_exec_next(A, g, s, &dl) == kFolExecRun; ++s, ++n) b += fol_round16(dl);
+        A.cnt[g] = n;
+        A.bytes[g] = b;
+    }
+}
+
+__global__ void __launch_bounds__(kFolThreads) fol_exec_place_kernel(const __grid_constant__ FolExecArgs A) {
+    bool full = false, null_ent = false;
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kFolThreads;
+    for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kFolThreads + threadIdx.x; g < A.G; g += stride) {
+        const uint64_t s0 = fol_exec_start(A, g);
+        uint64_t ro = A.cnt[g], bo = A.bytes[g], s = s0;
+        uint32_t dl = 0u, r;
+        while ((r = fol_exec_next(A, g, s, &dl)) == kFolExecRun) {
+            const uint64_t sz = fol_round16(dl);
+            if (ro >= A.rec_cap || bo > A.out_cap || sz > A.out_cap - bo) { full = true; break; }
+            A.rec_group[ro] = static_cast<uint32_t>(g);
+            A.rec_slot[ro] = s;
+            A.rec_off[ro] = bo;
+            A.rec_len[ro] = dl;
+            ++ro;
+            bo += sz;
+            ++s;
+        }
+        null_ent |= r == kFolExecNull;
+        if (s != s0) {
+            A.last_exec[g] = s - 1u;
+            atomicMax(reinterpret_cast<unsigned long long *>(A.n_exec), static_cast<unsigned long long>(ro));
+        }
+    }
+    if (full) atomicOr(A.status, SS_DEV_STATUS_EXEC_FULL);
+    if (null_ent) atomicOr(A.status, SS_DEV_STATUS_EXEC_NULL);
+}
+
+// a warp per record: held shard of rank k at shard_addr + k * SS_CW_SLOT_PITCH(L), the store layout of the append
+__global__ void __launch_bounds__(kExecThreads) fol_exec_payload_kernel(const __grid_constant__ FolExecArgs A) {
+    __shared__ ExecShared S;
+    exec_tables_init(S);
+    const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+    const uint64_t n = *A.n_exec;
+    const uint64_t nwarps = static_cast<uint64_t>(gridDim.x) * kExecWarps;
+    for (uint64_t r = static_cast<uint64_t>(blockIdx.x) * kExecWarps + w; r < n; r += nwarps) {
+        const uint64_t g = A.rec_group[r], pos = g * A.W + (A.rec_slot[r] & (A.W - 1u));
+        const uint32_t dlen = A.rec_len[r];
+        const uint64_t pitch = SS_CW_SLOT_PITCH((dlen + A.d - 1u) / A.d);
+        warp_exec_payload(S, w, lane, A.d, A.held[pos], dlen, A.matrix, reinterpret_cast<const uint8_t *>(A.shard_addr[pos]), pitch,
+                          A.out + A.rec_off[r]);
+    }
+}
+
 // the leader's side: PeerMessage::Msg{AppendEntriesReply{term, end_slot, conflict}} frames -> ingest records
 struct ReplyParseArgs {
     const uint8_t *buf;
@@ -612,7 +717,8 @@ int ss_follower_destroy(ss_follower *f) {
         cudaStreamSynchronize(f->ctx->stream);
     }
     void *bufs[] = {f->start_slot, f->log_end, f->curr_term, f->last_commit, f->last_snap, f->leader, f->term, f->shard_addr,
-                    f->held, f->data_len, f->hdr, f->keys, f->idx, f->partials, f->sort_tmp, f->words};
+                    f->held, f->data_len, f->last_exec, f->matrix, f->ex_cnt, f->ex_bytes, f->ex_partials, f->ex_words, f->hdr,
+                    f->keys, f->idx, f->partials, f->sort_tmp, f->words};
     for (void *b : bufs)
         if (b) cudaFree(b);
     if (f->ctx) ctx_release(f->ctx);
@@ -652,9 +758,19 @@ int ss_follower_create(ss_ctx *ctx, const ss_follower_config *cfg, uint64_t G, s
     if ((rc = fol_alloc(ctx, &f->start_slot, G)) || (rc = fol_alloc(ctx, &f->log_end, G)) || (rc = fol_alloc(ctx, &f->curr_term, G)) ||
         (rc = fol_alloc(ctx, &f->last_commit, G)) || (rc = fol_alloc(ctx, &f->last_snap, G)) || (rc = fol_alloc(ctx, &f->leader, G)) ||
         (rc = fol_alloc(ctx, &f->term, G * W)) || (rc = fol_alloc(ctx, &f->shard_addr, G * W)) ||
-        (rc = fol_alloc(ctx, &f->held, G * W)) || (rc = fol_alloc(ctx, &f->data_len, G * W)) || (rc = fol_alloc(ctx, &f->words, 4))) {
+        (rc = fol_alloc(ctx, &f->held, G * W)) || (rc = fol_alloc(ctx, &f->data_len, G * W)) || (rc = fol_alloc(ctx, &f->words, 4)) ||
+        (rc = fol_alloc(ctx, &f->last_exec, G)) || (rc = fol_alloc(ctx, &f->matrix, size_t(f->T) * f->d, false)) ||
+        (rc = fol_alloc(ctx, &f->ex_cnt, G, false)) || (rc = fol_alloc(ctx, &f->ex_bytes, G, false)) ||
+        (rc = fol_alloc(ctx, &f->ex_partials, scan_tiles(G), false)) || (rc = fol_alloc(ctx, &f->ex_words, 3, false))) {
         ss_follower_destroy(f);
         return rc;
+    }
+    // the coder's matrix, whose rows ss_follower_execute inverts on the device; a pageable source is staged before the
+    // call returns
+    const gf::Matrix m = gf::coding_matrix(static_cast<int>(f->d), static_cast<int>(f->T - f->d));
+    if (cudaMemcpyAsync(f->matrix, m.v.data(), m.v.size(), cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) {
+        ss_follower_destroy(f);
+        return set_error(SS_ERR_CUDA, "coding matrix upload failed");
     }
     follower_init_kernel<<<fol_grid(ctx, G, kFolThreads), kFolThreads, 0, ctx->stream>>>(G, f->log_end, f->leader);
     if ((rc = launched(ctx)) != SS_OK) {
@@ -681,6 +797,41 @@ int ss_follower_advance(ss_follower *f, const uint64_t *upto) {
     ss_ctx *ctx = f->ctx;
     SS_TRY(ctx_bind(ctx));
     follower_advance_kernel<<<fol_grid(ctx, f->G, kFolThreads), kFolThreads, 0, ctx->stream>>>(upto, f->G, f->start_slot, f->last_commit);
+    return launched(ctx);
+}
+
+int ss_follower_exec_view_get(ss_follower *f, ss_follower_exec_view *v) {
+    if (f == nullptr || v == nullptr) return set_error(SS_ERR_INVALID_ARG, "null argument");
+    memset(v, 0, sizeof(*v));
+    v->n_groups = f->G;
+    v->last_exec = f->last_exec;
+    return SS_OK;
+}
+
+int ss_follower_execute(ss_follower *f, uint8_t *out, uint64_t out_capacity, uint32_t *rec_group, uint64_t *rec_slot, uint64_t *rec_off,
+                        uint32_t *rec_len, uint64_t rec_capacity, uint64_t *totals) {
+    if (f == nullptr) return set_error(SS_ERR_INVALID_ARG, "null follower");
+    if (!out || !rec_group || !rec_slot || !rec_off || !rec_len) return set_error(SS_ERR_INVALID_ARG, "null buffer");
+    if (reinterpret_cast<uintptr_t>(out) & 15u) return set_error(SS_ERR_INVALID_ARG, "out must be 16-byte aligned");
+    ss_ctx *ctx = f->ctx;
+    SS_TRY(ctx_bind(ctx));
+    FolExecArgs A{};
+    A.G = f->G; A.W = f->W; A.d = f->d;
+    A.start_slot = f->start_slot; A.last_commit = f->last_commit; A.shard_addr = f->shard_addr; A.held = f->held; A.data_len = f->data_len;
+    A.matrix = f->matrix; A.last_exec = f->last_exec; A.cnt = f->ex_cnt; A.bytes = f->ex_bytes; A.n_exec = f->ex_words;
+    A.out = out; A.out_cap = out_capacity; A.rec_group = rec_group; A.rec_slot = rec_slot; A.rec_off = rec_off; A.rec_len = rec_len;
+    A.rec_cap = rec_capacity; A.status = ctx->dev_status;
+    uint64_t *tot = totals != nullptr ? totals : f->ex_words + 1;
+    const uint32_t grid = fol_grid(ctx, f->G, kFolThreads);
+    SS_CUDA(cudaMemsetAsync(f->ex_words, 0, 8, ctx->stream));
+    fol_exec_count_kernel<<<grid, kFolThreads, 0, ctx->stream>>>(A);
+    SS_TRY(launched(ctx));
+    SS_TRY(launch_exclusive_scan_u64(ctx, f->ex_cnt, f->G, f->ex_partials, tot));
+    SS_TRY(launch_exclusive_scan_u64(ctx, f->ex_bytes, f->G, f->ex_partials, tot + 1));
+    fol_exec_place_kernel<<<grid, kFolThreads, 0, ctx->stream>>>(A);
+    SS_TRY(launched(ctx));
+    // a warp per entry the ring can hold, up to the grid cap; warps past the executed count return at once
+    fol_exec_payload_kernel<<<fol_grid(ctx, f->G * f->W, kExecWarps), kExecThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
 }
 

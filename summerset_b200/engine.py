@@ -33,10 +33,13 @@ torch tensors (zero-copy views) so tests can read results and install state; it 
         pack_append(me, out, max_frames[, want_end, heartbeat])   AppendEntries frames (craft/durability.rs:12-127)
         backoff(buf, frame_off, frame_group, frame_peer, rec_kind)   the conflict branch (craft/messages.rs:386-406)
         advance_log(upto) / log_view()      the snapshot's start_slot move; log_start, try_next and the entry rings
+        execute(out, rec_capacity) / exec_view()   the committed entries' request batches (craft/messages.rs:316-359)
+        set_full_copy(on)                   the commit threshold of full-copy mode (craft/leadership.rs:282-288)
     Follower(ctx, G, population, me[, window])   the CRaft follower
         append(buf, frame_off, frame_group, frame_peer, store, wal)   handle_msg_append_entries (craft/messages.rs:14-252):
                                             store, LogEntry / Metadata records, AppendEntriesReply cells
         advance(upto)                       the snapshot's start_slot move
+        execute(out, rec_capacity)          the committed entries' request batches (craft/messages.rs:198-240)
     append_reply_parse(ctx, buf, frame_off, frame_group, frame_peer, curr_term, G)   the leader's side: AppendEntriesReply
                                             frames -> RaftEngine.on_append_replies records
 """
@@ -61,6 +64,21 @@ class _DevArray:
 
     def __init__(self, ptr: int, shape: Tuple[int, ...], typestr: str):
         self.__cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (ptr, False), "version": 2}
+
+
+def _execute(fn, h, out: torch.Tensor, rec_capacity: int, out_capacity: Optional[int]) -> dict:
+    """one call of an execution walk with ss_acceptor_execute's argument list after the handle"""
+    assert out.dtype == torch.uint8 and out.is_contiguous()
+    dev = out.device
+    res = dict(rec_group=torch.empty(rec_capacity, dtype=torch.int32, device=dev),
+               rec_slot=torch.empty(rec_capacity, dtype=torch.int64, device=dev),
+               rec_off=torch.empty(rec_capacity, dtype=torch.int64, device=dev),
+               rec_len=torch.empty(rec_capacity, dtype=torch.int32, device=dev),
+               totals=torch.empty(2, dtype=torch.int64, device=dev))
+    p = lambda x: x.data_ptr()
+    check(fn(h, p(out), out.numel() if out_capacity is None else out_capacity, p(res["rec_group"]), p(res["rec_slot"]),
+             p(res["rec_off"]), p(res["rec_len"]), rec_capacity, p(res["totals"])))
+    return res
 
 
 class _EngineBase:
@@ -290,6 +308,24 @@ class RaftEngine(_EngineBase):
         """log_start moves towards upto (int64 [G]), never past min(last_snap, last_commit)."""
         assert upto.is_cuda and upto.dtype == torch.int64 and upto.numel() == self.G
         check(self.lib.ss_engine_craft_advance(self.h, upto.data_ptr()))
+
+    def set_full_copy(self, on: bool) -> None:
+        """The commit threshold of the next tick: majority when on, majority + fault_tolerance when off."""
+        check(self.lib.ss_engine_craft_set_full_copy(self.h, 1 if on else 0))
+        check(self.lib.ss_engine_view_get(self.h, C.byref(self.view)))
+        self.threshold = self.view.threshold
+
+    def exec_view(self) -> dict:
+        """Takes the log into use and returns last_exec int64 [G] (zero-copy)."""
+        v = _lib.CraftExecView()
+        check(self.lib.ss_engine_craft_exec_view_get(self.h, C.byref(v)))
+        return dict(last_exec=self._tensor(v.last_exec, (self.G,), "<i8", torch.int64))
+
+    def execute(self, out: torch.Tensor, rec_capacity: int, out_capacity: Optional[int] = None) -> dict:
+        """Executes the committed entries from last_exec + 1: payloads into out (uint8, 16-byte aligned, one
+        round_up(data_len, 16) region each).  Returns device tensors rec_group (int32), rec_slot, rec_off (int64),
+        rec_len (int32), each [rec_capacity], and totals (int64 [2]: records and bytes asked for)."""
+        return _execute(self.lib.ss_engine_craft_execute, self.h, out, rec_capacity, out_capacity)
 
 
 class Acceptor:
@@ -570,6 +606,9 @@ class Follower:
         self.shard_addr = t(v.shard_addr, (G, W), "<i8", torch.int64)
         self.held = t(v.held, (G, W), "<i4", torch.int32)
         self.data_len = t(v.data_len, (G, W), "<i4", torch.int32)
+        ev = self.exec_view = _lib.FollowerExecView()
+        check(self.lib.ss_follower_exec_view_get(self.h, C.byref(ev)))
+        self.last_exec = t(ev.last_exec, (G,), "<i8", torch.int64)
 
     def append(self, buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor, frame_peer: torch.Tensor,
                store: torch.Tensor, wal: torch.Tensor, store_capacity: Optional[int] = None,
@@ -600,6 +639,11 @@ class Follower:
         """The snapshot's start_slot move, never past last_commit (upto int64 [G], absolute slots)."""
         assert upto.is_cuda and upto.dtype == torch.int64 and upto.numel() == self.G
         check(self.lib.ss_follower_advance(self.h, upto.data_ptr()))
+
+    def execute(self, out: torch.Tensor, rec_capacity: int, out_capacity: Optional[int] = None) -> dict:
+        """Executes the committed entries from last_exec + 1, regenerating missing data shards: payloads into out
+        (uint8, 16-byte aligned, one round_up(data_len, 16) region each).  Returns what Acceptor.execute returns."""
+        return _execute(self.lib.ss_follower_execute, self.h, out, rec_capacity, out_capacity)
 
     def close(self) -> None:
         if getattr(self, "h", None) is not None and self.h:

@@ -419,6 +419,16 @@ class Follower {
         check(ss_follower_view_get(fol_, &v));
         return v;
     }
+    ss_follower_exec_view exec_view() const {
+        ss_follower_exec_view v{};
+        check(ss_follower_exec_view_get(fol_, &v));
+        return v;
+    }
+    // the committed entries' request batches (see ss_follower_execute); pass last_exec to advance_start_slot
+    void execute(uint8_t *out, uint64_t out_capacity, uint32_t *rec_group, uint64_t *rec_slot, uint64_t *rec_off, uint32_t *rec_len,
+                 uint64_t rec_capacity, uint64_t *totals = nullptr) {
+        check(ss_follower_execute(fol_, out, out_capacity, rec_group, rec_slot, rec_off, rec_len, rec_capacity, totals));
+    }
 
   private:
     ss_follower *fol_ = nullptr;
@@ -458,5 +468,15 @@ inline void craft_backoff(ss_engine *e, const uint8_t *buf, uint64_t buf_len, co
     check(ss_engine_craft_backoff(e, buf, buf_len, frame_off, frame_group, frame_peer, rec_kind, n_frames, reply_variant, want_end));
 }
 inline void craft_advance(ss_engine *e, const uint64_t *upto) { check(ss_engine_craft_advance(e, upto)); }
+inline void craft_set_full_copy(ss_engine *e, bool full_copy) { check(ss_engine_craft_set_full_copy(e, full_copy ? 1 : 0)); }
+inline ss_engine_craft_exec_view craft_exec_view(ss_engine *e) {
+    ss_engine_craft_exec_view v{};
+    check(ss_engine_craft_exec_view_get(e, &v));
+    return v;
+}
+inline void craft_execute(ss_engine *e, uint8_t *out, uint64_t out_capacity, uint32_t *rec_group, uint64_t *rec_slot, uint64_t *rec_off,
+                          uint32_t *rec_len, uint64_t rec_capacity, uint64_t *totals = nullptr) {
+    check(ss_engine_craft_execute(e, out, out_capacity, rec_group, rec_slot, rec_off, rec_len, rec_capacity, totals));
+}
 
 }  // namespace ssb
