@@ -1213,11 +1213,12 @@ int ss_engine_craft_exec_view_get(ss_engine *engine, ss_engine_craft_exec_view *
  * (craft/messages.rs:316-359): for every group, from max(last_exec + 1, log_start) while the slot is at most
  * last_commit, an entry with data_len == 0 is a null codeword get_data refuses (rscoding.rs:581-583): it does not
  * execute and its group's walk stops there (SS_DEV_STATUS_EXEC_NULL); any other executes and last_exec moves to it.
- * The leader's last_commit is the reference's new_commit: the leader holds every shard of its own entries, so none is
- * postponed and no Reconstruct is needed, and the reference's last_commit equals new_commit on every path the device
- * reaches.  The payload is get_data's output, the first data_len bytes of data shards 0..d-1 concatenated
- * (rscoding.rs:581-683), read at shard_addr + j * plane_stride: the stores of ss_engine_craft_propose must still hold
- * the entries.  Outputs, records, capacities, totals and status bits are those of ss_acceptor_execute (see
+ * An entry holding fewer than d shards (one a step-up took over and no absorb has completed; ss_engine_craft_recon_view)
+ * stops the walk with no status bit, as in ss_follower_execute: ss_engine_craft_reconstruct_reads lists it.  The payload
+ * is get_data's output, the first data_len bytes of data shards 0..d-1 concatenated (rscoding.rs:581-683), read at
+ * shard_addr + j * plane_stride; a missing data shard is regenerated from the first d held shards in index order, as
+ * reconstruct_data chooses them (rscoding.rs:490-537).  The planes of ss_engine_craft_propose and ss_engine_craft_step_up
+ * must still hold the entries.  Outputs, records, capacities, totals and status bits are those of ss_acceptor_execute (see
  * ss_follower_execute).  Takes the log into use, and is refused once ss_engine_raft_append has run. */
 int ss_engine_craft_execute(ss_engine *engine, uint8_t *out, uint64_t out_capacity, uint32_t *rec_group, uint64_t *rec_slot,
                             uint64_t *rec_off, uint32_t *rec_len, uint64_t rec_capacity, uint64_t *totals);
@@ -1266,6 +1267,104 @@ int ss_frame_append_pack_dev(ss_engine *engine, const ss_append_pack_spec *spec,
 int ss_engine_craft_backoff(ss_engine *engine, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off,
                             const uint32_t *frame_group, const uint8_t *frame_peer, const uint32_t *rec_kind, uint64_t n_frames,
                             uint32_t reply_variant, uint64_t *want_end);
+
+/* ---- CRaft leader fail-over: step-up and reconstruct reads (SS_PROTO_CRAFT engines) ------------------------------------
+ * A new leader's log comes from this replica's follower (ss_engine_craft_step_up, the log half of become_the_leader,
+ * craft/leadership.rs:212-246).  In 1-shard mode a follower holds one shard of most entries, so the leader then lists the
+ * committed entries it holds fewer than d = majority shards of (ss_engine_craft_reconstruct_reads, craft/messages.rs:316-371),
+ * the followers serve them (ss_follower_reconstruct_serve, messages.rs:621-662), the leader absorbs the replies
+ * (ss_engine_craft_absorb, messages.rs:664-744 without its execution loop) and ss_engine_craft_execute runs what now holds
+ * d shards, regenerating missing data shards.
+ * Two more arrays of the leader's log: held ([G][raft_window] shard masks; ss_engine_craft_propose writes every shard's bit,
+ * step-up the follower's mask) and last_recon ([G], the reference's last_recon, mod.rs:345-347; zero when the log is taken
+ * into use, left alone by step-up: the reference keeps it across roles).  An entry's AppendEntries carries held & wanted
+ * (subset_copy, rscoding.rs:255-293): a shard the leader does not hold goes out as None.  A log that is never stepped up
+ * holds every shard of every entry and behaves as before.
+ * Stated differences from the reference:
+ *   1. elections (RequestVote, RequestVoteReply, become_a_candidate, voted_for), heartbeats and the `external` flag of
+ *      unreplied entries (leadership.rs:236-243) stay with the host; step-down (engine -> follower) is not built;
+ *   2. the packer's leader_commit is the engine's last_commit, the quorum commit point; the reference sends its executed
+ *      prefix, which lags behind while reconstruct reads are outstanding;
+ *   3. execution after an absorb goes up to the tick's last_commit, which keeps the current-term rule; the reference's loop
+ *      runs to shadow_last_commit (the k-th match, no term check; messages.rs:673-686), which ss_raft_kth_match_dev gives a
+ *      host that wants it;
+ *   4. served codewords carry the held shards only; a reference follower that executed also sends regenerated data
+ *      shards and data_copy;
+ *   5. absorb ignores slots at or past log_end, where the reference would index past its vector;
+ *   6. an entry failing absorb_other's checks is rejected alone; in the reference it aborts the rest of the message, in
+ *      HashMap order. */
+typedef struct ss_engine_craft_recon_view {
+    uint64_t n_groups;
+    uint32_t raft_window, total_shards;
+    uint32_t *held;             /* [G][raft_window] shard masks */
+    uint64_t *last_recon;       /* [G] the last slot a reconstruct read listed */
+} ss_engine_craft_recon_view;
+/* Takes the log into use.  The held masks are kept from the first call of this view, step-up, reconstruct reads or
+ * absorb on (every mask starts full: only ss_engine_craft_propose made entries until then); before that propose does not
+ * write them and pack and execute do not read them. */
+int ss_engine_craft_recon_view_get(ss_engine *engine, ss_engine_craft_recon_view *view);
+/* verdict[i] of ss_engine_craft_step_up; every one but DONE leaves the group unchanged */
+#define SS_STEPUP_VERDICT_DONE 0u
+#define SS_STEPUP_VERDICT_IGNORED 1u      /* group >= n_groups, or listed earlier in the same call */
+#define SS_STEPUP_VERDICT_WINDOW 2u       /* the follower's log_end - start_slot > raft_window */
+#define SS_STEPUP_VERDICT_RANGE 3u        /* log_end, last_snap, a ring term or term[i] >= 2^32 (the engine's arrays are u32) */
+#define SS_STEPUP_VERDICT_STALE_TERM 4u   /* term[i] < the follower's curr_term */
+#define SS_STEPUP_VERDICT_STORE_FULL 5u   /* the group's slots end past plane_stride (SS_DEV_STATUS_STORE_FULL) */
+/* Step-up for the listed groups (device u32 [n_listed]; a group >= n_groups, or one listed before in the call, is
+ * ignored), each in term[i] (device u64 [n_listed], the term the host's election won), from `follower`, this replica's
+ * follower (same context, population, n_groups and protocol; SS_ERR_INVALID_ARG otherwise, and for an engine that ran
+ * ss_engine_raft_append).  The verdicts above are checked in that order.  For a stepped-up group g:
+ *   - [start_slot, log_end) of the follower's ring goes into the engine's: terms, data_len, held, log_offset 0;
+ *   - every non-null entry gets a SS_CW_SLOT_PITCH(ceil(data_len / d)) slot in every plane shards + j * plane_stride,
+ *     the slots placed in (listing, slot) order by an exclusive scan (shard_off[i]: listing i's first slot, UINT64_MAX
+ *     when not stepped up; *need, device, may be NULL: the bytes asked for).  Held shard j (rank k in the follower's
+ *     store) is copied to plane j, round_up(shard_len, 16) bytes; the absent ones stay reserved for an absorb;
+ *   - log_start = start_slot, log_end, last_commit, last_snap and last_exec (ss_follower_exec_view) are the follower's,
+ *     curr_term = term[i]; for every peer next_slot = try_next = log_end and match = 0 (leadership.rs:225-234);
+ *     last_recon is left alone.  The log_offset ring is the host's to rewrite through ss_engine_craft_log_view.
+ * The offsets are monotone, so the groups cut by plane_stride are a suffix of those that passed the other checks.
+ * plane_stride: a non-zero multiple of 32, the same as every ss_engine_craft_propose's; shards 16-byte aligned and alive
+ * while the entries are.  The follower's state is only read.
+ * Cost: a thread per listing sizes and writes the state; the copies take a warp per entry, with aligned 128-bit accesses. */
+int ss_engine_craft_step_up(ss_engine *engine, const ss_follower *follower, const uint32_t *groups, uint64_t n_listed,
+                            const uint64_t *term, uint8_t *shards, uint64_t plane_stride, uint64_t *shard_off, uint64_t *need,
+                            uint32_t *verdict);
+/* Reconstruct reads: for each listed group (groups device u32 [n_listed], NULL = every group in index order; a group >=
+ * n_groups is ignored, one listed twice is planned twice from the state before the call), the slots s from
+ * max(last_exec + 1, log_start, last_recon + 1) through last_commit whose entry holds fewer than d shards are listed as
+ * (s, term); then last_recon = the last slot listed.  The list is cut into frames of chunk_size (>= 1) entries: 8-byte
+ * big-endian length + PeerMessage::Msg{Reconstruct{slots: Vec<(usize, Term)>}} (reconstruct_variant, 4; mod.rs:239-246),
+ * each with frame_dst 0xff: the host broadcasts it.  Outputs, placement, totals and the per-group capacity cut are those of
+ * ss_acceptor_step_up_reads; a cut group keeps its last_recon.  Cost: a thread per listed group. */
+int ss_engine_craft_reconstruct_reads(ss_engine *engine, const uint32_t *groups, uint64_t n_listed, uint64_t chunk_size,
+                                      uint32_t reconstruct_variant, uint8_t *out, uint64_t out_capacity, uint32_t *frame_group,
+                                      uint8_t *frame_dst, uint64_t *frame_off, uint32_t *frame_len, uint64_t frame_capacity,
+                                      uint64_t *totals);
+/* Serve on the follower: frame i (taken as by ss_follower_append) is PeerMessage::Msg{Reconstruct{slots: Vec<(usize,
+ * Term)>}}.  A listed (slot, term) is skipped when the slot is outside [start_slot, log_end) or the ring's term differs;
+ * otherwise the entry is the held shards as an RSCodeword (d, p, data_len, shard_len, T shard Options, data_copy None).
+ * A (slot, term) listed again is one entry; entries follow their first occurrence.  The reply is
+ * PeerMessage::Msg{ReconstructReply{slots_data: HashMap<usize, RSCodeword>}} (reply_variant, 5) for frame_peer[i]; an
+ * empty map gets no reply.  Verdicts, outputs, placement, the out_capacity cut and *total are those of
+ * ss_acceptor_reconstruct_serve.  Follower state is not changed.  Cost: a thread per frame sizes, a warp per reply writes;
+ * a frame of k entries takes O(k^2) decode steps for the repeat check. */
+int ss_follower_reconstruct_serve(ss_follower *follower, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off,
+                                  const uint32_t *frame_group, const uint8_t *frame_peer, uint64_t n_frames,
+                                  uint32_t reconstruct_variant, uint32_t reply_variant, uint8_t *out, uint64_t out_capacity,
+                                  uint64_t *reply_off, uint64_t *reply_len, uint32_t *verdict, uint64_t *total);
+/* Absorb on the leader: frame i is PeerMessage::Msg{ReconstructReply{slots_data: HashMap<usize, RSCodeword>}}, decoded by
+ * ss_acceptor_absorb's rules (this d and p, shard_len = ceil(data_len / d), exactly T shard Options each present one
+ * shard_len bytes, data_copy None or Some followed by exactly data_len bytes); a frame that does not decode so is
+ * malformed (also a group >= n_groups) and absorbs nothing.  A key repeated in a frame keeps its last value.  Entries are
+ * taken in frame order, then wire order: one is ignored when its slot is outside [log_start, log_end), the entry is null
+ * or its data_len differs; otherwise each shard the entry lacks is written to its reserved plane slot (round_up(shard_len,
+ * 16) bytes, the pad zero) and its held bit set, so the first carrier of a shard index wins (absorb_other,
+ * rscoding.rs:296-343).  No store capacity is needed: step-up reserved every slot.  absorbed[i] = the entries of frame i
+ * that added shards; verdict[i]: SS_ACCEPT_VERDICT_ACCEPTED, another message's variant index or SS_FRAME_KIND_MALFORMED.
+ * ss_engine_craft_execute runs afterwards.  Cost: a group's frames are walked by one warp, the copies take the warp. */
+int ss_engine_craft_absorb(ss_engine *engine, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off,
+                           const uint32_t *frame_group, const uint8_t *frame_peer, uint64_t n_frames, uint32_t reply_variant,
+                           uint32_t *absorbed, uint32_t *verdict);
 
 /* ---- tuning / introspection (bench + tests) ------------------------------------------------ */
 /* Tuning knob for experiments; 0 = the defaults.

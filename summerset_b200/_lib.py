@@ -150,6 +150,11 @@ SIGNATURES = {
     "ss_engine_craft_execute": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp]),
     "ss_follower_exec_view_get": (_i, [_vp, _vp]),
     "ss_follower_execute": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp]),
+    "ss_engine_craft_recon_view_get": (_i, [_vp, _vp]),
+    "ss_engine_craft_step_up": (_i, [_vp, _vp, _vp, _u64, _vp, _vp, _u64, _vp, _vp, _vp]),
+    "ss_engine_craft_reconstruct_reads": (_i, [_vp, _vp, _u64, _u64, _u32, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp]),
+    "ss_follower_reconstruct_serve": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _u32, _vp, _u64, _vp, _vp, _vp, _vp]),
+    "ss_engine_craft_absorb": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _vp, _vp]),
     "ss_rs_set_variant": (_i, [_vp, _i]),
     "ss_rs_last_kernel": (C.c_char_p, [_vp]),
     "ss_rs_jit_status": (C.c_char_p, [_vp]),
@@ -250,6 +255,12 @@ class CraftExecView(C.Structure):
     _fields_ = [("n_groups", C.c_uint64), ("last_exec", C.c_void_p)]
 
 
+class CraftReconView(C.Structure):
+    """ss_engine_craft_recon_view"""
+    _fields_ = [("n_groups", C.c_uint64), ("raft_window", C.c_uint32), ("total_shards", C.c_uint32), ("held", C.c_void_p),
+                ("last_recon", C.c_void_p)]
+
+
 class FollowerExecView(C.Structure):
     """ss_follower_exec_view"""
     _fields_ = [("n_groups", C.c_uint64), ("last_exec", C.c_void_p)]
@@ -295,6 +306,9 @@ SS_APPEND_REPLY_INGEST = 0xFFFFFFF0
 SS_APPEND_REPLY_CONFLICT = 0xFFFFFFF1
 SS_APPEND_REPLY_HIGHER_TERM = 0xFFFFFFF2
 SS_APPEND_REPLY_END_RANGE = 0xFFFFFFF3
+# verdicts of ss_engine_craft_step_up
+SS_STEPUP_VERDICT_DONE, SS_STEPUP_VERDICT_IGNORED, SS_STEPUP_VERDICT_WINDOW, SS_STEPUP_VERDICT_RANGE, \
+    SS_STEPUP_VERDICT_STALE_TERM, SS_STEPUP_VERDICT_STORE_FULL = range(6)
 # pair statuses of ss_frame_append_pack_dev
 SS_APPEND_PAIR_SENT, SS_APPEND_PAIR_NOTHING, SS_APPEND_PAIR_SNAPSHOTTED, SS_APPEND_PAIR_OVERFLOW = range(4)
 

@@ -23,6 +23,8 @@
 //     (engine.cu's scan)            record indices and payload regions
 //     craft_exec_place_kernel       a thread per group: capacities, the records, last_exec
 //     craft_exec_payload_kernel     a warp per record: get_data's bytes gathered from the planes (exec_payload.cuh)
+//     craft_exec_regen_kernel       the same after a step-up, a missing data shard regenerated from the first d held ones
+// Step-up, reconstruct reads and absorb, which fill the held masks below, are in craft_recon.cu.
 //   ss_engine_craft_advance   the snapshot's start_slot move (craft/snapshot.rs:142,184)
 #include <cub/device/device_radix_sort.cuh>
 
@@ -32,6 +34,7 @@
 #include "device_common.cuh"
 #include "engine_state.hpp"
 #include "exec_payload.cuh"
+#include "gf256.hpp"
 #include "ss_internal.hpp"
 #include "wire_common.cuh"
 
@@ -40,20 +43,6 @@ namespace ssb {
 constexpr int kClThreads = 256;
 constexpr uint32_t kLogEntryVariant = 1u;          // DurEntry::LogEntry (craft/mod.rs:148-159: Metadata 0, LogEntry 1)
 constexpr uint32_t kClVariantLimit = 1u << 16;
-
-static inline uint32_t cl_grid(ss_ctx *ctx, uint64_t items, uint32_t per_cta) {
-    uint64_t ctas = (items + per_cta - 1) / per_cta;
-    const uint64_t cap = static_cast<uint64_t>(ctx->sm_count) * 8ull * 8ull;
-    if (ctas > cap) ctas = cap;
-    if (ctas == 0) ctas = 1;
-    return static_cast<uint32_t>(ctas);
-}
-
-__device__ __forceinline__ uint64_t cl_round16(uint64_t x) { return (x + 15u) & ~15ull; }
-
-__device__ __forceinline__ void cl_put_be64(uint8_t *p, uint64_t v) {
-    for (int b = 0; b < 8; ++b) p[b] = static_cast<uint8_t>(v >> (8 * (7 - b)));
-}
 
 // one status write per warp, not one per flagged item
 __device__ __forceinline__ void cl_warp_status(bool flag, uint32_t bit, uint32_t *status) {
@@ -115,7 +104,7 @@ struct ProposeArgs {
     const uint64_t *log_start;
     uint32_t *log_end, *terms;
     const uint32_t *curr_term;
-    uint32_t *ent_len;
+    uint32_t *ent_len, *held;
     uint64_t *ent_addr, *ent_log_offset;
     uint32_t *eff;
     uint64_t *rec_len;
@@ -175,6 +164,7 @@ __global__ void __launch_bounds__(kClThreads) craft_propose_commit_kernel(const 
         const uint64_t pos = g * A.W + (s & (A.W - 1u));
         A.terms[pos] = A.curr_term[g];
         A.ent_len[pos] = len;
+        if (A.held != nullptr) A.held[pos] = A.T >= 32u ? 0xffffffffu : (1u << A.T) - 1u;   // every shard: the encode writes them all
         A.ent_addr[pos] = reinterpret_cast<uint64_t>(A.shards + off);
         A.ent_log_offset[pos] = A.log_offset != nullptr ? A.log_offset[g] : 0ull;
         A.log_end[g] = s + 1u;
@@ -221,6 +211,7 @@ struct PackArgs {
     uint32_t *try_next;
     const uint64_t *log_start;
     const uint32_t *ent_len;
+    const uint32_t *held;           // read by the kHeld instances only (after a step-up or the recon view)
     const uint64_t *ent_addr, *ent_log_offset;
     uint64_t plane_stride;
     uint8_t *out;
@@ -279,8 +270,25 @@ __device__ __forceinline__ PairPlan plan_pair(const PackArgs &A, uint64_t p) {
     return r;
 }
 
-__device__ __forceinline__ uint64_t ent_bytes(const PackArgs &A, uint64_t row, uint64_t s, uint32_t nsh) {
+// the shards peer q's entries carry, before the held mask cuts them (subset_copy, rscoding.rs:255-293): the peer's
+// own, or 0..majority in full copy
+__device__ __forceinline__ uint32_t peer_want(const PackArgs &A, uint64_t q) {
+    const uint32_t r = static_cast<uint32_t>(q) < A.me ? static_cast<uint32_t>(q) : static_cast<uint32_t>(q) + 1u;
+    return own_mask(A.full_copy, A.majority, r);
+}
+
+// the shards of `want` the entry at ring position pos carries.  kHeld false: every entry holds every shard (a log that
+// was never stepped up), and the pack kernels compile without the held loads
+template <bool kHeld>
+__device__ __forceinline__ uint32_t pack_mask(const PackArgs &A, uint64_t pos, uint32_t want) {
+    return kHeld ? want & A.held[pos] : want;
+}
+
+// an entry's bytes; nsh: its shard count when every shard is held
+template <bool kHeld>
+__device__ __forceinline__ uint64_t ent_bytes(const PackArgs &A, uint64_t row, uint64_t s, uint32_t want, uint32_t nsh) {
     const uint64_t pos = row + (s & (A.W - 1u));
+    if (kHeld) nsh = static_cast<uint32_t>(__popc(pack_mask<kHeld>(A, pos, want)));
     return wv_len(A.terms[pos]) + cw_bytes(A.ent_len[pos], A.d, A.T, nsh) + 1u + wv_len(A.ent_log_offset[pos]);
 }
 
@@ -292,12 +300,13 @@ __device__ __forceinline__ void chunk_span(const PackArgs &A, uint64_t lo, uint6
 }
 
 // PeerMessage::Msg{AppendEntries{term, prev_slot, prev_term, entries, leader_commit, last_snap}} behind its length
-__device__ __forceinline__ uint64_t frame_bytes(const PackArgs &A, uint64_t g, uint64_t first, uint64_t n) {
+template <bool kHeld>
+__device__ __forceinline__ uint64_t frame_bytes(const PackArgs &A, uint64_t g, uint64_t first, uint64_t n, uint32_t want) {
     const uint64_t row = g * A.W, prev = first - 1u;
     const uint32_t nsh = A.full_copy ? A.majority : 1u;
     uint64_t b = 8u + 1u + wv_len(A.variant) + wv_len(A.curr_term[g]) + wv_len(prev) + wv_len(A.terms[row + (prev & (A.W - 1u))]) +
                  wv_len(n) + wv_len(A.last_commit[g]) + wv_len(A.last_snap[g]);
-    for (uint64_t k = 0; k < n; ++k) b += ent_bytes(A, row, first + k, nsh);
+    for (uint64_t k = 0; k < n; ++k) b += ent_bytes<kHeld>(A, row, first + k, want, nsh);
     return b;
 }
 
@@ -307,6 +316,7 @@ __device__ __forceinline__ uint64_t warp_sum(uint64_t v) {
     return v;
 }
 
+template <bool kHeld>
 __global__ void __launch_bounds__(kClThreads) append_plan_kernel(const __grid_constant__ PackArgs A) {
     const uint32_t lane = threadIdx.x & 31u;
     const uint64_t warp = (static_cast<uint64_t>(blockIdx.x) * kClThreads + threadIdx.x) >> 5;
@@ -314,11 +324,12 @@ __global__ void __launch_bounds__(kClThreads) append_plan_kernel(const __grid_co
     for (uint64_t p = warp; p < A.PG; p += nwarps) {
         const PairPlan r = plan_pair(A, p);
         const uint64_t g = p % A.G;
+        const uint32_t want = kHeld ? peer_want(A, p / A.G) : 0u;
         uint64_t bytes = 0;
         for (uint64_t c = lane; c < r.nf; c += 32u) {
             uint64_t first, n;
             chunk_span(A, r.lo, r.hi, c, first, n);
-            bytes += cl_round16(frame_bytes(A, g, first, n));
+            bytes += cl_round16(frame_bytes<kHeld>(A, g, first, n, want));
         }
         bytes = warp_sum(bytes);
         if (lane == 0u) {
@@ -331,6 +342,7 @@ __global__ void __launch_bounds__(kClThreads) append_plan_kernel(const __grid_co
 }
 
 // the cut, try_next, and the frame arrays of every pair written
+template <bool kHeld>
 __global__ void __launch_bounds__(kClThreads) append_place_kernel(const __grid_constant__ PackArgs A) {
     const uint32_t lane = threadIdx.x & 31u;
     const uint64_t warp = (static_cast<uint64_t>(blockIdx.x) * kClThreads + threadIdx.x) >> 5;
@@ -356,6 +368,7 @@ __global__ void __launch_bounds__(kClThreads) append_place_kernel(const __grid_c
         }
         const uint64_t rng = A.pk_range[p], lo = rng & 0xffffffffull, hi = rng >> 32;
         const uint64_t g = p % A.G;
+        const uint32_t want = kHeld ? peer_want(A, p / A.G) : 0u;
         if (lane == 0u) A.try_next[p] = A.heartbeat ? t : static_cast<uint32_t>(hi + 1u);   // durability.rs:124-125
         uint64_t run = off;
         for (uint64_t c0 = 0; c0 < nf_end - base; c0 += 32u) {
@@ -364,7 +377,7 @@ __global__ void __launch_bounds__(kClThreads) append_place_kernel(const __grid_c
             if (c < nf_end - base) {
                 uint64_t first, n;
                 chunk_span(A, lo, hi, c, first, n);
-                len = frame_bytes(A, g, first, n);
+                len = frame_bytes<kHeld>(A, g, first, n, want);
             }
             const uint64_t r = cl_round16(len);
             uint64_t x = r;
@@ -386,6 +399,7 @@ __global__ void __launch_bounds__(kClThreads) append_place_kernel(const __grid_c
 }
 
 // a warp per written frame
+template <bool kHeld>
 __global__ void __launch_bounds__(kClThreads) append_write_kernel(const __grid_constant__ PackArgs A) {
     const uint32_t lane = threadIdx.x & 31u;
     const uint64_t warp = (static_cast<uint64_t>(blockIdx.x) * kClThreads + threadIdx.x) >> 5;
@@ -399,8 +413,7 @@ __global__ void __launch_bounds__(kClThreads) append_write_kernel(const __grid_c
         chunk_span(A, rng & 0xffffffffull, rng >> 32, c, first, n);
         const uint64_t row = g * A.W, wm = A.W - 1u, prev = first - 1u;
         const uint32_t ct = A.curr_term[g], pt = A.terms[row + (prev & wm)];
-        const uint32_t replica = static_cast<uint32_t>(q) < A.me ? static_cast<uint32_t>(q) : static_cast<uint32_t>(q) + 1u;
-        const uint32_t mask = own_mask(A.full_copy, A.majority, replica);
+        const uint32_t want = peer_want(A, q);
         uint8_t *fr = A.out + A.frame_off[f];
         if (lane == 0u) {
             cl_put_be64(fr, A.frame_len[f] - 8u);
@@ -414,13 +427,14 @@ __global__ void __launch_bounds__(kClThreads) append_write_kernel(const __grid_c
         }
         uint64_t m = 9u + wv_len(A.variant) + wv_len(ct) + wv_len(prev) + wv_len(pt) + wv_len(n);
         for (uint64_t k = 0; k < n; ++k) {
-            // LogEntry{term, reqs_cw: subset_copy({peer}) or {0..majority}, external: false, log_offset}
+            // LogEntry{term, reqs_cw: subset_copy({peer}) or {0..majority}, external: false, log_offset}; a shard the
+            // leader does not hold goes out as None
             const uint64_t pos = row + ((first + k) & wm);
             const uint32_t et = A.terms[pos];
             const uint64_t lof = A.ent_log_offset[pos];
             if (lane == 0u) wv_put(fr + m, et);
             m += wv_len(et);
-            m += warp_put_cw(fr + m, A.ent_len[pos], A.d, A.T, mask, reinterpret_cast<const uint8_t *>(A.ent_addr[pos]), A.plane_stride, lane);
+            m += warp_put_cw(fr + m, A.ent_len[pos], A.d, A.T, pack_mask<kHeld>(A, pos, want), reinterpret_cast<const uint8_t *>(A.ent_addr[pos]), A.plane_stride, lane);
             if (lane == 0u) {
                 fr[m] = 0u;
                 wv_put(fr + m + 1u, lof);
@@ -529,6 +543,8 @@ struct CraftExecArgs {
     uint32_t W, d;
     uint64_t plane_stride;
     const uint32_t *last_commit, *ent_len;
+    const uint32_t *held;           // nullptr while every entry holds every shard (no step-up, no recon view)
+    const uint8_t *matrix;          // [T*d]
     const uint64_t *log_start, *ent_addr;
     uint64_t *last_exec;
     uint64_t *cnt, *bytes;          // [G] per group: records, payload bytes; then their exclusive scans
@@ -547,17 +563,25 @@ __device__ __forceinline__ uint64_t craft_exec_start(const CraftExecArgs &A, uin
     return s > ls ? s : ls;
 }
 
-// the data_len of the entry at slot s, or 0 past last_commit (a stop) or at a null entry
-__device__ __forceinline__ uint32_t craft_exec_len(const CraftExecArgs &A, uint64_t g, uint64_t s) {
-    return s <= A.last_commit[g] ? A.ent_len[g * A.W + (s & (A.W - 1u))] : 0u;
+enum : uint32_t { kClExecStop = 0u, kClExecRun = 1u, kClExecNull = 2u };
+
+// what the walk does at slot s of group g: stop (past last_commit, or fewer than d shards held: an entry a step-up
+// took over that no absorb has completed yet), run it (*dlen = its data_len), or stop at a null entry, which get_data
+// refuses (rscoding.rs:581-583)
+__device__ __forceinline__ uint32_t craft_exec_next(const CraftExecArgs &A, uint64_t g, uint64_t s, uint32_t *dlen) {
+    if (s > A.last_commit[g]) return kClExecStop;
+    const uint64_t pos = g * A.W + (s & (A.W - 1u));
+    if (A.held != nullptr && static_cast<uint32_t>(__popc(A.held[pos])) < A.d) return kClExecStop;
+    *dlen = A.ent_len[pos];
+    return *dlen == 0u ? kClExecNull : kClExecRun;
 }
 
 __global__ void __launch_bounds__(kClThreads) craft_exec_count_kernel(const __grid_constant__ CraftExecArgs A) {
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kClThreads;
     for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kClThreads + threadIdx.x; g < A.G; g += stride) {
         uint64_t n = 0u, b = 0u;
-        uint32_t dl;
-        for (uint64_t s = craft_exec_start(A, g); (dl = craft_exec_len(A, g, s)) != 0u; ++s, ++n) b += cl_round16(dl);
+        uint32_t dl = 0u;
+        for (uint64_t s = craft_exec_start(A, g); craft_exec_next(A, g, s, &dl) == kClExecRun; ++s, ++n) b += cl_round16(dl);
         A.cnt[g] = n;
         A.bytes[g] = b;
     }
@@ -567,13 +591,12 @@ __global__ void __launch_bounds__(kClThreads) craft_exec_place_kernel(const __gr
     bool full = false, null_ent = false;
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kClThreads;
     for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kClThreads + threadIdx.x; g < A.G; g += stride) {
-        const uint64_t s0 = craft_exec_start(A, g), lc = A.last_commit[g];
+        const uint64_t s0 = craft_exec_start(A, g);
         uint64_t ro = A.cnt[g], bo = A.bytes[g], s = s0;
-        uint32_t dl;
-        bool cut = false;
-        while ((dl = craft_exec_len(A, g, s)) != 0u) {
+        uint32_t dl = 0u, r;
+        while ((r = craft_exec_next(A, g, s, &dl)) == kClExecRun) {
             const uint64_t sz = cl_round16(dl);
-            if (ro >= A.rec_cap || bo > A.out_cap || sz > A.out_cap - bo) { cut = true; break; }
+            if (ro >= A.rec_cap || bo > A.out_cap || sz > A.out_cap - bo) { full = true; break; }
             A.rec_group[ro] = static_cast<uint32_t>(g);
             A.rec_slot[ro] = s;
             A.rec_off[ro] = bo;
@@ -582,8 +605,7 @@ __global__ void __launch_bounds__(kClThreads) craft_exec_place_kernel(const __gr
             bo += sz;
             ++s;
         }
-        full |= cut;
-        null_ent |= !cut && s <= lc;                                        // stopped inside the committed prefix
+        null_ent |= r == kClExecNull;
         if (s != s0) {
             A.last_exec[g] = s - 1u;
             atomicMax(reinterpret_cast<unsigned long long *>(A.n_exec), static_cast<unsigned long long>(ro));
@@ -593,8 +615,8 @@ __global__ void __launch_bounds__(kClThreads) craft_exec_place_kernel(const __gr
     if (null_ent) atomicOr(A.status, SS_DEV_STATUS_EXEC_NULL);
 }
 
-// a warp per record: the leader holds every shard of its entries, shard j at shard_addr + j * plane_stride, so the
-// gather never regenerates one and needs neither the coder's matrix nor the GF(2^8) tables
+// a warp per record while every entry holds every shard (a log that was never stepped up): shard j at shard_addr +
+// j * plane_stride, so the gather never regenerates one and needs neither the coder's matrix nor the GF(2^8) tables
 __global__ void __launch_bounds__(kExecThreads) craft_exec_payload_kernel(const __grid_constant__ CraftExecArgs A) {
     __shared__ ExecShared S;
     const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
@@ -605,6 +627,21 @@ __global__ void __launch_bounds__(kExecThreads) craft_exec_payload_kernel(const 
         const uint64_t g = A.rec_group[r], pos = g * A.W + (A.rec_slot[r] & (A.W - 1u));
         warp_exec_payload(S, w, lane, A.d, all, A.rec_len[r], nullptr, reinterpret_cast<const uint8_t *>(A.ent_addr[pos]), A.plane_stride,
                           A.out + A.rec_off[r]);
+    }
+}
+
+// the same once a held mask may lack shards (after a step-up): shard j of the held mask at shard_addr + j *
+// plane_stride, a missing data shard regenerated from the first d held ones
+__global__ void __launch_bounds__(kExecThreads) craft_exec_regen_kernel(const __grid_constant__ CraftExecArgs A) {
+    __shared__ ExecShared S;
+    exec_tables_init(S);
+    const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+    const uint64_t n = *A.n_exec;
+    const uint64_t nwarps = static_cast<uint64_t>(gridDim.x) * kExecWarps;
+    for (uint64_t r = static_cast<uint64_t>(blockIdx.x) * kExecWarps + w; r < n; r += nwarps) {
+        const uint64_t g = A.rec_group[r], pos = g * A.W + (A.rec_slot[r] & (A.W - 1u));
+        warp_exec_payload<true>(S, w, lane, A.d, A.held[pos], A.rec_len[r], A.matrix, reinterpret_cast<const uint8_t *>(A.ent_addr[pos]),
+                                A.plane_stride, A.out + A.rec_off[r]);
     }
 }
 
@@ -631,13 +668,13 @@ static int cl_alloc(ss_ctx *ctx, T **p, size_t count, bool zero) {
 void craft_log_free(ss_engine *e) {
     void *bufs[] = {e->log_start, e->try_next, e->ent_len, e->ent_addr, e->ent_log_offset, e->cl_partials, e->cl_words, e->cl_eff,
                     e->cl_wal, e->pk_frames, e->pk_bytes, e->pk_range, e->last_exec, e->ex_cnt, e->ex_bytes, e->ex_words, e->bo_keys,
-                    e->bo_idx, e->bo_sort_tmp};
+                    e->bo_idx, e->bo_sort_tmp, e->held, e->last_recon, e->matrix, e->rc_words};
     for (void *b : bufs)
         if (b) cudaFree(b);
 }
 
 // the configuration checks every log call makes
-static int craft_check(ss_engine *e) {
+int craft_check(ss_engine *e) {
     if (e == nullptr) return set_error(SS_ERR_INVALID_ARG, "null engine");
     if (e->cfg.protocol != SS_PROTO_CRAFT) return set_error(SS_ERR_INVALID_ARG, "the leader's log serves CRaft engines only");
     if (e->raft_appended) return set_error(SS_ERR_INVALID_ARG, "ss_engine_raft_append ran on this engine: its entries have no codeword");
@@ -645,8 +682,32 @@ static int craft_check(ss_engine *e) {
     return SS_OK;
 }
 
+// the coder's matrix, whose rows execute inverts on the device; a pageable source is staged before the call returns
+static int upload_matrix(ss_engine *e) {
+    const gf::Matrix m = gf::coding_matrix(static_cast<int>(e->majority), static_cast<int>(e->n - e->majority));
+    SS_CUDA(cudaMemcpyAsync(e->matrix, m.v.data(), m.v.size(), cudaMemcpyHostToDevice, e->ctx->stream));
+    return SS_OK;
+}
+
+// every ring position: every shard
+__global__ void __launch_bounds__(kClThreads) craft_held_fill_kernel(uint32_t *held, uint64_t n, uint32_t all) {
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kClThreads;
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kClThreads + threadIdx.x; i < n; i += stride) held[i] = all;
+}
+
+int craft_held_in_use(ss_engine *e) {
+    if (e->held_partial) return SS_OK;
+    // until now every entry was proposed, so it holds every shard: the masks start full
+    ss_ctx *ctx = e->ctx;
+    const uint64_t n = e->G * e->W;
+    craft_held_fill_kernel<<<cl_grid(ctx, n, kClThreads), kClThreads, 0, ctx->stream>>>(e->held, n, e->n >= 32u ? 0xffffffffu : (1u << e->n) - 1u);
+    SS_TRY(launched(ctx));
+    e->held_partial = true;
+    return SS_OK;
+}
+
 // takes the log into use: its state, scratch and coder on the first call
-static int craft_log_init(ss_engine *e) {
+int craft_log_init(ss_engine *e) {
     ss_ctx *ctx = e->ctx;
     SS_TRY(ctx_bind(ctx));
     if (e->log_in_use) return SS_OK;
@@ -660,7 +721,9 @@ static int craft_log_init(ss_engine *e) {
         (rc = cl_alloc(ctx, &e->pk_frames, PG, false)) || (rc = cl_alloc(ctx, &e->pk_bytes, PG, false)) ||
         (rc = cl_alloc(ctx, &e->pk_range, PG, false)) || (rc = cl_alloc(ctx, &e->log_start, G, true)) ||
         (rc = cl_alloc(ctx, &e->last_exec, G, true)) || (rc = cl_alloc(ctx, &e->ex_cnt, G, false)) ||
-        (rc = cl_alloc(ctx, &e->ex_bytes, G, false)) || (rc = cl_alloc(ctx, &e->ex_words, 3, false))) {
+        (rc = cl_alloc(ctx, &e->ex_bytes, G, false)) || (rc = cl_alloc(ctx, &e->ex_words, 3, false)) ||
+        (rc = cl_alloc(ctx, &e->held, GW, true)) || (rc = cl_alloc(ctx, &e->last_recon, G, true)) ||
+        (rc = cl_alloc(ctx, &e->matrix, size_t(e->n) * e->majority, false)) || (rc = upload_matrix(e))) {
         // nothing half-built stays behind: a later call starts over, and raft_append stays allowed
         cudaStreamSynchronize(ctx->stream);
         craft_log_free(e);
@@ -669,19 +732,20 @@ static int craft_log_init(ss_engine *e) {
         e->pk_frames = nullptr; e->pk_bytes = nullptr; e->pk_range = nullptr;
         e->last_exec = nullptr; e->ex_cnt = nullptr; e->ex_bytes = nullptr; e->ex_words = nullptr;
         e->bo_keys = nullptr; e->bo_idx = nullptr; e->bo_sort_tmp = nullptr; e->bo_cap = 0;
+        e->held = nullptr; e->last_recon = nullptr; e->matrix = nullptr; e->rc_words = nullptr; e->rc_cap = 0;
         return rc;
     }
     e->log_in_use = true;
     return SS_OK;
 }
 
-static int key_bits(uint64_t v) {
+int key_bits(uint64_t v) {
     int b = 1;
     while (b < 32 && (v >> b) != 0u) ++b;
     return b;
 }
 
-static int backoff_scratch(ss_engine *e, uint64_t n, int bits) {
+int backoff_scratch(ss_engine *e, uint64_t n, int bits) {
     if (n <= e->bo_cap) return SS_OK;
     ss_ctx *ctx = e->ctx;
     SS_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -741,7 +805,9 @@ int ss_engine_craft_propose(ss_engine *e, uint32_t me, const uint8_t *arena, con
     A.data_len = data_len; A.log_offset = log_offset; A.shards = shards; A.plane_stride = plane_stride; A.wal_capacity = wal_capacity;
     A.shard_off = shard_off; A.slot_out = slot_out; A.wal_off = wal_off; A.wal_len = wal_len; A.wal = wal;
     A.log_start = e->log_start; A.log_end = e->log_end; A.terms = e->terms; A.curr_term = e->curr_term;
-    A.ent_len = e->ent_len; A.ent_addr = e->ent_addr; A.ent_log_offset = e->ent_log_offset; A.eff = e->cl_eff; A.rec_len = e->cl_wal;
+    A.ent_len = e->ent_len; A.held = e->held_partial ? e->held : nullptr; A.ent_addr = e->ent_addr; A.ent_log_offset = e->ent_log_offset;
+    A.eff = e->cl_eff;
+    A.rec_len = e->cl_wal;
     A.status = ctx->dev_status;
     const uint32_t grid = cl_grid(ctx, e->G, kClThreads);
     craft_propose_prepare_kernel<<<grid, kClThreads, 0, ctx->stream>>>(A);
@@ -777,21 +843,27 @@ int ss_frame_append_pack_dev(ss_engine *e, const ss_append_pack_spec *spec, cons
     A.heartbeat = spec->heartbeat ? 1u : 0u;
     A.want_end = spec->heartbeat ? nullptr : want_end;
     A.next_slot = e->next_slot; A.log_end = e->log_end; A.curr_term = e->curr_term; A.terms = e->terms; A.last_commit = e->last_commit;
-    A.last_snap = e->last_snap; A.try_next = e->try_next; A.log_start = e->log_start; A.ent_len = e->ent_len; A.ent_addr = e->ent_addr;
+    A.last_snap = e->last_snap; A.try_next = e->try_next; A.log_start = e->log_start; A.ent_len = e->ent_len;
+    A.held = e->held_partial ? e->held : nullptr; A.ent_addr = e->ent_addr;
     A.ent_log_offset = e->ent_log_offset; A.plane_stride = e->log_plane_stride;
     A.out = out; A.out_capacity = out_capacity; A.max_frames = max_frames; A.frame_off = frame_off; A.frame_len = frame_len;
     A.frame_group = frame_group; A.frame_peer = frame_peer; A.n_frames = n_frames; A.total = total != nullptr ? total : e->cl_words + 3;
     A.pair_status = pair_status; A.pk_frames = e->pk_frames; A.pk_bytes = e->pk_bytes; A.pk_range = e->pk_range;
     A.frames_total = e->cl_words; A.status = ctx->dev_status;
     const uint32_t grid_w = cl_grid(ctx, A.PG, kClThreads / 32);
-    append_plan_kernel<<<grid_w, kClThreads, 0, ctx->stream>>>(A);
+    const bool held = e->held_partial;
+    if (held) append_plan_kernel<true><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
+    else append_plan_kernel<false><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     SS_TRY(launch_exclusive_scan_u64(ctx, e->pk_frames, A.PG, e->cl_partials, e->cl_words));
     SS_TRY(launch_exclusive_scan_u64(ctx, e->pk_bytes, A.PG, e->cl_partials, A.total));
     SS_CUDA(cudaMemcpyAsync(n_frames, e->cl_words, 8, cudaMemcpyDeviceToDevice, ctx->stream));
-    append_place_kernel<<<grid_w, kClThreads, 0, ctx->stream>>>(A);
+    if (held) append_place_kernel<true><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
+    else append_place_kernel<false><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
-    append_write_kernel<<<cl_grid(ctx, max_frames, kClThreads / 32), kClThreads, 0, ctx->stream>>>(A);
+    const uint32_t grid_f = cl_grid(ctx, max_frames, kClThreads / 32);
+    if (held) append_write_kernel<true><<<grid_f, kClThreads, 0, ctx->stream>>>(A);
+    else append_write_kernel<false><<<grid_f, kClThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
 }
 
@@ -845,7 +917,8 @@ int ss_engine_craft_execute(ss_engine *e, uint8_t *out, uint64_t out_capacity, u
     ss_ctx *ctx = e->ctx;
     CraftExecArgs A{};
     A.G = e->G; A.W = e->W; A.d = e->majority; A.plane_stride = e->log_plane_stride;
-    A.last_commit = e->last_commit; A.ent_len = e->ent_len; A.log_start = e->log_start; A.ent_addr = e->ent_addr;
+    A.last_commit = e->last_commit; A.ent_len = e->ent_len; A.held = e->held_partial ? e->held : nullptr; A.matrix = e->matrix;
+    A.log_start = e->log_start; A.ent_addr = e->ent_addr;
     A.last_exec = e->last_exec; A.cnt = e->ex_cnt; A.bytes = e->ex_bytes; A.n_exec = e->ex_words;
     A.out = out; A.out_cap = out_capacity; A.rec_group = rec_group; A.rec_slot = rec_slot; A.rec_off = rec_off; A.rec_len = rec_len;
     A.rec_cap = rec_capacity; A.status = ctx->dev_status;
@@ -859,7 +932,9 @@ int ss_engine_craft_execute(ss_engine *e, uint8_t *out, uint64_t out_capacity, u
     craft_exec_place_kernel<<<grid, kClThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     // a warp per entry the ring can hold, up to the grid cap; warps past the executed count return at once
-    craft_exec_payload_kernel<<<cl_grid(ctx, e->G * e->W, kExecWarps), kExecThreads, 0, ctx->stream>>>(A);
+    const uint32_t grid_p = cl_grid(ctx, e->G * e->W, kExecWarps);
+    if (e->held_partial) craft_exec_regen_kernel<<<grid_p, kExecThreads, 0, ctx->stream>>>(A);
+    else craft_exec_payload_kernel<<<grid_p, kExecThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
 }
 

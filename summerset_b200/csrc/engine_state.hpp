@@ -44,6 +44,14 @@ struct ss_engine {
     uint64_t *cl_wal = nullptr;             // [G] propose: WAL record lengths
     uint64_t *pk_frames = nullptr, *pk_bytes = nullptr, *pk_range = nullptr;   // [P*G] pack scratch
     uint64_t *last_exec = nullptr;          // [G] last executed slot (ss_engine_craft_execute)
+    uint32_t *held = nullptr;               // [G][W] shards the leader holds (propose: all; step-up: the follower's),
+                                            // kept from the first step-up or recon view on (craft_held_in_use)
+    uint64_t *last_recon = nullptr;         // [G] last slot a reconstruct read listed (ss_engine_craft_reconstruct_reads)
+    uint8_t *matrix = nullptr;              // [T*d] the coder's coding matrix: execute regenerates missing data shards
+    bool held_partial = false;              // a held mask may lack shards (step-up ran, or the recon view was handed out);
+                                            // until then propose, pack and execute neither write nor read held
+    uint64_t *rc_words = nullptr;           // [n] recon scratch (listed groups / frames), grow-only with rc_cap
+    uint64_t rc_cap = 0;
     uint64_t *ex_cnt = nullptr, *ex_bytes = nullptr;   // [G] execute scratch: records and payload bytes, then their scans
     uint64_t *ex_words = nullptr;           // [3] records written, and the totals when the caller passes none
     uint64_t bo_cap = 0;                    // backoff scratch, grow-only
@@ -55,4 +63,28 @@ struct ss_engine {
 namespace ssb {
 // frees the CRaft log's state and scratch (craft_leader.cu)
 void craft_log_free(ss_engine *e);
+// the configuration checks every log call makes, and taking the log into use on the first call (craft_leader.cu)
+int craft_check(ss_engine *e);
+int craft_log_init(ss_engine *e);
+// held is kept from here on: every mask starts full (only propose made entries so far), and propose writes it (craft_leader.cu)
+int craft_held_in_use(ss_engine *e);
+// bits of a radix-sort key up to v, and the log's grow-only sort scratch (bo_*) for n keys of that many bits, shared by
+// the back-off and absorb (craft_leader.cu)
+int key_bits(uint64_t v);
+int backoff_scratch(ss_engine *e, uint64_t n, int bits);
+
+// the log calls' grid: enough CTAs of per_cta items, capped at 64 per SM
+inline uint32_t cl_grid(ss_ctx *ctx, uint64_t items, uint32_t per_cta) {
+    uint64_t ctas = (items + per_cta - 1) / per_cta;
+    const uint64_t cap = static_cast<uint64_t>(ctx->sm_count) * 8ull * 8ull;
+    if (ctas > cap) ctas = cap;
+    if (ctas == 0) ctas = 1;
+    return static_cast<uint32_t>(ctas);
+}
+
+__device__ __forceinline__ uint64_t cl_round16(uint64_t x) { return (x + 15u) & ~15ull; }
+
+__device__ __forceinline__ void cl_put_be64(uint8_t *p, uint64_t v) {
+    for (int b = 0; b < 8; ++b) p[b] = static_cast<uint8_t>(v >> (8 * (7 - b)));
+}
 }  // namespace ssb

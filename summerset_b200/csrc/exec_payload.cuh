@@ -2,9 +2,10 @@
 //
 // Shared by the three execution walks: the acceptor's (acceptor.cu), the CRaft follower's (follower.cu) and the CRaft
 // leader's (craft_leader.cu).  Each calls warp_exec_payload once per record with the entry's held mask and the address
-// rule of its shards: held shard j of rank k (k-th set bit of held) is at src + k * stride.  The acceptor and the
-// follower keep only their held shards in padded store slots (stride SS_CW_SLOT_PITCH(L)); the leader holds every shard
-// of its entries in planes (stride plane_stride, rank = shard index) and so never regenerates one.
+// rule of its shards, chosen at compile time: by rank (the default), held shard j of rank k (k-th set bit of held) is
+// at src + k * stride -- the acceptor and the follower keep only their held shards in padded store slots (stride
+// SS_CW_SLOT_PITCH(L)); by index, shard j is at src + j * stride -- the leader's planes (stride plane_stride), where a
+// stepped-up leader reserves a slot for every shard and holds some of them.
 #pragma once
 #include <cstdint>
 
@@ -48,10 +49,12 @@ __device__ __forceinline__ void exec_tables_init(ExecShared &S) {
 }
 
 // Output-stationary: lane v writes payload bytes [16v, 16v + 16) of dst with one aligned 128-bit store (zero past dlen).
-// Data shard i is payload bytes [i*L, (i+1)*L); a held one is read at src + rank(i)*stride, a missing one is the
+// Data shard i is payload bytes [i*L, (i+1)*L); a held one is read at src + rank(i)*stride (kByIndex: src + i*stride),
+// a missing one is the
 // GF(2^8) combination of the first d held shards (ranks 0..d-1) with row i of inverse(M[sources]), reconstruct_data's
 // choice of sources (rscoding.rs:490-537).  matrix: the coder's [T*d] coding matrix; held has at least d bits below T.
 // Ends with __syncwarp: the warp's next record may overwrite the rows this one read.
+template <bool kByIndex = false>
 __device__ __forceinline__ void warp_exec_payload(ExecShared &S, uint32_t w, uint32_t lane, uint32_t d, uint32_t held, uint32_t dlen,
                                                   const uint8_t *matrix, const uint8_t *src, uint64_t stride, uint8_t *dst) {
     uint8_t (*ra)[32] = S.a[w];
@@ -96,9 +99,13 @@ __device__ __forceinline__ void warp_exec_payload(ExecShared &S, uint32_t w, uin
     }
     // bytes [o, o + c) of data shard i (c <= 16) as the low c bytes of a uint4, the rest zero
     auto shard16 = [&](uint32_t i, uint32_t o, int c) -> uint4 {
-        if ((held >> i) & 1u) return dev::load16(src + __popc(held & ((1u << i) - 1u)) * stride + o, c);
+        if ((held >> i) & 1u) {
+            if (kByIndex) return dev::load16(src + i * stride + o, c);
+            return dev::load16(src + __popc(held & ((1u << i) - 1u)) * stride + o, c);
+        }
         const uint8_t *coef = ri[piv[i]];
         uint4 acc = make_uint4(0u, 0u, 0u, 0u);
+        uint32_t rest = held;                                          // kByIndex: the held shards not yet a source
         for (uint32_t q0 = 0; q0 < d; q0 += kChunk) {
             uint32_t cq[kChunk], top = 0u;
             dev::Raw16 raw[kChunk];
@@ -107,7 +114,12 @@ __device__ __forceinline__ void warp_exec_payload(ExecShared &S, uint32_t w, uin
                 const bool in = q0 + q < d;
                 cq[q] = in ? coef[q0 + q] : 0u;
                 top |= cq[q];
-                raw[q] = dev::raw16_issue(src + (q0 + q) * stride + o, in && cq[q] != 0u ? c : 0);
+                uint32_t at = q0 + q;                                  // source q0 + q
+                if (kByIndex) {
+                    at = in ? static_cast<uint32_t>(__ffs(static_cast<int>(rest))) - 1u : 0u;
+                    if (in) rest &= rest - 1u;
+                }
+                raw[q] = dev::raw16_issue(src + at * stride + o, in && cq[q] != 0u ? c : 0);
             }
             uint4 x[kChunk];
 #pragma unroll

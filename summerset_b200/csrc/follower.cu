@@ -27,6 +27,8 @@
 //   fol_exec_place_kernel    a thread per group: capacities, the records, last_exec
 //   fol_exec_payload_kernel  a warp per record: get_data's bytes from the held shards, a missing data shard regenerated
 //                            from the first d held ones (exec_payload.cuh)
+//
+// Serving a new leader's Reconstruct reads (ss_follower_reconstruct_serve) is in craft_recon.cu.
 #include <cub/device/device_radix_sort.cuh>
 
 #include <cstring>
@@ -35,6 +37,7 @@
 #include "codeword_wire.cuh"
 #include "device_common.cuh"
 #include "exec_payload.cuh"
+#include "follower_state.hpp"
 #include "gf256.hpp"
 #include "ss_internal.hpp"
 #include "wire_common.cuh"
@@ -57,28 +60,6 @@ struct Ent {
 };
 
 }  // namespace ssb
-
-struct ss_follower {
-    ss_ctx *ctx = nullptr;
-    ss_follower_config cfg{};
-    uint32_t d = 0, T = 0, W = 0;
-    uint64_t G = 0;
-    uint64_t *start_slot = nullptr, *log_end = nullptr, *curr_term = nullptr, *last_commit = nullptr, *last_snap = nullptr;
-    uint8_t *leader = nullptr;
-    uint64_t *term = nullptr, *shard_addr = nullptr;
-    uint32_t *held = nullptr, *data_len = nullptr;
-    uint64_t *last_exec = nullptr;  // [G] last executed slot (ss_follower_execute)
-    uint8_t *matrix = nullptr;      // [T*d] the coder's coding matrix (gf256.hpp), row-major
-    uint64_t *ex_cnt = nullptr, *ex_bytes = nullptr, *ex_partials = nullptr, *ex_words = nullptr;   // execute scratch
-    // per-call scratch, grow-only
-    uint64_t cap_frames = 0;
-    ssb::FolHdr *hdr = nullptr;
-    uint32_t *keys = nullptr, *idx = nullptr;   // [2][cap]
-    uint64_t *partials = nullptr;
-    void *sort_tmp = nullptr;
-    size_t sort_tmp_bytes = 0;
-    uint64_t *words = nullptr;      // [4]: cut key, absorb cursor, totals when the caller passes none
-};
 
 namespace ssb {
 
@@ -673,7 +654,7 @@ static int fol_key_bits(uint64_t G) {
     return b;
 }
 
-static int fol_scratch(ss_follower *f, uint64_t n) {
+int fol_scratch(ss_follower *f, uint64_t n) {
     if (n <= f->cap_frames) return SS_OK;
     ss_ctx *ctx = f->ctx;
     SS_CUDA(cudaStreamSynchronize(ctx->stream));

@@ -34,12 +34,15 @@ torch tensors (zero-copy views) so tests can read results and install state; it 
         backoff(buf, frame_off, frame_group, frame_peer, rec_kind)   the conflict branch (craft/messages.rs:386-406)
         advance_log(upto) / log_view()      the snapshot's start_slot move; log_start, try_next and the entry rings
         execute(out, rec_capacity) / exec_view()   the committed entries' request batches (craft/messages.rs:316-359)
+        step_up(follower, groups, term, store) / reconstruct_reads(out, ...) / absorb(buf, ...) / recon_view()
+                                            fail-over: become_the_leader's log half, Reconstruct reads, their replies
         set_full_copy(on)                   the commit threshold of full-copy mode (craft/leadership.rs:282-288)
     Follower(ctx, G, population, me[, window])   the CRaft follower
         append(buf, frame_off, frame_group, frame_peer, store, wal)   handle_msg_append_entries (craft/messages.rs:14-252):
                                             store, LogEntry / Metadata records, AppendEntriesReply cells
         advance(upto)                       the snapshot's start_slot move
         execute(out, rec_capacity)          the committed entries' request batches (craft/messages.rs:198-240)
+        reconstruct_serve(buf, ...)         a new leader's Reconstruct reads (craft/messages.rs:621-662)
     append_reply_parse(ctx, buf, frame_off, frame_group, frame_peer, curr_term, G)   the leader's side: AppendEntriesReply
                                             frames -> RaftEngine.on_append_replies records
 """
@@ -326,6 +329,58 @@ class RaftEngine(_EngineBase):
         round_up(data_len, 16) region each).  Returns device tensors rec_group (int32), rec_slot, rec_off (int64),
         rec_len (int32), each [rec_capacity], and totals (int64 [2]: records and bytes asked for)."""
         return _execute(self.lib.ss_engine_craft_execute, self.h, out, rec_capacity, out_capacity)
+
+    # ---- fail-over: step-up from this replica's follower, reconstruct reads, absorbing the replies ----
+    def recon_view(self) -> dict:
+        """Takes the log into use and returns zero-copy views: held int32 [G, W] (shard masks) and last_recon int64 [G]."""
+        v = _lib.CraftReconView()
+        check(self.lib.ss_engine_craft_recon_view_get(self.h, C.byref(v)))
+        return dict(held=self._tensor(v.held, (self.G, self.W), "<i4", torch.int32),
+                    last_recon=self._tensor(v.last_recon, (self.G,), "<i8", torch.int64))
+
+    def step_up(self, follower: "Follower", groups: torch.Tensor, term: torch.Tensor, store: torch.Tensor) -> dict:
+        """The log half of become_the_leader for the listed groups (int32 [n]) in term (int64 [n]), taken from this
+        replica's follower; the entries' shards go into store (uint8 [T, plane_stride], caller-owned, alive while the
+        entries are).  Returns device tensors shard_off (int64 [n], -1 = not stepped up), verdict (int32 [n]) and need
+        (int64 [1])."""
+        assert groups.dtype == torch.int32 and term.dtype == torch.int64 and groups.numel() == term.numel()
+        assert store.dtype == torch.uint8 and store.dim() == 2 and store.is_contiguous()
+        n, dev = groups.numel(), self.dev
+        out = dict(shard_off=torch.empty(n, dtype=torch.int64, device=dev), verdict=torch.empty(n, dtype=torch.int32, device=dev),
+                   need=torch.empty(1, dtype=torch.int64, device=dev))
+        p = lambda x: x.data_ptr()
+        check(self.lib.ss_engine_craft_step_up(self.h, follower.h, p(groups), n, p(term), p(store), store.shape[1], p(out["shard_off"]),
+                                               p(out["need"]), p(out["verdict"])))
+        return out
+
+    def reconstruct_reads(self, out: torch.Tensor, frame_capacity: int, chunk_size: int, groups: Optional[torch.Tensor] = None,
+                          out_capacity: Optional[int] = None, reconstruct_variant: int = 4) -> dict:
+        """Reconstruct{slots: Vec<(slot, term)>} frames for the committed entries past last_recon holding fewer than d
+        shards, each to be broadcast.  Outputs as Acceptor.step_up_reads()."""
+        assert out.dtype == torch.uint8 and (groups is None or groups.dtype == torch.int32)
+        dev, cap = out.device, max(frame_capacity, 1)
+        res = dict(frame_group=torch.empty(cap, dtype=torch.int32, device=dev), frame_dst=torch.empty(cap, dtype=torch.uint8, device=dev),
+                   frame_off=torch.empty(cap, dtype=torch.int64, device=dev), frame_len=torch.empty(cap, dtype=torch.int32, device=dev),
+                   totals=torch.empty(2, dtype=torch.int64, device=dev))
+        p = lambda x: None if x is None else x.data_ptr()
+        check(self.lib.ss_engine_craft_reconstruct_reads(self.h, p(groups), 0 if groups is None else groups.numel(), chunk_size,
+                                                         reconstruct_variant, p(out), out.numel() if out_capacity is None else out_capacity,
+                                                         p(res["frame_group"]), p(res["frame_dst"]), p(res["frame_off"]),
+                                                         p(res["frame_len"]), frame_capacity, p(res["totals"])))
+        return res
+
+    def absorb(self, buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor, frame_peer: torch.Tensor,
+               reply_variant: int = 5) -> dict:
+        """Absorbs ReconstructReply frames into the slots step_up reserved.  Returns device tensors absorbed (int32: entries
+        of each frame that added shards) and verdict (int32)."""
+        assert buf.dtype == torch.uint8 and frame_off.dtype == torch.int64 and frame_group.dtype == torch.int32
+        assert frame_peer.dtype == torch.uint8
+        n, dev = frame_off.numel(), buf.device
+        res = dict(absorbed=torch.empty(n, dtype=torch.int32, device=dev), verdict=torch.empty(n, dtype=torch.int32, device=dev))
+        p = lambda x: x.data_ptr()
+        check(self.lib.ss_engine_craft_absorb(self.h, p(buf), buf.numel(), p(frame_off), p(frame_group), p(frame_peer), n, reply_variant,
+                                              p(res["absorbed"]), p(res["verdict"])))
+        return res
 
 
 class Acceptor:
@@ -644,6 +699,23 @@ class Follower:
         """Executes the committed entries from last_exec + 1, regenerating missing data shards: payloads into out
         (uint8, 16-byte aligned, one round_up(data_len, 16) region each).  Returns what Acceptor.execute returns."""
         return _execute(self.lib.ss_follower_execute, self.h, out, rec_capacity, out_capacity)
+
+    def reconstruct_serve(self, buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor, frame_peer: torch.Tensor,
+                          out: torch.Tensor, out_capacity: Optional[int] = None, reconstruct_variant: int = 4,
+                          reply_variant: int = 5) -> dict:
+        """Serves a new leader's Reconstruct{slots: Vec<(slot, term)>} frames from the held shards.  Outputs as
+        Acceptor.reconstruct_serve()."""
+        assert buf.dtype == torch.uint8 and frame_off.dtype == torch.int64 and frame_group.dtype == torch.int32
+        assert frame_peer.dtype == torch.uint8 and out.dtype == torch.uint8
+        n, dev = frame_off.numel(), buf.device
+        res = dict(reply_off=torch.empty(n, dtype=torch.int64, device=dev), reply_len=torch.empty(n, dtype=torch.int64, device=dev),
+                   verdict=torch.empty(n, dtype=torch.int32, device=dev), total=torch.empty(1, dtype=torch.int64, device=dev))
+        p = lambda x: x.data_ptr()
+        check(self.lib.ss_follower_reconstruct_serve(self.h, p(buf), buf.numel(), p(frame_off), p(frame_group), p(frame_peer), n,
+                                                     reconstruct_variant, reply_variant, p(out),
+                                                     out.numel() if out_capacity is None else out_capacity, p(res["reply_off"]),
+                                                     p(res["reply_len"]), p(res["verdict"]), p(res["total"])))
+        return res
 
     def close(self) -> None:
         if getattr(self, "h", None) is not None and self.h:

@@ -429,6 +429,16 @@ class Follower {
                  uint64_t rec_capacity, uint64_t *totals = nullptr) {
         check(ss_follower_execute(fol_, out, out_capacity, rec_group, rec_slot, rec_off, rec_len, rec_capacity, totals));
     }
+    // a new leader's Reconstruct frames answered from the held shards (see ss_follower_reconstruct_serve)
+    void handle_msg_reconstruct(const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
+                                const uint8_t *frame_peer, uint64_t n_frames, uint8_t *out, uint64_t out_capacity, uint64_t *reply_off,
+                                uint64_t *reply_len, uint32_t *verdict, uint64_t *total = nullptr, uint32_t reconstruct_variant = 4,
+                                uint32_t reply_variant = 5) {
+        check(ss_follower_reconstruct_serve(fol_, buf, buf_len, frame_off, frame_group, frame_peer, n_frames, reconstruct_variant,
+                                            reply_variant, out, out_capacity, reply_off, reply_len, verdict, total));
+    }
+    // the handle, for ss_engine_craft_step_up
+    const ss_follower *get() const { return fol_; }
 
   private:
     ss_follower *fol_ = nullptr;
@@ -477,6 +487,27 @@ inline ss_engine_craft_exec_view craft_exec_view(ss_engine *e) {
 inline void craft_execute(ss_engine *e, uint8_t *out, uint64_t out_capacity, uint32_t *rec_group, uint64_t *rec_slot, uint64_t *rec_off,
                           uint32_t *rec_len, uint64_t rec_capacity, uint64_t *totals = nullptr) {
     check(ss_engine_craft_execute(e, out, out_capacity, rec_group, rec_slot, rec_off, rec_len, rec_capacity, totals));
+}
+// fail-over: step-up from this replica's follower, the Reconstruct reads, the replies absorbed (ss_engine_craft_step_up ...)
+inline ss_engine_craft_recon_view craft_recon_view(ss_engine *e) {
+    ss_engine_craft_recon_view v{};
+    check(ss_engine_craft_recon_view_get(e, &v));
+    return v;
+}
+inline void craft_step_up(ss_engine *e, const Follower &follower, const uint32_t *groups, uint64_t n_listed, const uint64_t *term,
+                          uint8_t *shards, uint64_t plane_stride, uint64_t *shard_off, uint32_t *verdict, uint64_t *need = nullptr) {
+    check(ss_engine_craft_step_up(e, follower.get(), groups, n_listed, term, shards, plane_stride, shard_off, need, verdict));
+}
+inline void craft_reconstruct_reads(ss_engine *e, const uint32_t *groups, uint64_t n_listed, uint64_t chunk_size, uint8_t *out,
+                                    uint64_t out_capacity, uint32_t *frame_group, uint8_t *frame_dst, uint64_t *frame_off,
+                                    uint32_t *frame_len, uint64_t frame_capacity, uint64_t *totals = nullptr,
+                                    uint32_t reconstruct_variant = 4) {
+    check(ss_engine_craft_reconstruct_reads(e, groups, n_listed, chunk_size, reconstruct_variant, out, out_capacity, frame_group,
+                                            frame_dst, frame_off, frame_len, frame_capacity, totals));
+}
+inline void craft_absorb(ss_engine *e, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
+                         const uint8_t *frame_peer, uint64_t n_frames, uint32_t *absorbed, uint32_t *verdict, uint32_t reply_variant = 5) {
+    check(ss_engine_craft_absorb(e, buf, buf_len, frame_off, frame_group, frame_peer, n_frames, reply_variant, absorbed, verdict));
 }
 
 }  // namespace ssb
