@@ -12,6 +12,7 @@ pad, last_exec and payload byte with the restatement and with the request batche
 from __future__ import annotations
 
 import ctypes as C
+import functools
 import random
 
 import numpy as np
@@ -72,8 +73,10 @@ for _i in range(255):
     _LOG[_v] = _i
     _v = (_v << 1) ^ (0x11D if _v & 0x80 else 0)
 gmul = lambda a, b: _EXP[_LOG[a] + _LOG[b]] if a and b else 0
+_MUL = np.array([[gmul(a, b) for b in range(256)] for a in range(256)], dtype=np.uint8)   # _MUL[a][x] = a * x
 
 
+@functools.lru_cache(maxsize=None)
 def decode_rows(d, p, held):
     """inverse(M[the first d held shards]) by the warp's Gauss-Jordan: pivots in column order, rows never swapped;
     -> rows[i] = the coefficients of data shard i over sources 0..d-1"""
@@ -102,20 +105,21 @@ def payload(stored, held, d, p, dl):
     """the bytes the warp writes: stored[k] = the held shard of rank k (L bytes); round_up(dl, 16) bytes, zero past dl"""
     L = -(-dl // d)
     rows = decode_rows(d, p, held) if held & ((1 << d) - 1) != (1 << d) - 1 else None
+    src = [np.frombuffer(bytes(x), dtype=np.uint8)[:L] for x in stored]
 
-    def shard_byte(i, o):
+    def shard(i):                                                 # data shard i: held, or regenerated from sources 0..d-1
         if held >> i & 1:
-            return stored[popc(held & ((1 << i) - 1))][o]
-        acc = 0
+            return src[popc(held & ((1 << i) - 1))]
+        acc = np.zeros(L, dtype=np.uint8)
         for q in range(d):
-            acc ^= gmul(rows[i][q], stored[q][o])
+            acc ^= _MUL[rows[i][q]][src[q]]
         return acc
 
-    out = bytearray(r16(dl))
-    for v in range(-(-dl // 16)):                                 # output-stationary 16-byte columns
-        for pos in range(16 * v, min(dl, 16 * v + 16)):
-            out[pos] = shard_byte(pos // L, pos % L)              # a column may straddle shards
-    return bytes(out)
+    data = np.stack([shard(i) for i in range(d)])
+    pos = np.arange(dl)
+    out = np.zeros(r16(dl), dtype=np.uint8)
+    out[:dl] = data[pos // L, pos % L]                            # byte pos of a 16-byte column, which may straddle shards
+    return out.tobytes()
 
 
 def coded(batch, d, p):
@@ -443,13 +447,14 @@ def test_leader_execute_matches_the_restatement(n):
     eng.close()
 
 
-def _install(fol, G, groups, W):
+def _install(fol, G, groups, W, fill=0, skew=0):
     """state through the follower's view: groups[g] = dict(start, lc, le, ent={slot: (data_len, held, batch)}); shards
-    from the oracle's encoder in the padded layout (held shard of rank k at shard_addr + k * pitch(L)) -> the store"""
+    from the oracle's encoder in the padded layout (held shard of rank k at shard_addr + k * pitch(L)), each slot's pad
+    filled with the byte `fill`, every entry `skew` bytes past a 32-byte boundary of the store -> the store"""
     import torch
     d, p = fol.d, fol.T - fol.d
     dev = "cuda:0"
-    blob, addr = bytearray(), {}
+    blob, addr = bytearray([fill] * skew), {}
     for g, gr in enumerate(groups):
         for s, (dl, held, b) in gr["ent"].items():
             if dl == 0:
@@ -459,11 +464,11 @@ def _install(fol, G, groups, W):
             addr[(g, s)] = len(blob)
             for j in range(d + p):
                 if held >> j & 1:
-                    blob += sh[j].tobytes() + bytes(pitch(L) - L)
+                    blob += sh[j].tobytes() + bytes([fill] * (pitch(L) - L))
     store = torch.tensor(np.frombuffer(bytes(blob) + bytes(16), dtype=np.uint8), device=dev)
     base = store.data_ptr()
     sa = np.zeros((G, W), dtype=np.int64)
-    held = np.zeros((G, W), dtype=np.int32)
+    held = np.zeros((G, W), dtype=np.uint32)                       # shard 31's bit does not fit an int32
     dlen = np.zeros((G, W), dtype=np.int32)
     term = np.zeros((G, W), dtype=np.int64)
     for g, gr in enumerate(groups):
@@ -472,7 +477,7 @@ def _install(fol, G, groups, W):
             held[g][s % W], dlen[g][s % W], term[g][s % W] = h, dl, 1
     t = lambda a: torch.tensor(a, device=dev)
     fol.shard_addr.copy_(t(sa))
-    fol.held.copy_(t(held))
+    fol.held.copy_(t(held.view(np.int32)))
     fol.data_len.copy_(t(dlen))
     fol.term.copy_(t(term))
     fol.start_slot.copy_(t(np.array([gr["start"] for gr in groups], dtype=np.int64)))

@@ -738,17 +738,17 @@ def _failover(n, full_copy):
     keep, batch = [], {}
     stride = G * pitch(-(-3000 // d)) * 8                       # every plane call of a log takes the same stride
 
-    def propose(eng, me):
+    def propose(eng, me, fc=full_copy):
         lens = [rng.choice((1, 15, 16, 17, 300, 3000)) for _ in range(G)]
-        store, got = _propose(eng, me, lens, stride, full_copy)
+        store, got = _propose(eng, me, lens, stride, fc)
         keep.append(store)
         for g, (s, b) in got.items():
             batch[(g, s)] = b
 
-    def round_trip(eng, me, live, want=None, heartbeat=False):
+    def round_trip(eng, me, live, want=None, heartbeat=False, fc=full_copy):
         """pack, deliver to the live replicas, ingest the replies, back off -> (want_end or None, frames to each replica)"""
         out = torch.zeros(1 << 22, dtype=torch.uint8, device=dev)
-        o = eng.pack_append(me, out, 1 << 12, want_end=want, heartbeat=heartbeat, full_copy=full_copy, msg_chunk_size=chunk)
+        o = eng.pack_append(me, out, 1 << 12, want_end=want, heartbeat=heartbeat, full_copy=fc, msg_chunk_size=chunk)
         torch.cuda.synchronize()
         nf = int(o["n_frames"][0])
         fo, fg, fp = o["frame_off"][:nf], o["frame_group"][:nf], o["frame_peer"][:nf]
@@ -777,28 +777,30 @@ def _failover(n, full_copy):
         torch.cuda.synchronize()
         return (want if (want != -1).any() else None), sent
 
-    def settle(eng, me, live):
-        want, _ = round_trip(eng, me, live)
+    def settle(eng, me, live, fc=full_copy):
+        want, _ = round_trip(eng, me, live, fc=fc)
         for _ in range(8):
             if want is None:
                 break
-            want, _ = round_trip(eng, me, live, want)
+            want, _ = round_trip(eng, me, live, want, fc=fc)
         assert want is None
-        round_trip(eng, me, live, heartbeat=True)
+        round_trip(eng, me, live, heartbeat=True, fc=fc)
 
     # 1. the first leader, replica 0: three terms of entries; replica 1 misses the first term's second round (it catches
-    #    up through a back-off), replica n - 1 misses the whole last term
+    #    up through a back-off), replica n - 1 misses the whole last term.  The code survives n - d lost shards: from
+    #    n = 5 up, the crashed leader's and the lagging replica's.  At n = 3 and 4 coded copies of the last term would not
+    #    survive both, so that term goes out in full copy, CRaft's fallback: the new leader holds its d data shards
     old = RaftEngine(ctx, G, n, craft=True, window=W)
     old.log_view()
-    if full_copy:
-        old.set_full_copy(True)
     lag = n - 1
     for term in (1, 2, 3):
+        fc = full_copy or (term == 3 and n - d < 2)
+        old.set_full_copy(fc)
         old.curr_term.fill_(term)
         for k in range(2):
-            propose(old, 0)
+            propose(old, 0, fc)
             live = [r for r in fols if not (term == 1 and k == 1 and r == 1) and not (term == 3 and r == lag)]
-            settle(old, 0, live)
+            settle(old, 0, live, fc)
     old.close()
     # 2. the vote rule over the survivors' logs: the highest (last term, last slot), the lowest id among equals
     views = {r: _fol_state(f) for r, f in fols.items()}
