@@ -1000,8 +1000,9 @@ int ss_prepare_reply_parse_dev(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len
  *   2. a non-empty frame whose entries are all present with matching terms appends nothing and gets the immediate reply
  *      {curr_term, prev_slot + n, None}; the reference, with first_new left at prev_slot + 1, would push every entry
  *      again at the end of its log (messages.rs:102-182).  The reply's bytes are the same; no record is written;
- *   3. role is not tracked: the host submits frames only for the groups it follows; the candidate same-term hack,
- *      heard_heartbeat and the timers stay on the host;
+ *   3. the append does not track role: the host submits frames only for the groups it follows; heard_heartbeat and the
+ *      timers stay on the host; the elections keep their role beside this state (CRaft elections, below), where a
+ *      same-term frame ends a candidacy as the candidate same-term hack does;
  *   4. the capacity cut is a suffix in frame order (below);
  *   5. absorbed entries (messages.rs:143-154) take a region after every frame's region, placed in the order the group
  *      walks reach them; one that does not fit keeps the shards it held (SS_DEV_STATUS_STORE_FULL). */
@@ -1281,8 +1282,8 @@ int ss_engine_craft_backoff(ss_engine *engine, const uint8_t *buf, uint64_t buf_
  * (subset_copy, rscoding.rs:255-293): a shard the leader does not hold goes out as None.  A log that is never stepped up
  * holds every shard of every entry and behaves as before.
  * Stated differences from the reference:
- *   1. elections (RequestVote, RequestVoteReply, become_a_candidate, voted_for), heartbeats and the `external` flag of
- *      unreplied entries (leadership.rs:236-243) stay with the host; step-down (engine -> follower) is not built;
+ *   1. heartbeats and the `external` flag of unreplied entries (leadership.rs:236-243) stay with the host; step-down
+ *      (engine -> follower) is not built; elections run on the follower (ss_follower_campaign / _vote / _tally, below);
  *   2. the packer's leader_commit is the engine's last_commit, the quorum commit point; the reference sends its executed
  *      prefix, which lags behind while reconstruct reads are outstanding;
  *   3. execution after an absorb goes up to the tick's last_commit, which keeps the current-term rule; the reference's loop
@@ -1365,6 +1366,100 @@ int ss_follower_reconstruct_serve(ss_follower *follower, const uint8_t *buf, uin
 int ss_engine_craft_absorb(ss_engine *engine, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off,
                            const uint32_t *frame_group, const uint8_t *frame_peer, uint64_t n_frames, uint32_t reply_variant,
                            uint32_t *absorbed, uint32_t *verdict);
+
+/* ---- CRaft elections on the follower ---------------------------------------------------------------------------------
+ * Choosing a new leader: a replica campaigns for the groups whose leader timed out (become_a_candidate,
+ * craft/leadership.rs:143-209), the other replicas answer its RequestVote frames (handle_msg_request_vote,
+ * craft/messages.rs:499-591) and the candidate tallies the RequestVoteReply frames (handle_msg_request_vote_reply,
+ * messages.rs:593-619) into won_group / won_term, which go straight to ss_engine_craft_step_up (n_listed = n_groups).
+ * The PeerMsg variant indices are arguments: RequestVote 2, RequestVoteReply 3 (mod.rs:239-246); each < 2^16.
+ * State, per group, allocated on the first call below or of the view: vote_term, voted_for (0xff = None), role_term,
+ * role (SS_FOLLOWER_ROLE_*) and votes (a mask by replica id).  They are read through the follower's curr_term and leader:
+ *   - voted_for counts only while vote_term == curr_term;
+ *   - a group is a candidate or elected only while role_term == curr_term and leader == me.
+ * So ss_follower_append changes none of them, yet its check_term (a higher term: voted_for None, votes cleared, role
+ * Follower) ends a vote and a candidacy, and so does a same-term AppendEntries, which sets leader to its sender (the
+ * candidate same-term hack, messages.rs:33-43).
+ * Stated differences from the reference:
+ *   1. a campaign sets leader = me, which is how the state above knows a candidacy;
+ *   2. the candidate's Metadata record is made durable before its RequestVote goes out; the reference sends first;
+ *   3. a reply is counted only when the group is a candidate at curr_term, reply.term == curr_term and granted; the
+ *      reference counts any reply past check_term, a refusal or a reply to an older campaign included;
+ *   4. election timers, heartbeats, disallow_step_up and step-down stay with the host. */
+#define SS_FOLLOWER_ROLE_FOLLOWER 0u
+#define SS_FOLLOWER_ROLE_CANDIDATE 1u
+#define SS_FOLLOWER_ROLE_ELECTED 2u
+typedef struct ss_follower_vote_view {
+    uint64_t n_groups;
+    uint64_t *vote_term;        /* [G] the term voted_for belongs to */
+    uint8_t *voted_for;         /* [G] 0xff = None */
+    uint64_t *role_term;        /* [G] the term role belongs to */
+    uint8_t *role;              /* [G] SS_FOLLOWER_ROLE_* */
+    uint32_t *votes;            /* [G] votes granted to this replica's candidacy, bit r = replica r */
+} ss_follower_vote_view;
+int ss_follower_vote_view_get(ss_follower *follower, ss_follower_vote_view *view);
+/* verdict[i] of ss_follower_campaign, checked in this order; every one but DONE leaves the group unchanged */
+#define SS_CAMPAIGN_VERDICT_DONE 0u
+#define SS_CAMPAIGN_VERDICT_IGNORED 1u        /* group >= n_groups, or listed earlier in the same call */
+#define SS_CAMPAIGN_VERDICT_NOT_FOLLOWER 2u   /* already a candidate or elected at curr_term */
+#define SS_CAMPAIGN_VERDICT_OTHER_LEADER 3u   /* leader is set and is not timeout_source[i] */
+#define SS_CAMPAIGN_VERDICT_RANGE 4u          /* curr_term + 1 >= 2^32: the engine's terms are u32 */
+/* Campaigns for the listed groups (device u32 [n_listed]); timeout_source (device u8 [n_listed], NULL = no check) is the
+ * replica whose silence started listing i.  For a DONE group: curr_term += 1, voted_for = me, votes = {me}, role
+ * candidate, leader = me; DurEntry::Metadata{curr_term, voted_for: me} in the 32-byte cell meta + 32*i (meta_len[i]
+ * bytes, the cell format of ss_follower_append); PeerMessage::Msg{RequestVote{term: curr_term, last_slot: log_end - 1,
+ * last_term: the ring's term at last_slot}} (request_vote_variant) behind its 8-byte big-endian length in the 48-byte
+ * cell frames + 48*i (frame_len[i] bytes, frame_dst[i] = 0xff: the same bytes go to every peer).  The host makes the
+ * record durable, then broadcasts the frame.  Other listings: meta_len and frame_len 0, frame_dst 0xff, cells not
+ * written.  Cells are zero past their length.  Cost: a sort of the listings and a thread per listing. */
+int ss_follower_campaign(ss_follower *follower, const uint32_t *groups, uint64_t n_listed, const uint8_t *timeout_source,
+                         uint32_t request_vote_variant, uint8_t *meta, uint32_t *meta_len, uint8_t *frames, uint32_t *frame_len,
+                         uint8_t *frame_dst, uint32_t *verdict);
+/* Verdicts of ss_follower_vote, beside the PeerMsg variant index k (another message; 0x80000000 | k for the
+ * PeerMessage variants) and SS_FRAME_KIND_MALFORMED */
+#define SS_VOTE_VERDICT_GRANTED 0xfffffff0u       /* reply {curr_term, true} */
+#define SS_VOTE_VERDICT_DENIED_STALE 0xfffffff1u  /* term < curr_term: reply {curr_term, false} */
+#define SS_VOTE_VERDICT_NO_REPLY 0xfffffff2u      /* voted for another candidate, or its log is behind: no reply */
+/* RequestVote frames, taken as ss_follower_append takes frames: frame i is PeerMessage::Msg{RequestVote{term, last_slot,
+ * last_term}} (request_vote_variant) from candidate frame_peer[i] for group frame_group[i].  Malformed: truncated,
+ * trailing bytes, a variant >= 2^16, a peer that is `me` or >= population, a group >= n_groups.
+ * Each group's frames are replayed in frame order:
+ *   check_term: term > curr_term raises curr_term, clears the vote and sets leader = the candidate;
+ *   term < curr_term: reply {curr_term, false};
+ *   otherwise the vote is granted when voted_for is None or the candidate, and last_term >= the term of this log's last
+ *     entry || (last_term == curr_term && last_slot + 1 >= log_end) -- the reference's test verbatim, which also grants
+ *     an equal last term with a shorter log; a grant sets voted_for; a vote not granted gets no reply.
+ * Outputs per frame: DurEntry::Metadata{curr_term, voted_for} as the frame left them in the 32-byte cell meta + 32*i
+ * when the frame raised the term or granted (meta_len[i], 0 = none); PeerMessage::Msg{RequestVoteReply{term, granted}}
+ * (reply_variant) in the 32-byte cell replies + 32*i (reply_len[i], 0 = none) for reply_dst[i] (0xff = none), sent once
+ * the frame's record is durable; the verdict.  Cells are zero past their length and not written when it is 0.
+ * Cost: a sort of the frames and a thread per group's run of them. */
+int ss_follower_vote(ss_follower *follower, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off,
+                     const uint32_t *frame_group, const uint8_t *frame_peer, uint64_t n_frames, uint32_t request_vote_variant,
+                     uint32_t reply_variant, uint8_t *meta, uint32_t *meta_len, uint8_t *replies, uint32_t *reply_len,
+                     uint8_t *reply_dst, uint32_t *verdict);
+/* Verdicts of ss_follower_tally, checked in this order, beside another message's variant index and
+ * SS_FRAME_KIND_MALFORMED */
+#define SS_TALLY_VERDICT_HIGHER_TERM 0xfffffff0u      /* term > curr_term: stepped down, Metadata{term, None} */
+#define SS_TALLY_VERDICT_ELECTED_ALREADY 0xfffffff1u  /* the group is elected at curr_term: ignored */
+#define SS_TALLY_VERDICT_NOT_CANDIDATE 0xfffffff2u    /* the group is not a candidate at curr_term */
+#define SS_TALLY_VERDICT_STALE_TERM 0xfffffff3u       /* a reply to an older campaign */
+#define SS_TALLY_VERDICT_DENIED 0xfffffff4u           /* granted == false */
+#define SS_TALLY_VERDICT_DUPLICATE 0xfffffff5u        /* this peer's vote is counted already */
+#define SS_TALLY_VERDICT_COUNTED 0xfffffff6u          /* counted, no majority yet */
+#define SS_TALLY_VERDICT_WON 0xfffffff7u              /* counted, and the votes reach majority: role elected */
+/* RequestVoteReply frames, taken as ss_follower_vote takes frames: frame i is PeerMessage::Msg{RequestVoteReply{term,
+ * granted}} (reply_variant; granted a 0/1 byte, anything else malformed) from frame_peer[i].  Each group's frames are
+ * replayed in frame order with the verdicts above; a HIGHER_TERM frame writes DurEntry::Metadata{term, None} into the
+ * 32-byte cell meta + 32*i (meta_len[i], 0 = none) and sets leader = frame_peer[i].
+ * won_group (device u32 [n_groups]): the groups this call elected and that are still elected at its end, in group
+ * order, then UINT32_MAX up to n_groups; won_term (device u64 [n_groups]) their curr_term, 0 past them; *n_won (device
+ * u64, may be NULL) their count.  Pass won_group / won_term to ss_engine_craft_step_up with n_listed = n_groups: it
+ * ignores the UINT32_MAX entries.  Cost: a sort of the frames, a thread per group's run of them, a scan. */
+int ss_follower_tally(ss_follower *follower, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off,
+                      const uint32_t *frame_group, const uint8_t *frame_peer, uint64_t n_frames, uint32_t reply_variant,
+                      uint8_t *meta, uint32_t *meta_len, uint32_t *verdict, uint32_t *won_group, uint64_t *won_term,
+                      uint64_t *n_won);
 
 /* ---- tuning / introspection (bench + tests) ------------------------------------------------ */
 /* Tuning knob for experiments; 0 = the defaults.

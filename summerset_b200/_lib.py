@@ -155,6 +155,10 @@ SIGNATURES = {
     "ss_engine_craft_reconstruct_reads": (_i, [_vp, _vp, _u64, _u64, _u32, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp]),
     "ss_follower_reconstruct_serve": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _u32, _vp, _u64, _vp, _vp, _vp, _vp]),
     "ss_engine_craft_absorb": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _vp, _vp]),
+    "ss_follower_vote_view_get": (_i, [_vp, _vp]),
+    "ss_follower_campaign": (_i, [_vp, _vp, _u64, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "ss_follower_vote": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "ss_follower_tally": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ss_rs_set_variant": (_i, [_vp, _i]),
     "ss_rs_last_kernel": (C.c_char_p, [_vp]),
     "ss_rs_jit_status": (C.c_char_p, [_vp]),
@@ -266,6 +270,12 @@ class FollowerExecView(C.Structure):
     _fields_ = [("n_groups", C.c_uint64), ("last_exec", C.c_void_p)]
 
 
+class FollowerVoteView(C.Structure):
+    """ss_follower_vote_view"""
+    _fields_ = [("n_groups", C.c_uint64), ("vote_term", C.c_void_p), ("voted_for", C.c_void_p), ("role_term", C.c_void_p),
+                ("role", C.c_void_p), ("votes", C.c_void_p)]
+
+
 class AppendPackSpec(C.Structure):
     """ss_append_pack_spec"""
     _fields_ = [("me", C.c_uint32), ("append_variant", C.c_uint32), ("msg_chunk_size", C.c_uint32), ("full_copy", C.c_uint32),
@@ -309,6 +319,13 @@ SS_APPEND_REPLY_END_RANGE = 0xFFFFFFF3
 # verdicts of ss_engine_craft_step_up
 SS_STEPUP_VERDICT_DONE, SS_STEPUP_VERDICT_IGNORED, SS_STEPUP_VERDICT_WINDOW, SS_STEPUP_VERDICT_RANGE, \
     SS_STEPUP_VERDICT_STALE_TERM, SS_STEPUP_VERDICT_STORE_FULL = range(6)
+# CRaft elections: follower roles, verdicts of ss_follower_campaign, ss_follower_vote and ss_follower_tally
+SS_FOLLOWER_ROLE_FOLLOWER, SS_FOLLOWER_ROLE_CANDIDATE, SS_FOLLOWER_ROLE_ELECTED = range(3)
+SS_CAMPAIGN_VERDICT_DONE, SS_CAMPAIGN_VERDICT_IGNORED, SS_CAMPAIGN_VERDICT_NOT_FOLLOWER, SS_CAMPAIGN_VERDICT_OTHER_LEADER, \
+    SS_CAMPAIGN_VERDICT_RANGE = range(5)
+SS_VOTE_VERDICT_GRANTED, SS_VOTE_VERDICT_DENIED_STALE, SS_VOTE_VERDICT_NO_REPLY = range(0xFFFFFFF0, 0xFFFFFFF3)
+SS_TALLY_VERDICT_HIGHER_TERM, SS_TALLY_VERDICT_ELECTED_ALREADY, SS_TALLY_VERDICT_NOT_CANDIDATE, SS_TALLY_VERDICT_STALE_TERM, \
+    SS_TALLY_VERDICT_DENIED, SS_TALLY_VERDICT_DUPLICATE, SS_TALLY_VERDICT_COUNTED, SS_TALLY_VERDICT_WON = range(0xFFFFFFF0, 0xFFFFFFF8)
 # pair statuses of ss_frame_append_pack_dev
 SS_APPEND_PAIR_SENT, SS_APPEND_PAIR_NOTHING, SS_APPEND_PAIR_SNAPSHOTTED, SS_APPEND_PAIR_OVERFLOW = range(4)
 

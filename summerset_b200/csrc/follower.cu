@@ -28,7 +28,8 @@
 //   fol_exec_payload_kernel  a warp per record: get_data's bytes from the held shards, a missing data shard regenerated
 //                            from the first d held ones (exec_payload.cuh)
 //
-// Serving a new leader's Reconstruct reads (ss_follower_reconstruct_serve) is in craft_recon.cu.
+// Serving a new leader's Reconstruct reads (ss_follower_reconstruct_serve) is in craft_recon.cu; campaigns, votes and
+// their tally (ss_follower_campaign / _vote / _tally) are in craft_election.cu.
 #include <cub/device/device_radix_sort.cuh>
 
 #include <cstring>
@@ -699,7 +700,8 @@ int ss_follower_destroy(ss_follower *f) {
     }
     void *bufs[] = {f->start_slot, f->log_end, f->curr_term, f->last_commit, f->last_snap, f->leader, f->term, f->shard_addr,
                     f->held, f->data_len, f->last_exec, f->matrix, f->ex_cnt, f->ex_bytes, f->ex_partials, f->ex_words, f->hdr,
-                    f->keys, f->idx, f->partials, f->sort_tmp, f->words};
+                    f->keys, f->idx, f->partials, f->sort_tmp, f->words, f->vote_term, f->role_term, f->voted_for, f->role,
+                    f->votes, f->won_flag};
     for (void *b : bufs)
         if (b) cudaFree(b);
     if (f->ctx) ctx_release(f->ctx);

@@ -1,5 +1,5 @@
-// follower_state.hpp -- the CRaft follower handle (ss_follower_*), shared by follower.cu and the reconstruct serve and
-// step-up calls (craft_recon.cu).
+// follower_state.hpp -- the CRaft follower handle (ss_follower_*), shared by follower.cu, the reconstruct serve and
+// step-up calls (craft_recon.cu) and the elections (craft_election.cu).
 #pragma once
 #include "ss_internal.hpp"
 
@@ -33,4 +33,10 @@ struct ss_follower {
     void *sort_tmp = nullptr;
     size_t sort_tmp_bytes = 0;
     uint64_t *words = nullptr;      // [4]: cut key, absorb cursor, totals when the caller passes none
+    // elections (craft_election.cu), allocated on first use: [G] each
+    uint64_t *vote_term = nullptr, *role_term = nullptr;
+    uint8_t *voted_for = nullptr, *role = nullptr;
+    uint32_t *votes = nullptr;
+    uint64_t won_cap = 0;
+    uint64_t *won_flag = nullptr;   // [won_cap + 1] the tally's per-segment flags and their scan, grow-only
 };

@@ -43,6 +43,9 @@ torch tensors (zero-copy views) so tests can read results and install state; it 
         advance(upto)                       the snapshot's start_slot move
         execute(out, rec_capacity)          the committed entries' request batches (craft/messages.rs:198-240)
         reconstruct_serve(buf, ...)         a new leader's Reconstruct reads (craft/messages.rs:621-662)
+        campaign(groups) / vote(buf, ...) / tally(buf, ...) / vote_view()   elections: become_a_candidate
+                                            (craft/leadership.rs:143-209), handle_msg_request_vote and _reply
+                                            (craft/messages.rs:499-619); tally's won_group / won_term feed step_up
     append_reply_parse(ctx, buf, frame_off, frame_group, frame_peer, curr_term, G)   the leader's side: AppendEntriesReply
                                             frames -> RaftEngine.on_append_replies records
 """
@@ -637,6 +640,8 @@ class Follower:
 
     REPLY_CELL = 48
     META_CELL = 32
+    VOTE_CELL = 48              # RequestVote frames of campaign()
+    VOTE_REPLY_CELL = 32        # RequestVoteReply frames of vote()
 
     def __init__(self, ctx: Context, n_groups: int, population: int, me: int, window: int = 0, append_variant: int = 0,
                  reply_variant: int = 1, meta_variant: int = 0, log_variant: int = 1):
@@ -716,6 +721,69 @@ class Follower:
                                                      out.numel() if out_capacity is None else out_capacity, p(res["reply_off"]),
                                                      p(res["reply_len"]), p(res["verdict"]), p(res["total"])))
         return res
+
+    # ---- elections: campaigns, RequestVote frames answered, votes tallied ----
+    def vote_view(self) -> dict:
+        """Takes the election state into use and returns zero-copy views: vote_term int64 [G], voted_for uint8 [G] (0xff =
+        None), role_term int64 [G], role uint8 [G] (SS_FOLLOWER_ROLE_*) and votes int32 [G] (bit r = replica r).  voted_for
+        counts while vote_term == curr_term, role while role_term == curr_term and leader == me."""
+        v = _lib.FollowerVoteView()
+        check(self.lib.ss_follower_vote_view_get(self.h, C.byref(v)))
+        G = self.G
+        t = lambda ptr, ts, dt: torch.as_tensor(_DevArray(ptr, (G,), ts), device=self.dev).view(dt).view((G,))
+        return dict(vote_term=t(v.vote_term, "<i8", torch.int64), voted_for=t(v.voted_for, "|u1", torch.uint8),
+                    role_term=t(v.role_term, "<i8", torch.int64), role=t(v.role, "|u1", torch.uint8),
+                    votes=t(v.votes, "<i4", torch.int32))
+
+    def campaign(self, groups: torch.Tensor, timeout_source: Optional[torch.Tensor] = None, request_vote_variant: int = 2) -> dict:
+        """become_a_candidate for the listed groups (int32 [n]; timeout_source uint8 [n] or None = no leader check).
+        Returns device tensors meta (uint8 [n, 32]) and meta_len, frames (uint8 [n, 48]: the RequestVote to broadcast) and
+        frame_len, frame_dst (uint8) and verdict (int32)."""
+        assert groups.dtype == torch.int32 and (timeout_source is None or timeout_source.dtype == torch.uint8)
+        n, dev = groups.numel(), groups.device
+        e = lambda dt: torch.empty(n, dtype=dt, device=dev)
+        out = dict(meta=torch.zeros((n, self.META_CELL), dtype=torch.uint8, device=dev), meta_len=e(torch.int32),
+                   frames=torch.zeros((n, self.VOTE_CELL), dtype=torch.uint8, device=dev), frame_len=e(torch.int32),
+                   frame_dst=e(torch.uint8), verdict=e(torch.int32))
+        p = lambda x: None if x is None else x.data_ptr()
+        check(self.lib.ss_follower_campaign(self.h, p(groups), n, p(timeout_source), request_vote_variant, p(out["meta"]),
+                                            p(out["meta_len"]), p(out["frames"]), p(out["frame_len"]), p(out["frame_dst"]),
+                                            p(out["verdict"])))
+        return out
+
+    def vote(self, buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor, frame_peer: torch.Tensor,
+             request_vote_variant: int = 2, reply_variant: int = 3) -> dict:
+        """handle_msg_request_vote over a batch of RequestVote frames (taken as append takes frames).  Returns device
+        tensors meta (uint8 [n, 32]) and meta_len, replies (uint8 [n, 32]) and reply_len, reply_dst (uint8) and verdict."""
+        assert buf.dtype == torch.uint8 and frame_off.dtype == torch.int64 and frame_group.dtype == torch.int32
+        assert frame_peer.dtype == torch.uint8
+        n, dev = frame_off.numel(), buf.device
+        e = lambda dt: torch.empty(n, dtype=dt, device=dev)
+        out = dict(meta=torch.zeros((n, self.META_CELL), dtype=torch.uint8, device=dev), meta_len=e(torch.int32),
+                   replies=torch.zeros((n, self.VOTE_REPLY_CELL), dtype=torch.uint8, device=dev), reply_len=e(torch.int32),
+                   reply_dst=e(torch.uint8), verdict=e(torch.int32))
+        p = lambda x: x.data_ptr()
+        check(self.lib.ss_follower_vote(self.h, p(buf), buf.numel(), p(frame_off), p(frame_group), p(frame_peer), n,
+                                        request_vote_variant, reply_variant, p(out["meta"]), p(out["meta_len"]), p(out["replies"]),
+                                        p(out["reply_len"]), p(out["reply_dst"]), p(out["verdict"])))
+        return out
+
+    def tally(self, buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor, frame_peer: torch.Tensor,
+              reply_variant: int = 3) -> dict:
+        """handle_msg_request_vote_reply over a batch of RequestVoteReply frames.  Returns device tensors meta (uint8
+        [n, 32]) and meta_len, verdict, and won_group (int32 [G], -1 past the elected groups), won_term (int64 [G]) and
+        n_won (int64 [1]): pass won_group / won_term to RaftEngine.step_up."""
+        assert buf.dtype == torch.uint8 and frame_off.dtype == torch.int64 and frame_group.dtype == torch.int32
+        assert frame_peer.dtype == torch.uint8
+        n, dev = frame_off.numel(), buf.device
+        out = dict(meta=torch.zeros((n, self.META_CELL), dtype=torch.uint8, device=dev), meta_len=torch.empty(n, dtype=torch.int32, device=dev),
+                   verdict=torch.empty(n, dtype=torch.int32, device=dev), won_group=torch.empty(self.G, dtype=torch.int32, device=dev),
+                   won_term=torch.empty(self.G, dtype=torch.int64, device=dev), n_won=torch.empty(1, dtype=torch.int64, device=dev))
+        p = lambda x: x.data_ptr()
+        check(self.lib.ss_follower_tally(self.h, p(buf), buf.numel(), p(frame_off), p(frame_group), p(frame_peer), n, reply_variant,
+                                         p(out["meta"]), p(out["meta_len"]), p(out["verdict"]), p(out["won_group"]),
+                                         p(out["won_term"]), p(out["n_won"])))
+        return out
 
     def close(self) -> None:
         if getattr(self, "h", None) is not None and self.h:

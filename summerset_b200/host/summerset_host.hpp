@@ -437,6 +437,33 @@ class Follower {
         check(ss_follower_reconstruct_serve(fol_, buf, buf_len, frame_off, frame_group, frame_peer, n_frames, reconstruct_variant,
                                             reply_variant, out, out_capacity, reply_off, reply_len, verdict, total));
     }
+    // elections: the state beside the follower's, allocated on first use (see ss_follower_vote_view)
+    ss_follower_vote_view vote_view() const {
+        ss_follower_vote_view v{};
+        check(ss_follower_vote_view_get(fol_, &v));
+        return v;
+    }
+    // become_a_candidate for the listed groups: Metadata cells, then RequestVote frames to broadcast (see ss_follower_campaign)
+    void become_a_candidate(const uint32_t *groups, uint64_t n_listed, const uint8_t *timeout_source, uint8_t *meta, uint32_t *meta_len,
+                            uint8_t *frames, uint32_t *frame_len, uint8_t *frame_dst, uint32_t *verdict, uint32_t request_vote_variant = 2) {
+        check(ss_follower_campaign(fol_, groups, n_listed, timeout_source, request_vote_variant, meta, meta_len, frames, frame_len, frame_dst,
+                                   verdict));
+    }
+    // RequestVote frames answered (see ss_follower_vote)
+    void handle_msg_request_vote(const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
+                                 const uint8_t *frame_peer, uint64_t n_frames, uint8_t *meta, uint32_t *meta_len, uint8_t *replies,
+                                 uint32_t *reply_len, uint8_t *reply_dst, uint32_t *verdict, uint32_t request_vote_variant = 2,
+                                 uint32_t reply_variant = 3) {
+        check(ss_follower_vote(fol_, buf, buf_len, frame_off, frame_group, frame_peer, n_frames, request_vote_variant, reply_variant, meta,
+                               meta_len, replies, reply_len, reply_dst, verdict));
+    }
+    // RequestVoteReply frames tallied; won_group / won_term ([n_groups]) go to craft_step_up (see ss_follower_tally)
+    void handle_msg_request_vote_reply(const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
+                                       const uint8_t *frame_peer, uint64_t n_frames, uint8_t *meta, uint32_t *meta_len, uint32_t *verdict,
+                                       uint32_t *won_group, uint64_t *won_term, uint64_t *n_won = nullptr, uint32_t reply_variant = 3) {
+        check(ss_follower_tally(fol_, buf, buf_len, frame_off, frame_group, frame_peer, n_frames, reply_variant, meta, meta_len, verdict,
+                                won_group, won_term, n_won));
+    }
     // the handle, for ss_engine_craft_step_up
     const ss_follower *get() const { return fol_; }
 
