@@ -1236,6 +1236,8 @@ typedef struct ss_append_pack_spec {
 #define SS_APPEND_PAIR_NOTHING 1u       /* nothing to send */
 #define SS_APPEND_PAIR_SNAPSHOTTED 2u   /* prev_slot < log_start: the reference errs ("snapshotted slot queried") */
 #define SS_APPEND_PAIR_OVERFLOW 3u      /* cut by out_capacity or max_frames: nothing written, try_next unchanged */
+#define SS_APPEND_PAIR_NOT_LEADER 4u    /* the engine does not lead the group (ss_engine_craft_role_view): nothing written,
+                                           try_next unchanged */
 /* AppendEntries frames for every (peer q, group g), after try = max(try_next, next_slot):
  *   entries (heartbeat == 0): end = want_end ? min(want_end[q*G + g], log_end - 1) : log_end - 1 (want_end device
  *     [P][G], may be NULL; UINT64_MAX: NOTHING for that pair).  try < 1 or prev_slot = try - 1 >= log_end: NOTHING;
@@ -1283,7 +1285,8 @@ int ss_engine_craft_backoff(ss_engine *engine, const uint8_t *buf, uint64_t buf_
  * holds every shard of every entry and behaves as before.
  * Stated differences from the reference:
  *   1. heartbeats and the `external` flag of unreplied entries (leadership.rs:236-243) stay with the host; step-down
- *      (engine -> follower) is not built; elections run on the follower (ss_follower_campaign / _vote / _tally, below);
+ *      (engine -> follower) is ss_engine_craft_step_down and elections run on the follower (ss_follower_campaign /
+ *      _vote / _tally), both below;
  *   2. the packer's leader_commit is the engine's last_commit, the quorum commit point; the reference sends its executed
  *      prefix, which lags behind while reconstruct reads are outstanding;
  *   3. execution after an absorb goes up to the tick's last_commit, which keeps the current-term rule; the reference's loop
@@ -1385,7 +1388,8 @@ int ss_engine_craft_absorb(ss_engine *engine, const uint8_t *buf, uint64_t buf_l
  *   2. the candidate's Metadata record is made durable before its RequestVote goes out; the reference sends first;
  *   3. a reply is counted only when the group is a candidate at curr_term, reply.term == curr_term and granted; the
  *      reference counts any reply past check_term, a refusal or a reply to an older campaign included;
- *   4. election timers, heartbeats, disallow_step_up and step-down stay with the host. */
+ *   4. election timers, heartbeats and disallow_step_up stay with the host; a leader steps down through
+ *      ss_engine_craft_step_down (below), run on each batch before these calls take it. */
 #define SS_FOLLOWER_ROLE_FOLLOWER 0u
 #define SS_FOLLOWER_ROLE_CANDIDATE 1u
 #define SS_FOLLOWER_ROLE_ELECTED 2u
@@ -1460,6 +1464,82 @@ int ss_follower_tally(ss_follower *follower, const uint8_t *buf, uint64_t buf_le
                       const uint32_t *frame_group, const uint8_t *frame_peer, uint64_t n_frames, uint32_t reply_variant,
                       uint8_t *meta, uint32_t *meta_len, uint32_t *verdict, uint32_t *won_group, uint64_t *won_term,
                       uint64_t *n_won);
+
+/* ---- CRaft step-down: check_term for the groups a replica leads (SS_PROTO_CRAFT engines) -------------------------------
+ * An engine leads the groups whose `led` byte is set.  The bytes are allocated on the first ss_engine_craft_step_down or
+ * ss_engine_craft_role_view_get, every one set (until then the engine leads every group, as before); a host whose
+ * replica leads only some groups clears the others through the view; ss_engine_craft_step_up sets it for the groups it
+ * steps up.  For a group whose byte is clear:
+ *   - ss_engine_craft_propose refuses it as it refuses a full window (shard_off, slot_out, wal_off UINT64_MAX, wal_len 0,
+ *     no WAL record) and sets SS_DEV_STATUS_NOT_LEADER;
+ *   - ss_frame_append_pack_dev gives its pairs SS_APPEND_PAIR_NOT_LEADER in entry and heartbeat mode: no frame, try_next
+ *     unchanged;
+ *   - ss_engine_craft_execute skips it (it executes on the follower now);
+ *   - ss_engine_craft_reconstruct_reads lists nothing for it and keeps its last_recon.
+ * Back-off, absorb, ingest and tick only touch the engine's own words; the raised curr_term keeps the tick's current-term
+ * rule from committing the group.  An engine that never allocates `led` runs the same kernels as before. */
+#define SS_DEV_STATUS_NOT_LEADER 128u
+typedef struct ss_engine_craft_role_view {
+    uint64_t n_groups;
+    uint8_t *led;               /* [G] 1: this engine leads the group */
+} ss_engine_craft_role_view;
+int ss_engine_craft_role_view_get(ss_engine *engine, ss_engine_craft_role_view *view);
+/* PeerMsg variant indices of the messages that carry a term (mod.rs:207-247), each < 2^16 */
+typedef struct ss_step_down_spec {
+    uint32_t append_variant;        /* AppendEntries, 0 */
+    uint32_t append_reply_variant;  /* AppendEntriesReply, 1 */
+    uint32_t request_vote_variant;  /* RequestVote, 2 */
+    uint32_t vote_reply_variant;    /* RequestVoteReply, 3 */
+} ss_step_down_spec;
+/* verdict[i] of ss_engine_craft_step_down, beside SS_FRAME_KIND_MALFORMED and 0x80000000 | k (a PeerMessage variant
+ * other than Msg), checked in this order */
+#define SS_STEPDOWN_VERDICT_PASS 0xfffffff0u        /* hand the frame to its usual handler */
+#define SS_STEPDOWN_VERDICT_RANGE 0xfffffff1u       /* a led group's term >= 2^32 (the engine's terms are u32): unchanged */
+#define SS_STEPDOWN_VERDICT_STORE_FULL 0xfffffff2u  /* cut by store_capacity: the group stays led (SS_DEV_STATUS_STORE_FULL) */
+#define SS_STEPDOWN_VERDICT_DEPOSED 0xfffffff3u     /* this frame stepped the group down */
+/* check_term (craft/leadership.rs:16-75) of the four messages that carry a term, for a batch of incoming frames, run
+ * before the batch goes to ss_follower_append, ss_follower_vote, ss_follower_tally or ss_append_reply_parse_dev.  Frames
+ * are taken as ss_follower_append takes them.  `engine` and `follower` are this replica's: same context, population,
+ * n_groups and protocol, and the follower's window >= the engine's raft_window (SS_ERR_INVALID_ARG otherwise).
+ * Each frame is decoded by the rules of the call that takes it (AppendEntries: ss_follower_append's; RequestVote and
+ * RequestVoteReply: ss_follower_vote's and _tally's; AppendEntriesReply: ss_append_reply_parse_dev's, and a frame_peer
+ * that is a peer, since it becomes the follower's leader); one that does not decode is SS_FRAME_KIND_MALFORMED and deposes
+ * nobody.  Every PeerMsg variant other than the four (CRaft's are Reconstruct and ReconstructReply) carries no term and
+ * PASSes, whatever its index: its own handler reports an unknown one.  Each group's frames are replayed in frame order: for a led group the first frame with
+ * term > the engine's curr_term (and < 2^32) deposes it (DEPOSED); its later frames, and every frame of a group that is
+ * not led, PASS, as do frames with a stale or equal term.  The host drops a DEPOSED frame, as the reference does, unless
+ * it is a RequestVote, which goes on to ss_follower_vote.
+ * A deposed group g, on the follower:
+ *   - start_slot = max(start_slot, log_start), log_end = the engine's; each slot of [start_slot, log_end) holds the
+ *     engine's term, data_len and held (every shard while the engine's held masks are not in use);
+ *   - last_commit, last_snap and last_exec become the max of the follower's and the engine's, so no executed entry runs
+ *     again;
+ *   - curr_term = max(curr_term, term); when it rises, DurEntry::Metadata{curr_term, None} goes into the 32-byte cell
+ *     meta + 32*i (meta_len[i], 0 = none; the cell format of ss_follower_append); leader = frame_peer[i];
+ * and on the engine: led = 0, curr_term = term, match = 0 for its peers; nothing else changes.
+ * Shards: an entry the follower held already -- the same slot inside its old [start_slot, log_end), the same term,
+ * data_len and held -- keeps its shard_addr (Log Matching: the same bytes).  Every other non-null entry is copied from
+ * the engine's planes into store, its held shards in rank order SS_CW_SLOT_PITCH(ceil(data_len / d)) apart,
+ * round_up(shard_len, 16) bytes each; the regions are placed by an exclusive scan over the DEPOSED frames in frame order
+ * (store_off[i]: the frame's first byte, UINT64_MAX for the other frames; *need, device, may be NULL: the bytes asked
+ * for).  The offsets are monotone, so the frames cut by store_capacity are a suffix; their groups stay led and unchanged,
+ * and every term-carrying frame of a cut group after its deposing frame is STORE_FULL too, so none reaches a handler.
+ * The same batch with a larger store finishes them (groups deposed already PASS).  Afterwards the follower references
+ * nothing in the engine's planes.  store: 16-byte aligned.
+ * Stated differences from the reference:
+ *   1. check_term runs over the whole batch before the handlers, not message by message;
+ *   2. the RANGE verdict;
+ *   3. the capacity cut;
+ *   4. the reuse rule above;
+ *   5. timers and heartbeats stay with the host, as for the elections.
+ * Cost: a thread per frame decodes, a thread per DEPOSED frame walks its group's span, and the copies take a warp per
+ * copied entry.  Device scratch, grow-only and kept by the engine: 8 * (n_groups + 3 * n_frames + min(n_frames, n_groups)
+ * * raft_window) bytes plus scan tiles (the copy list is sized for every slot of every deposed span: 512 MiB for 2^20
+ * groups at raft_window 64). */
+int ss_engine_craft_step_down(ss_engine *engine, ss_follower *follower, const ss_step_down_spec *spec, const uint8_t *buf,
+                              uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group, const uint8_t *frame_peer,
+                              uint64_t n_frames, uint8_t *store, uint64_t store_capacity, uint64_t *store_off, uint8_t *meta,
+                              uint32_t *meta_len, uint32_t *verdict, uint64_t *need);
 
 /* ---- tuning / introspection (bench + tests) ------------------------------------------------ */
 /* Tuning knob for experiments; 0 = the defaults.

@@ -156,6 +156,8 @@ SIGNATURES = {
     "ss_follower_reconstruct_serve": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _u32, _vp, _u64, _vp, _vp, _vp, _vp]),
     "ss_engine_craft_absorb": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _vp, _vp]),
     "ss_follower_vote_view_get": (_i, [_vp, _vp]),
+    "ss_engine_craft_role_view_get": (_i, [_vp, _vp]),
+    "ss_engine_craft_step_down": (_i, [_vp, _vp, _vp, _vp, _u64, _vp, _vp, _vp, _u64, _vp, _u64, _vp, _vp, _vp, _vp, _vp]),
     "ss_follower_campaign": (_i, [_vp, _vp, _u64, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ss_follower_vote": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ss_follower_tally": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
@@ -265,6 +267,17 @@ class CraftReconView(C.Structure):
                 ("last_recon", C.c_void_p)]
 
 
+class CraftRoleView(C.Structure):
+    """ss_engine_craft_role_view"""
+    _fields_ = [("n_groups", C.c_uint64), ("led", C.c_void_p)]
+
+
+class StepDownSpec(C.Structure):
+    """ss_step_down_spec"""
+    _fields_ = [("append_variant", C.c_uint32), ("append_reply_variant", C.c_uint32), ("request_vote_variant", C.c_uint32),
+                ("vote_reply_variant", C.c_uint32)]
+
+
 class FollowerExecView(C.Structure):
     """ss_follower_exec_view"""
     _fields_ = [("n_groups", C.c_uint64), ("last_exec", C.c_void_p)]
@@ -327,7 +340,10 @@ SS_VOTE_VERDICT_GRANTED, SS_VOTE_VERDICT_DENIED_STALE, SS_VOTE_VERDICT_NO_REPLY 
 SS_TALLY_VERDICT_HIGHER_TERM, SS_TALLY_VERDICT_ELECTED_ALREADY, SS_TALLY_VERDICT_NOT_CANDIDATE, SS_TALLY_VERDICT_STALE_TERM, \
     SS_TALLY_VERDICT_DENIED, SS_TALLY_VERDICT_DUPLICATE, SS_TALLY_VERDICT_COUNTED, SS_TALLY_VERDICT_WON = range(0xFFFFFFF0, 0xFFFFFFF8)
 # pair statuses of ss_frame_append_pack_dev
-SS_APPEND_PAIR_SENT, SS_APPEND_PAIR_NOTHING, SS_APPEND_PAIR_SNAPSHOTTED, SS_APPEND_PAIR_OVERFLOW = range(4)
+SS_APPEND_PAIR_SENT, SS_APPEND_PAIR_NOTHING, SS_APPEND_PAIR_SNAPSHOTTED, SS_APPEND_PAIR_OVERFLOW, SS_APPEND_PAIR_NOT_LEADER = range(5)
+# CRaft step-down: verdicts of ss_engine_craft_step_down, and the status bit of a call refused for a group not led
+SS_STEPDOWN_VERDICT_PASS, SS_STEPDOWN_VERDICT_RANGE, SS_STEPDOWN_VERDICT_STORE_FULL, SS_STEPDOWN_VERDICT_DEPOSED = range(0xFFFFFFF0, 0xFFFFFFF4)
+SS_DEV_STATUS_NOT_LEADER = 128
 
 
 class SummersetError(RuntimeError):

@@ -26,6 +26,7 @@
 
 #include <cstring>
 
+#include "craft_frames.cuh"
 #include "device_common.cuh"
 #include "engine_state.hpp"
 #include "follower_state.hpp"
@@ -35,21 +36,7 @@
 namespace ssb {
 
 constexpr int kElThreads = 256;
-constexpr uint32_t kElVariantLimit = 1u << 16;
-constexpr uint32_t kElPending = 0xfffffffeu;
-constexpr uint8_t kNone = 0xffu;                 // ReplicaId::MAX: voted_for None, leader None
-constexpr uint32_t kMetaCell = 32u, kVoteCell = 48u, kReplyCell = 32u;
-
-// DurEntry::Metadata{curr_term, voted_for} into a 32-byte cell (at most 8 + 3 + 9 + 1 bytes), zero to its end
-__device__ __forceinline__ uint32_t el_put_meta(uint8_t *cell, uint32_t variant, uint64_t term, uint8_t voted_for) {
-    uint32_t m = 8u;
-    m += wv_put(cell + m, variant);
-    m += wv_put(cell + m, term);
-    cell[m++] = voted_for;
-    cl_put_be64(cell, m - 8u);
-    for (uint32_t q = m; q < kMetaCell; ++q) cell[q] = 0u;
-    return m;
-}
+constexpr uint32_t kVoteCell = 48u, kReplyCell = 32u;
 
 // ---- campaign ------------------------------------------------------------------------------------------------------
 struct CampaignArgs {
@@ -131,68 +118,7 @@ __global__ void __launch_bounds__(kElThreads) campaign_kernel(const __grid_const
 }
 
 // ---- vote and tally ------------------------------------------------------------------------------------------------
-struct ElectArgs {
-    const uint8_t *buf;
-    uint64_t buf_len;
-    const uint64_t *frame_off;
-    const uint32_t *frame_group;
-    const uint8_t *frame_peer;
-    uint64_t n, G;
-    uint32_t W, me, population, majority, variant, reply_variant, meta_variant;
-    const uint64_t *log_end, *term;
-    uint64_t *curr_term;
-    uint8_t *leader;
-    uint64_t *vote_term, *role_term;
-    uint8_t *voted_for, *role;
-    uint32_t *votes;
-    uint32_t *key_in, *idx_in;
-    const uint32_t *key, *idx;
-    uint8_t *meta;
-    uint32_t *meta_len;
-    uint8_t *replies;               // vote only
-    uint32_t *reply_len;
-    uint8_t *reply_dst;
-    uint32_t *verdict;
-    uint64_t *won_flag;             // tally only: [n] per sorted frame, then its exclusive scan
-    const uint64_t *n_won;
-    uint32_t *won_group;
-    uint64_t *won_term;
-};
-
-// Frame i: PeerMessage::Msg{RequestVote{term, last_slot, last_term}} (kReply false) or
-// PeerMessage::Msg{RequestVoteReply{term, granted}} (kReply true: f1 = granted).  kElPending when it is one, else its
-// verdict: another message's variant index (0x80000000 | k for PeerMessage variants) or SS_FRAME_KIND_MALFORMED
-template <bool kReply>
-__device__ __forceinline__ uint32_t el_decode(const ElectArgs &A, uint64_t i, uint64_t &f0, uint64_t &f1, uint64_t &f2) {
-    const uint32_t g = A.frame_group[i];
-    const uint64_t off = A.frame_off[i];
-    const uint8_t peer = A.frame_peer[i];
-    if (g >= A.G || peer == A.me || peer >= A.population || off > A.buf_len || A.buf_len - off < 8u) return SS_FRAME_KIND_MALFORMED;
-    const uint8_t *fr = A.buf + off;
-    uint64_t len = 0;
-    for (int k = 0; k < 8; ++k) len = (len << 8) | fr[k];
-    if (len > A.buf_len - off - 8u) return SS_FRAME_KIND_MALFORMED;
-    const uint8_t *b = fr + 8;
-    uint64_t n = 0, v = 0;
-    uint32_t c;
-#define SS_GET(dst) do { if (!(c = wv_get(b + n, len - n, (dst)))) return SS_FRAME_KIND_MALFORMED; n += c; } while (0)
-    SS_GET(v);
-    if (v != 0u) return v < kElVariantLimit ? 0x80000000u | static_cast<uint32_t>(v) : SS_FRAME_KIND_MALFORMED;
-    SS_GET(v);
-    if (v != A.variant) return v < kElVariantLimit ? static_cast<uint32_t>(v) : SS_FRAME_KIND_MALFORMED;
-    SS_GET(f0);
-    if (kReply) {
-        if (n >= len || b[n] > 1u) return SS_FRAME_KIND_MALFORMED;  // bool
-        f1 = b[n++];
-        f2 = 0u;
-    } else {
-        SS_GET(f1);
-        SS_GET(f2);
-    }
-#undef SS_GET
-    return n == len ? kElPending : SS_FRAME_KIND_MALFORMED;
-}
-
+// ElectArgs and el_decode are in craft_frames.cuh, beside the other term-carrying messages' decoders
 template <bool kReply>
 __device__ __forceinline__ void el_head(const ElectArgs &A) {
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kElThreads;

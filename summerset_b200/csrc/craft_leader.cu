@@ -109,6 +109,7 @@ struct ProposeArgs {
     uint32_t *eff;
     uint64_t *rec_len;
     uint32_t *status;
+    const uint8_t *led;             // read by the kLed instances only (ss_engine_craft_role_view)
 };
 
 __device__ __forceinline__ uint32_t own_mask(uint32_t full_copy, uint32_t majority, uint32_t replica) {
@@ -120,12 +121,18 @@ __device__ __forceinline__ uint64_t wal_rec_len(uint32_t t, uint64_t dl, uint32_
     return 8u + wv_len(kLogEntryVariant) + wv_len(t) + cw_bytes(dl, d, T, nsh) + 2u;
 }
 
+// kLed: a group the engine does not lead is refused as a full window is, under SS_DEV_STATUS_NOT_LEADER
+template <bool kLed>
 __global__ void __launch_bounds__(kClThreads) craft_propose_prepare_kernel(const __grid_constant__ ProposeArgs A) {
-    bool full = false;
+    bool full = false, fenced = false;
     const uint32_t nsh = A.full_copy ? A.majority : 1u;
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kClThreads;
     for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kClThreads + threadIdx.x; g < A.G; g += stride) {
         uint32_t len = A.data_len[g];
+        if (kLed && len != 0u && A.led[g] == 0u) {
+            fenced = true;
+            len = 0u;
+        }
         // every slot of [log_start, log_end] must stay in the ring: the packer reads the terms of lagging peers' entries
         if (len != 0u && static_cast<uint64_t>(A.log_end[g]) + 1u - A.log_start[g] > A.W) {
             full = true;
@@ -138,6 +145,7 @@ __global__ void __launch_bounds__(kClThreads) craft_propose_prepare_kernel(const
         A.wal_off[g] = cl_round16(rl);
     }
     cl_warp_status(full, SS_DEV_STATUS_RAFT_WINDOW_FULL, A.status);
+    if (kLed) cl_warp_status(fenced, SS_DEV_STATUS_NOT_LEADER, A.status);
 }
 
 __global__ void __launch_bounds__(kClThreads) craft_propose_commit_kernel(const __grid_constant__ ProposeArgs A) {
@@ -223,6 +231,7 @@ struct PackArgs {
     uint32_t *pair_status;
     uint64_t *pk_frames, *pk_bytes, *pk_range, *frames_total;
     uint32_t *status;
+    const uint8_t *led;             // read by the kLed instances only (ss_engine_craft_role_view)
 };
 
 // what goes to pair p = q*G + g: SENT with entries [lo, hi] (hi = lo - 1: a heartbeat), NOTHING or SNAPSHOTTED
@@ -316,13 +325,14 @@ __device__ __forceinline__ uint64_t warp_sum(uint64_t v) {
     return v;
 }
 
-template <bool kHeld>
+// kLed: the pairs of a group the engine does not lead send nothing (SS_APPEND_PAIR_NOT_LEADER)
+template <bool kHeld, bool kLed>
 __global__ void __launch_bounds__(kClThreads) append_plan_kernel(const __grid_constant__ PackArgs A) {
     const uint32_t lane = threadIdx.x & 31u;
     const uint64_t warp = (static_cast<uint64_t>(blockIdx.x) * kClThreads + threadIdx.x) >> 5;
     const uint64_t nwarps = (static_cast<uint64_t>(gridDim.x) * kClThreads) >> 5;
     for (uint64_t p = warp; p < A.PG; p += nwarps) {
-        const PairPlan r = plan_pair(A, p);
+        const PairPlan r = kLed && A.led[p % A.G] == 0u ? PairPlan{SS_APPEND_PAIR_NOT_LEADER, 0u, 0ull, 0ull, 0ull} : plan_pair(A, p);
         const uint64_t g = p % A.G;
         const uint32_t want = kHeld ? peer_want(A, p / A.G) : 0u;
         uint64_t bytes = 0;
@@ -341,8 +351,8 @@ __global__ void __launch_bounds__(kClThreads) append_plan_kernel(const __grid_co
     }
 }
 
-// the cut, try_next, and the frame arrays of every pair written
-template <bool kHeld>
+// the cut, try_next, and the frame arrays of every pair written; a NOT_LEADER pair keeps its try_next
+template <bool kHeld, bool kLed>
 __global__ void __launch_bounds__(kClThreads) append_place_kernel(const __grid_constant__ PackArgs A) {
     const uint32_t lane = threadIdx.x & 31u;
     const uint64_t warp = (static_cast<uint64_t>(blockIdx.x) * kClThreads + threadIdx.x) >> 5;
@@ -352,7 +362,7 @@ __global__ void __launch_bounds__(kClThreads) append_place_kernel(const __grid_c
         const uint32_t st = A.pair_status[p];
         const uint32_t t = pair_try(A, p);
         if (st != SS_APPEND_PAIR_SENT) {
-            if (lane == 0u) A.try_next[p] = t;                              // try_next >= next_slot from here on
+            if (lane == 0u && !(kLed && st == SS_APPEND_PAIR_NOT_LEADER)) A.try_next[p] = t;   // try_next >= next_slot from here on
             continue;
         }
         const uint64_t base = A.pk_frames[p], off = A.pk_bytes[p];
@@ -556,6 +566,7 @@ struct CraftExecArgs {
     uint32_t *rec_len;
     uint64_t rec_cap;
     uint32_t *status;
+    const uint8_t *led;             // read by the kLed instances only: a group the engine does not lead is skipped
 };
 
 __device__ __forceinline__ uint64_t craft_exec_start(const CraftExecArgs &A, uint64_t g) {
@@ -576,21 +587,25 @@ __device__ __forceinline__ uint32_t craft_exec_next(const CraftExecArgs &A, uint
     return *dlen == 0u ? kClExecNull : kClExecRun;
 }
 
+template <bool kLed>
 __global__ void __launch_bounds__(kClThreads) craft_exec_count_kernel(const __grid_constant__ CraftExecArgs A) {
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kClThreads;
     for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kClThreads + threadIdx.x; g < A.G; g += stride) {
         uint64_t n = 0u, b = 0u;
         uint32_t dl = 0u;
-        for (uint64_t s = craft_exec_start(A, g); craft_exec_next(A, g, s, &dl) == kClExecRun; ++s, ++n) b += cl_round16(dl);
+        if (!(kLed && A.led[g] == 0u))
+            for (uint64_t s = craft_exec_start(A, g); craft_exec_next(A, g, s, &dl) == kClExecRun; ++s, ++n) b += cl_round16(dl);
         A.cnt[g] = n;
         A.bytes[g] = b;
     }
 }
 
+template <bool kLed>
 __global__ void __launch_bounds__(kClThreads) craft_exec_place_kernel(const __grid_constant__ CraftExecArgs A) {
     bool full = false, null_ent = false;
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kClThreads;
     for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kClThreads + threadIdx.x; g < A.G; g += stride) {
+        if (kLed && A.led[g] == 0u) continue;
         const uint64_t s0 = craft_exec_start(A, g);
         uint64_t ro = A.cnt[g], bo = A.bytes[g], s = s0;
         uint32_t dl = 0u, r;
@@ -668,7 +683,7 @@ static int cl_alloc(ss_ctx *ctx, T **p, size_t count, bool zero) {
 void craft_log_free(ss_engine *e) {
     void *bufs[] = {e->log_start, e->try_next, e->ent_len, e->ent_addr, e->ent_log_offset, e->cl_partials, e->cl_words, e->cl_eff,
                     e->cl_wal, e->pk_frames, e->pk_bytes, e->pk_range, e->last_exec, e->ex_cnt, e->ex_bytes, e->ex_words, e->bo_keys,
-                    e->bo_idx, e->bo_sort_tmp, e->held, e->last_recon, e->matrix, e->rc_words};
+                    e->bo_idx, e->bo_sort_tmp, e->held, e->last_recon, e->matrix, e->rc_words, e->led};
     for (void *b : bufs)
         if (b) cudaFree(b);
 }
@@ -732,7 +747,7 @@ int craft_log_init(ss_engine *e) {
         e->pk_frames = nullptr; e->pk_bytes = nullptr; e->pk_range = nullptr;
         e->last_exec = nullptr; e->ex_cnt = nullptr; e->ex_bytes = nullptr; e->ex_words = nullptr;
         e->bo_keys = nullptr; e->bo_idx = nullptr; e->bo_sort_tmp = nullptr; e->bo_cap = 0;
-        e->held = nullptr; e->last_recon = nullptr; e->matrix = nullptr; e->rc_words = nullptr; e->rc_cap = 0;
+        e->held = nullptr; e->last_recon = nullptr; e->matrix = nullptr; e->rc_words = nullptr; e->rc_cap = 0; e->led = nullptr;
         return rc;
     }
     e->log_in_use = true;
@@ -809,8 +824,10 @@ int ss_engine_craft_propose(ss_engine *e, uint32_t me, const uint8_t *arena, con
     A.eff = e->cl_eff;
     A.rec_len = e->cl_wal;
     A.status = ctx->dev_status;
+    A.led = e->led;
     const uint32_t grid = cl_grid(ctx, e->G, kClThreads);
-    craft_propose_prepare_kernel<<<grid, kClThreads, 0, ctx->stream>>>(A);
+    if (e->led != nullptr) craft_propose_prepare_kernel<true><<<grid, kClThreads, 0, ctx->stream>>>(A);
+    else craft_propose_prepare_kernel<false><<<grid, kClThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     SS_TRY(launch_exclusive_scan_u64(ctx, shard_off, e->G, e->cl_partials, need != nullptr ? need : e->cl_words + 2));
     SS_TRY(launch_exclusive_scan_u64(ctx, wal_off, e->G, e->cl_partials, e->cl_words + 1));
@@ -849,17 +866,21 @@ int ss_frame_append_pack_dev(ss_engine *e, const ss_append_pack_spec *spec, cons
     A.out = out; A.out_capacity = out_capacity; A.max_frames = max_frames; A.frame_off = frame_off; A.frame_len = frame_len;
     A.frame_group = frame_group; A.frame_peer = frame_peer; A.n_frames = n_frames; A.total = total != nullptr ? total : e->cl_words + 3;
     A.pair_status = pair_status; A.pk_frames = e->pk_frames; A.pk_bytes = e->pk_bytes; A.pk_range = e->pk_range;
-    A.frames_total = e->cl_words; A.status = ctx->dev_status;
+    A.frames_total = e->cl_words; A.status = ctx->dev_status; A.led = e->led;
     const uint32_t grid_w = cl_grid(ctx, A.PG, kClThreads / 32);
-    const bool held = e->held_partial;
-    if (held) append_plan_kernel<true><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
-    else append_plan_kernel<false><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
+    const bool held = e->held_partial, led = e->led != nullptr;
+    if (held && led) append_plan_kernel<true, true><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
+    else if (held) append_plan_kernel<true, false><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
+    else if (led) append_plan_kernel<false, true><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
+    else append_plan_kernel<false, false><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     SS_TRY(launch_exclusive_scan_u64(ctx, e->pk_frames, A.PG, e->cl_partials, e->cl_words));
     SS_TRY(launch_exclusive_scan_u64(ctx, e->pk_bytes, A.PG, e->cl_partials, A.total));
     SS_CUDA(cudaMemcpyAsync(n_frames, e->cl_words, 8, cudaMemcpyDeviceToDevice, ctx->stream));
-    if (held) append_place_kernel<true><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
-    else append_place_kernel<false><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
+    if (held && led) append_place_kernel<true, true><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
+    else if (held) append_place_kernel<true, false><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
+    else if (led) append_place_kernel<false, true><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
+    else append_place_kernel<false, false><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     const uint32_t grid_f = cl_grid(ctx, max_frames, kClThreads / 32);
     if (held) append_write_kernel<true><<<grid_f, kClThreads, 0, ctx->stream>>>(A);
@@ -921,15 +942,17 @@ int ss_engine_craft_execute(ss_engine *e, uint8_t *out, uint64_t out_capacity, u
     A.log_start = e->log_start; A.ent_addr = e->ent_addr;
     A.last_exec = e->last_exec; A.cnt = e->ex_cnt; A.bytes = e->ex_bytes; A.n_exec = e->ex_words;
     A.out = out; A.out_cap = out_capacity; A.rec_group = rec_group; A.rec_slot = rec_slot; A.rec_off = rec_off; A.rec_len = rec_len;
-    A.rec_cap = rec_capacity; A.status = ctx->dev_status;
+    A.rec_cap = rec_capacity; A.status = ctx->dev_status; A.led = e->led;
     uint64_t *tot = totals != nullptr ? totals : e->ex_words + 1;
     const uint32_t grid = cl_grid(ctx, e->G, kClThreads);
     SS_CUDA(cudaMemsetAsync(e->ex_words, 0, 8, ctx->stream));
-    craft_exec_count_kernel<<<grid, kClThreads, 0, ctx->stream>>>(A);
+    if (e->led != nullptr) craft_exec_count_kernel<true><<<grid, kClThreads, 0, ctx->stream>>>(A);
+    else craft_exec_count_kernel<false><<<grid, kClThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     SS_TRY(launch_exclusive_scan_u64(ctx, e->ex_cnt, e->G, e->cl_partials, tot));
     SS_TRY(launch_exclusive_scan_u64(ctx, e->ex_bytes, e->G, e->cl_partials, tot + 1));
-    craft_exec_place_kernel<<<grid, kClThreads, 0, ctx->stream>>>(A);
+    if (e->led != nullptr) craft_exec_place_kernel<true><<<grid, kClThreads, 0, ctx->stream>>>(A);
+    else craft_exec_place_kernel<false><<<grid, kClThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     // a warp per entry the ring can hold, up to the grid cap; warps past the executed count return at once
     const uint32_t grid_p = cl_grid(ctx, e->G * e->W, kExecWarps);

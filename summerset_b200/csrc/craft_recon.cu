@@ -26,6 +26,7 @@
 #include <cstring>
 
 #include "codeword_wire.cuh"
+#include "craft_frames.cuh"
 #include "device_common.cuh"
 #include "engine_state.hpp"
 #include "follower_state.hpp"
@@ -35,32 +36,6 @@
 namespace ssb {
 
 constexpr int kRcThreads = 256;
-constexpr uint32_t kRcVariantLimit = 1u << 16;
-constexpr uint32_t kRcPending = 0xfffffffeu;
-
-// the 8-byte length, PeerMessage::Msg and the PeerMsg variant of the frame at buf + off; kRcPending with b / len / n past
-// the element count (cnt) when it is `variant`
-__device__ __forceinline__ uint32_t rc_head(const uint8_t *buf, uint64_t buf_len, uint64_t off, uint32_t variant, const uint8_t *&b,
-                                            uint64_t &len, uint64_t &n, uint64_t &cnt) {
-    if (off > buf_len || buf_len - off < 8u) return SS_FRAME_KIND_MALFORMED;
-    const uint8_t *fr = buf + off;
-    len = 0;
-    for (int k = 0; k < 8; ++k) len = (len << 8) | fr[k];
-    if (len > buf_len - off - 8u) return SS_FRAME_KIND_MALFORMED;
-    b = fr + 8;
-    n = 0;
-    uint64_t v = 0;
-    uint32_t c;
-    if (!(c = wv_get(b + n, len - n, v))) return SS_FRAME_KIND_MALFORMED;
-    n += c;
-    if (v != 0u) return v < kRcVariantLimit ? 0x80000000u | static_cast<uint32_t>(v) : SS_FRAME_KIND_MALFORMED;
-    if (!(c = wv_get(b + n, len - n, v))) return SS_FRAME_KIND_MALFORMED;
-    n += c;
-    if (v != variant) return v < kRcVariantLimit ? static_cast<uint32_t>(v) : SS_FRAME_KIND_MALFORMED;
-    if (!(c = wv_get(b + n, len - n, cnt))) return SS_FRAME_KIND_MALFORMED;
-    n += c;
-    return kRcPending;
-}
 
 // ---- step-up -------------------------------------------------------------------------------------------------------
 struct StepUpArgs {
@@ -217,6 +192,7 @@ struct ReadsArgs {
     uint32_t *frame_len;
     uint64_t frame_cap;
     uint32_t *status;
+    const uint8_t *led;             // read by the kLed instances only: a group the engine does not lead lists nothing
 };
 
 __device__ __forceinline__ uint32_t reads_group(const ReadsArgs &A, uint64_t i) { return A.groups != nullptr ? A.groups[i] : static_cast<uint32_t>(i); }
@@ -239,12 +215,13 @@ __device__ __forceinline__ uint64_t reads_frame_len(const ReadsArgs &A, uint64_t
     return 9u + wv_len(A.variant) + wv_len(m) + ebytes;
 }
 
+template <bool kLed>
 __global__ void __launch_bounds__(kRcThreads) recon_size_kernel(const __grid_constant__ ReadsArgs A) {
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kRcThreads;
     for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kRcThreads + threadIdx.x; i < A.n; i += stride) {
         const uint32_t g = reads_group(A, i);
         uint64_t frames = 0, bytes = 0;
-        if (g < A.G) {
+        if (g < A.G && !(kLed && A.led[g] == 0u)) {
             const uint64_t lr0 = A.last_recon[g];
             uint64_t m = 0, eb = 0;
             reads_walk(A, g, lr0, [&](uint64_t s, uint32_t t) {
@@ -266,12 +243,13 @@ __global__ void __launch_bounds__(kRcThreads) recon_size_kernel(const __grid_con
     }
 }
 
+template <bool kLed>
 __global__ void __launch_bounds__(kRcThreads) recon_write_kernel(const __grid_constant__ ReadsArgs A) {
     bool full = false;
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kRcThreads;
     for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kRcThreads + threadIdx.x; i < A.n; i += stride) {
         const uint32_t g = reads_group(A, i);
-        if (g >= A.G) continue;
+        if (g >= A.G || (kLed && A.led[g] == 0u)) continue;
         const uint64_t f0 = A.cnt[i], o0 = A.bytes[i];
         const uint64_t f1 = i + 1u < A.n ? A.cnt[i + 1u] : A.totals[0], o1 = i + 1u < A.n ? A.bytes[i + 1u] : A.totals[1];
         if (f1 > A.frame_cap || o1 > A.out_cap) {                          // the ends are monotone: a suffix is cut
@@ -624,7 +602,7 @@ __global__ void __launch_bounds__(kRcThreads, 1) absorb_apply_kernel(const __gri
 }
 
 // the engine's recon scratch, grow-only: `words` u64
-static int rc_scratch(ss_engine *e, uint64_t words) {
+int rc_scratch(ss_engine *e, uint64_t words) {
     if (words <= e->rc_cap) return SS_OK;
     SS_CUDA(cudaStreamSynchronize(e->ctx->stream));
     if (e->rc_words) cudaFree(e->rc_words);
@@ -699,7 +677,8 @@ int ss_engine_craft_step_up(ss_engine *e, const ss_follower *f, const uint32_t *
     stepup_commit_kernel<<<grid, kRcThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     stepup_copy_kernel<<<cl_grid(ctx, n_listed * e->W, kRcThreads / 32), kRcThreads, 0, ctx->stream>>>(A);
-    return launched(ctx);
+    SS_TRY(launched(ctx));
+    return craft_led_mark(e, groups, verdict, n_listed);                   // a stepped-up group is led again
 }
 
 int ss_engine_craft_reconstruct_reads(ss_engine *e, const uint32_t *groups, uint64_t n_listed, uint64_t chunk_size,
@@ -729,13 +708,15 @@ int ss_engine_craft_reconstruct_reads(ss_engine *e, const uint32_t *groups, uint
     uint64_t *partials = e->rc_words + 3u * n, *tot = totals != nullptr ? totals : partials + scan_tiles(n);
     A.totals = tot;
     A.out = out; A.out_cap = out_capacity; A.frame_group = frame_group; A.frame_dst = frame_dst; A.frame_off = frame_off;
-    A.frame_len = frame_len; A.frame_cap = frame_capacity; A.status = ctx->dev_status;
+    A.frame_len = frame_len; A.frame_cap = frame_capacity; A.status = ctx->dev_status; A.led = e->led;
     const uint32_t grid = cl_grid(ctx, n, kRcThreads);
-    recon_size_kernel<<<grid, kRcThreads, 0, ctx->stream>>>(A);
+    if (e->led != nullptr) recon_size_kernel<true><<<grid, kRcThreads, 0, ctx->stream>>>(A);
+    else recon_size_kernel<false><<<grid, kRcThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     SS_TRY(launch_exclusive_scan_u64(ctx, A.cnt, n, partials, tot));
     SS_TRY(launch_exclusive_scan_u64(ctx, A.bytes, n, partials, tot + 1));
-    recon_write_kernel<<<grid, kRcThreads, 0, ctx->stream>>>(A);
+    if (e->led != nullptr) recon_write_kernel<true><<<grid, kRcThreads, 0, ctx->stream>>>(A);
+    else recon_write_kernel<false><<<grid, kRcThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
 }
 

@@ -50,6 +50,9 @@ struct ss_engine {
     uint8_t *matrix = nullptr;              // [T*d] the coder's coding matrix: execute regenerates missing data shards
     bool held_partial = false;              // a held mask may lack shards (step-up ran, or the recon view was handed out);
                                             // until then propose, pack and execute neither write nor read held
+    uint8_t *led = nullptr;                 // [G] 1: the engine leads the group (craft_stepdown.cu), allocated on the first
+                                            // step-down or role view; until then every group is led and the log calls run
+                                            // their kLed = false kernels
     uint64_t *rc_words = nullptr;           // [n] recon scratch (listed groups / frames), grow-only with rc_cap
     uint64_t rc_cap = 0;
     uint64_t *ex_cnt = nullptr, *ex_bytes = nullptr;   // [G] execute scratch: records and payload bytes, then their scans
@@ -68,10 +71,16 @@ int craft_check(ss_engine *e);
 int craft_log_init(ss_engine *e);
 // held is kept from here on: every mask starts full (only propose made entries so far), and propose writes it (craft_leader.cu)
 int craft_held_in_use(ss_engine *e);
+// the led bytes, allocated on first use with every group led (craft_stepdown.cu)
+int craft_led_in_use(ss_engine *e);
+// led = 1 for the groups of the listings step-up took (verdict DONE), once the bytes exist (craft_stepdown.cu)
+int craft_led_mark(ss_engine *e, const uint32_t *groups, const uint32_t *verdict, uint64_t n);
 // bits of a radix-sort key up to v, and the log's grow-only sort scratch (bo_*) for n keys of that many bits, shared by
 // the back-off and absorb (craft_leader.cu)
 int key_bits(uint64_t v);
 int backoff_scratch(ss_engine *e, uint64_t n, int bits);
+// the recon / step-down scratch (rc_words), grow-only: `words` u64 (craft_recon.cu)
+int rc_scratch(ss_engine *e, uint64_t words);
 
 // the log calls' grid: enough CTAs of per_cta items, capped at 64 per SM
 inline uint32_t cl_grid(ss_ctx *ctx, uint64_t items, uint32_t per_cta) {

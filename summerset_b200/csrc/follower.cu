@@ -36,6 +36,7 @@
 #include <new>
 
 #include "codeword_wire.cuh"
+#include "craft_frames.cuh"
 #include "device_common.cuh"
 #include "exec_payload.cuh"
 #include "follower_state.hpp"
@@ -45,143 +46,8 @@
 
 namespace ssb {
 
-// one decoded AppendEntries frame
-struct FolHdr {
-    uint64_t term, prev, prev_term, n_ent, commit, snap;
-    uint64_t store_sz, wal_sz;      // the regions the frame reserves
-    uint32_t ents_at;               // offset of entry 0 inside the frame
-    uint32_t kind;                  // verdict so far
-    uint64_t first_k;               // replay: index of the first appended entry (n_ent: none appended)
-};
-
-// one LogEntry inside a frame; offsets count from the frame's start
-struct Ent {
-    uint64_t term, dl, sl;
-    uint32_t held, tags_at, start, ext_end, next;
-};
-
-}  // namespace ssb
-
-namespace ssb {
-
 constexpr int kFolThreads = 256;
-constexpr uint32_t kFolPending = 0xfffffffeu;
-constexpr uint32_t kFolVariantLimit = 1u << 16;
-constexpr uint64_t kFolMaxBody = 0xffffffffull - 64u;
 constexpr uint64_t kTag = 1ull << 63;          // shard_addr of an entry appended by this call: its frame and shard tags
-
-struct FolArgs {
-    const uint8_t *buf;
-    uint64_t buf_len;
-    const uint64_t *frame_off;
-    const uint32_t *frame_group;
-    const uint8_t *frame_peer;
-    uint64_t n, G;
-    uint32_t d, T, W, me, population, append_variant, reply_variant, meta_variant, log_variant;
-    uint64_t *start_slot, *log_end, *curr_term, *last_commit, *last_snap;
-    uint8_t *leader;
-    uint64_t *term, *shard_addr;
-    uint32_t *held, *data_len;
-    FolHdr *hdr;
-    uint32_t *key_in, *idx_in;
-    const uint32_t *key, *idx;
-    uint64_t *cut, *abs_cursor, *tot;
-    uint8_t *store;
-    uint64_t store_cap, *store_off;
-    uint8_t *wal;
-    uint64_t wal_cap, *wal_off, *wal_len;
-    uint8_t *meta;
-    uint32_t *meta_len;
-    uint8_t *replies;
-    uint32_t *reply_len;
-    uint8_t *reply_dst;
-    uint64_t *trunc_slot;
-    uint32_t *verdict, *status;
-};
-
-__device__ __forceinline__ uint64_t fol_round16(uint64_t x) { return (x + 15u) & ~15ull; }
-
-// entry at frame offset `at` of a frame whose body is fr[8 .. end): term, the codeword, external (a raw bool byte),
-// log_offset
-__device__ __forceinline__ bool ent_parse(const uint8_t *fr, uint64_t end, uint64_t at, uint32_t d, uint32_t T, Ent &e) {
-    const uint8_t *b = fr + 8;
-    const uint64_t len = end - 8u;
-    uint64_t n = at - 8u, v = 0, term = 0, dl = 0, sl = 0;
-    uint32_t c, tags_at = 0, held = 0;
-    if (!(c = wv_get(b + n, len - n, term))) return false;
-    n += c;
-    if (!cw_parse(b, len, n, d, T, dl, sl, tags_at, held, v)) return false;
-    if (n >= len || b[n] > 1u) return false;                                // external: bool
-    const uint32_t ext_end = static_cast<uint32_t>(8u + n + 1u);
-    ++n;
-    if (!(c = wv_get(b + n, len - n, v))) return false;                     // log_offset, dropped
-    n += c;
-    e.term = term; e.dl = dl; e.sl = sl; e.held = held; e.tags_at = tags_at;
-    e.start = static_cast<uint32_t>(at); e.ext_end = ext_end; e.next = static_cast<uint32_t>(8u + n);
-    return true;
-}
-
-__device__ __forceinline__ uint64_t ent_store_bytes(const Ent &e) {
-    return static_cast<uint64_t>(__popc(e.held)) * SS_CW_SLOT_PITCH(e.sl);
-}
-__device__ __forceinline__ uint64_t ent_rec_len(const Ent &e, uint32_t log_variant) {
-    return 8u + static_cast<uint64_t>(wv_len(log_variant)) + (e.ext_end - e.start) + 1u;
-}
-
-// decodes frame i: PeerMessage::Msg{AppendEntries{term, prev_slot, prev_term, entries, leader_commit, last_snap}}
-__device__ __forceinline__ FolHdr fol_decode(const FolArgs &A, uint64_t i) {
-    FolHdr h{};
-    h.kind = SS_FRAME_KIND_MALFORMED;
-    const uint32_t grp = A.frame_group[i];
-    const uint64_t off = A.frame_off[i];
-    if (grp >= A.G || A.frame_peer[i] == A.me || A.frame_peer[i] >= A.population || off > A.buf_len || A.buf_len - off < 8u) return h;
-    const uint8_t *fr = A.buf + off;
-    uint64_t len = 0;
-    for (int b = 0; b < 8; ++b) len = (len << 8) | fr[b];
-    if (len > A.buf_len - off - 8u || len > kFolMaxBody) return h;
-    const uint8_t *b = fr + 8;
-    uint64_t n = 0, v = 0;
-    uint32_t c;
-#define SS_GET(dst) do { if (!(c = wv_get(b + n, len - n, (dst)))) return h; n += c; } while (0)
-    SS_GET(v);
-    if (v != 0u) {                                                          // LeaseMsg / Leave / LeaveReply
-        if (v < kFolVariantLimit) h.kind = 0x80000000u | static_cast<uint32_t>(v);
-        return h;
-    }
-    SS_GET(v);
-    if (v != A.append_variant) {                                            // another PeerMsg: the host's business
-        if (v < kFolVariantLimit) h.kind = static_cast<uint32_t>(v);
-        return h;
-    }
-    uint64_t term = 0, prev = 0, prev_term = 0, n_ent = 0;
-    SS_GET(term);
-    SS_GET(prev);
-    SS_GET(prev_term);
-    SS_GET(n_ent);
-    const uint64_t ents_at = 8u + n;
-    uint64_t sz = 0, wz = 0;
-    for (uint64_t k = 0; k < n_ent; ++k) {
-        Ent e;
-        if (!ent_parse(fr, 8u + len, 8u + n, A.d, A.T, e)) return h;
-        sz += ent_store_bytes(e);
-        wz += fol_round16(ent_rec_len(e, A.log_variant));
-        n = e.next - 8u;
-    }
-    uint64_t commit = 0, snap = 0;
-    SS_GET(commit);
-    SS_GET(snap);
-#undef SS_GET
-    if (n != len) return h;
-    h.term = term; h.prev = prev; h.prev_term = prev_term; h.n_ent = n_ent; h.commit = commit; h.snap = snap;
-    h.store_sz = sz; h.wal_sz = wz;
-    h.ents_at = static_cast<uint32_t>(ents_at);
-    h.first_k = n_ent;
-    // every entry inside [start_slot, start_slot + window): the ring holds them
-    const uint64_t start = A.start_slot[grp];
-    const bool beyond = n_ent != 0u && (prev + n_ent < prev || prev + n_ent >= start + A.W);
-    h.kind = beyond ? SS_FOLLOWER_VERDICT_BEYOND_WINDOW : kFolPending;
-    return h;
-}
 
 __global__ void __launch_bounds__(kFolThreads) follower_header_kernel(const __grid_constant__ FolArgs A) {
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kFolThreads;
@@ -582,46 +448,10 @@ struct ReplyParseArgs {
 __global__ void __launch_bounds__(kFolThreads) append_reply_parse_kernel(const __grid_constant__ ReplyParseArgs A) {
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kFolThreads;
     for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kFolThreads + threadIdx.x; i < A.n; i += stride) {
-        uint32_t kind = SS_FRAME_KIND_MALFORMED;
         uint64_t term = 0, end = 0, c_term = 0, c_slot = 0;
         const uint32_t grp = A.frame_group[i];
         const uint64_t off = A.frame_off[i];
-        do {
-            if (grp >= A.G || off > A.buf_len || A.buf_len - off < 8u) break;
-            const uint8_t *fr = A.buf + off;
-            uint64_t len = 0;
-            for (int b = 0; b < 8; ++b) len = (len << 8) | fr[b];
-            if (len > A.buf_len - off - 8u) break;
-            const uint8_t *b = fr + 8;
-            uint64_t n = 0, v = 0;
-            uint32_t c;
-            if (!(c = wv_get(b + n, len - n, v))) break;
-            n += c;
-            if (v != 0u) { if (v < kFolVariantLimit) kind = 0x80000000u | static_cast<uint32_t>(v); break; }
-            if (!(c = wv_get(b + n, len - n, v))) break;
-            n += c;
-            if (v != A.reply_variant) { if (v < kFolVariantLimit) kind = static_cast<uint32_t>(v); break; }
-            if (!(c = wv_get(b + n, len - n, term))) break;
-            n += c;
-            if (!(c = wv_get(b + n, len - n, end))) break;
-            n += c;
-            if (n >= len) break;
-            const uint8_t tag = b[n++];
-            if (tag == 1u) {
-                if (!(c = wv_get(b + n, len - n, c_term))) break;
-                n += c;
-                if (!(c = wv_get(b + n, len - n, c_slot))) break;
-                n += c;
-            } else if (tag != 0u) {
-                break;
-            }
-            if (n != len) break;
-            // check_term first (messages.rs:272-274): a higher term makes the leader step down and drop the reply
-            kind = term > A.curr_term[grp] ? SS_APPEND_REPLY_HIGHER_TERM
-                 : tag == 1u               ? SS_APPEND_REPLY_CONFLICT
-                 : end > 0xffffffffull     ? SS_APPEND_REPLY_END_RANGE
-                                           : SS_APPEND_REPLY_INGEST;
-        } while (false);
+        const uint32_t kind = reply_parse(A.buf, A.buf_len, off, grp, A.G, A.reply_variant, A.curr_term, term, end, c_term, c_slot);
         if (kind < SS_APPEND_REPLY_INGEST || kind > SS_APPEND_REPLY_END_RANGE) term = end = c_term = c_slot = 0u;   // not decoded
         const bool ok = kind == SS_APPEND_REPLY_INGEST;
         A.rec_group[i] = ok ? grp : 0xffffffffu;

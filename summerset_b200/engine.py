@@ -356,6 +356,36 @@ class RaftEngine(_EngineBase):
                                                p(out["need"]), p(out["verdict"])))
         return out
 
+    # ---- step-down: check_term for the groups this engine leads ----
+    def role_view(self) -> dict:
+        """Takes the log into use and returns a zero-copy view: led uint8 [G] (1: this engine leads the group; every byte set
+        on first use).  Clearing a byte fences the group from propose, pack, execute and reconstruct_reads."""
+        v = _lib.CraftRoleView()
+        check(self.lib.ss_engine_craft_role_view_get(self.h, C.byref(v)))
+        return dict(led=self._tensor(v.led, (self.G,), "|u1", torch.uint8))
+
+    def step_down(self, follower: "Follower", buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor,
+                  frame_peer: torch.Tensor, store: torch.Tensor, store_capacity: Optional[int] = None, append_variant: int = 0,
+                  append_reply_variant: int = 1, request_vote_variant: int = 2, vote_reply_variant: int = 3) -> dict:
+        """check_term over a batch of incoming frames (taken as Follower.append takes frames) before their handlers run:
+        the first higher-term frame of a led group deposes it, and the engine's log goes back to this replica's follower,
+        the entries it lacks copied into store (uint8, 16-byte aligned, alive while the entries are).  Returns device
+        tensors store_off (int64 [n], -1 = no region), meta (uint8 [n, 32]) and meta_len, verdict (int32 [n]) and need
+        (int64 [1])."""
+        assert buf.dtype == torch.uint8 and frame_off.dtype == torch.int64 and frame_group.dtype == torch.int32
+        assert frame_peer.dtype == torch.uint8 and store.dtype == torch.uint8
+        n, dev = frame_off.numel(), buf.device
+        out = dict(store_off=torch.empty(n, dtype=torch.int64, device=dev), meta=torch.zeros((n, 32), dtype=torch.uint8, device=dev),
+                   meta_len=torch.empty(n, dtype=torch.int32, device=dev), verdict=torch.empty(n, dtype=torch.int32, device=dev),
+                   need=torch.empty(1, dtype=torch.int64, device=dev))
+        spec = _lib.StepDownSpec(append_variant, append_reply_variant, request_vote_variant, vote_reply_variant)
+        p = lambda x: x.data_ptr()
+        check(self.lib.ss_engine_craft_step_down(self.h, follower.h, C.byref(spec), p(buf), buf.numel(), p(frame_off), p(frame_group),
+                                                 p(frame_peer), n, p(store), store.numel() if store_capacity is None else store_capacity,
+                                                 p(out["store_off"]), p(out["meta"]), p(out["meta_len"]), p(out["verdict"]),
+                                                 p(out["need"])))
+        return out
+
     def reconstruct_reads(self, out: torch.Tensor, frame_capacity: int, chunk_size: int, groups: Optional[torch.Tensor] = None,
                           out_capacity: Optional[int] = None, reconstruct_variant: int = 4) -> dict:
         """Reconstruct{slots: Vec<(slot, term)>} frames for the committed entries past last_recon holding fewer than d

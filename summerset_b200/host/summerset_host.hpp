@@ -525,6 +525,19 @@ inline void craft_step_up(ss_engine *e, const Follower &follower, const uint32_t
                           uint8_t *shards, uint64_t plane_stride, uint64_t *shard_off, uint32_t *verdict, uint64_t *need = nullptr) {
     check(ss_engine_craft_step_up(e, follower.get(), groups, n_listed, term, shards, plane_stride, shard_off, need, verdict));
 }
+// step-down: the led bytes, and check_term over a batch of incoming frames (ss_engine_craft_step_down)
+inline ss_engine_craft_role_view craft_role_view(ss_engine *e) {
+    ss_engine_craft_role_view v{};
+    check(ss_engine_craft_role_view_get(e, &v));
+    return v;
+}
+inline void craft_step_down(ss_engine *e, Follower &follower, const ss_step_down_spec &spec, const uint8_t *buf, uint64_t buf_len,
+                            const uint64_t *frame_off, const uint32_t *frame_group, const uint8_t *frame_peer, uint64_t n_frames,
+                            uint8_t *store, uint64_t store_capacity, uint64_t *store_off, uint8_t *meta, uint32_t *meta_len,
+                            uint32_t *verdict, uint64_t *need = nullptr) {
+    check(ss_engine_craft_step_down(e, const_cast<ss_follower *>(follower.get()), &spec, buf, buf_len, frame_off, frame_group, frame_peer, n_frames, store,
+                                    store_capacity, store_off, meta, meta_len, verdict, need));
+}
 inline void craft_reconstruct_reads(ss_engine *e, const uint32_t *groups, uint64_t n_listed, uint64_t chunk_size, uint8_t *out,
                                     uint64_t out_capacity, uint32_t *frame_group, uint8_t *frame_dst, uint64_t *frame_off,
                                     uint32_t *frame_len, uint64_t frame_capacity, uint64_t *totals = nullptr,
