@@ -25,12 +25,10 @@
 //   heartbeat_keys_kernel    a thread per record: sort keys (the records are then stably sorted by group as above)
 //   heartbeat_walk_kernel    a thread per group segment: check_leader, the ballot / exec_bar filters and the commit walk
 //                            of every record of the group in record order
-//   exec_count_kernel        a thread per group: how many instances the walk executes, and their payload bytes
-//   (engine.cu's scan)       record indices and payload regions
-//   exec_place_kernel        a thread per group: capacities, the records, commit_bar
-//   exec_payload_kernel      a warp per executed instance: get_data's bytes, with reconstruct_data's regeneration of
-//                            missing data shards from the first d held shards (Gauss-Jordan on the device, then packed
-//                            GF(2^8) Horner rows on the byte stream)
+//   (exec_walk.cuh, AccLog)  a thread per group: how many instances the walk executes, their payload bytes, then the
+//                            records and commit_bar; a warp per executed instance: get_data's bytes, with
+//                            reconstruct_data's regeneration of missing data shards from the first d held shards
+//                            (Gauss-Jordan on the device, then packed GF(2^8) Horner rows on the byte stream)
 //
 // Reconstruct reads, for the instances the follower cannot execute from its own shards: handle_msg_reconstruct
 // (rspaxos/messages.rs:468-516, crossword/messages.rs:577-632) and handle_msg_reconstruct_reply
@@ -81,7 +79,7 @@
 
 #include "codeword_wire.cuh"
 #include "device_common.cuh"
-#include "exec_payload.cuh"
+#include "exec_walk.cuh"
 #include "gf256.hpp"
 #include "ss_internal.hpp"
 #include "gossip_walk.cuh"
@@ -158,7 +156,7 @@ struct ss_acceptor {
 namespace ssb {
 
 constexpr int kAccThreads = 256;
-static_assert(kAccThreads == kExecThreads, "exec_payload_kernel runs kExecThreads-thread CTAs");
+static_assert(kAccThreads == kExecThreads, "the warp kernels run kExecWarps warps per kAccThreads-thread CTA");
 constexpr uint32_t kPending = 0xfffffffeu;          // in the window, ballot not yet checked
 constexpr uint32_t kVariantLimit = 1u << 16;        // no enum of the protocol has this many variants: malformed
 constexpr uint64_t kMaxFrameBody = 0xffffffffull - 64u;   // longer frames are malformed: every record length fits a u32
@@ -203,7 +201,6 @@ __device__ __forceinline__ uint64_t store_bytes(const FrameHdr &h) {
 __device__ __forceinline__ uint64_t wal_bytes(const FrameHdr &h, uint32_t wal_variant) {
     return 8u + static_cast<uint64_t>(wv_len(wal_variant)) + (h.end - h.slot_at);
 }
-__device__ __forceinline__ uint64_t round16(uint64_t x) { return (x + 15u) & ~15ull; }
 
 // decodes frame i as ssor_decode_accept reads it, plus the acceptor's own checks (code, shard_len, assignment shape)
 __device__ __forceinline__ FrameHdr decode_frame(const AccArgs &A, uint64_t i) {
@@ -516,98 +513,37 @@ __global__ void __launch_bounds__(kAccThreads) heartbeat_walk_kernel(const __gri
 }
 
 // ---- execute -----------------------------------------------------------------------------------------------------
-struct ExecArgs {
-    uint64_t G;
-    uint32_t d, T;
+// handle_logged_commit_slot's walk (exec_walk.cuh) over the 64-slot window, from max(commit_bar, window_base): stop past
+// the window, at an instance not committed, or at fewer than d shards (postponed); stop at a null codeword, which
+// get_data and reconstruct_data both refuse (rscoding.rs:495-497, 581-583).  A held shard of rank k is at shard_addr +
+// k * pitch, the store slots.
+struct AccLog {
+    uint32_t d;
     const uint64_t *window_base, *committed, *shard_addr;
     const uint32_t *held, *data_len;
-    const uint8_t *matrix;          // [T*d]
     uint64_t *commit_bar;
-    uint64_t *cnt, *bytes;          // [G] per group: records, payload bytes; then their exclusive scans
-    uint64_t *n_exec;               // records written (they are a prefix: the offsets are monotone)
-    uint8_t *out;
-    uint64_t out_cap;
-    uint32_t *rec_group;
-    uint64_t *rec_slot, *rec_off;
-    uint32_t *rec_len;
-    uint64_t rec_cap;
-    uint32_t *status;
+
+    struct Walk { uint64_t s, base, com; };
+    static constexpr bool kTables = true, kByIndex = false;
+
+    __device__ __forceinline__ bool live(uint64_t) const { return true; }
+    __device__ __forceinline__ Walk start(uint64_t g) const {
+        const uint64_t base = window_base[g], com = committed[g], cb = commit_bar[g];
+        return {cb > base ? cb : base, base, com};
+    }
+    __device__ __forceinline__ uint32_t next(const Walk &w, uint64_t g, uint64_t s, uint32_t *dlen) const {
+        if (s - w.base >= 64u || !((w.com >> (s & 63u)) & 1u)) return kExecStop;
+        const uint64_t at = g * 64u + (s & 63u);
+        if (static_cast<uint32_t>(__popc(held[at])) < d) return kExecStop;
+        *dlen = data_len[at];
+        return *dlen == 0u ? kExecNull : kExecRun;
+    }
+    __device__ __forceinline__ void finish(uint64_t g, uint64_t s) const { commit_bar[g] = s; }
+    __device__ __forceinline__ ExecSrc source(uint64_t g, uint64_t s, uint32_t dlen) const {
+        const uint64_t at = g * 64u + (s & 63u);
+        return {held[at], reinterpret_cast<const uint8_t *>(shard_addr[at]), SS_CW_SLOT_PITCH((dlen + d - 1u) / d)};
+    }
 };
-
-enum : uint32_t { kExecStop = 0u, kExecRun = 1u, kExecNull = 2u };
-
-// what handle_logged_commit_slot's walk does at slot s of group g: stop (past the window, not committed, or fewer than
-// d shards: postponed), run it (*dlen = its data_len), or stop at a null codeword, which get_data and reconstruct_data
-// both refuse (rscoding.rs:495-497, 581-583)
-__device__ __forceinline__ uint32_t exec_next(const ExecArgs &A, uint64_t g, uint64_t s, uint64_t base, uint64_t com, uint32_t *dlen) {
-    if (s - base >= 64u || !((com >> (s & 63u)) & 1u)) return kExecStop;
-    const uint64_t at = g * 64u + (s & 63u);
-    if (static_cast<uint32_t>(__popc(A.held[at])) < A.d) return kExecStop;
-    *dlen = A.data_len[at];
-    return *dlen == 0u ? kExecNull : kExecRun;
-}
-
-__device__ __forceinline__ uint64_t exec_start(const ExecArgs &A, uint64_t g) {
-    const uint64_t cb = A.commit_bar[g], base = A.window_base[g];
-    return cb > base ? cb : base;
-}
-
-__global__ void __launch_bounds__(kAccThreads) exec_count_kernel(const __grid_constant__ ExecArgs A) {
-    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
-    for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; g < A.G; g += stride) {
-        const uint64_t base = A.window_base[g], com = A.committed[g];
-        uint64_t n = 0u, b = 0u;
-        uint32_t dl = 0u;
-        for (uint64_t s = exec_start(A, g); exec_next(A, g, s, base, com, &dl) == kExecRun; ++s, ++n) b += round16(dl);
-        A.cnt[g] = n;
-        A.bytes[g] = b;
-    }
-}
-
-__global__ void __launch_bounds__(kAccThreads) exec_place_kernel(const __grid_constant__ ExecArgs A) {
-    bool full = false, null_cw = false;
-    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
-    for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; g < A.G; g += stride) {
-        const uint64_t base = A.window_base[g], com = A.committed[g], s0 = exec_start(A, g);
-        uint64_t ro = A.cnt[g], bo = A.bytes[g], s = s0;
-        uint32_t dl = 0u, r;
-        while ((r = exec_next(A, g, s, base, com, &dl)) == kExecRun) {
-            const uint64_t sz = round16(dl);
-            if (ro >= A.rec_cap || bo > A.out_cap || sz > A.out_cap - bo) { full = true; break; }
-            A.rec_group[ro] = static_cast<uint32_t>(g);
-            A.rec_slot[ro] = s;
-            A.rec_off[ro] = bo;
-            A.rec_len[ro] = dl;
-            ++ro;
-            bo += sz;
-            ++s;
-        }
-        null_cw |= r == kExecNull;
-        if (s != s0) {
-            A.commit_bar[g] = s;
-            atomicMax(reinterpret_cast<unsigned long long *>(A.n_exec), static_cast<unsigned long long>(ro));
-        }
-    }
-    if (full) atomicOr(A.status, SS_DEV_STATUS_EXEC_FULL);
-    if (null_cw) atomicOr(A.status, SS_DEV_STATUS_EXEC_NULL);
-}
-
-// a warp per executed instance (exec_payload.cuh): held shard of rank k at shard_addr + k*pitch, the store slots
-__global__ void __launch_bounds__(kAccThreads) exec_payload_kernel(const __grid_constant__ ExecArgs A) {
-    __shared__ ExecShared S;
-    exec_tables_init(S);
-    const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
-    const uint32_t d = A.d;
-    const uint64_t n = *A.n_exec;
-    const uint64_t nwarps = static_cast<uint64_t>(gridDim.x) * kExecWarps;
-    for (uint64_t r = static_cast<uint64_t>(blockIdx.x) * kExecWarps + w; r < n; r += nwarps) {
-        const uint64_t g = A.rec_group[r], s = A.rec_slot[r], at = g * 64u + (s & 63u);
-        const uint32_t dlen = A.rec_len[r], held = A.held[at];
-        const uint64_t pitch = SS_CW_SLOT_PITCH((dlen + d - 1u) / d);
-        warp_exec_payload(S, w, lane, d, held, dlen, A.matrix, reinterpret_cast<const uint8_t *>(A.shard_addr[at]), pitch,
-                          A.out + A.rec_off[r]);
-    }
-}
 
 // ---- reconstruct reads ---------------------------------------------------------------------------------------------
 struct RecArgs {
@@ -1669,29 +1605,6 @@ __global__ void __launch_bounds__(kAccThreads) request_write_kernel(const __grid
     if (full && lane == 0u) atomicOr(A.status, SS_DEV_STATUS_FRAME_OVERFLOW);
 }
 
-static inline uint32_t acc_grid(ss_ctx *ctx, uint64_t items, uint32_t per_cta) {
-    uint64_t ctas = (items + per_cta - 1) / per_cta;
-    const uint64_t cap = static_cast<uint64_t>(ctx->sm_count) * 8ull * 8ull;
-    if (ctas > cap) ctas = cap;
-    if (ctas == 0) ctas = 1;
-    return static_cast<uint32_t>(ctas);
-}
-
-// zeroed on the context's stream: a cudaMemset would go to the legacy default stream, which a non-blocking context
-// stream does not wait for, so it could land after the caller's first writes (window_base) or the first accept
-template <typename T>
-static int acc_alloc(ss_ctx *ctx, T **p, size_t count, bool zero = true) {
-    SS_CUDA(cudaMalloc(reinterpret_cast<void **>(p), count * sizeof(T) ? count * sizeof(T) : 1));
-    if (zero) SS_CUDA(cudaMemsetAsync(*p, 0, count * sizeof(T), ctx->stream));
-    return SS_OK;
-}
-
-static int key_bits(uint64_t G) {
-    int b = 1;
-    while (b < 32 && (G >> b) != 0u) ++b;                                    // keys run 0..G
-    return b;
-}
-
 static int ensure_scratch(ss_acceptor *a, uint64_t n) {
     if (n <= a->cap_frames) return SS_OK;
     ss_ctx *ctx = a->ctx;
@@ -1702,11 +1615,11 @@ static int ensure_scratch(ss_acceptor *a, uint64_t n) {
     a->hdr = nullptr; a->keys = nullptr; a->idx = nullptr; a->partials = nullptr; a->fcnt = nullptr; a->sort_tmp = nullptr;
     a->cap_frames = 0;
     // the header pass writes hdr, key_in and idx_in (and fcnt) of every frame, the sort the rest, the scan its partials
-    SS_TRY(acc_alloc(ctx, &a->hdr, n, false));
-    SS_TRY(acc_alloc(ctx, &a->keys, 2 * n, false));
-    SS_TRY(acc_alloc(ctx, &a->idx, 2 * n, false));
-    SS_TRY(acc_alloc(ctx, &a->partials, scan_tiles(n), false));
-    SS_TRY(acc_alloc(ctx, &a->fcnt, n, false));
+    SS_TRY(dalloc(ctx, &a->hdr, n, false));
+    SS_TRY(dalloc(ctx, &a->keys, 2 * n, false));
+    SS_TRY(dalloc(ctx, &a->idx, 2 * n, false));
+    SS_TRY(dalloc(ctx, &a->partials, scan_tiles(n), false));
+    SS_TRY(dalloc(ctx, &a->fcnt, n, false));
     size_t bytes = 0;
     SS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, a->keys, a->keys + n, a->idx, a->idx + n, static_cast<int>(n), 0,
                                             key_bits(a->G), ctx->stream));
@@ -1765,20 +1678,20 @@ int ss_acceptor_create(ss_ctx *ctx, const ss_acceptor_config *cfg, uint64_t G, s
     a->ctx = ctx; a->cfg = *cfg; a->G = G;
     ctx_retain(ctx);
     int rc = SS_OK;
-    if ((rc = acc_alloc(ctx, &a->window_base, G)) || (rc = acc_alloc(ctx, &a->bal_max_seen, G)) ||
-        (rc = acc_alloc(ctx, &a->inst_bal, G * 64)) || (rc = acc_alloc(ctx, &a->accepting, G)) ||
-        (rc = acc_alloc(ctx, &a->shard_addr, G * 64)) || (rc = acc_alloc(ctx, &a->held, G * 64)) ||
-        (rc = acc_alloc(ctx, &a->data_len, G * 64)) || (rc = acc_alloc(ctx, &a->source, G * 64)) || (rc = acc_alloc(ctx, &a->totals, 2)) ||
-        (cfg->protocol == SS_PROTO_CROSSWORD && (rc = acc_alloc(ctx, &a->assignment, G * 64))) ||
-        (cfg->protocol == SS_PROTO_CROSSWORD && (rc = acc_alloc(ctx, &a->assign_rows, G * 64 * cfg->population))) ||
-        (rc = acc_alloc(ctx, &a->gossip_bar, G)) ||
-        (rc = acc_alloc(ctx, &a->committed, G)) || (rc = acc_alloc(ctx, &a->commit_bar, G)) || (rc = acc_alloc(ctx, &a->exec_bar, G)) ||
-        (rc = acc_alloc(ctx, &a->preparing, G)) || (rc = acc_alloc(ctx, &a->voted_bal, G * 64)) ||
-        (rc = acc_alloc(ctx, &a->voted_mask, G * 64)) || (rc = acc_alloc(ctx, &a->prep_trigger, G * 64)) ||
-        (rc = acc_alloc(ctx, &a->prep_span, G * 64)) ||
-        (rc = acc_alloc(ctx, &a->ex_cnt, G, false)) || (rc = acc_alloc(ctx, &a->ex_bytes, G, false)) ||
-        (rc = acc_alloc(ctx, &a->ex_partials, scan_tiles(G), false)) || (rc = acc_alloc(ctx, &a->ex_n, 1, false)) ||
-        (rc = acc_alloc(ctx, &a->matrix, size_t(cfg->total_shards) * cfg->data_shards, false))) {
+    if ((rc = dalloc(ctx, &a->window_base, G)) || (rc = dalloc(ctx, &a->bal_max_seen, G)) ||
+        (rc = dalloc(ctx, &a->inst_bal, G * 64)) || (rc = dalloc(ctx, &a->accepting, G)) ||
+        (rc = dalloc(ctx, &a->shard_addr, G * 64)) || (rc = dalloc(ctx, &a->held, G * 64)) ||
+        (rc = dalloc(ctx, &a->data_len, G * 64)) || (rc = dalloc(ctx, &a->source, G * 64)) || (rc = dalloc(ctx, &a->totals, 2)) ||
+        (cfg->protocol == SS_PROTO_CROSSWORD && (rc = dalloc(ctx, &a->assignment, G * 64))) ||
+        (cfg->protocol == SS_PROTO_CROSSWORD && (rc = dalloc(ctx, &a->assign_rows, G * 64 * cfg->population))) ||
+        (rc = dalloc(ctx, &a->gossip_bar, G)) ||
+        (rc = dalloc(ctx, &a->committed, G)) || (rc = dalloc(ctx, &a->commit_bar, G)) || (rc = dalloc(ctx, &a->exec_bar, G)) ||
+        (rc = dalloc(ctx, &a->preparing, G)) || (rc = dalloc(ctx, &a->voted_bal, G * 64)) ||
+        (rc = dalloc(ctx, &a->voted_mask, G * 64)) || (rc = dalloc(ctx, &a->prep_trigger, G * 64)) ||
+        (rc = dalloc(ctx, &a->prep_span, G * 64)) ||
+        (rc = dalloc(ctx, &a->ex_cnt, G, false)) || (rc = dalloc(ctx, &a->ex_bytes, G, false)) ||
+        (rc = dalloc(ctx, &a->ex_partials, scan_tiles(G), false)) || (rc = dalloc(ctx, &a->ex_n, 1, false)) ||
+        (rc = dalloc(ctx, &a->matrix, size_t(cfg->total_shards) * cfg->data_shards, false))) {
         ss_acceptor_destroy(a);
         return rc;
     }
@@ -1817,7 +1730,7 @@ int ss_acceptor_heartbeat(ss_acceptor *a, const uint32_t *hb_group, const uint8_
     H.window_base = a->window_base; H.inst_bal = a->inst_bal; H.commit_bar = a->commit_bar; H.exec_bar = a->exec_bar;
     H.bal_max_seen = a->bal_max_seen; H.accepting = a->accepting; H.committed = a->committed; H.newly = newly;
     H.key_in = a->keys; H.idx_in = a->idx; H.key = a->keys + n; H.idx = a->idx + n;
-    const uint32_t grid = acc_grid(ctx, n, kAccThreads);
+    const uint32_t grid = launch_grid(ctx, n, kAccThreads);
     heartbeat_keys_kernel<<<grid, kAccThreads, 0, ctx->stream>>>(H);
     SS_TRY(launched(ctx));
     size_t bytes = a->sort_tmp_bytes;
@@ -1835,24 +1748,10 @@ int ss_acceptor_execute(ss_acceptor *a, uint8_t *out, uint64_t out_capacity, uin
     if (reinterpret_cast<uintptr_t>(out) & 15u) return set_error(SS_ERR_INVALID_ARG, "out must be 16-byte aligned");
     ss_ctx *ctx = a->ctx;
     SS_TRY(ctx_bind(ctx));
-    ExecArgs E{};
-    E.G = a->G; E.d = a->cfg.data_shards; E.T = a->cfg.total_shards;
-    E.window_base = a->window_base; E.committed = a->committed; E.shard_addr = a->shard_addr; E.held = a->held; E.data_len = a->data_len;
-    E.matrix = a->matrix; E.commit_bar = a->commit_bar; E.cnt = a->ex_cnt; E.bytes = a->ex_bytes; E.n_exec = a->ex_n;
-    E.out = out; E.out_cap = out_capacity; E.rec_group = rec_group; E.rec_slot = rec_slot; E.rec_off = rec_off; E.rec_len = rec_len;
-    E.rec_cap = rec_capacity; E.status = ctx->dev_status;
-    uint64_t *tot = totals != nullptr ? totals : a->totals;
-    const uint32_t grid = acc_grid(ctx, a->G, kAccThreads);
-    SS_CUDA(cudaMemsetAsync(a->ex_n, 0, 8, ctx->stream));
-    exec_count_kernel<<<grid, kAccThreads, 0, ctx->stream>>>(E);
-    SS_TRY(launched(ctx));
-    SS_TRY(launch_exclusive_scan_u64(ctx, a->ex_cnt, a->G, a->ex_partials, tot));
-    SS_TRY(launch_exclusive_scan_u64(ctx, a->ex_bytes, a->G, a->ex_partials, tot + 1));
-    exec_place_kernel<<<grid, kAccThreads, 0, ctx->stream>>>(E);
-    SS_TRY(launched(ctx));
-    // a warp per instance the window can hold, up to the grid cap; warps past the executed count return at once
-    exec_payload_kernel<<<acc_grid(ctx, a->G * 64u, kExecWarps), kAccThreads, 0, ctx->stream>>>(E);
-    return launched(ctx);
+    const ExecOut o{a->matrix, a->ex_cnt, a->ex_bytes, a->ex_n, out, out_capacity, rec_group, rec_slot, rec_off,
+                    rec_len, rec_capacity, ctx->dev_status};
+    const AccLog log{a->cfg.data_shards, a->window_base, a->committed, a->shard_addr, a->held, a->data_len, a->commit_bar};
+    return launch_execute(ctx, o, log, log, a->G, a->G * 64u, a->ex_partials, totals != nullptr ? totals : a->totals);
 }
 
 int ss_acceptor_view_get(ss_acceptor *a, ss_acceptor_view *v) {
@@ -1875,7 +1774,7 @@ int ss_acceptor_advance(ss_acceptor *a, const uint64_t *upto) {
     if (a == nullptr || upto == nullptr) return set_error(SS_ERR_INVALID_ARG, "null acceptor or upto");
     ss_ctx *ctx = a->ctx;
     SS_TRY(ctx_bind(ctx));
-    acceptor_advance_kernel<<<acc_grid(ctx, a->G, kAccThreads), kAccThreads, 0, ctx->stream>>>(upto, a->G, a->window_base, a->accepting,
+    acceptor_advance_kernel<<<launch_grid(ctx, a->G, kAccThreads), kAccThreads, 0, ctx->stream>>>(upto, a->G, a->window_base, a->accepting,
                                                                                                a->committed, a->preparing);
     return launched(ctx);
 }
@@ -1914,7 +1813,7 @@ int ss_acceptor_accept(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, con
     A.store = store; A.store_cap = store_capacity; A.store_off = store_off;
     A.wal = wal; A.wal_cap = wal_capacity; A.wal_off = wal_off; A.wal_len = wal_len;
     A.replies = replies; A.reply_len = reply_len; A.reply_dst = reply_dst; A.verdict = verdict; A.status = ctx->dev_status;
-    const uint32_t grid_t = acc_grid(ctx, n, kAccThreads);
+    const uint32_t grid_t = launch_grid(ctx, n, kAccThreads);
     acceptor_header_kernel<<<grid_t, kAccThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     size_t bytes = a->sort_tmp_bytes;
@@ -1927,7 +1826,7 @@ int ss_acceptor_accept(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, con
     SS_TRY(launch_exclusive_scan_u64(ctx, wal_off, n, a->partials, tot + 1));
     acceptor_place_kernel<<<grid_t, kAccThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
-    acceptor_copy_kernel<<<acc_grid(ctx, n, kAccThreads / 32), kAccThreads, 0, ctx->stream>>>(A);
+    acceptor_copy_kernel<<<launch_grid(ctx, n, kAccThreads / 32), kAccThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
 }
 
@@ -1962,7 +1861,7 @@ int ss_acceptor_reconstruct_serve(ss_acceptor *a, const uint8_t *buf, uint64_t b
     RecArgs R = rec_args(a, buf, buf_len, frame_off, frame_group, n, reconstruct_variant);
     R.reply_variant = reply_variant; R.out = out; R.out_cap = out_capacity; R.reply_off = reply_off; R.reply_len = reply_len;
     R.verdict = verdict;
-    const uint32_t grid_w = acc_grid(ctx, n, kExecWarps);
+    const uint32_t grid_w = launch_grid(ctx, n, kExecWarps);
     serve_count_kernel<<<grid_w, kAccThreads, 0, ctx->stream>>>(R);
     SS_TRY(launched(ctx));
     SS_TRY(launch_exclusive_scan_u64(ctx, reply_off, n, a->partials, total != nullptr ? total : a->totals));
@@ -1989,14 +1888,14 @@ int ss_acceptor_absorb(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, con
     R.key_in = a->keys; R.idx_in = a->idx; R.key = a->keys + n; R.idx = a->idx + n;
     R.grp_bytes = a->ex_bytes;      // execute's per-group scratch: both calls are ordered on the context's stream
     R.store = store; R.store_cap = store_capacity; R.absorbed = absorbed; R.verdict = verdict;
-    absorb_decode_kernel<<<acc_grid(ctx, n, kAccThreads), kAccThreads, 0, ctx->stream>>>(R);
+    absorb_decode_kernel<<<launch_grid(ctx, n, kAccThreads), kAccThreads, 0, ctx->stream>>>(R);
     SS_TRY(launched(ctx));
     size_t bytes = a->sort_tmp_bytes;
     SS_CUDA(cub::DeviceRadixSort::SortPairs(a->sort_tmp, bytes, a->keys, a->keys + n, a->idx, a->idx + n, static_cast<int>(n), 0,
                                             key_bits(a->G), ctx->stream));
     SS_TRY(launched(ctx));
     SS_CUDA(cudaMemsetAsync(a->ex_bytes, 0, a->G * 8, ctx->stream));
-    const uint32_t grid_w = acc_grid(ctx, n, kExecWarps);
+    const uint32_t grid_w = launch_grid(ctx, n, kExecWarps);
     absorb_plan_kernel<<<grid_w, kAccThreads, 0, ctx->stream>>>(R);
     SS_TRY(launched(ctx));
     SS_TRY(launch_exclusive_scan_u64(ctx, a->ex_bytes, a->G, a->ex_partials, total != nullptr ? total : a->totals));
@@ -2043,7 +1942,7 @@ int ss_acceptor_prepare(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, co
     P.cap = rec_capacity < wal_cells ? rec_capacity : wal_cells;
     P.wal = wal; P.rec_group = rec_group; P.rec_slot = rec_slot; P.rec_frame = rec_frame; P.verdict = verdict;
     P.status = ctx->dev_status;
-    const uint32_t grid_t = acc_grid(ctx, n, kAccThreads);
+    const uint32_t grid_t = launch_grid(ctx, n, kAccThreads);
     prepare_header_kernel<<<grid_t, kAccThreads, 0, ctx->stream>>>(P);
     SS_TRY(launched(ctx));
     size_t bytes = a->sort_tmp_bytes;
@@ -2055,7 +1954,7 @@ int ss_acceptor_prepare(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, co
     SS_TRY(launch_exclusive_scan_u64(ctx, a->fcnt, n, a->partials, P.totals));
     prepare_apply_kernel<<<grid_t, kAccThreads, 0, ctx->stream>>>(P);
     SS_TRY(launched(ctx));
-    prepare_write_kernel<<<acc_grid(ctx, n, kAccThreads / 32), kAccThreads, 0, ctx->stream>>>(P);
+    prepare_write_kernel<<<launch_grid(ctx, n, kAccThreads / 32), kAccThreads, 0, ctx->stream>>>(P);
     return launched(ctx);
 }
 
@@ -2081,10 +1980,10 @@ int ss_acceptor_prepare_reply(ss_acceptor *a, const uint32_t *rec_group, const u
     R.voted_mask = a->voted_mask; R.held = a->held; R.data_len = a->data_len; R.source = a->source; R.prep_span = a->prep_span;
     R.out = out; R.out_cap = out_capacity; R.reply_off = reply_off; R.reply_len = reply_len; R.reply_dst = reply_dst;
     R.status = ctx->dev_status;
-    prep_reply_size_kernel<<<acc_grid(ctx, n, kAccThreads), kAccThreads, 0, ctx->stream>>>(R);
+    prep_reply_size_kernel<<<launch_grid(ctx, n, kAccThreads), kAccThreads, 0, ctx->stream>>>(R);
     SS_TRY(launched(ctx));
     SS_TRY(launch_exclusive_scan_u64(ctx, reply_off, n, a->partials, total != nullptr ? total : a->totals));
-    prep_reply_copy_kernel<<<acc_grid(ctx, n, kExecWarps), kAccThreads, 0, ctx->stream>>>(R);
+    prep_reply_copy_kernel<<<launch_grid(ctx, n, kExecWarps), kAccThreads, 0, ctx->stream>>>(R);
     return launched(ctx);
 }
 
@@ -2130,7 +2029,7 @@ static int acceptor_requests(ss_acceptor *a, bool step_up, const uint32_t *group
     R.totals = tot;
     R.out = out; R.out_cap = out_capacity; R.frame_group = frame_group; R.frame_dst = frame_dst; R.frame_off = frame_off;
     R.frame_len = frame_len; R.frame_cap = frame_capacity; R.status = ctx->dev_status;
-    const uint32_t grid_w = acc_grid(ctx, n, kExecWarps);
+    const uint32_t grid_w = launch_grid(ctx, n, kExecWarps);
     request_size_kernel<<<grid_w, kAccThreads, 0, ctx->stream>>>(R);
     SS_TRY(launched(ctx));
     SS_TRY(launch_exclusive_scan_u64(ctx, R.cnt, n, a->partials, tot));

@@ -363,7 +363,7 @@ int ss_follower_campaign(ss_follower *f, const uint32_t *groups, uint64_t n_list
     A.vote_term = f->vote_term; A.role_term = f->role_term; A.voted_for = f->voted_for; A.role = f->role; A.votes = f->votes;
     A.key_in = f->keys; A.idx_in = f->idx; A.key = f->keys + n_listed; A.idx = f->idx + n_listed;
     A.meta = meta; A.meta_len = meta_len; A.frames = frames; A.frame_len = frame_len; A.frame_dst = frame_dst; A.verdict = verdict;
-    const uint32_t grid = cl_grid(ctx, n_listed, kElThreads);
+    const uint32_t grid = launch_grid(ctx, n_listed, kElThreads);
     campaign_key_kernel<<<grid, kElThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     SS_TRY(el_sort(f, n_listed));
@@ -390,7 +390,7 @@ int ss_follower_vote(ss_follower *f, const uint8_t *buf, uint64_t buf_len, const
     A.buf = buf; A.buf_len = buf_len; A.frame_off = frame_off; A.frame_group = frame_group; A.frame_peer = frame_peer;
     A.variant = request_vote_variant; A.reply_variant = reply_variant;
     A.meta = meta; A.meta_len = meta_len; A.replies = replies; A.reply_len = reply_len; A.reply_dst = reply_dst; A.verdict = verdict;
-    const uint32_t grid = cl_grid(ctx, n, kElThreads);
+    const uint32_t grid = launch_grid(ctx, n, kElThreads);
     vote_head_kernel<<<grid, kElThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     SS_TRY(el_sort(f, n));
@@ -425,7 +425,7 @@ int ss_follower_tally(ss_follower *f, const uint8_t *buf, uint64_t buf_len, cons
     A.meta = meta; A.meta_len = meta_len; A.verdict = verdict;
     uint64_t *tot = n_won != nullptr ? n_won : f->won_flag + n;
     A.won_flag = f->won_flag; A.n_won = tot; A.won_group = won_group; A.won_term = won_term;
-    const uint32_t grid = cl_grid(ctx, n, kElThreads);
+    const uint32_t grid = launch_grid(ctx, n, kElThreads);
     tally_head_kernel<<<grid, kElThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     SS_TRY(el_sort(f, n));

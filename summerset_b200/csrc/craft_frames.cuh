@@ -86,8 +86,6 @@ struct FolArgs {
     uint32_t *verdict, *status;
 };
 
-__device__ __forceinline__ uint64_t fol_round16(uint64_t x) { return (x + 15u) & ~15ull; }
-
 // entry at frame offset `at` of a frame whose body is fr[8 .. end): term, the codeword, external (a raw bool byte),
 // log_offset
 __device__ __forceinline__ bool ent_parse(const uint8_t *fr, uint64_t end, uint64_t at, uint32_t d, uint32_t T, Ent &e) {
@@ -151,7 +149,7 @@ __device__ __forceinline__ FolHdr fol_decode(const FolArgs &A, uint64_t i) {
         Ent e;
         if (!ent_parse(fr, 8u + len, 8u + n, A.d, A.T, e)) return h;
         sz += ent_store_bytes(e);
-        wz += fol_round16(ent_rec_len(e, A.log_variant));
+        wz += round16(ent_rec_len(e, A.log_variant));
         n = e.next - 8u;
     }
     uint64_t commit = 0, snap = 0;

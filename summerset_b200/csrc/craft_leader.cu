@@ -19,11 +19,10 @@
 //     (CUB radix sort)              stable: each pair's conflicts in frame order
 //     backoff_walk_kernel           a thread per pair: the walk-back over the terms ring, try_next and want_end
 //   ss_engine_craft_execute   the execution half of handle_msg_append_entries_reply's success branch (craft/messages.rs:316-359):
-//     craft_exec_count_kernel       a thread per group: the entries the walk executes, and their payload bytes
-//     (engine.cu's scan)            record indices and payload regions
-//     craft_exec_place_kernel       a thread per group: capacities, the records, last_exec
-//     craft_exec_payload_kernel     a warp per record: get_data's bytes gathered from the planes (exec_payload.cuh)
-//     craft_exec_regen_kernel       the same after a step-up, a missing data shard regenerated from the first d held ones
+//     (exec_walk.cuh, CraftLog)     a thread per group: the entries the walk executes, their payload bytes, then the
+//                                   records and last_exec
+//     (exec_walk.cuh, CraftShards)  a warp per record: get_data's bytes gathered from the planes; after a step-up, a
+//                                   missing data shard regenerated from the first d held ones
 // Step-up, reconstruct reads and absorb, which fill the held masks below, are in craft_recon.cu.
 //   ss_engine_craft_advance   the snapshot's start_slot move (craft/snapshot.rs:142,184)
 #include <cub/device/device_radix_sort.cuh>
@@ -33,7 +32,7 @@
 
 #include "device_common.cuh"
 #include "engine_state.hpp"
-#include "exec_payload.cuh"
+#include "exec_walk.cuh"
 #include "gf256.hpp"
 #include "ss_internal.hpp"
 #include "wire_common.cuh"
@@ -142,7 +141,7 @@ __global__ void __launch_bounds__(kClThreads) craft_propose_prepare_kernel(const
         A.shard_off[g] = len == 0u ? 0ull : SS_CW_SLOT_PITCH((static_cast<uint64_t>(len) + A.d - 1u) / A.d);
         const uint64_t rl = len == 0u ? 0ull : wal_rec_len(A.curr_term[g], len, A.d, A.T, nsh);
         A.rec_len[g] = rl;
-        A.wal_off[g] = cl_round16(rl);
+        A.wal_off[g] = round16(rl);
     }
     cl_warp_status(full, SS_DEV_STATUS_RAFT_WINDOW_FULL, A.status);
     if (kLed) cl_warp_status(fenced, SS_DEV_STATUS_NOT_LEADER, A.status);
@@ -156,7 +155,7 @@ __global__ void __launch_bounds__(kClThreads) craft_propose_commit_kernel(const 
         const uint64_t off = A.shard_off[g], wo = A.wal_off[g], rl = A.rec_len[g];
         const uint64_t pitch = SS_CW_SLOT_PITCH((static_cast<uint64_t>(len) + A.d - 1u) / A.d);
         const bool s_over = len != 0u && (off > A.plane_stride || pitch > A.plane_stride - off);
-        const bool w_over = len != 0u && (wo > A.wal_capacity || cl_round16(rl) > A.wal_capacity - wo);
+        const bool w_over = len != 0u && (wo > A.wal_capacity || round16(rl) > A.wal_capacity - wo);
         if (len == 0u || s_over || w_over) {
             s_full |= s_over;
             w_full |= w_over;
@@ -339,7 +338,7 @@ __global__ void __launch_bounds__(kClThreads) append_plan_kernel(const __grid_co
         for (uint64_t c = lane; c < r.nf; c += 32u) {
             uint64_t first, n;
             chunk_span(A, r.lo, r.hi, c, first, n);
-            bytes += cl_round16(frame_bytes<kHeld>(A, g, first, n, want));
+            bytes += round16(frame_bytes<kHeld>(A, g, first, n, want));
         }
         bytes = warp_sum(bytes);
         if (lane == 0u) {
@@ -389,7 +388,7 @@ __global__ void __launch_bounds__(kClThreads) append_place_kernel(const __grid_c
                 chunk_span(A, lo, hi, c, first, n);
                 len = frame_bytes<kHeld>(A, g, first, n, want);
             }
-            const uint64_t r = cl_round16(len);
+            const uint64_t r = round16(len);
             uint64_t x = r;
 #pragma unroll
             for (int o = 1; o < 32; o <<= 1) {
@@ -548,117 +547,50 @@ __global__ void __launch_bounds__(kClThreads) backoff_walk_kernel(const __grid_c
 }
 
 // ---- execution -----------------------------------------------------------------------------------------------------
-struct CraftExecArgs {
-    uint64_t G;
+// the log's ring as the execution walk (exec_walk.cuh) reads it
+struct CraftRing {
     uint32_t W, d;
     uint64_t plane_stride;
     const uint32_t *last_commit, *ent_len;
     const uint32_t *held;           // nullptr while every entry holds every shard (no step-up, no recon view)
-    const uint8_t *matrix;          // [T*d]
     const uint64_t *log_start, *ent_addr;
     uint64_t *last_exec;
-    uint64_t *cnt, *bytes;          // [G] per group: records, payload bytes; then their exclusive scans
-    uint64_t *n_exec;               // records written (a prefix: the offsets are monotone)
-    uint8_t *out;
-    uint64_t out_cap;
-    uint32_t *rec_group;
-    uint64_t *rec_slot, *rec_off;
-    uint32_t *rec_len;
-    uint64_t rec_cap;
-    uint32_t *status;
     const uint8_t *led;             // read by the kLed instances only: a group the engine does not lead is skipped
 };
 
-__device__ __forceinline__ uint64_t craft_exec_start(const CraftExecArgs &A, uint64_t g) {
-    const uint64_t s = A.last_exec[g] + 1u, ls = A.log_start[g];
-    return s > ls ? s : ls;
-}
-
-enum : uint32_t { kClExecStop = 0u, kClExecRun = 1u, kClExecNull = 2u };
-
-// what the walk does at slot s of group g: stop (past last_commit, or fewer than d shards held: an entry a step-up
-// took over that no absorb has completed yet), run it (*dlen = its data_len), or stop at a null entry, which get_data
-// refuses (rscoding.rs:581-583)
-__device__ __forceinline__ uint32_t craft_exec_next(const CraftExecArgs &A, uint64_t g, uint64_t s, uint32_t *dlen) {
-    if (s > A.last_commit[g]) return kClExecStop;
-    const uint64_t pos = g * A.W + (s & (A.W - 1u));
-    if (A.held != nullptr && static_cast<uint32_t>(__popc(A.held[pos])) < A.d) return kClExecStop;
-    *dlen = A.ent_len[pos];
-    return *dlen == 0u ? kClExecNull : kClExecRun;
-}
-
+// the walk from max(last_exec + 1, log_start): stop past last_commit, or at fewer than d shards held (an entry a step-up
+// took over that no absorb has completed yet); stop at a null entry, which get_data refuses (rscoding.rs:581-583)
 template <bool kLed>
-__global__ void __launch_bounds__(kClThreads) craft_exec_count_kernel(const __grid_constant__ CraftExecArgs A) {
-    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kClThreads;
-    for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kClThreads + threadIdx.x; g < A.G; g += stride) {
-        uint64_t n = 0u, b = 0u;
-        uint32_t dl = 0u;
-        if (!(kLed && A.led[g] == 0u))
-            for (uint64_t s = craft_exec_start(A, g); craft_exec_next(A, g, s, &dl) == kClExecRun; ++s, ++n) b += cl_round16(dl);
-        A.cnt[g] = n;
-        A.bytes[g] = b;
-    }
-}
+struct CraftLog : CraftRing {
+    struct Walk { uint64_t s; };
 
-template <bool kLed>
-__global__ void __launch_bounds__(kClThreads) craft_exec_place_kernel(const __grid_constant__ CraftExecArgs A) {
-    bool full = false, null_ent = false;
-    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kClThreads;
-    for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kClThreads + threadIdx.x; g < A.G; g += stride) {
-        if (kLed && A.led[g] == 0u) continue;
-        const uint64_t s0 = craft_exec_start(A, g);
-        uint64_t ro = A.cnt[g], bo = A.bytes[g], s = s0;
-        uint32_t dl = 0u, r;
-        while ((r = craft_exec_next(A, g, s, &dl)) == kClExecRun) {
-            const uint64_t sz = cl_round16(dl);
-            if (ro >= A.rec_cap || bo > A.out_cap || sz > A.out_cap - bo) { full = true; break; }
-            A.rec_group[ro] = static_cast<uint32_t>(g);
-            A.rec_slot[ro] = s;
-            A.rec_off[ro] = bo;
-            A.rec_len[ro] = dl;
-            ++ro;
-            bo += sz;
-            ++s;
-        }
-        null_ent |= r == kClExecNull;
-        if (s != s0) {
-            A.last_exec[g] = s - 1u;
-            atomicMax(reinterpret_cast<unsigned long long *>(A.n_exec), static_cast<unsigned long long>(ro));
-        }
+    __device__ __forceinline__ bool live(uint64_t g) const { return !(kLed && led[g] == 0u); }
+    __device__ __forceinline__ Walk start(uint64_t g) const {
+        const uint64_t s = last_exec[g] + 1u, ls = log_start[g];
+        return {s > ls ? s : ls};
     }
-    if (full) atomicOr(A.status, SS_DEV_STATUS_EXEC_FULL);
-    if (null_ent) atomicOr(A.status, SS_DEV_STATUS_EXEC_NULL);
-}
+    __device__ __forceinline__ uint32_t next(const Walk &, uint64_t g, uint64_t s, uint32_t *dlen) const {
+        if (s > last_commit[g]) return kExecStop;
+        const uint64_t pos = g * W + (s & (W - 1u));
+        if (held != nullptr && static_cast<uint32_t>(__popc(held[pos])) < d) return kExecStop;
+        *dlen = ent_len[pos];
+        return *dlen == 0u ? kExecNull : kExecRun;
+    }
+    __device__ __forceinline__ void finish(uint64_t g, uint64_t s) const { last_exec[g] = s - 1u; }
+};
 
-// a warp per record while every entry holds every shard (a log that was never stepped up): shard j at shard_addr +
-// j * plane_stride, so the gather never regenerates one and needs neither the coder's matrix nor the GF(2^8) tables
-__global__ void __launch_bounds__(kExecThreads) craft_exec_payload_kernel(const __grid_constant__ CraftExecArgs A) {
-    __shared__ ExecShared S;
-    const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
-    const uint32_t all = (1u << A.d) - 1u;
-    const uint64_t n = *A.n_exec;
-    const uint64_t nwarps = static_cast<uint64_t>(gridDim.x) * kExecWarps;
-    for (uint64_t r = static_cast<uint64_t>(blockIdx.x) * kExecWarps + w; r < n; r += nwarps) {
-        const uint64_t g = A.rec_group[r], pos = g * A.W + (A.rec_slot[r] & (A.W - 1u));
-        warp_exec_payload(S, w, lane, A.d, all, A.rec_len[r], nullptr, reinterpret_cast<const uint8_t *>(A.ent_addr[pos]), A.plane_stride,
-                          A.out + A.rec_off[r]);
-    }
-}
+// shard j at ent_addr + j * plane_stride.  kRegen = false while every entry holds every shard (a log that was never
+// stepped up): the gather never regenerates one and needs neither the coder's matrix nor the GF(2^8) tables.  kRegen
+// once a held mask may lack shards (after a step-up): a missing data shard regenerated from the first d held ones.
+template <bool kRegen>
+struct CraftShards : CraftRing {
+    static constexpr bool kTables = kRegen, kByIndex = kRegen;
 
-// the same once a held mask may lack shards (after a step-up): shard j of the held mask at shard_addr + j *
-// plane_stride, a missing data shard regenerated from the first d held ones
-__global__ void __launch_bounds__(kExecThreads) craft_exec_regen_kernel(const __grid_constant__ CraftExecArgs A) {
-    __shared__ ExecShared S;
-    exec_tables_init(S);
-    const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
-    const uint64_t n = *A.n_exec;
-    const uint64_t nwarps = static_cast<uint64_t>(gridDim.x) * kExecWarps;
-    for (uint64_t r = static_cast<uint64_t>(blockIdx.x) * kExecWarps + w; r < n; r += nwarps) {
-        const uint64_t g = A.rec_group[r], pos = g * A.W + (A.rec_slot[r] & (A.W - 1u));
-        warp_exec_payload<true>(S, w, lane, A.d, A.held[pos], A.rec_len[r], A.matrix, reinterpret_cast<const uint8_t *>(A.ent_addr[pos]),
-                                A.plane_stride, A.out + A.rec_off[r]);
+    __device__ __forceinline__ ExecSrc source(uint64_t g, uint64_t s, uint32_t) const {
+        const uint64_t pos = g * W + (s & (W - 1u));
+        return {kRegen ? held[pos] : (1u << d) - 1u, reinterpret_cast<const uint8_t *>(ent_addr[pos]), plane_stride};
     }
-}
+};
 
 // start_slot moves by clamp(upto - log_start, 0, min(last_snap, last_commit) - log_start)
 __global__ void __launch_bounds__(kClThreads)
@@ -671,13 +603,6 @@ craft_advance_kernel(const uint64_t *__restrict__ upto, uint64_t G, uint64_t *__
         const uint64_t lim = sn < lc ? sn : lc;
         if (u > s && lim > s) log_start[g] = u < lim ? u : lim;
     }
-}
-
-template <typename T>
-static int cl_alloc(ss_ctx *ctx, T **p, size_t count, bool zero) {
-    SS_CUDA(cudaMalloc(reinterpret_cast<void **>(p), count * sizeof(T) ? count * sizeof(T) : 1));
-    if (zero) SS_CUDA(cudaMemsetAsync(*p, 0, count * sizeof(T), ctx->stream));
-    return SS_OK;
 }
 
 void craft_log_free(ss_engine *e) {
@@ -715,7 +640,7 @@ int craft_held_in_use(ss_engine *e) {
     // until now every entry was proposed, so it holds every shard: the masks start full
     ss_ctx *ctx = e->ctx;
     const uint64_t n = e->G * e->W;
-    craft_held_fill_kernel<<<cl_grid(ctx, n, kClThreads), kClThreads, 0, ctx->stream>>>(e->held, n, e->n >= 32u ? 0xffffffffu : (1u << e->n) - 1u);
+    craft_held_fill_kernel<<<launch_grid(ctx, n, kClThreads), kClThreads, 0, ctx->stream>>>(e->held, n, e->n >= 32u ? 0xffffffffu : (1u << e->n) - 1u);
     SS_TRY(launched(ctx));
     e->held_partial = true;
     return SS_OK;
@@ -729,16 +654,16 @@ int craft_log_init(ss_engine *e) {
     const uint64_t G = e->G, PG = uint64_t(e->n_peers) * G, GW = G * e->W;
     if (e->coder == nullptr) SS_TRY(ss_rs_coder_create(ctx, static_cast<int>(e->majority), static_cast<int>(e->n - e->majority), &e->coder));
     int rc = SS_OK;
-    if ((rc = cl_alloc(ctx, &e->try_next, PG, true)) || (rc = cl_alloc(ctx, &e->ent_len, GW, true)) ||
-        (rc = cl_alloc(ctx, &e->ent_addr, GW, true)) || (rc = cl_alloc(ctx, &e->ent_log_offset, GW, true)) ||
-        (rc = cl_alloc(ctx, &e->cl_partials, scan_tiles(PG > G ? PG : G), false)) || (rc = cl_alloc(ctx, &e->cl_words, 4, false)) ||
-        (rc = cl_alloc(ctx, &e->cl_eff, G, false)) || (rc = cl_alloc(ctx, &e->cl_wal, G, false)) ||
-        (rc = cl_alloc(ctx, &e->pk_frames, PG, false)) || (rc = cl_alloc(ctx, &e->pk_bytes, PG, false)) ||
-        (rc = cl_alloc(ctx, &e->pk_range, PG, false)) || (rc = cl_alloc(ctx, &e->log_start, G, true)) ||
-        (rc = cl_alloc(ctx, &e->last_exec, G, true)) || (rc = cl_alloc(ctx, &e->ex_cnt, G, false)) ||
-        (rc = cl_alloc(ctx, &e->ex_bytes, G, false)) || (rc = cl_alloc(ctx, &e->ex_words, 3, false)) ||
-        (rc = cl_alloc(ctx, &e->held, GW, true)) || (rc = cl_alloc(ctx, &e->last_recon, G, true)) ||
-        (rc = cl_alloc(ctx, &e->matrix, size_t(e->n) * e->majority, false)) || (rc = upload_matrix(e))) {
+    if ((rc = dalloc(ctx, &e->try_next, PG, true)) || (rc = dalloc(ctx, &e->ent_len, GW, true)) ||
+        (rc = dalloc(ctx, &e->ent_addr, GW, true)) || (rc = dalloc(ctx, &e->ent_log_offset, GW, true)) ||
+        (rc = dalloc(ctx, &e->cl_partials, scan_tiles(PG > G ? PG : G), false)) || (rc = dalloc(ctx, &e->cl_words, 4, false)) ||
+        (rc = dalloc(ctx, &e->cl_eff, G, false)) || (rc = dalloc(ctx, &e->cl_wal, G, false)) ||
+        (rc = dalloc(ctx, &e->pk_frames, PG, false)) || (rc = dalloc(ctx, &e->pk_bytes, PG, false)) ||
+        (rc = dalloc(ctx, &e->pk_range, PG, false)) || (rc = dalloc(ctx, &e->log_start, G, true)) ||
+        (rc = dalloc(ctx, &e->last_exec, G, true)) || (rc = dalloc(ctx, &e->ex_cnt, G, false)) ||
+        (rc = dalloc(ctx, &e->ex_bytes, G, false)) || (rc = dalloc(ctx, &e->ex_words, 3, false)) ||
+        (rc = dalloc(ctx, &e->held, GW, true)) || (rc = dalloc(ctx, &e->last_recon, G, true)) ||
+        (rc = dalloc(ctx, &e->matrix, size_t(e->n) * e->majority, false)) || (rc = upload_matrix(e))) {
         // nothing half-built stays behind: a later call starts over, and raft_append stays allowed
         cudaStreamSynchronize(ctx->stream);
         craft_log_free(e);
@@ -754,12 +679,6 @@ int craft_log_init(ss_engine *e) {
     return SS_OK;
 }
 
-int key_bits(uint64_t v) {
-    int b = 1;
-    while (b < 32 && (v >> b) != 0u) ++b;
-    return b;
-}
-
 int backoff_scratch(ss_engine *e, uint64_t n, int bits) {
     if (n <= e->bo_cap) return SS_OK;
     ss_ctx *ctx = e->ctx;
@@ -769,8 +688,8 @@ int backoff_scratch(ss_engine *e, uint64_t n, int bits) {
         if (b) cudaFree(b);
     e->bo_keys = nullptr; e->bo_idx = nullptr; e->bo_sort_tmp = nullptr;
     e->bo_cap = 0;
-    SS_TRY(cl_alloc(ctx, &e->bo_keys, 2 * n, false));
-    SS_TRY(cl_alloc(ctx, &e->bo_idx, 2 * n, false));
+    SS_TRY(dalloc(ctx, &e->bo_keys, 2 * n, false));
+    SS_TRY(dalloc(ctx, &e->bo_idx, 2 * n, false));
     size_t bytes = 0;
     SS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, e->bo_keys, e->bo_keys + n, e->bo_idx, e->bo_idx + n, static_cast<int>(n), 0, bits,
                                             ctx->stream));
@@ -825,7 +744,7 @@ int ss_engine_craft_propose(ss_engine *e, uint32_t me, const uint8_t *arena, con
     A.rec_len = e->cl_wal;
     A.status = ctx->dev_status;
     A.led = e->led;
-    const uint32_t grid = cl_grid(ctx, e->G, kClThreads);
+    const uint32_t grid = launch_grid(ctx, e->G, kClThreads);
     if (e->led != nullptr) craft_propose_prepare_kernel<true><<<grid, kClThreads, 0, ctx->stream>>>(A);
     else craft_propose_prepare_kernel<false><<<grid, kClThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
@@ -837,7 +756,7 @@ int ss_engine_craft_propose(ss_engine *e, uint32_t me, const uint8_t *arena, con
     // into planes 0..d-1, parity into planes d..T-1, each at the group's slot
     SS_TRY(ss_rs_encode_batch_dev(e->coder, arena, data_off, e->cl_eff, e->G, shards + uint64_t(e->majority) * plane_stride, plane_stride,
                                   shard_off, SS_RS_OUT_PADDED16 | SS_RS_EMIT_DATA));
-    craft_propose_wal_kernel<<<cl_grid(ctx, e->G, kClThreads / 32), kClThreads, 0, ctx->stream>>>(A);
+    craft_propose_wal_kernel<<<launch_grid(ctx, e->G, kClThreads / 32), kClThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
 }
 
@@ -867,7 +786,7 @@ int ss_frame_append_pack_dev(ss_engine *e, const ss_append_pack_spec *spec, cons
     A.frame_group = frame_group; A.frame_peer = frame_peer; A.n_frames = n_frames; A.total = total != nullptr ? total : e->cl_words + 3;
     A.pair_status = pair_status; A.pk_frames = e->pk_frames; A.pk_bytes = e->pk_bytes; A.pk_range = e->pk_range;
     A.frames_total = e->cl_words; A.status = ctx->dev_status; A.led = e->led;
-    const uint32_t grid_w = cl_grid(ctx, A.PG, kClThreads / 32);
+    const uint32_t grid_w = launch_grid(ctx, A.PG, kClThreads / 32);
     const bool held = e->held_partial, led = e->led != nullptr;
     if (held && led) append_plan_kernel<true, true><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
     else if (held) append_plan_kernel<true, false><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
@@ -882,7 +801,7 @@ int ss_frame_append_pack_dev(ss_engine *e, const ss_append_pack_spec *spec, cons
     else if (led) append_place_kernel<false, true><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
     else append_place_kernel<false, false><<<grid_w, kClThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
-    const uint32_t grid_f = cl_grid(ctx, max_frames, kClThreads / 32);
+    const uint32_t grid_f = launch_grid(ctx, max_frames, kClThreads / 32);
     if (held) append_write_kernel<true><<<grid_f, kClThreads, 0, ctx->stream>>>(A);
     else append_write_kernel<false><<<grid_f, kClThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
@@ -908,7 +827,7 @@ int ss_engine_craft_backoff(ss_engine *e, const uint8_t *buf, uint64_t buf_len, 
     A.n = n_frames; A.G = e->G; A.PG = PG; A.P = e->n_peers; A.W = e->W; A.variant = reply_variant;
     A.key_in = e->bo_keys; A.idx_in = e->bo_idx; A.key = e->bo_keys + n_frames; A.idx = e->bo_idx + n_frames;
     A.next_slot = e->next_slot; A.try_next = e->try_next; A.terms = e->terms; A.log_start = e->log_start; A.want_end = want_end;
-    const uint32_t grid = cl_grid(ctx, n_frames, kClThreads);
+    const uint32_t grid = launch_grid(ctx, n_frames, kClThreads);
     backoff_key_kernel<<<grid, kClThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     size_t bytes = e->bo_sort_bytes;
@@ -936,29 +855,15 @@ int ss_engine_craft_execute(ss_engine *e, uint8_t *out, uint64_t out_capacity, u
     SS_TRY(craft_check(e));
     SS_TRY(craft_log_init(e));
     ss_ctx *ctx = e->ctx;
-    CraftExecArgs A{};
-    A.G = e->G; A.W = e->W; A.d = e->majority; A.plane_stride = e->log_plane_stride;
-    A.last_commit = e->last_commit; A.ent_len = e->ent_len; A.held = e->held_partial ? e->held : nullptr; A.matrix = e->matrix;
-    A.log_start = e->log_start; A.ent_addr = e->ent_addr;
-    A.last_exec = e->last_exec; A.cnt = e->ex_cnt; A.bytes = e->ex_bytes; A.n_exec = e->ex_words;
-    A.out = out; A.out_cap = out_capacity; A.rec_group = rec_group; A.rec_slot = rec_slot; A.rec_off = rec_off; A.rec_len = rec_len;
-    A.rec_cap = rec_capacity; A.status = ctx->dev_status; A.led = e->led;
+    const ExecOut o{e->matrix, e->ex_cnt, e->ex_bytes, e->ex_words, out, out_capacity, rec_group, rec_slot, rec_off, rec_len,
+                    rec_capacity, ctx->dev_status};
+    const CraftRing ring{e->W, e->majority, e->log_plane_stride, e->last_commit, e->ent_len, e->held_partial ? e->held : nullptr, e->log_start,
+                         e->ent_addr, e->last_exec, e->led};
     uint64_t *tot = totals != nullptr ? totals : e->ex_words + 1;
-    const uint32_t grid = cl_grid(ctx, e->G, kClThreads);
-    SS_CUDA(cudaMemsetAsync(e->ex_words, 0, 8, ctx->stream));
-    if (e->led != nullptr) craft_exec_count_kernel<true><<<grid, kClThreads, 0, ctx->stream>>>(A);
-    else craft_exec_count_kernel<false><<<grid, kClThreads, 0, ctx->stream>>>(A);
-    SS_TRY(launched(ctx));
-    SS_TRY(launch_exclusive_scan_u64(ctx, e->ex_cnt, e->G, e->cl_partials, tot));
-    SS_TRY(launch_exclusive_scan_u64(ctx, e->ex_bytes, e->G, e->cl_partials, tot + 1));
-    if (e->led != nullptr) craft_exec_place_kernel<true><<<grid, kClThreads, 0, ctx->stream>>>(A);
-    else craft_exec_place_kernel<false><<<grid, kClThreads, 0, ctx->stream>>>(A);
-    SS_TRY(launched(ctx));
-    // a warp per entry the ring can hold, up to the grid cap; warps past the executed count return at once
-    const uint32_t grid_p = cl_grid(ctx, e->G * e->W, kExecWarps);
-    if (e->held_partial) craft_exec_regen_kernel<<<grid_p, kExecThreads, 0, ctx->stream>>>(A);
-    else craft_exec_payload_kernel<<<grid_p, kExecThreads, 0, ctx->stream>>>(A);
-    return launched(ctx);
+    const auto run = [&](auto log, auto shards) { return launch_execute(ctx, o, log, shards, e->G, e->G * e->W, e->cl_partials, tot); };
+    const bool led = e->led != nullptr;
+    if (e->held_partial) return led ? run(CraftLog<true>{ring}, CraftShards<true>{ring}) : run(CraftLog<false>{ring}, CraftShards<true>{ring});
+    return led ? run(CraftLog<true>{ring}, CraftShards<false>{ring}) : run(CraftLog<false>{ring}, CraftShards<false>{ring});
 }
 
 int ss_engine_craft_set_full_copy(ss_engine *e, int full_copy) {
@@ -974,7 +879,7 @@ int ss_engine_craft_advance(ss_engine *e, const uint64_t *upto) {
     if (upto == nullptr) return set_error(SS_ERR_INVALID_ARG, "null upto");
     SS_TRY(craft_log_init(e));
     ss_ctx *ctx = e->ctx;
-    craft_advance_kernel<<<cl_grid(ctx, e->G, kClThreads), kClThreads, 0, ctx->stream>>>(upto, e->G, e->log_start, e->last_snap,
+    craft_advance_kernel<<<launch_grid(ctx, e->G, kClThreads), kClThreads, 0, ctx->stream>>>(upto, e->G, e->log_start, e->last_snap,
                                                                                       e->last_commit);
     return launched(ctx);
 }

@@ -227,13 +227,13 @@ __global__ void __launch_bounds__(kRcThreads) recon_size_kernel(const __grid_con
             reads_walk(A, g, lr0, [&](uint64_t s, uint32_t t) {
                 eb += wv_len(s) + wv_len(t);
                 if (++m == A.chunk) {
-                    bytes += cl_round16(reads_frame_len(A, m, eb));
+                    bytes += round16(reads_frame_len(A, m, eb));
                     ++frames;
                     m = eb = 0;
                 }
             });
             if (m != 0u) {
-                bytes += cl_round16(reads_frame_len(A, m, eb));
+                bytes += round16(reads_frame_len(A, m, eb));
                 ++frames;
             }
             A.recon0[i] = lr0;
@@ -289,7 +289,7 @@ __global__ void __launch_bounds__(kRcThreads) recon_write_kernel(const __grid_co
                 A.frame_off[f] = o;
                 A.frame_len[f] = static_cast<uint32_t>(at);
                 ++f;
-                o += cl_round16(at);
+                o += round16(at);
             }
         });
         if (total != 0u) A.last_recon[g] = last;
@@ -378,7 +378,7 @@ __global__ void __launch_bounds__(kRcThreads) serve_size_kernel(const __grid_con
         else bytes += 9u + wv_len(A.reply_variant) + wv_len(cnt);
         A.verdict[i] = kind;
         A.reply_len[i] = bytes;
-        A.reply_off[i] = cl_round16(bytes);
+        A.reply_off[i] = round16(bytes);
     }
 }
 
@@ -392,7 +392,7 @@ __global__ void __launch_bounds__(kRcThreads, 1) serve_write_kernel(const __grid
     bool full = false;
     for (uint64_t i = warp; i < A.n; i += nwarps) {
         const uint64_t len = A.reply_len[i], off = A.reply_off[i];
-        if (len == 0u || off > A.out_cap || cl_round16(len) > A.out_cap - off) {
+        if (len == 0u || off > A.out_cap || round16(len) > A.out_cap - off) {
             if (lane == 0u) {
                 if (len != 0u) {
                     A.verdict[i] = SS_RECON_VERDICT_OUT_FULL;
@@ -667,7 +667,7 @@ int ss_engine_craft_step_up(ss_engine *e, const ss_follower *f, const uint32_t *
     A.log_end = e->log_end; A.last_commit = e->last_commit; A.last_snap = e->last_snap; A.curr_term = e->curr_term; A.terms = e->terms;
     A.ent_len = e->ent_len; A.held = e->held; A.match = e->match; A.next_slot = e->next_slot; A.try_next = e->try_next;
     A.status = ctx->dev_status;
-    const uint32_t grid = cl_grid(ctx, n_listed, kRcThreads);
+    const uint32_t grid = launch_grid(ctx, n_listed, kRcThreads);
     SS_CUDA(cudaMemsetAsync(e->rc_words, 0xff, e->G * 8, ctx->stream));
     stepup_first_kernel<<<grid, kRcThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
@@ -676,7 +676,7 @@ int ss_engine_craft_step_up(ss_engine *e, const ss_follower *f, const uint32_t *
     SS_TRY(launch_exclusive_scan_u64(ctx, shard_off, n_listed, partials, tot));
     stepup_commit_kernel<<<grid, kRcThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
-    stepup_copy_kernel<<<cl_grid(ctx, n_listed * e->W, kRcThreads / 32), kRcThreads, 0, ctx->stream>>>(A);
+    stepup_copy_kernel<<<launch_grid(ctx, n_listed * e->W, kRcThreads / 32), kRcThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     return craft_led_mark(e, groups, verdict, n_listed);                   // a stepped-up group is led again
 }
@@ -709,7 +709,7 @@ int ss_engine_craft_reconstruct_reads(ss_engine *e, const uint32_t *groups, uint
     A.totals = tot;
     A.out = out; A.out_cap = out_capacity; A.frame_group = frame_group; A.frame_dst = frame_dst; A.frame_off = frame_off;
     A.frame_len = frame_len; A.frame_cap = frame_capacity; A.status = ctx->dev_status; A.led = e->led;
-    const uint32_t grid = cl_grid(ctx, n, kRcThreads);
+    const uint32_t grid = launch_grid(ctx, n, kRcThreads);
     if (e->led != nullptr) recon_size_kernel<true><<<grid, kRcThreads, 0, ctx->stream>>>(A);
     else recon_size_kernel<false><<<grid, kRcThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
@@ -745,10 +745,10 @@ int ss_follower_reconstruct_serve(ss_follower *f, const uint8_t *buf, uint64_t b
     A.data_len = f->data_len;
     A.out = out; A.out_cap = out_capacity; A.reply_off = reply_off; A.reply_len = reply_len; A.verdict = verdict;
     A.status = ctx->dev_status;
-    serve_size_kernel<<<cl_grid(ctx, n, kRcThreads), kRcThreads, 0, ctx->stream>>>(A);
+    serve_size_kernel<<<launch_grid(ctx, n, kRcThreads), kRcThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     SS_TRY(launch_exclusive_scan_u64(ctx, reply_off, n, f->partials, total != nullptr ? total : f->words + 2));
-    serve_write_kernel<<<cl_grid(ctx, n, kRcThreads / 32), kRcThreads, 0, ctx->stream>>>(A);
+    serve_write_kernel<<<launch_grid(ctx, n, kRcThreads / 32), kRcThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
 }
 
@@ -772,13 +772,13 @@ int ss_engine_craft_absorb(ss_engine *e, const uint8_t *buf, uint64_t buf_len, c
     A.log_start = e->log_start; A.ent_addr = e->ent_addr; A.log_end = e->log_end; A.ent_len = e->ent_len; A.held = e->held;
     A.fr_at = e->rc_words; A.key_in = e->bo_keys; A.idx_in = e->bo_idx; A.key = e->bo_keys + n; A.idx = e->bo_idx + n;
     A.absorbed = absorbed; A.verdict = verdict;
-    absorb_head_kernel<<<cl_grid(ctx, n, kRcThreads), kRcThreads, 0, ctx->stream>>>(A);
+    absorb_head_kernel<<<launch_grid(ctx, n, kRcThreads), kRcThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     size_t bytes = e->bo_sort_bytes;
     SS_CUDA(cub::DeviceRadixSort::SortPairs(e->bo_sort_tmp, bytes, e->bo_keys, e->bo_keys + n, e->bo_idx, e->bo_idx + n, static_cast<int>(n), 0,
                                             bits, ctx->stream));
     SS_TRY(launched(ctx));
-    absorb_apply_kernel<<<cl_grid(ctx, n, kRcThreads / 32), kRcThreads, 0, ctx->stream>>>(A);
+    absorb_apply_kernel<<<launch_grid(ctx, n, kRcThreads / 32), kRcThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
 }
 

@@ -252,7 +252,7 @@ int craft_led_in_use(ss_engine *e) {
 int craft_led_mark(ss_engine *e, const uint32_t *groups, const uint32_t *verdict, uint64_t n) {
     if (e->led == nullptr || n == 0) return SS_OK;
     ss_ctx *ctx = e->ctx;
-    led_mark_kernel<<<cl_grid(ctx, n, kSdThreads), kSdThreads, 0, ctx->stream>>>(groups, verdict, n, e->G, e->led);
+    led_mark_kernel<<<launch_grid(ctx, n, kSdThreads), kSdThreads, 0, ctx->stream>>>(groups, verdict, n, e->G, e->led);
     return launched(ctx);
 }
 
@@ -330,7 +330,7 @@ int ss_engine_craft_step_down(ss_engine *e, ss_follower *f, const ss_step_down_s
     A.log_start = e->log_start; A.last_exec = e->last_exec; A.ent_addr = e->ent_addr; A.log_end = e->log_end;
     A.last_commit = e->last_commit; A.last_snap = e->last_snap; A.terms = e->terms; A.ent_len = e->ent_len;
     A.held = e->held_partial ? e->held : nullptr; A.curr_term = e->curr_term; A.match = e->match; A.led = e->led;
-    const uint32_t grid = cl_grid(ctx, n, kSdThreads);
+    const uint32_t grid = launch_grid(ctx, n, kSdThreads);
     SS_CUDA(cudaMemsetAsync(A.first, 0xff, G * 8, ctx->stream));
     sd_head_kernel<<<grid, kSdThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
@@ -341,7 +341,7 @@ int ss_engine_craft_step_down(ss_engine *e, ss_follower *f, const ss_step_down_s
     sd_commit_kernel<<<grid, kSdThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     // a warp per entry the deposed spans can copy, up to the grid cap; warps past the copied count return at once
-    sd_copy_kernel<<<cl_grid(ctx, span > n ? span : n, kSdThreads / 32), kSdThreads, 0, ctx->stream>>>(A);
+    sd_copy_kernel<<<launch_grid(ctx, span > n ? span : n, kSdThreads / 32), kSdThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
 }
 

@@ -454,15 +454,6 @@ engine_raft_snap_kernel(const uint32_t *__restrict__ match, uint32_t P, uint64_t
     }
 }
 
-// zeroed on the context's stream: a cudaMemset would go to the legacy default stream, which a non-blocking context
-// stream does not wait for, so it could land after the caller's first writes (set_prepared_ballots, window_base)
-template <typename T>
-static int dalloc(ss_ctx *ctx, T **p, size_t count, bool zero = true) {
-    SS_CUDA(cudaMalloc(reinterpret_cast<void **>(p), count * sizeof(T) ? count * sizeof(T) : 1));
-    if (zero) SS_CUDA(cudaMemsetAsync(*p, 0, count * sizeof(T), ctx->stream));
-    return SS_OK;
-}
-
 uint64_t scan_tiles(uint64_t n) { return (n + kScanTile - 1) / kScanTile; }
 
 int launch_exclusive_scan_u64(ss_ctx *ctx, uint64_t *x, uint64_t n, uint64_t *partials, uint64_t *total) {

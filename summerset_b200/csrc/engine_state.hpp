@@ -75,23 +75,10 @@ int craft_held_in_use(ss_engine *e);
 int craft_led_in_use(ss_engine *e);
 // led = 1 for the groups of the listings step-up took (verdict DONE), once the bytes exist (craft_stepdown.cu)
 int craft_led_mark(ss_engine *e, const uint32_t *groups, const uint32_t *verdict, uint64_t n);
-// bits of a radix-sort key up to v, and the log's grow-only sort scratch (bo_*) for n keys of that many bits, shared by
-// the back-off and absorb (craft_leader.cu)
-int key_bits(uint64_t v);
+// the log's grow-only sort scratch (bo_*) for n keys of `bits` bits, shared by the back-off and absorb (craft_leader.cu)
 int backoff_scratch(ss_engine *e, uint64_t n, int bits);
 // the recon / step-down scratch (rc_words), grow-only: `words` u64 (craft_recon.cu)
 int rc_scratch(ss_engine *e, uint64_t words);
-
-// the log calls' grid: enough CTAs of per_cta items, capped at 64 per SM
-inline uint32_t cl_grid(ss_ctx *ctx, uint64_t items, uint32_t per_cta) {
-    uint64_t ctas = (items + per_cta - 1) / per_cta;
-    const uint64_t cap = static_cast<uint64_t>(ctx->sm_count) * 8ull * 8ull;
-    if (ctas > cap) ctas = cap;
-    if (ctas == 0) ctas = 1;
-    return static_cast<uint32_t>(ctas);
-}
-
-__device__ __forceinline__ uint64_t cl_round16(uint64_t x) { return (x + 15u) & ~15ull; }
 
 __device__ __forceinline__ void cl_put_be64(uint8_t *p, uint64_t v) {
     for (int b = 0; b < 8; ++b) p[b] = static_cast<uint8_t>(v >> (8 * (7 - b)));

@@ -22,11 +22,9 @@
 //
 // Execution of the committed entries (the walk in handle_msg_append_entries, craft/messages.rs:198-240):
 //
-//   fol_exec_count_kernel    a thread per group: the entries the walk executes, and their payload bytes
-//   (engine.cu's scan)       record indices and payload regions
-//   fol_exec_place_kernel    a thread per group: capacities, the records, last_exec
-//   fol_exec_payload_kernel  a warp per record: get_data's bytes from the held shards, a missing data shard regenerated
-//                            from the first d held ones (exec_payload.cuh)
+//   (exec_walk.cuh, FolLog)  a thread per group: the entries the walk executes, their payload bytes, then the records
+//                            and last_exec; a warp per record: get_data's bytes from the held shards, a missing data
+//                            shard regenerated from the first d held ones
 //
 // Serving a new leader's Reconstruct reads (ss_follower_reconstruct_serve) is in craft_recon.cu; campaigns, votes and
 // their tally (ss_follower_campaign / _vote / _tally) are in craft_election.cu.
@@ -38,7 +36,7 @@
 #include "codeword_wire.cuh"
 #include "craft_frames.cuh"
 #include "device_common.cuh"
-#include "exec_payload.cuh"
+#include "exec_walk.cuh"
 #include "follower_state.hpp"
 #include "gf256.hpp"
 #include "ss_internal.hpp"
@@ -117,7 +115,7 @@ __device__ __forceinline__ const uint8_t *shard_in_frame(const uint8_t *tags, ui
 // or -- for an entry this call appended, whose slots the copy pass has not written yet -- from its own frame.
 __device__ void absorb_copy(const FolArgs &A, uint8_t *dst, uint64_t old_addr, uint32_t old_held, const uint8_t *new_tags,
                             uint32_t new_held, uint64_t L) {
-    const uint64_t pitch = SS_CW_SLOT_PITCH(L), padded = fol_round16(L);
+    const uint64_t pitch = SS_CW_SLOT_PITCH(L), padded = round16(L);
     const uint32_t uni = old_held | new_held;
     const uint8_t *old_tags = nullptr;
     if (old_addr & kTag) {
@@ -229,7 +227,7 @@ __global__ void __launch_bounds__(kFolThreads) follower_replay_kernel(const __gr
                     A.data_len[pos] = static_cast<uint32_t>(e.dl);
                     A.shard_addr[pos] = kTag | (static_cast<uint64_t>(i) << 32) | e.tags_at;
                     le = s + 1u;
-                    wl += fol_round16(ent_rec_len(e, A.log_variant));
+                    wl += round16(ent_rec_len(e, A.log_variant));
                 } else {
                     const uint32_t oh = A.held[pos];
                     if (static_cast<uint32_t>(__popc(oh & dmask)) < A.d && A.data_len[pos] == e.dl && oh != e.held) {
@@ -316,7 +314,7 @@ __global__ void __launch_bounds__(kFolThreads) follower_copy_kernel(const __grid
                 const uint64_t pos = row + ((h.prev + 1u + q) & wm);
                 if (lane == 0u && A.shard_addr[pos] == (kTag | (i << 32) | e.tags_at))
                     A.shard_addr[pos] = reinterpret_cast<uint64_t>(A.store + so);
-                wo += fol_round16(8u + body);
+                wo += round16(8u + body);
                 so += ent_store_bytes(e);
             }
             at = e.next;
@@ -337,96 +335,37 @@ follower_advance_kernel(const uint64_t *__restrict__ upto, uint64_t G, uint64_t 
 }
 
 // ---- execution -----------------------------------------------------------------------------------------------------
-struct FolExecArgs {
-    uint64_t G;
+// the walk in handle_msg_append_entries (exec_walk.cuh), from max(last_exec + 1, start_slot): stop past last_commit, or
+// at fewer than d shards held, which the commit walk already excludes but state a host installed may hold; stop at a
+// null entry, which get_data refuses (rscoding.rs:581-583).  A held shard of rank k is at shard_addr + k *
+// SS_CW_SLOT_PITCH(L), the store layout of the append.
+struct FolLog {
     uint32_t W, d;
     const uint64_t *start_slot, *last_commit, *shard_addr;
     const uint32_t *held, *data_len;
-    const uint8_t *matrix;          // [T*d]
     uint64_t *last_exec;
-    uint64_t *cnt, *bytes;          // [G] per group: records, payload bytes; then their exclusive scans
-    uint64_t *n_exec;               // records written (a prefix: the offsets are monotone)
-    uint8_t *out;
-    uint64_t out_cap;
-    uint32_t *rec_group;
-    uint64_t *rec_slot, *rec_off;
-    uint32_t *rec_len;
-    uint64_t rec_cap;
-    uint32_t *status;
+
+    struct Walk { uint64_t s; };
+    static constexpr bool kTables = true, kByIndex = false;
+
+    __device__ __forceinline__ bool live(uint64_t) const { return true; }
+    __device__ __forceinline__ Walk start(uint64_t g) const {
+        const uint64_t s = last_exec[g] + 1u, st = start_slot[g];
+        return {s > st ? s : st};
+    }
+    __device__ __forceinline__ uint32_t next(const Walk &, uint64_t g, uint64_t s, uint32_t *dlen) const {
+        if (s > last_commit[g]) return kExecStop;
+        const uint64_t pos = g * W + (s & (W - 1u));
+        if (static_cast<uint32_t>(__popc(held[pos])) < d) return kExecStop;
+        *dlen = data_len[pos];
+        return *dlen == 0u ? kExecNull : kExecRun;
+    }
+    __device__ __forceinline__ void finish(uint64_t g, uint64_t s) const { last_exec[g] = s - 1u; }
+    __device__ __forceinline__ ExecSrc source(uint64_t g, uint64_t s, uint32_t dlen) const {
+        const uint64_t pos = g * W + (s & (W - 1u));
+        return {held[pos], reinterpret_cast<const uint8_t *>(shard_addr[pos]), SS_CW_SLOT_PITCH((dlen + d - 1u) / d)};
+    }
 };
-
-enum : uint32_t { kFolExecStop = 0u, kFolExecRun = 1u, kFolExecNull = 2u };
-
-__device__ __forceinline__ uint64_t fol_exec_start(const FolExecArgs &A, uint64_t g) {
-    const uint64_t s = A.last_exec[g] + 1u, st = A.start_slot[g];
-    return s > st ? s : st;
-}
-
-// what the walk does at slot s of group g: stop (past last_commit, or fewer than d shards held, which the commit walk
-// already excludes but state a host installed may hold), run it (*dlen = its data_len), or stop at a null entry, which
-// get_data refuses (rscoding.rs:581-583)
-__device__ __forceinline__ uint32_t fol_exec_next(const FolExecArgs &A, uint64_t g, uint64_t s, uint32_t *dlen) {
-    if (s > A.last_commit[g]) return kFolExecStop;
-    const uint64_t pos = g * A.W + (s & (A.W - 1u));
-    if (static_cast<uint32_t>(__popc(A.held[pos])) < A.d) return kFolExecStop;
-    *dlen = A.data_len[pos];
-    return *dlen == 0u ? kFolExecNull : kFolExecRun;
-}
-
-__global__ void __launch_bounds__(kFolThreads) fol_exec_count_kernel(const __grid_constant__ FolExecArgs A) {
-    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kFolThreads;
-    for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kFolThreads + threadIdx.x; g < A.G; g += stride) {
-        uint64_t n = 0u, b = 0u;
-        uint32_t dl = 0u;
-        for (uint64_t s = fol_exec_start(A, g); fol_exec_next(A, g, s, &dl) == kFolExecRun; ++s, ++n) b += fol_round16(dl);
-        A.cnt[g] = n;
-        A.bytes[g] = b;
-    }
-}
-
-__global__ void __launch_bounds__(kFolThreads) fol_exec_place_kernel(const __grid_constant__ FolExecArgs A) {
-    bool full = false, null_ent = false;
-    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kFolThreads;
-    for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kFolThreads + threadIdx.x; g < A.G; g += stride) {
-        const uint64_t s0 = fol_exec_start(A, g);
-        uint64_t ro = A.cnt[g], bo = A.bytes[g], s = s0;
-        uint32_t dl = 0u, r;
-        while ((r = fol_exec_next(A, g, s, &dl)) == kFolExecRun) {
-            const uint64_t sz = fol_round16(dl);
-            if (ro >= A.rec_cap || bo > A.out_cap || sz > A.out_cap - bo) { full = true; break; }
-            A.rec_group[ro] = static_cast<uint32_t>(g);
-            A.rec_slot[ro] = s;
-            A.rec_off[ro] = bo;
-            A.rec_len[ro] = dl;
-            ++ro;
-            bo += sz;
-            ++s;
-        }
-        null_ent |= r == kFolExecNull;
-        if (s != s0) {
-            A.last_exec[g] = s - 1u;
-            atomicMax(reinterpret_cast<unsigned long long *>(A.n_exec), static_cast<unsigned long long>(ro));
-        }
-    }
-    if (full) atomicOr(A.status, SS_DEV_STATUS_EXEC_FULL);
-    if (null_ent) atomicOr(A.status, SS_DEV_STATUS_EXEC_NULL);
-}
-
-// a warp per record: held shard of rank k at shard_addr + k * SS_CW_SLOT_PITCH(L), the store layout of the append
-__global__ void __launch_bounds__(kExecThreads) fol_exec_payload_kernel(const __grid_constant__ FolExecArgs A) {
-    __shared__ ExecShared S;
-    exec_tables_init(S);
-    const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
-    const uint64_t n = *A.n_exec;
-    const uint64_t nwarps = static_cast<uint64_t>(gridDim.x) * kExecWarps;
-    for (uint64_t r = static_cast<uint64_t>(blockIdx.x) * kExecWarps + w; r < n; r += nwarps) {
-        const uint64_t g = A.rec_group[r], pos = g * A.W + (A.rec_slot[r] & (A.W - 1u));
-        const uint32_t dlen = A.rec_len[r];
-        const uint64_t pitch = SS_CW_SLOT_PITCH((dlen + A.d - 1u) / A.d);
-        warp_exec_payload(S, w, lane, A.d, A.held[pos], dlen, A.matrix, reinterpret_cast<const uint8_t *>(A.shard_addr[pos]), pitch,
-                          A.out + A.rec_off[r]);
-    }
-}
 
 // the leader's side: PeerMessage::Msg{AppendEntriesReply{term, end_slot, conflict}} frames -> ingest records
 struct ReplyParseArgs {
@@ -464,27 +403,6 @@ __global__ void __launch_bounds__(kFolThreads) append_reply_parse_kernel(const _
     }
 }
 
-static inline uint32_t fol_grid(ss_ctx *ctx, uint64_t items, uint32_t per_cta) {
-    uint64_t ctas = (items + per_cta - 1) / per_cta;
-    const uint64_t cap = static_cast<uint64_t>(ctx->sm_count) * 8ull * 8ull;
-    if (ctas > cap) ctas = cap;
-    if (ctas == 0) ctas = 1;
-    return static_cast<uint32_t>(ctas);
-}
-
-template <typename T>
-static int fol_alloc(ss_ctx *ctx, T **p, size_t count, bool zero = true) {
-    SS_CUDA(cudaMalloc(reinterpret_cast<void **>(p), count * sizeof(T) ? count * sizeof(T) : 1));
-    if (zero) SS_CUDA(cudaMemsetAsync(*p, 0, count * sizeof(T), ctx->stream));
-    return SS_OK;
-}
-
-static int fol_key_bits(uint64_t G) {
-    int b = 1;
-    while (b < 32 && (G >> b) != 0u) ++b;
-    return b;
-}
-
 int fol_scratch(ss_follower *f, uint64_t n) {
     if (n <= f->cap_frames) return SS_OK;
     ss_ctx *ctx = f->ctx;
@@ -494,13 +412,13 @@ int fol_scratch(ss_follower *f, uint64_t n) {
         if (b) cudaFree(b);
     f->hdr = nullptr; f->keys = nullptr; f->idx = nullptr; f->partials = nullptr; f->sort_tmp = nullptr;
     f->cap_frames = 0;
-    SS_TRY(fol_alloc(ctx, &f->hdr, n, false));
-    SS_TRY(fol_alloc(ctx, &f->keys, 2 * n, false));
-    SS_TRY(fol_alloc(ctx, &f->idx, 2 * n, false));
-    SS_TRY(fol_alloc(ctx, &f->partials, scan_tiles(n), false));
+    SS_TRY(dalloc(ctx, &f->hdr, n, false));
+    SS_TRY(dalloc(ctx, &f->keys, 2 * n, false));
+    SS_TRY(dalloc(ctx, &f->idx, 2 * n, false));
+    SS_TRY(dalloc(ctx, &f->partials, scan_tiles(n), false));
     size_t bytes = 0;
     SS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, f->keys, f->keys + n, f->idx, f->idx + n, static_cast<int>(n), 0,
-                                            fol_key_bits(f->G), ctx->stream));
+                                            key_bits(f->G), ctx->stream));
     SS_CUDA(cudaMalloc(&f->sort_tmp, bytes ? bytes : 1));
     f->sort_tmp_bytes = bytes;
     f->cap_frames = n;
@@ -568,13 +486,13 @@ int ss_follower_create(ss_ctx *ctx, const ss_follower_config *cfg, uint64_t G, s
     f->T = cfg->population;
     ctx_retain(ctx);
     int rc = SS_OK;
-    if ((rc = fol_alloc(ctx, &f->start_slot, G)) || (rc = fol_alloc(ctx, &f->log_end, G)) || (rc = fol_alloc(ctx, &f->curr_term, G)) ||
-        (rc = fol_alloc(ctx, &f->last_commit, G)) || (rc = fol_alloc(ctx, &f->last_snap, G)) || (rc = fol_alloc(ctx, &f->leader, G)) ||
-        (rc = fol_alloc(ctx, &f->term, G * W)) || (rc = fol_alloc(ctx, &f->shard_addr, G * W)) ||
-        (rc = fol_alloc(ctx, &f->held, G * W)) || (rc = fol_alloc(ctx, &f->data_len, G * W)) || (rc = fol_alloc(ctx, &f->words, 4)) ||
-        (rc = fol_alloc(ctx, &f->last_exec, G)) || (rc = fol_alloc(ctx, &f->matrix, size_t(f->T) * f->d, false)) ||
-        (rc = fol_alloc(ctx, &f->ex_cnt, G, false)) || (rc = fol_alloc(ctx, &f->ex_bytes, G, false)) ||
-        (rc = fol_alloc(ctx, &f->ex_partials, scan_tiles(G), false)) || (rc = fol_alloc(ctx, &f->ex_words, 3, false))) {
+    if ((rc = dalloc(ctx, &f->start_slot, G)) || (rc = dalloc(ctx, &f->log_end, G)) || (rc = dalloc(ctx, &f->curr_term, G)) ||
+        (rc = dalloc(ctx, &f->last_commit, G)) || (rc = dalloc(ctx, &f->last_snap, G)) || (rc = dalloc(ctx, &f->leader, G)) ||
+        (rc = dalloc(ctx, &f->term, G * W)) || (rc = dalloc(ctx, &f->shard_addr, G * W)) ||
+        (rc = dalloc(ctx, &f->held, G * W)) || (rc = dalloc(ctx, &f->data_len, G * W)) || (rc = dalloc(ctx, &f->words, 4)) ||
+        (rc = dalloc(ctx, &f->last_exec, G)) || (rc = dalloc(ctx, &f->matrix, size_t(f->T) * f->d, false)) ||
+        (rc = dalloc(ctx, &f->ex_cnt, G, false)) || (rc = dalloc(ctx, &f->ex_bytes, G, false)) ||
+        (rc = dalloc(ctx, &f->ex_partials, scan_tiles(G), false)) || (rc = dalloc(ctx, &f->ex_words, 3, false))) {
         ss_follower_destroy(f);
         return rc;
     }
@@ -585,7 +503,7 @@ int ss_follower_create(ss_ctx *ctx, const ss_follower_config *cfg, uint64_t G, s
         ss_follower_destroy(f);
         return set_error(SS_ERR_CUDA, "coding matrix upload failed");
     }
-    follower_init_kernel<<<fol_grid(ctx, G, kFolThreads), kFolThreads, 0, ctx->stream>>>(G, f->log_end, f->leader);
+    follower_init_kernel<<<launch_grid(ctx, G, kFolThreads), kFolThreads, 0, ctx->stream>>>(G, f->log_end, f->leader);
     if ((rc = launched(ctx)) != SS_OK) {
         ss_follower_destroy(f);
         return rc;
@@ -609,7 +527,7 @@ int ss_follower_advance(ss_follower *f, const uint64_t *upto) {
     if (f == nullptr || upto == nullptr) return set_error(SS_ERR_INVALID_ARG, "null follower or upto");
     ss_ctx *ctx = f->ctx;
     SS_TRY(ctx_bind(ctx));
-    follower_advance_kernel<<<fol_grid(ctx, f->G, kFolThreads), kFolThreads, 0, ctx->stream>>>(upto, f->G, f->start_slot, f->last_commit);
+    follower_advance_kernel<<<launch_grid(ctx, f->G, kFolThreads), kFolThreads, 0, ctx->stream>>>(upto, f->G, f->start_slot, f->last_commit);
     return launched(ctx);
 }
 
@@ -628,24 +546,10 @@ int ss_follower_execute(ss_follower *f, uint8_t *out, uint64_t out_capacity, uin
     if (reinterpret_cast<uintptr_t>(out) & 15u) return set_error(SS_ERR_INVALID_ARG, "out must be 16-byte aligned");
     ss_ctx *ctx = f->ctx;
     SS_TRY(ctx_bind(ctx));
-    FolExecArgs A{};
-    A.G = f->G; A.W = f->W; A.d = f->d;
-    A.start_slot = f->start_slot; A.last_commit = f->last_commit; A.shard_addr = f->shard_addr; A.held = f->held; A.data_len = f->data_len;
-    A.matrix = f->matrix; A.last_exec = f->last_exec; A.cnt = f->ex_cnt; A.bytes = f->ex_bytes; A.n_exec = f->ex_words;
-    A.out = out; A.out_cap = out_capacity; A.rec_group = rec_group; A.rec_slot = rec_slot; A.rec_off = rec_off; A.rec_len = rec_len;
-    A.rec_cap = rec_capacity; A.status = ctx->dev_status;
-    uint64_t *tot = totals != nullptr ? totals : f->ex_words + 1;
-    const uint32_t grid = fol_grid(ctx, f->G, kFolThreads);
-    SS_CUDA(cudaMemsetAsync(f->ex_words, 0, 8, ctx->stream));
-    fol_exec_count_kernel<<<grid, kFolThreads, 0, ctx->stream>>>(A);
-    SS_TRY(launched(ctx));
-    SS_TRY(launch_exclusive_scan_u64(ctx, f->ex_cnt, f->G, f->ex_partials, tot));
-    SS_TRY(launch_exclusive_scan_u64(ctx, f->ex_bytes, f->G, f->ex_partials, tot + 1));
-    fol_exec_place_kernel<<<grid, kFolThreads, 0, ctx->stream>>>(A);
-    SS_TRY(launched(ctx));
-    // a warp per entry the ring can hold, up to the grid cap; warps past the executed count return at once
-    fol_exec_payload_kernel<<<fol_grid(ctx, f->G * f->W, kExecWarps), kExecThreads, 0, ctx->stream>>>(A);
-    return launched(ctx);
+    const ExecOut o{f->matrix, f->ex_cnt, f->ex_bytes, f->ex_words, out, out_capacity, rec_group, rec_slot, rec_off, rec_len,
+                    rec_capacity, ctx->dev_status};
+    const FolLog log{f->W, f->d, f->start_slot, f->last_commit, f->shard_addr, f->held, f->data_len, f->last_exec};
+    return launch_execute(ctx, o, log, log, f->G, f->G * f->W, f->ex_partials, totals != nullptr ? totals : f->ex_words + 1);
 }
 
 int ss_follower_append(ss_follower *f, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
@@ -684,13 +588,13 @@ int ss_follower_append(ss_follower *f, const uint8_t *buf, uint64_t buf_len, con
     A.wal = wal; A.wal_cap = wal_capacity; A.wal_off = wal_off; A.wal_len = wal_len;
     A.meta = meta; A.meta_len = meta_len; A.replies = replies; A.reply_len = reply_len; A.reply_dst = reply_dst;
     A.trunc_slot = trunc_slot; A.verdict = verdict; A.status = ctx->dev_status;
-    const uint32_t grid_t = fol_grid(ctx, n, kFolThreads);
+    const uint32_t grid_t = launch_grid(ctx, n, kFolThreads);
     SS_CUDA(cudaMemsetAsync(f->words, 0xff, 8, ctx->stream));
     follower_header_kernel<<<grid_t, kFolThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     size_t bytes = f->sort_tmp_bytes;
     SS_CUDA(cub::DeviceRadixSort::SortPairs(f->sort_tmp, bytes, f->keys, f->keys + n, f->idx, f->idx + n, static_cast<int>(n), 0,
-                                            fol_key_bits(f->G), ctx->stream));
+                                            key_bits(f->G), ctx->stream));
     SS_TRY(launched(ctx));
     SS_TRY(launch_exclusive_scan_u64(ctx, store_off, n, f->partials, tot));
     SS_TRY(launch_exclusive_scan_u64(ctx, wal_off, n, f->partials, tot + 1));
@@ -698,7 +602,7 @@ int ss_follower_append(ss_follower *f, const uint8_t *buf, uint64_t buf_len, con
     SS_TRY(launched(ctx));
     follower_replay_kernel<<<grid_t, kFolThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
-    follower_copy_kernel<<<fol_grid(ctx, n, kFolThreads / 32), kFolThreads, 0, ctx->stream>>>(A);
+    follower_copy_kernel<<<launch_grid(ctx, n, kFolThreads / 32), kFolThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
 }
 
@@ -717,7 +621,7 @@ int ss_append_reply_parse_dev(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len,
     A.curr_term = curr_term; A.n = n_frames; A.G = n_groups; A.reply_variant = reply_variant;
     A.rec_group = rec_group; A.rec_peer = rec_peer; A.rec_end_slot = rec_end_slot; A.rec_term = rec_term;
     A.rec_conflict_term = rec_conflict_term; A.rec_conflict_slot = rec_conflict_slot; A.rec_kind = rec_kind;
-    append_reply_parse_kernel<<<fol_grid(ctx, n_frames, kFolThreads), kFolThreads, 0, ctx->stream>>>(A);
+    append_reply_parse_kernel<<<launch_grid(ctx, n_frames, kFolThreads), kFolThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
 }
 

@@ -135,6 +135,31 @@ inline int launched(ss_ctx *ctx) {
     return SS_OK;
 }
 
+// enough CTAs of per_cta items, capped at 64 per SM
+inline uint32_t launch_grid(ss_ctx *ctx, uint64_t items, uint32_t per_cta) {
+    uint64_t ctas = (items + per_cta - 1) / per_cta;
+    const uint64_t cap = static_cast<uint64_t>(ctx->sm_count) * 8ull * 8ull;
+    if (ctas > cap) ctas = cap;
+    if (ctas == 0) ctas = 1;
+    return static_cast<uint32_t>(ctas);
+}
+
+// zeroed on the context's stream: a cudaMemset would go to the legacy default stream, which a non-blocking context
+// stream does not wait for, so it could land after the caller's first writes (window_base) or the first accept
+template <typename T>
+int dalloc(ss_ctx *ctx, T **p, size_t count, bool zero = true) {
+    SS_CUDA(cudaMalloc(reinterpret_cast<void **>(p), count * sizeof(T) ? count * sizeof(T) : 1));
+    if (zero) SS_CUDA(cudaMemsetAsync(*p, 0, count * sizeof(T), ctx->stream));
+    return SS_OK;
+}
+
+// bits of a radix-sort key up to v
+inline int key_bits(uint64_t v) {
+    int b = 1;
+    while (b < 32 && (v >> b) != 0u) ++b;
+    return b;
+}
+
 // exclusive prefix sum of x[0..n) in place (engine.cu); partials: scan_tiles(n) words of device scratch; total (device,
 // may be NULL) = the sum of all n values.  Deterministic: integer sums in a fixed order.
 uint64_t scan_tiles(uint64_t n);

@@ -1,9 +1,12 @@
-// wire_common.cuh -- device helpers shared by the wire kernels (wire_kernels.cu) and the acceptor (acceptor.cu):
-// bincode 2 standard-config u64 varints and warp-cooperative byte copies.
+// wire_common.cuh -- device helpers shared by the wire kernels (wire_kernels.cu), the acceptor (acceptor.cu) and the
+// CRaft calls: 16-byte region rounding, bincode 2 standard-config u64 varints and warp-cooperative byte copies.
 #pragma once
 #include "device_common.cuh"
 
 namespace ssb {
+
+// a region's bytes: every record and frame region starts 16-byte aligned
+__device__ __forceinline__ uint64_t round16(uint64_t x) { return (x + 15u) & ~15ull; }
 
 __device__ __forceinline__ int wv_put(uint8_t *p, uint64_t v) {
     if (v < 251ull) { p[0] = static_cast<uint8_t>(v); return 1; }

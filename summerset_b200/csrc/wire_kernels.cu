@@ -413,14 +413,6 @@ __global__ void __launch_bounds__(kWireThreads) reconstruct_serve_kernel(const _
     }
 }
 
-static inline uint32_t wire_grid(ss_ctx *ctx, uint64_t items, uint32_t per_cta) {
-    uint64_t ctas = (items + per_cta - 1) / per_cta;
-    const uint64_t cap = static_cast<uint64_t>(ctx->sm_count) * 8ull * 8ull;
-    if (ctas > cap) ctas = cap;
-    if (ctas == 0) ctas = 1;
-    return static_cast<uint32_t>(ctas);
-}
-
 }  // namespace ssb
 
 using namespace ssb;
@@ -461,7 +453,7 @@ int ss_frame_accept_pack_dev(ss_ctx *ctx, const ss_frame_spec *s, const uint8_t 
     A.population = s->population; A.peer = peer; A.with_assignment = s->with_assignment; A.assign_size = s->assign_size;
     A.slot = slot; A.ballot = ballot; A.n = n; A.out = out; A.frame_stride = frame_stride; A.frame_off = frame_off; A.frame_len = frame_len;
     if (shard_stride < ((uint64_t(A.L) + 15) & ~uint64_t(15))) return set_error(SS_ERR_INVALID_ARG, "shard_stride shorter than a padded shard");
-    frame_pack_kernel<<<wire_grid(ctx, n, kWireThreads / 32), kWireThreads, 0, ctx->stream>>>(A);
+    frame_pack_kernel<<<launch_grid(ctx, n, kWireThreads / 32), kWireThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
 }
 
@@ -496,10 +488,10 @@ int ss_frame_accept_pack_ragged_dev(ss_ctx *ctx, const ss_frame_spec *s, const u
     A.shard_off = shard_off; A.lens = data_len; A.capacity = out_capacity;
     void *scr = nullptr;
     SS_TRY(ctx_scratch(ctx, scan_tiles(n) * 8, &scr));
-    frame_size_ragged_kernel<<<wire_grid(ctx, n, kWireThreads), kWireThreads, 0, ctx->stream>>>(A);
+    frame_size_ragged_kernel<<<launch_grid(ctx, n, kWireThreads), kWireThreads, 0, ctx->stream>>>(A);
     SS_TRY(launched(ctx));
     SS_TRY(launch_exclusive_scan_u64(ctx, frame_off, n, static_cast<uint64_t *>(scr), total));
-    frame_pack_ragged_kernel<<<wire_grid(ctx, n, kWireThreads / 32), kWireThreads, 0, ctx->stream>>>(A);
+    frame_pack_ragged_kernel<<<launch_grid(ctx, n, kWireThreads / 32), kWireThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
 }
 
@@ -516,7 +508,7 @@ int ss_accept_reply_parse_dev(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len,
     A.buf = buf; A.buf_len = buf_len; A.frame_off = frame_off; A.frame_group = frame_group; A.frame_peer = frame_peer;
     A.window_base = window_base; A.n_frames = n_frames; A.G = n_groups; A.reply_variant = reply_variant; A.with_size = with_size ? 1u : 0u;
     A.rec_group = rec_group; A.rec_slot = rec_slot; A.rec_peer = rec_peer; A.rec_ballot = rec_ballot; A.rec_kind = rec_kind;
-    accept_reply_parse_kernel<<<wire_grid(ctx, n_frames, kWireThreads), kWireThreads, 0, ctx->stream>>>(A);
+    accept_reply_parse_kernel<<<launch_grid(ctx, n_frames, kWireThreads), kWireThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
 }
 
@@ -531,7 +523,7 @@ int ss_prepare_reply_parse_dev(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len
     PrepParseArgs A;
     A.buf = buf; A.buf_len = buf_len; A.frame_off = frame_off; A.n_frames = n_frames;
     A.d = data_shards; A.T = total_shards; A.reply_variant = reply_variant; A.rec = rec;
-    prepare_reply_parse_kernel<<<wire_grid(ctx, n_frames, kWireThreads), kWireThreads, 0, ctx->stream>>>(A);
+    prepare_reply_parse_kernel<<<launch_grid(ctx, n_frames, kWireThreads), kWireThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
 }
 
@@ -542,7 +534,7 @@ int ss_wal_commit_pack_dev(ss_ctx *ctx, const uint64_t *newly, const uint64_t *w
     if (!newly || !window_base || !entries || !entry_group || !entry_len || !n_entries) return set_error(SS_ERR_INVALID_ARG, "null buffer");
     SS_CUDA(cudaMemsetAsync(n_entries, 0, 8, ctx->stream));
     if (n_groups == 0) return SS_OK;
-    wal_commit_pack_kernel<<<wire_grid(ctx, n_groups, kWireThreads), kWireThreads, 0, ctx->stream>>>(
+    wal_commit_pack_kernel<<<launch_grid(ctx, n_groups, kWireThreads), kWireThreads, 0, ctx->stream>>>(
         newly, window_base, n_groups, commit_variant, entries, entry_group, entry_len, capacity, reinterpret_cast<unsigned long long *>(n_entries));
     return launched(ctx);
 }
@@ -563,7 +555,7 @@ int ss_reconstruct_serve_dev(ss_ctx *ctx, const uint8_t *shard_planes, uint64_t 
     A.planes = shard_planes; A.plane_stride = plane_stride; A.shard_stride = shard_stride; A.T = total_shards; A.L = shard_len;
     A.req_group = req_group; A.req_held = req_held; A.req_excl = req_excl; A.req_status = req_status; A.reply_off = reply_off;
     A.n = n_requests; A.reply_mask = reply_mask; A.out = out;
-    reconstruct_serve_kernel<<<wire_grid(ctx, n_requests, kWireThreads / 32), kWireThreads, 0, ctx->stream>>>(A);
+    reconstruct_serve_kernel<<<launch_grid(ctx, n_requests, kWireThreads / 32), kWireThreads, 0, ctx->stream>>>(A);
     return launched(ctx);
 }
 

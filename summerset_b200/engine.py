@@ -507,17 +507,7 @@ class Acceptor:
         """Executes the committed instances handle_logged_commit_slot would: payloads into out (uint8, 16-byte aligned,
         one round_up(data_len, 16) region each).  Returns device tensors rec_group (int32), rec_slot, rec_off (int64),
         rec_len (int32), each [rec_capacity], and totals (int64 [2]: records and bytes asked for)."""
-        assert out.dtype == torch.uint8 and out.is_contiguous()
-        dev = out.device
-        res = dict(rec_group=torch.empty(rec_capacity, dtype=torch.int32, device=dev),
-                   rec_slot=torch.empty(rec_capacity, dtype=torch.int64, device=dev),
-                   rec_off=torch.empty(rec_capacity, dtype=torch.int64, device=dev),
-                   rec_len=torch.empty(rec_capacity, dtype=torch.int32, device=dev),
-                   totals=torch.empty(2, dtype=torch.int64, device=dev))
-        p = lambda x: x.data_ptr()
-        check(self.lib.ss_acceptor_execute(self.h, p(out), out.numel() if out_capacity is None else out_capacity, p(res["rec_group"]),
-                                           p(res["rec_slot"]), p(res["rec_off"]), p(res["rec_len"]), rec_capacity, p(res["totals"])))
-        return res
+        return _execute(self.lib.ss_acceptor_execute, self.h, out, rec_capacity, out_capacity)
 
     def reconstruct_serve(self, buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor, frame_peer: torch.Tensor,
                           out: torch.Tensor, out_capacity: Optional[int] = None, reconstruct_variant: int = 4,

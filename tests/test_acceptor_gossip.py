@@ -466,7 +466,7 @@ def test_reaccept_defines_assign_rows(ctx):
 
 
 def _warp_cap(ctx):
-    return ctx.sm_count * 64 * 8          # acc_grid: 64 CTAs per SM, 8 warps per CTA
+    return ctx.sm_count * 64 * 8          # launch_grid: 64 CTAs per SM, 8 warps per CTA
 
 
 @pytest.mark.gpu

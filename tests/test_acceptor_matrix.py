@@ -312,7 +312,7 @@ def test_acceptor_widest_reply_and_data_len_bound(ctx, oracle):
 # D: batch sizes, scan tiles and grid caps
 # ---------------------------------------------------------------------------------------------
 def _copy_cap(ctx):
-    return ctx.sm_count * 64 * 8          # acc_grid: 64 CTAs per SM; the copy kernel runs 8 warps (frames) per CTA
+    return ctx.sm_count * 64 * 8          # launch_grid: 64 CTAs per SM; the copy kernel runs 8 warps (frames) per CTA
 
 
 def _thread_cap(ctx):

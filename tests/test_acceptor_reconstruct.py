@@ -722,7 +722,7 @@ def test_absorb_exec_bar_and_stale_ballot(ctx):
 
 
 def _warp_cap(ctx):
-    return ctx.sm_count * 64 * 8          # acc_grid: 64 CTAs per SM, 8 warps per CTA: frames / segments per sweep
+    return ctx.sm_count * 64 * 8          # launch_grid: 64 CTAs per SM, 8 warps per CTA: frames / segments per sweep
 
 
 def _thread_cap(ctx):

@@ -1,9 +1,9 @@
 """CRaft execution's shard decode: the bytes executed are the bytes proposed, on every CRaft path that decodes.
 
-Three kernels turn CRaft shards back into request batches through warp_exec_payload (csrc/exec_payload.cuh):
-craft_exec_payload_kernel (the leader before any step-up, every shard held), craft_exec_regen_kernel (the leader once
-the recon view is taken: shard j at shard_addr + j * plane_stride, the sources of a missing data shard the first d held
-shards) and fol_exec_payload_kernel (the follower: held shard of rank k at shard_addr + k * pitch(L)).  Every record is
+Three instances of exec_payload_kernel (csrc/exec_walk.cuh) turn CRaft shards back into request batches through
+warp_exec_payload: CraftShards<false> (the leader before any step-up, every shard held), CraftShards<true> (the leader
+once the recon view is taken: shard j at shard_addr + j * plane_stride, the sources of a missing data shard the first d
+held shards) and FolLog (the follower: held shard of rank k at shard_addr + k * pitch(L)).  Every record is
 compared with the request batch it was proposed from and with the C oracle's Reed-Solomon reconstruct fed the first d
 held shards; the CPU tier pins the restatement in tests/test_craft_execute.py to the same oracle.
 
@@ -108,8 +108,8 @@ def _no_status(ctx):
 @pytest.mark.parametrize("n", range(3, 13))
 def test_leader_decodes_every_held_mask(n):
     """G = every mask + 1 groups, entry k of group g of length lengths[(g + k) % K]: one execute call covers every
-    (mask, length) cell.  The fully held log runs through craft_exec_payload_kernel before the recon view and through
-    craft_exec_regen_kernel after it, byte-identically; then each group's mask is written into held, the planes of
+    (mask, length) cell.  The fully held log runs through the gather-only payload kernel before the recon view and
+    through the regenerating one after it, byte-identically; then each group's mask is written into held, the planes of
     the shards it lacks are poisoned, and the regen kernel must still execute the batches."""
     import torch
     from summerset_b200.engine import RaftEngine
@@ -149,10 +149,10 @@ def test_leader_decodes_every_held_mask(n):
     # the same fully held log through both kernels
     every = walk(state(lambda g, s: full), G * K, 1 << 40)
     assert len(every["records"]) == G * K
-    o_a, out_a = run(every)                                       # craft_exec_payload_kernel
+    o_a, out_a = run(every)                                       # the gather-only payload kernel
     rv = eng.recon_view()
     assert (rv["held"][:, 1:K + 1] == full).all()
-    o_b, out_b = run(every)                                       # craft_exec_regen_kernel, every mask full
+    o_b, out_b = run(every)                                       # the regenerating payload kernel, every mask full
     assert np.array_equal(out_a, out_b) and all(np.array_equal(o_a[k], o_b[k]) for k in o_a)
     # each group's mask, the other shards' plane slots poisoned
     hv = np.zeros((G, W), dtype=np.int64)
@@ -257,7 +257,7 @@ def _propose_np(eng, lens, rng, stride):
 
 @pytest.mark.gpu
 def test_leader_regen_past_the_payload_grid_cap():
-    """sm_count * 64 * 8 + 4099 records in one call, more than the capped grid of craft_exec_regen_kernel has warps:
+    """sm_count * 64 * 8 + 4099 records in one call, more than the capped grid of the regenerating payload kernel has warps:
     two entries per group (one in the last group), full and partial masks mixed, the planes of the missing shards
     poisoned"""
     import torch
@@ -318,9 +318,9 @@ def _sample_check(out, rec_off, rec_len, src, src_off, held, d, p, rng):
 
 @pytest.mark.gpu
 def test_leader_past_the_group_grid_cap():
-    """sm_count * 64 * 256 + 1000 groups, more than the capped grids of craft_exec_count_kernel and
-    craft_exec_place_kernel have threads: one short entry per group, some not proposed and some not committed, so the
-    group scan places records unevenly; craft_exec_payload_kernel strides past its cap too"""
+    """sm_count * 64 * 256 + 1000 groups, more than the capped grids of the leader's exec_count_kernel and
+    exec_place_kernel have threads: one short entry per group, some not proposed and some not committed, so the
+    group scan places records unevenly; the gather-only payload kernel strides past its cap too"""
     import torch
     from summerset_b200.engine import RaftEngine
     ctx = tx._ctx()
@@ -351,8 +351,8 @@ def test_leader_past_the_group_grid_cap():
 
 @pytest.mark.gpu
 def test_follower_past_the_group_grid_cap():
-    """sm_count * 64 * 256 + 1000 groups, more than the capped grids of fol_exec_count_kernel and fol_exec_place_kernel
-    have threads, and far more records than fol_exec_payload_kernel's capped grid has warps: one short entry per group
+    """sm_count * 64 * 256 + 1000 groups, more than the capped grids of the follower's exec_count_kernel and
+    exec_place_kernel have threads, and far more records than its exec_payload_kernel's capped grid has warps: one short entry per group
     installed through the views, held masks of every decodable kind, some of d - 1 shards (the walk stops) and some
     not committed; entries 16 bytes past a 32-byte boundary, slot pads poisoned"""
     import torch

@@ -4,7 +4,7 @@
 `walk` restates both execution walks -- the leader's (the execution half of handle_msg_append_entries_reply's success
 branch, craft/messages.rs:316-359) and the follower's (handle_msg_append_entries, craft/messages.rs:198-240) -- with the
 record placement, the capacity cuts and last_exec of ss_acceptor_execute's contract.  `payload` restates the payload
-warp (csrc/exec_payload.cuh): 16-byte output columns gathered across shard boundaries, a missing data shard regenerated
+warp (csrc/exec_walk.cuh): 16-byte output columns gathered across shard boundaries, a missing data shard regenerated
 with the inverse of M[first d held shards].  The leader's and the follower's per-message restatements and the bincode
 encoders come from tests/test_craft_leader.py and tests/test_follower.py.  GPU tests compare every record, offset, zero
 pad, last_exec and payload byte with the restatement and with the request batches themselves.
