@@ -899,6 +899,59 @@ int ss_acceptor_prepare(ss_acceptor *acceptor, const uint8_t *buf, uint64_t buf_
 int ss_acceptor_prepare_reply(ss_acceptor *acceptor, const uint32_t *rec_group, const uint64_t *rec_slot, uint64_t n_records,
                               uint32_t reply_variant, uint8_t *out, uint64_t out_capacity, uint64_t *reply_off,
                               uint64_t *reply_len, uint8_t *reply_dst, uint64_t *total);
+/* WAL recovery on the acceptor: recover_apply_entry and recover_from_wal (rspaxos/recovery.rs:10-181,
+ * crossword/recovery.rs:10-186) for the records the acceptor writes -- WalEntry::PrepareBal{slot, ballot}
+ * (ss_acceptor_prepare), AcceptData{slot, ballot, reqs_cw[, assignment]} (ss_acceptor_accept) and CommitSlot{slot}
+ * (ss_wal_commit_pack_dev) -- replayed into the window and the shard store without a record crossing to the host.
+ * Record i is at buf + rec_off[i] (any byte alignment) as the device writes it: an 8-byte big-endian length, then the
+ * bincode WalEntry, whose variant is prepare_variant (PrepareBal, 0), cfg.wal_variant (AcceptData, 1) or commit_variant
+ * (CommitSlot, 2); the three must differ.  Record i belongs to group rec_group[i]; a group's records are replayed in
+ * array order, which is WAL order, on top of the state the acceptor holds (normally a fresh acceptor whose window_base
+ * the host installed from the snapshot's start_slot); groups are independent.
+ *   PrepareBal: inst_bal = ballot, Status::Preparing (also over Accepting or Committed).
+ *   AcceptData: inst_bal = ballot, Status::Accepting (also out of Committed), held = the record's shards with its
+ *               data_len, voted = (ballot, held); Crossword: assignment[me] and the whole row set into assign_rows.  The
+ *               record is decoded by the rules ss_acceptor_accept applies to the Accept body (code, shard_len, shard
+ *               lengths, assignment shape, non-minimal varints).
+ *   CommitSlot: Status::Committed (also on a null position, as the reference does).
+ * A position that was null (neither Preparing, Accepting nor Committed) when a record first touches it starts as a
+ * fresh null_instance(): inst_bal 0, no shards, data_len 0, voted None (Crossword: empty assignment), so a retired
+ * position leaks nothing into the replay.  Every position a record touches gets source 0xff and trigger / span 0
+ * (replica_bk is None after recovery).  bal_max_seen[g] = max(before, the ballot of every applied record).
+ * commit_bar, exec_bar and gossip_bar are not changed.
+ * Shards: of the applied AcceptData records of one (group, slot) the last defines the instance; only its shards are
+ * copied into `store`, popcount(held) * SS_CW_SLOT_PITCH(L) bytes in the padded layout ss_acceptor_accept writes, and
+ * shard_addr names that copy.  Regions are placed by an exclusive scan in (group, window position) order; *total
+ * (device u64, may be NULL) = the store bytes the batch asked for.  store 16-byte aligned.
+ * verdict[i]:
+ *   SS_ACCEPT_VERDICT_ACCEPTED         applied;
+ *   SS_ACCEPT_VERDICT_STALE_SLOT       slot < window_base: ignored, as in the reference;
+ *   SS_ACCEPT_VERDICT_BEYOND_WINDOW    slot >= window_base + 64: this record and every later record of its group are
+ *                                      not applied; the host executes, advances and re-submits them;
+ *   SS_FRAME_KIND_MALFORMED            the length runs past buf_len, trailing bytes, a variant that is none of the
+ *                                      three, a record that fails the accept decode rules, or a group >= n_groups.  For
+ *                                      a valid group the group's log ends there, as the reference's read loop ends at
+ *                                      the first entry it cannot decode and truncates: every later record of the group
+ *                                      gets SS_RECOVER_VERDICT_AFTER_END;
+ *   SS_ACCEPT_VERDICT_STORE_FULL       the capacity cut is per group: a group whose store region ends past
+ *                                      store_capacity applies nothing, its records that would apply get STORE_FULL and
+ *                                      SS_DEV_STATUS_STORE_FULL is set.  The offsets are monotone, so the placed groups
+ *                                      are a prefix in group order; re-submitting the STORE_FULL records finishes the job.
+ * Stated differences from the reference:
+ *   1. the 64-slot window, with the suffix cut and re-submission above (the reference grows its log with null
+ *      instances);
+ *   2. execution is not replayed: the reference executes each contiguous committed prefix as it reads and then sets
+ *      exec_bar = commit_bar; here the host runs ss_acceptor_execute after the call and installs exec_bar as it does
+ *      today.  The two differ only for a slot whose CommitSlot is followed in the same WAL by a PrepareBal or AcceptData
+ *      of that slot: the reference has already executed it, here it waits for a heartbeat to commit it again;
+ *   3. the per-group capacity cut;
+ *   4. bal_prep_sent and bal_prepared are leader words, which the acceptor does not have: they are not recovered.
+ * Cost: the walk and the replay take a thread per group segment, so a batch costs its largest per-group run of records
+ * there; the shard copies take a warp per defining record. */
+#define SS_RECOVER_VERDICT_AFTER_END 0xfffffff9u   /* after a malformed record of its group: the group's log ended */
+int ss_acceptor_recover(ss_acceptor *acceptor, const uint8_t *buf, uint64_t buf_len, const uint64_t *rec_off,
+                        const uint32_t *rec_group, uint64_t n_records, uint32_t prepare_variant, uint32_t commit_variant,
+                        uint8_t *store, uint64_t store_capacity, uint32_t *verdict, uint64_t *total);
 /* Reconstruct requests from the acceptor, for the committed instances it cannot execute from its own shards: Crossword
  * follower gossip (trigger_gossiping with gossip_targets_excl, crossword/gossiping.rs:35-192; the reference runs it on
  * the gossip timer in the groups this replica does not lead, crossword/mod.rs:1150) and the reconstruct half of a new

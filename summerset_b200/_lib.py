@@ -129,6 +129,7 @@ SIGNATURES = {
     "ss_acceptor_prepare_view_get": (_i, [_vp, _vp]),
     "ss_acceptor_prepare": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _u32, _vp, _u64, _vp, _vp, _vp, _u64, _vp, _vp]),
     "ss_acceptor_prepare_reply": (_i, [_vp, _vp, _vp, _u64, _u32, _vp, _u64, _vp, _vp, _vp, _vp]),
+    "ss_acceptor_recover": (_i, [_vp, _vp, _u64, _vp, _vp, _u64, _u32, _u32, _vp, _u64, _vp, _vp]),
     "ss_acceptor_gossip_view_get": (_i, [_vp, _vp]),
     "ss_acceptor_gossip": (_i, [_vp, _vp, _u64, _vp, _u64, _u64, _u32, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp]),
     "ss_acceptor_step_up_reads": (_i, [_vp, _vp, _u64, _u64, _u32, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp]),
@@ -318,6 +319,8 @@ SS_FRAME_KIND_MALFORMED = 0xFFFFFFFF
 SS_RECON_VERDICT_NULL_CODEWORD = 0xFFFFFFF6
 SS_RECON_VERDICT_SHARD_RANGE = 0xFFFFFFF7
 SS_RECON_VERDICT_OUT_FULL = 0xFFFFFFF8
+# verdict of ss_acceptor_recover beside the accept verdicts: after a malformed record of its group
+SS_RECOVER_VERDICT_AFTER_END = 0xFFFFFFF9
 # verdicts of ss_follower_append (beside PeerMsg variant indices and SS_FRAME_KIND_MALFORMED)
 SS_FOLLOWER_VERDICT_ACCEPTED = 0xFFFFFFF0
 SS_FOLLOWER_VERDICT_REJECTED = 0xFFFFFFF1

@@ -77,6 +77,7 @@
 #include <cstring>
 #include <new>
 
+#include "acceptor_state.hpp"
 #include "codeword_wire.cuh"
 #include "device_common.cuh"
 #include "exec_walk.cuh"
@@ -87,18 +88,6 @@
 #include "wire_common.cuh"
 
 namespace ssb {
-
-// one decoded Accept frame (ss_acceptor_accept)
-struct FrameHdr {
-    uint64_t slot, ballot;
-    uint64_t end;                   // frame bytes: 8-byte length prefix + body
-    uint32_t kind;                  // verdict so far
-    uint32_t held, dlen, L;
-    uint32_t slot_at;               // offset of the `slot` varint inside the frame
-    uint32_t tags_at;               // offset of shard 0's Option tag
-    uint32_t asg;                   // Crossword: assignment[me]
-    uint32_t asg_at;                // Crossword: offset of assignment[0] inside the frame
-};
 
 // one decoded ReconstructReply frame (ss_acceptor_absorb); it lives in the FrameHdr scratch, which is at least as large
 struct ReplyHdr {
@@ -120,46 +109,7 @@ struct PrepHdr {
     uint32_t pad;
 };
 static_assert(sizeof(PrepHdr) <= sizeof(FrameHdr) && alignof(PrepHdr) <= alignof(FrameHdr), "PrepHdr reuses FrameHdr scratch");
-
-}  // namespace ssb
-
-struct ss_acceptor {
-    ss_ctx *ctx = nullptr;
-    ss_acceptor_config cfg{};
-    uint64_t G = 0;
-    uint64_t *window_base = nullptr, *bal_max_seen = nullptr, *inst_bal = nullptr, *accepting = nullptr, *shard_addr = nullptr;
-    uint32_t *held = nullptr, *data_len = nullptr, *assignment = nullptr;
-    uint8_t *source = nullptr;
-    uint64_t *committed = nullptr, *commit_bar = nullptr, *exec_bar = nullptr;
-    // Prepare: Status::Preparing (ring word), inst.voted = (voted_bal, voted_mask), replica_bk's trigger_slot and
-    // endprep_slot - trigger_slot
-    uint64_t *preparing = nullptr, *voted_bal = nullptr, *prep_trigger = nullptr;
-    uint32_t *voted_mask = nullptr;
-    uint8_t *prep_span = nullptr;
-    // Crossword follower gossip: the instance's whole assignment ([G*64][population] rows) and gossip_bar ([G])
-    uint32_t *assign_rows = nullptr;
-    uint64_t *gossip_bar = nullptr;
-    uint8_t *matrix = nullptr;      // [T*d] the coder's coding matrix (gf256.hpp), row-major
-    uint64_t *ex_cnt = nullptr, *ex_bytes = nullptr, *ex_partials = nullptr, *ex_n = nullptr;   // execute scratch
-    // per-call scratch, grow-only
-    uint64_t cap_frames = 0;
-    ssb::FrameHdr *hdr = nullptr;
-    uint32_t *keys = nullptr;       // [2][cap]: sort keys in / out
-    uint32_t *idx = nullptr;        // [2][cap]: frame indices in / out
-    uint64_t *partials = nullptr;   // [scan_tiles(cap)]
-    uint64_t *fcnt = nullptr;       // [cap]: ss_acceptor_prepare's per-frame record counts, then their scan
-    void *sort_tmp = nullptr;
-    size_t sort_tmp_bytes = 0;
-    uint64_t *totals = nullptr;     // [2] when the caller passes none
-};
-
-namespace ssb {
-
-constexpr int kAccThreads = 256;
 static_assert(kAccThreads == kExecThreads, "the warp kernels run kExecWarps warps per kAccThreads-thread CTA");
-constexpr uint32_t kPending = 0xfffffffeu;          // in the window, ballot not yet checked
-constexpr uint32_t kVariantLimit = 1u << 16;        // no enum of the protocol has this many variants: malformed
-constexpr uint64_t kMaxFrameBody = 0xffffffffull - 64u;   // longer frames are malformed: every record length fits a u32
 
 struct AccArgs {
     const uint8_t *buf;
@@ -195,91 +145,15 @@ struct AccArgs {
     uint32_t *status;
 };
 
-__device__ __forceinline__ uint64_t store_bytes(const FrameHdr &h) {
-    return static_cast<uint64_t>(__popc(h.held)) * SS_CW_SLOT_PITCH(h.L);
-}
 __device__ __forceinline__ uint64_t wal_bytes(const FrameHdr &h, uint32_t wal_variant) {
     return 8u + static_cast<uint64_t>(wv_len(wal_variant)) + (h.end - h.slot_at);
-}
-
-// decodes frame i as ssor_decode_accept reads it, plus the acceptor's own checks (code, shard_len, assignment shape)
-__device__ __forceinline__ FrameHdr decode_frame(const AccArgs &A, uint64_t i) {
-    FrameHdr h{};
-    h.kind = SS_FRAME_KIND_MALFORMED;
-    const uint32_t grp = A.frame_group[i];
-    const uint64_t off = A.frame_off[i];
-    if (grp >= A.G || off > A.buf_len || A.buf_len - off < 8u) return h;
-    const uint8_t *fr = A.buf + off;
-    uint64_t len = 0;
-    for (int b = 0; b < 8; ++b) len = (len << 8) | fr[b];
-    if (len > A.buf_len - off - 8u || len > kMaxFrameBody) return h;
-    const uint8_t *b = fr + 8;
-    uint64_t n = 0, v = 0;
-    uint32_t c;
-#define SS_GET(dst) do { if (!(c = wv_get(b + n, len - n, (dst)))) return h; n += c; } while (0)
-    SS_GET(v);
-    if (v != 0u) {                                                          // LeaseMsg / Leave / LeaveReply
-        if (v < kVariantLimit) h.kind = 0x80000000u | static_cast<uint32_t>(v);
-        return h;
-    }
-    SS_GET(v);
-    if (v != A.accept_variant) {                                            // another PeerMsg: the host's business
-        if (v < kVariantLimit) h.kind = static_cast<uint32_t>(v);
-        return h;
-    }
-    h.slot_at = static_cast<uint32_t>(8u + n);
-    SS_GET(h.slot);
-    SS_GET(h.ballot);
-    if (len - n < 2u || b[n] != A.d || b[n + 1] != A.T - A.d) return h;   // num_data_shards, num_parity_shards
-    n += 2;
-    uint64_t dl = 0, sl = 0;
-    SS_GET(dl);
-    SS_GET(sl);
-    SS_GET(v);
-    if (dl > 0xffffffffull || v != A.T || sl != (dl + A.d - 1u) / A.d) return h;   // rscoding.rs:177-181
-    h.tags_at = static_cast<uint32_t>(8u + n);
-    uint32_t held = 0;
-    for (uint32_t j = 0; j < A.T; ++j) {
-        if (n >= len) return h;
-        const uint8_t tag = b[n++];
-        if (tag == 0u) continue;
-        if (tag != 1u) return h;
-        SS_GET(v);
-        if (v != sl || len - n < sl) return h;
-        held |= 1u << j;
-        n += sl;
-    }
-    if (n >= len || b[n++] != 0u) return h;                                 // data_copy: None
-    if (A.crossword) {                                                      // assignment: Vec<Bitmap>, one row per replica
-        SS_GET(v);
-        if (v != A.population) return h;
-        h.asg_at = static_cast<uint32_t>(8u + n);
-        for (uint32_t r = 0; r < A.population; ++r) {
-            uint64_t sz = 0, nb = 0, blk = 0;
-            SS_GET(sz);
-            SS_GET(nb);
-            if (sz != A.T || nb != 1u) return h;
-            SS_GET(blk);
-            if (blk >> A.T) return h;
-            if (r == A.me) h.asg = static_cast<uint32_t>(blk);
-        }
-    }
-#undef SS_GET
-    if (n != len) return h;
-    h.end = 8u + len;
-    h.held = held;
-    h.dlen = static_cast<uint32_t>(dl);
-    h.L = static_cast<uint32_t>(sl);
-    const uint64_t base = A.window_base[grp];
-    h.kind = h.slot < base ? SS_ACCEPT_VERDICT_STALE_SLOT : h.slot - base >= 64u ? SS_ACCEPT_VERDICT_BEYOND_WINDOW : kPending;
-    return h;
 }
 
 // 1. a thread per frame: decode, filter, region sizes (0 for frames that cannot be accepted), sort keys
 __global__ void __launch_bounds__(kAccThreads) acceptor_header_kernel(const __grid_constant__ AccArgs A) {
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kAccThreads;
     for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kAccThreads + threadIdx.x; i < A.n; i += stride) {
-        const FrameHdr h = decode_frame(A, i);
+        const FrameHdr h = decode_frame<false>(A, i);
         A.hdr[i] = h;
         const bool pending = h.kind == kPending;
         A.store_off[i] = pending ? store_bytes(h) : 0ull;
@@ -357,14 +231,7 @@ __global__ void __launch_bounds__(kAccThreads) acceptor_place_kernel(const __gri
                         if (A.assignment != nullptr) {
                             A.assignment[at] = h.asg;
                             // the whole assignment, re-read from the rows the header pass validated
-                            const uint8_t *rb = A.buf + A.frame_off[i] + h.asg_at;
-                            uint64_t q = 0, sz = 0, nb = 0, blk = 0;
-                            for (uint32_t r = 0; r < A.population; ++r) {
-                                q += wv_get(rb + q, h.end - h.asg_at - q, sz);
-                                q += wv_get(rb + q, h.end - h.asg_at - q, nb);
-                                q += wv_get(rb + q, h.end - h.asg_at - q, blk);
-                                A.assign_rows[at * A.population + r] = static_cast<uint32_t>(blk);
-                            }
+                            read_assign_rows(A.buf + A.frame_off[i] + h.asg_at, h.end - h.asg_at, A.population, A.assign_rows, at * A.population);
                         }
                         A.voted_bal[at] = h.ballot;                     // inst.voted = (ballot, reqs_cw as accepted)
                         A.voted_mask[at] = h.held;
@@ -1605,7 +1472,7 @@ __global__ void __launch_bounds__(kAccThreads) request_write_kernel(const __grid
     if (full && lane == 0u) atomicOr(A.status, SS_DEV_STATUS_FRAME_OVERFLOW);
 }
 
-static int ensure_scratch(ss_acceptor *a, uint64_t n) {
+int acc_scratch(ss_acceptor *a, uint64_t n) {
     if (n <= a->cap_frames) return SS_OK;
     ss_ctx *ctx = a->ctx;
     SS_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -1723,7 +1590,7 @@ int ss_acceptor_heartbeat(ss_acceptor *a, const uint32_t *hb_group, const uint8_
     if (n == 0) return SS_OK;
     if (!hb_group || !hb_peer || !hb_ballot || !hb_commit_bar || !hb_exec_bar) return set_error(SS_ERR_INVALID_ARG, "null buffer");
     if (n > 0x7fffffffull) return set_error(SS_ERR_INVALID_ARG, "at most 2^31 - 1 records per call");
-    SS_TRY(ensure_scratch(a, n));
+    SS_TRY(acc_scratch(a, n));
     HbArgs H{};
     H.group = hb_group; H.peer = hb_peer; H.ballot = hb_ballot; H.hb_commit_bar = hb_commit_bar; H.hb_exec_bar = hb_exec_bar;
     H.n = n; H.G = a->G; H.me = a->cfg.me;
@@ -1796,7 +1663,7 @@ int ss_acceptor_accept(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, con
     if ((reinterpret_cast<uintptr_t>(store) | reinterpret_cast<uintptr_t>(wal)) & 15u)
         return set_error(SS_ERR_INVALID_ARG, "store and wal must be 16-byte aligned");
     if (n > 0x7fffffffull) return set_error(SS_ERR_INVALID_ARG, "at most 2^31 - 1 frames per call");
-    SS_TRY(ensure_scratch(a, n));
+    SS_TRY(acc_scratch(a, n));
     uint64_t *tot = totals != nullptr ? totals : a->totals;
     AccArgs A{};
     A.buf = buf; A.buf_len = buf_len; A.frame_off = frame_off; A.frame_group = frame_group; A.frame_peer = frame_peer;
@@ -1857,7 +1724,7 @@ int ss_acceptor_reconstruct_serve(ss_acceptor *a, const uint8_t *buf, uint64_t b
         return set_error(SS_ERR_INVALID_ARG, "null buffer");
     if (reinterpret_cast<uintptr_t>(out) & 15u) return set_error(SS_ERR_INVALID_ARG, "out must be 16-byte aligned");
     if (n > 0x7fffffffull) return set_error(SS_ERR_INVALID_ARG, "at most 2^31 - 1 frames per call");
-    SS_TRY(ensure_scratch(a, n));
+    SS_TRY(acc_scratch(a, n));
     RecArgs R = rec_args(a, buf, buf_len, frame_off, frame_group, n, reconstruct_variant);
     R.reply_variant = reply_variant; R.out = out; R.out_cap = out_capacity; R.reply_off = reply_off; R.reply_len = reply_len;
     R.verdict = verdict;
@@ -1882,7 +1749,7 @@ int ss_acceptor_absorb(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, con
     if (!buf || !frame_off || !frame_group || !frame_peer || !store || !absorbed || !verdict) return set_error(SS_ERR_INVALID_ARG, "null buffer");
     if (reinterpret_cast<uintptr_t>(store) & 15u) return set_error(SS_ERR_INVALID_ARG, "store must be 16-byte aligned");
     if (n > 0x7fffffffull) return set_error(SS_ERR_INVALID_ARG, "at most 2^31 - 1 frames per call");
-    SS_TRY(ensure_scratch(a, n));
+    SS_TRY(acc_scratch(a, n));
     RecArgs R = rec_args(a, buf, buf_len, frame_off, frame_group, n, reply_variant);
     R.rhdr = reinterpret_cast<ReplyHdr *>(a->hdr);   // the accept pass's per-frame header scratch, reused
     R.key_in = a->keys; R.idx_in = a->idx; R.key = a->keys + n; R.idx = a->idx + n;
@@ -1928,7 +1795,7 @@ int ss_acceptor_prepare(ss_acceptor *a, const uint8_t *buf, uint64_t buf_len, co
         return set_error(SS_ERR_INVALID_ARG, "null buffer");
     if (reinterpret_cast<uintptr_t>(wal) & 15u) return set_error(SS_ERR_INVALID_ARG, "wal must be 16-byte aligned");
     if (n > 0x7fffffffull) return set_error(SS_ERR_INVALID_ARG, "at most 2^31 - 1 frames per call");
-    SS_TRY(ensure_scratch(a, n));
+    SS_TRY(acc_scratch(a, n));
     PrepArgs P{};
     P.buf = buf; P.buf_len = buf_len; P.frame_off = frame_off; P.frame_group = frame_group; P.frame_peer = frame_peer;
     P.n = n; P.G = a->G; P.me = a->cfg.me; P.variant = prepare_variant; P.wal_variant = wal_variant;
@@ -1971,7 +1838,7 @@ int ss_acceptor_prepare_reply(ss_acceptor *a, const uint32_t *rec_group, const u
     if (!rec_group || !rec_slot || !out || !reply_off || !reply_len || !reply_dst) return set_error(SS_ERR_INVALID_ARG, "null buffer");
     if (reinterpret_cast<uintptr_t>(out) & 15u) return set_error(SS_ERR_INVALID_ARG, "out must be 16-byte aligned");
     if (n > 0x7fffffffull) return set_error(SS_ERR_INVALID_ARG, "at most 2^31 - 1 records per call");
-    SS_TRY(ensure_scratch(a, n));
+    SS_TRY(acc_scratch(a, n));
     PrepReplyArgs R{};
     R.rec_group = rec_group; R.rec_slot = rec_slot; R.n = n; R.G = a->G;
     R.d = a->cfg.data_shards; R.T = a->cfg.total_shards; R.variant = reply_variant;
@@ -2015,7 +1882,7 @@ static int acceptor_requests(ss_acceptor *a, bool step_up, const uint32_t *group
     if (!out || !frame_group || !frame_dst || !frame_off || !frame_len) return set_error(SS_ERR_INVALID_ARG, "null buffer");
     if (reinterpret_cast<uintptr_t>(out) & 15u) return set_error(SS_ERR_INVALID_ARG, "out must be 16-byte aligned");
     if (n > 0x7fffffffull) return set_error(SS_ERR_INVALID_ARG, "at most 2^31 - 1 listed groups per call");
-    SS_TRY(ensure_scratch(a, n));
+    SS_TRY(acc_scratch(a, n));
     ReqArgs R{};
     R.groups = groups; R.peer_alive = peer_alive; R.n = n; R.G = a->G; R.tail = tail_ignores; R.batch = batch < 64u ? batch : 64u;
     R.me = a->cfg.me; R.population = a->cfg.population; R.d = a->cfg.data_shards; R.T = a->cfg.total_shards; R.variant = variant;

@@ -580,6 +580,23 @@ class Acceptor:
                                                  p(res["reply_len"]), p(res["reply_dst"]), p(res["total"])))
         return res
 
+    def recover(self, buf: torch.Tensor, rec_off: torch.Tensor, rec_group: torch.Tensor, store: torch.Tensor,
+                store_capacity: Optional[int] = None, prepare_variant: int = 0, commit_variant: int = 2) -> dict:
+        """Replays WAL records (recover_apply_entry): buf uint8 holds PrepareBal, AcceptData and CommitSlot records as the
+        device wrote them (8-byte big-endian length + bincode WalEntry, any alignment), record i at rec_off[i] (int64) of
+        group rec_group[i] (int32), each group's records in WAL order.  The defining AcceptData shards go to store (uint8,
+        16-byte aligned, caller-owned; keep it alive while the instances hold it).  Returns device tensors verdict (int32
+        [n]) and total (int64 [1]: the store bytes the batch asked for)."""
+        assert buf.dtype == torch.uint8 and rec_off.dtype == torch.int64 and rec_group.dtype == torch.int32
+        assert store.dtype == torch.uint8 and rec_group.numel() == rec_off.numel()
+        n, dev = rec_off.numel(), buf.device
+        res = dict(verdict=torch.empty(n, dtype=torch.int32, device=dev), total=torch.empty(1, dtype=torch.int64, device=dev))
+        p = lambda x: x.data_ptr()
+        check(self.lib.ss_acceptor_recover(self.h, p(buf), buf.numel(), p(rec_off), p(rec_group), n, prepare_variant, commit_variant,
+                                           p(store), store.numel() if store_capacity is None else store_capacity, p(res["verdict"]),
+                                           p(res["total"])))
+        return res
+
     def _requests(self, step_up: bool, out: torch.Tensor, frame_capacity: int, groups: Optional[torch.Tensor], batch: int,
                   out_capacity: Optional[int], reconstruct_variant: int, peer_alive: Optional[torch.Tensor] = None,
                   tail_ignores: int = 0) -> dict:

@@ -353,6 +353,15 @@ class Acceptor {
         check(ss_acceptor_prepare_reply(acc_, rec_group, rec_slot, n_records, reply_variant, out, out_capacity, reply_off, reply_len,
                                         reply_dst, total));
     }
+    // recover_apply_entry over a group-tagged batch of WAL records (PrepareBal variant 0, AcceptData cfg.wal_variant,
+    // CommitSlot variant 2), each group's in WAL order; the defining shards go to store.  A group cut by the window or the
+    // store is finished by re-submitting its unapplied records (see the header)
+    void recover(const uint8_t *buf, uint64_t buf_len, const uint64_t *rec_off, const uint32_t *rec_group, uint64_t n_records,
+                 uint8_t *store, uint64_t store_capacity, uint32_t *verdict, uint64_t *total, uint32_t prepare_variant = 0,
+                 uint32_t commit_variant = 2) {
+        check(ss_acceptor_recover(acc_, buf, buf_len, rec_off, rec_group, n_records, prepare_variant, commit_variant, store,
+                                  store_capacity, verdict, total));
+    }
     // Crossword trigger_gossiping over the listed groups (NULL: all; leave out the groups this replica leads):
     // Reconstruct frames (variant 4) for peer frame_dst[f]; a capacity cut leaves a prefix of the groups written
     void gossip(const uint32_t *groups, uint64_t n_listed, const uint32_t *peer_alive, uint64_t tail_ignores, uint64_t batch_size,

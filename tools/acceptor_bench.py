@@ -49,7 +49,9 @@ def timed(fn, a):
     return ms
 
 
-def run(ctx, protocol, lens, spr, arena, data_off, a):
+def leader_frames(ctx, protocol, lens, spr, arena, data_off):
+    """the frames for peer 0 that the leader path builds -> (frames, frame_off, frame_len, frame_bytes, d, L, policies,
+    repack: a callable that packs them again)"""
     G = len(lens)
     dev = torch.device("cuda", 0)
     cw = protocol == "crossword"
@@ -89,8 +91,15 @@ def run(ctx, protocol, lens, spr, arena, data_off, a):
     pack(cap)
     assert ctx.device_status() == 0
     frame_bytes = int(fl.to(torch.int64).sum())
-    t_pack = timed(lambda: pack(cap), a)
-    del eng
+    return frames, off, fl, frame_bytes, d, L, policies, lambda: pack(cap)
+
+
+def run(ctx, protocol, lens, spr, arena, data_off, a):
+    G = len(lens)
+    dev = torch.device("cuda", 0)
+    cw = protocol == "crossword"
+    frames, off, fl, frame_bytes, d, L, policies, repack = leader_frames(ctx, protocol, lens, spr, arena, data_off)
+    t_pack = timed(repack, a)
     # the acceptor: peer 0's frames where the packer left them (16-byte regions; the shards inside are at any offset)
     acc = Acceptor(ctx, protocol, G, N, 0, d, 5)
     groups = torch.arange(G, dtype=torch.int32, device=dev)
@@ -120,7 +129,7 @@ def run(ctx, protocol, lens, spr, arena, data_off, a):
            "frame_pack": {**stats(t_pack), "bytes": frame_bytes, "GB/s": gbs(frame_bytes, t_pack)},
            "copy": {**stats(t_copy), "bytes": 2 * frame_bytes, "GB/s": gbs(2 * frame_bytes, t_copy)}}
     acc.close()
-    del store, frames, astore, wal, src, dst
+    del repack, frames, astore, wal, src, dst
     torch.cuda.empty_cache()
     return out, ok
 
