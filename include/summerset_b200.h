@@ -1175,7 +1175,8 @@ int ss_follower_append(ss_follower *follower, const uint8_t *buf, uint64_t buf_l
  * message's variant index (0x80000000 | k for PeerMessage variants) or SS_FRAME_KIND_MALFORMED (also a group >=
  * n_groups).  Every record but INGEST gets rec_group UINT32_MAX, which the ingest drops.  rec_term, rec_conflict_term and
  * rec_conflict_slot hold the decoded fields of a frame of one of the four kinds above (the conflict ones 0 for a
- * success reply); every field is 0 for another message or a malformed frame. */
+ * success reply); every field is 0 for another message or a malformed frame.  reply_variant < 2^16 (SS_ERR_INVALID_ARG
+ * otherwise, before any other check), as for ss_engine_craft_backoff. */
 #define SS_APPEND_REPLY_INGEST 0xfffffff0u
 #define SS_APPEND_REPLY_CONFLICT 0xfffffff1u
 #define SS_APPEND_REPLY_HIGHER_TERM 0xfffffff2u

@@ -610,6 +610,9 @@ int ss_append_reply_parse_dev(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len,
                               const uint8_t *frame_peer, const uint32_t *curr_term, uint64_t n_frames, uint64_t n_groups,
                               uint32_t reply_variant, uint32_t *rec_group, uint8_t *rec_peer, uint32_t *rec_end_slot,
                               uint64_t *rec_term, uint64_t *rec_conflict_term, uint64_t *rec_conflict_slot, uint32_t *rec_kind) {
+    // a frame's variant >= 2^16 is malformed, so no index from there on can name the reply (ss_engine_craft_backoff, which
+    // takes the same reply_variant, refuses it too)
+    if (reply_variant >= kFolVariantLimit) return set_error(SS_ERR_INVALID_ARG, "reply_variant must be < 2^16");
     if (ctx == nullptr) return set_error(SS_ERR_INVALID_ARG, "null context");
     SS_TRY(ctx_bind(ctx));
     if (n_frames == 0) return SS_OK;

@@ -52,9 +52,10 @@ def metadata(term, voted_for, variant=0) -> bytes:
 class Node(tf.Group):
     """one group's follower state at replica `me`, with the election words; returns what each message produces"""
 
-    def __init__(self, n, W, me):
-        super().__init__(n, W)
+    def __init__(self, n, W, me, request_vote_variant=RV, reply_variant=RVR, meta_variant=0):
+        super().__init__(n, W, meta_variant=meta_variant)
         self.me, self.maj, self.n = me, n // 2 + 1, n
+        self.rvv, self.rpv = request_vote_variant, reply_variant
         self.vt, self.vf, self.rt, self.role, self.votes = 0, NONE, 0, FOLLOWER, 0
 
     def voted(self):
@@ -75,7 +76,7 @@ class Node(tf.Group):
         self.ldr = self.me
         self.vt, self.vf, self.rt, self.role, self.votes = self.ct, self.me, self.ct, CANDIDATE, 1 << self.me
         last = self.le - 1
-        return DONE, metadata(self.ct, self.me), request_vote(self.ct, last, self.log[last][0])
+        return DONE, metadata(self.ct, self.me, self.mv), request_vote(self.ct, last, self.log[last][0], self.rvv)
 
     def vote(self, cand, term, last_slot, last_term):
         """-> (verdict, meta, reply)"""
@@ -83,21 +84,21 @@ class Node(tf.Group):
         if term > self.ct:                                        # check_term
             self.ct, vf, self.ldr, meta = term, NONE, cand, True
         if term < self.ct:
-            v, rep = DENIED_STALE, vote_reply(self.ct, False)
+            v, rep = DENIED_STALE, vote_reply(self.ct, False, self.rpv)
         elif (vf in (NONE, cand)) and (last_term >= self.log[self.le - 1][0] or (last_term == self.ct and last_slot + 1 >= self.le)):
             vf, meta = cand, True
-            v, rep = GRANTED, vote_reply(self.ct, True)
+            v, rep = GRANTED, vote_reply(self.ct, True, self.rpv)
         else:
             v, rep = NO_REPLY, None
         if meta:
             self.vt, self.vf = self.ct, vf
-        return v, metadata(self.ct, vf) if meta else None, rep
+        return v, metadata(self.ct, vf, self.mv) if meta else None, rep
 
     def tally(self, peer, term, granted):
         """-> (verdict, meta)"""
         if term > self.ct:                                        # check_term: step down
             self.ct, self.ldr, self.vt, self.vf = term, peer, term, NONE
-            return HIGHER, metadata(term, NONE)
+            return HIGHER, metadata(term, NONE, self.mv)
         r = self.role_now()
         if r == ELECTED:
             return ELECTED_ALREADY, None
@@ -306,7 +307,7 @@ def _cells_ok(cells, lens, want, width):
 class _Rig:
     """one device follower (replica `me`) and the restatement of each of its G groups"""
 
-    def __init__(self, n, G, seed):
+    def __init__(self, n, G, seed, request_vote_variant=RV, reply_variant=RVR, meta_variant=0):
         import torch
         from summerset_b200 import _lib
         from summerset_b200.engine import Follower
@@ -315,9 +316,10 @@ class _Rig:
         self.me = self.rng.randrange(n)
         self.ctx = ts._ctx()
         self.lib = self.ctx.lib
-        self.fol = Follower(self.ctx, G, n, self.me, window=self.W)
+        self.rvv, self.rpv = request_vote_variant, reply_variant
+        self.fol = Follower(self.ctx, G, n, self.me, window=self.W, meta_variant=meta_variant)
         self.vv = self.fol.vote_view()
-        self.nodes = [Node(n, self.W, self.me) for _ in range(G)]
+        self.nodes = [Node(n, self.W, self.me, request_vote_variant, reply_variant, meta_variant) for _ in range(G)]
         cts = [0, 1, 2, 5, 250, 251, 300, 70000, (1 << 32) - 2, U32, 1 << 40]
         ct_t, le_t, ld_t = [], [], []
         term = self.fol.term.cpu().numpy()
@@ -364,7 +366,7 @@ class _Rig:
         meta, ml, fr, fl, fd, vd = (_canary(32 * n, torch.uint8), _canary(n, torch.int32), _canary(48 * n, torch.uint8),
                                     _canary(n, torch.int32), _canary(n, torch.uint8), _canary(n, torch.int32))
         p = lambda x: None if x is None else x.data_ptr()
-        self._lib.check(self.lib.ss_follower_campaign(self.fol.h, p(grp), n, p(src), RV, p(meta), p(ml), p(fr), p(fl), p(fd), p(vd)))
+        self._lib.check(self.lib.ss_follower_campaign(self.fol.h, p(grp), n, p(src), self.rvv, p(meta), p(ml), p(fr), p(fl), p(fd), p(vd)))
         torch.cuda.synchronize()
         assert (vd.cpu().numpy()[:n].view(np.uint32) == [v for v, _, _ in want]).all() and _padded_ok(vd, n)
         _cells_ok(meta, ml, [m for _, m, _ in want], 32)
@@ -391,7 +393,7 @@ class _Rig:
         meta, ml, rep, rl, rd, vd = (_canary(32 * n, torch.uint8), _canary(n, torch.int32), _canary(32 * n, torch.uint8),
                                      _canary(n, torch.int32), _canary(n, torch.uint8), _canary(n, torch.int32))
         p = lambda x: x.data_ptr()
-        self._lib.check(self.lib.ss_follower_vote(self.fol.h, p(buf), buf.numel(), p(fo), p(fg), p(fp), n, RV, RVR, p(meta), p(ml),
+        self._lib.check(self.lib.ss_follower_vote(self.fol.h, p(buf), buf.numel(), p(fo), p(fg), p(fp), n, self.rvv, self.rpv, p(meta), p(ml),
                                                   p(rep), p(rl), p(rd), p(vd)))
         torch.cuda.synchronize()
         assert (vd.cpu().numpy()[:n].view(np.uint32) == [w[0] for w in want]).all() and _padded_ok(vd, n)
@@ -414,7 +416,7 @@ class _Rig:
         meta, ml, vd = _canary(32 * n, torch.uint8), _canary(n, torch.int32), _canary(n, torch.int32)
         wg, wt, nw = _canary(G, torch.int32), _canary(G, torch.int64), _canary(1, torch.int64)
         p = lambda x: x.data_ptr()
-        self._lib.check(self.lib.ss_follower_tally(self.fol.h, p(buf), buf.numel(), p(fo), p(fg), p(fp), n, RVR, p(meta), p(ml), p(vd),
+        self._lib.check(self.lib.ss_follower_tally(self.fol.h, p(buf), buf.numel(), p(fo), p(fg), p(fp), n, self.rpv, p(meta), p(ml), p(vd),
                                                    p(wg), p(wt), p(nw)))
         torch.cuda.synchronize()
         assert (vd.cpu().numpy()[:n].view(np.uint32) == [w[0] for w in want]).all() and _padded_ok(vd, n)
@@ -430,14 +432,15 @@ class _Rig:
 def _bad_votes(rig):
     """malformed and other-message RequestVote frames, and their verdicts"""
     G, n, me = rig.G, rig.n, rig.me
-    ok = request_vote(1, 0, 0)
+    ok = request_vote(1, 0, 0, rig.rvv)
     other = (me + 1) % n
+    foreign = 0 if rig.rvv else 1                                  # another PeerMsg (AppendEntries by default)
     return [(0, other, framed(ok[8:-1]), MALFORMED),                             # truncated body
             (0, other, framed(ok[8:] + b"\x00"), MALFORMED),                      # a trailing byte
             (1, me, ok, MALFORMED),                                               # from me
             (1, n if n < 32 else 200, ok, MALFORMED),                             # a peer past the population
             (G + 3, other, ok, MALFORMED),                                        # a group past n_groups
-            (2, other, request_vote(1, 0, 0, variant=0), 0),                      # AppendEntries
+            (2, other, request_vote(1, 0, 0, variant=foreign), foreign),          # another PeerMsg
             (2, other, framed(vi(1) + vi(0)), 0x80000001),                        # another PeerMessage
             (2, other, framed(vi(0) + vi(70000)), MALFORMED)]                     # a variant >= 2^16
 
@@ -445,10 +448,11 @@ def _bad_votes(rig):
 def _bad_replies(rig):
     G, n, me = rig.G, rig.n, rig.me
     other = (me + 1) % n
-    ok = vote_reply(1, True)
+    ok = vote_reply(1, True, rig.rpv)
+    foreign = 1 if rig.rpv != 1 else 0
     return [(0, other, framed(ok[8:-1]), MALFORMED), (0, other, framed(ok[8:] + b"\x01"), MALFORMED),
-            (0, other, framed(vi(0) + vi(RVR) + vi(1) + b"\x02"), MALFORMED),    # granted is not a bool
-            (1, me, ok, MALFORMED), (G, other, ok, MALFORMED), (1, other, vote_reply(1, True, variant=1), 1)]
+            (0, other, framed(vi(0) + vi(rig.rpv) + vi(1) + b"\x02"), MALFORMED),    # granted is not a bool
+            (1, me, ok, MALFORMED), (G, other, ok, MALFORMED), (1, other, vote_reply(1, True, variant=foreign), foreign)]
 
 
 def _round(rig, k_vote, k_tally):
@@ -474,7 +478,7 @@ def _round(rig, k_vote, k_tally):
         if rng.random() < 0.2:
             lt = term
         cand = rng.choice(peers)
-        f = (g, cand, request_vote(term, ls, lt), (term, ls, lt))
+        f = (g, cand, request_vote(term, ls, lt, rig.rvv), (term, ls, lt))
         frames.append(f)
         prev.append(f)
     bad = _bad_votes(rig)
@@ -492,13 +496,13 @@ def _round(rig, k_vote, k_tally):
         nd = rig.nodes[g]
         term = max(0, nd.ct + rng.choice([-1, 0, 0, 0, 0, 0, 1] if rng.random() < 0.9 else [3]))
         granted = rng.random() < 0.8
-        f = (g, rng.choice(peers), vote_reply(term, granted), (term, granted))
+        f = (g, rng.choice(peers), vote_reply(term, granted, rig.rpv), (term, granted))
         frames.append(f)
         prev.append(f)
     for g in cands[:len(cands) // 3]:                            # enough granted replies, first, to elect some groups
         ct = rig.nodes[g].ct
         for q in peers:
-            frames.insert(0, (g, q, vote_reply(ct, True), (ct, True)))
+            frames.insert(0, (g, q, vote_reply(ct, True, rig.rpv), (ct, True)))
     for b in _bad_replies(rig):
         frames.insert(rng.randrange(len(frames) + 1), b)
     return rig.tally(frames)
@@ -579,15 +583,16 @@ def _propose(eng, me, lens, stride, keep, batch, rng):
             batch[(g, slots[g])] = bs[g]
 
 
-def _replicate(ctx, eng, me, fols, keep, rng, groups=None):
+def _replicate(ctx, eng, me, fols, keep, rng, groups=None, append_variant=0, reply_variant=1):
     """the leader's entries, then a heartbeat, to every live follower (only the frames of `groups`, None = all: an
-    engine's heartbeat also goes out for the groups it never stepped up); their replies ingested and ticked"""
+    engine's heartbeat also goes out for the groups it never stepped up); their replies ingested and ticked.  The
+    followers must be configured with the same AppendEntries and AppendEntriesReply variants."""
     import torch
     from summerset_b200.engine import append_reply_parse
     dev = "cuda:0"
     for heartbeat in (False, True):
         out = torch.zeros(1 << 22, dtype=torch.uint8, device=dev)
-        o = eng.pack_append(me, out, 1 << 12, heartbeat=heartbeat, msg_chunk_size=4)
+        o = eng.pack_append(me, out, 1 << 12, heartbeat=heartbeat, msg_chunk_size=4, append_variant=append_variant)
         torch.cuda.synchronize()
         nf = int(o["n_frames"][0])
         fo, fg, fp = o["frame_off"][:nf], o["frame_group"][:nf], o["frame_peer"][:nf]
@@ -612,7 +617,7 @@ def _replicate(ctx, eng, me, fols, keep, rng, groups=None):
             continue
         tb, offs = ts._buf([x for _, _, x in replies], rng)
         fo2, fg2 = ts._t(offs, torch.int64), ts._t([x[0] for x in replies], torch.int32)
-        rec = append_reply_parse(ctx, tb, fo2, fg2, ts._t([x[1] for x in replies], torch.uint8), eng.curr_term, eng.G)
+        rec = append_reply_parse(ctx, tb, fo2, fg2, ts._t([x[1] for x in replies], torch.uint8), eng.curr_term, eng.G, reply_variant)
         eng.on_append_replies(rec["rec_group"], rec["rec_peer"], rec["rec_end_slot"])
         eng.tick()
         torch.cuda.synchronize()

@@ -584,6 +584,13 @@ def test_pack_matches_the_restatement(n):
 @pytest.mark.gpu
 @pytest.mark.parametrize("n", [5, 7])
 def test_closed_loop_with_device_followers(n):
+    closed_loop(n)
+
+
+def closed_loop(n, append_variant=0, reply_variant=1, meta_variant=0, log_variant=1, leader_reply_variant=None):
+    """leader 1 packs, device followers append and reply, the leader parses, ingests and backs off, all against the
+    restatements, with the given PeerMsg and DurEntry variant indices.  leader_reply_variant: the followers' replies are
+    re-encoded with this AppendEntriesReply index (one a follower cannot emit, >= 251) before the leader takes them."""
     import torch
     from summerset_b200.engine import Follower, RaftEngine, append_reply_parse
     ctx = _ctx()
@@ -599,8 +606,9 @@ def test_closed_loop_with_device_followers(n):
     for m in L:
         m.ct = term
     reps = [r for r in range(n) if r != me]                       # replica of peer q is reps[q]
-    fols = [Follower(ctx, G, n, r) for r in reps]
-    fmodels = [[tf.Group(n, fols[0].W) for _ in range(G)] for _ in reps]
+    fols = [Follower(ctx, G, n, r, 0, append_variant, reply_variant, meta_variant, log_variant) for r in reps]
+    fmodels = [[tf.Group(n, fols[0].W, reply_variant, meta_variant) for _ in range(G)] for _ in reps]
+    lrv = reply_variant if leader_reply_variant is None else leader_reply_variant
     keep = []                                                     # every store a live entry may point into
     seen = dict(conflict=0, trunc=0)
 
@@ -626,14 +634,15 @@ def test_closed_loop_with_device_followers(n):
             assert cells[i][:rl[i]].tobytes() == want["reply"], (q, g, i)
             seen["trunc"] += want["trunc"] is not None
             assert (int(tr[i]) != -1) == (want["trunc"] is not None)
-            out.append((g, q, want["reply"]))
+            tm, end, conf = tf._parse_reply_py(want["reply"], reply_variant)[1]
+            out.append((g, q, tf.reply(tm, end, conf, lrv)))
         return out
 
     def round_trip(want_np):
         """pack (want_end or all), compare, deliver, parse, ingest, back off -> the next want_end, or None when quiet"""
         out = torch.full((1 << 24,), 0xA5, dtype=torch.uint8, device=dev)
         wt = None if want_np is None else torch.tensor(want_np.view(np.int64), device=dev)
-        o = _pack_raw(eng, me, out, 1 << 24, 1 << 14, wt, chunk=3)
+        o = _pack_raw(eng, me, out, 1 << 24, 1 << 14, wt, chunk=3, variant=append_variant)
         out_np = out.cpu().numpy()
         # the restatement's frames, with their structure for the follower models
         per_q = [[] for _ in range(P)]
@@ -643,7 +652,7 @@ def test_closed_loop_with_device_followers(n):
                 st, frames, nt = m.plan(q, 3, None if want_np is None else int(want_np[q][g]))
                 assert int(o["pair_status"][q * G + g]) == st
                 for f in frames:
-                    x = m.frame_bytes(f)
+                    x = m.frame_bytes(f, append_variant)
                     off = int(o["frame_off"][k])
                     assert out_np[off:off + len(x)].tobytes() == x and o["frame_group"][k] == g and o["frame_peer"][k] == q
                     per_q[q].append((g, x, (f[0], f[1], f[2], m.lc, m.ls)))
@@ -661,19 +670,19 @@ def test_closed_loop_with_device_followers(n):
             buf += x
         tb = t(np.frombuffer(bytes(buf), dtype=np.uint8), torch.uint8)
         fo, fg, fp = t(offs, torch.int64), t([r[0] for r in replies], torch.int32), t([r[1] for r in replies], torch.uint8)
-        rec = append_reply_parse(ctx, tb, fo, fg, fp, eng.curr_term, G)
+        rec = append_reply_parse(ctx, tb, fo, fg, fp, eng.curr_term, G, lrv)
         eng.on_append_replies(rec["rec_group"], rec["rec_peer"], rec["rec_end_slot"])
-        want = eng.backoff(tb, fo, fg, fp, rec["rec_kind"])
+        want = eng.backoff(tb, fo, fg, fp, rec["rec_kind"], lrv)
         torch.cuda.synchronize()
         touched = set()
         for g, q, x in replies:                                   # success replies first, then conflicts in frame order
-            kind, fdec = tf._parse_reply_py(x, 1)
+            kind, fdec = tf._parse_reply_py(x, lrv)
             tm, end, conf = fdec
             if conf is None and L[g].success(q, end):
                 touched.add(g)
         want_model = np.full((P, G), U64, dtype=np.uint64)
         for g, q, x in replies:
-            tm, end, conf = tf._parse_reply_py(x, 1)[1]
+            tm, end, conf = tf._parse_reply_py(x, lrv)[1]
             if conf is not None:
                 seen["conflict"] += 1
                 want_model[q][g] = L[g].conflict(q, end, conf[0], conf[1])
@@ -701,7 +710,7 @@ def test_closed_loop_with_device_followers(n):
             if rng.random() < 0.5:
                 k = rng.randint(1, 3)
                 ents = [tf.Ent(1, d, p, 9, {reps[q]: rng.randbytes(-(-9 // d))}, True, 0) for _ in range(k)]
-                seed.append((g, tf.append_entries(1, 0, 0, [e.wire() for e in ents], 0, 0), (0, 0, ents, 0, 0)))
+                seed.append((g, tf.append_entries(1, 0, 0, [e.wire() for e in ents], 0, 0, append_variant), (0, 0, ents, 0, 0)))
         buf, offs = bytearray(), []
         for g, x, _ in seed:
             offs.append(len(buf))

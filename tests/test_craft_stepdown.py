@@ -114,6 +114,7 @@ class _Rig:
         import torch
         from summerset_b200.engine import Follower, RaftEngine
         self.n, self.G, self.W, self.d, self.me = n, G, W, n // 2 + 1, 1
+        self.meta_variant = 0
         self.ctx = ts._ctx()
         self.rng = rng = random.Random(9000 + n + seed)
         self.fols = {r: Follower(self.ctx, G, n, r, window=W) for r in range(1, n)}
@@ -189,9 +190,10 @@ def _check_deposed(rig, before, groups, term, peer, store, res, i_of, held_all=F
         assert int(F["last_exec"][g]) == max(int(B["last_exec"][g]), eex[g])
         assert int(F["curr_term"][g]) == max(int(B["curr_term"][g]), tt[g]) and int(F["leader"][g]) == peer
         raised = tt[g] > int(B["curr_term"][g])
-        assert ml[i] == (len(te.metadata(tt[g], NONE)) if raised else 0)
+        want_meta = te.metadata(tt[g], NONE, rig.meta_variant)
+        assert ml[i] == (len(want_meta) if raised else 0)
         if raised:
-            assert meta[i][:ml[i]].tobytes() == te.metadata(tt[g], NONE) and not meta[i][ml[i]:].any()
+            assert meta[i][:ml[i]].tobytes() == want_meta and not meta[i][ml[i]:].any()
         for s in range(ns, le):
             p = s % W
             et, dl, h = int(eterms[g][p]), int(edl[g][p]), int(held[g][p])
@@ -399,15 +401,18 @@ def test_fencing_after_step_down_and_through_the_role_view():
 # ---- every message kind, malformed frames, the held-free path, canaries ----------------------------------------------
 class _PlainRig:
     """replica 0 leads every group and was never stepped up (no held masks): two committed rounds of term-1 entries
-    replicated to 1.., one more proposed and not sent; replica 0's own follower is empty"""
+    replicated to 1.., one more proposed and not sent; replica 0's own follower is empty.  Every follower and the
+    replication between them use the given PeerMsg and DurEntry variant indices."""
 
-    def __init__(self, n, G=16, W=32):
+    def __init__(self, n, G=16, W=32, append_variant=0, reply_variant=1, meta_variant=0, log_variant=1):
         import torch
         from summerset_b200.engine import Follower, RaftEngine
         self.n, self.G, self.W, self.d, self.me = n, G, W, n // 2 + 1, 0
+        self.meta_variant = meta_variant
         self.ctx = ts._ctx()
         self.rng = rng = random.Random(7700 + n)
-        self.fols = {r: Follower(self.ctx, G, n, r, window=W) for r in range(n)}
+        self.fols = {r: Follower(self.ctx, G, n, r, window=W, append_variant=append_variant, reply_variant=reply_variant,
+                                 meta_variant=meta_variant, log_variant=log_variant) for r in range(n)}
         self.stride = G * tl.pitch(-(-3000 // self.d)) * 8
         self.keep, self.batch = [], {}
         self.eng = eng = RaftEngine(self.ctx, G, n, craft=True, window=W)
@@ -415,7 +420,8 @@ class _PlainRig:
         eng.curr_term.fill_(1)
         for _ in range(2):
             te._propose(eng, 0, [rng.choice((0, 1, 17, 300, 3000)) for _ in range(G)], self.stride, self.keep, self.batch, rng)
-            te._replicate(self.ctx, eng, 0, {r: f for r, f in self.fols.items() if r}, self.keep, rng)
+            te._replicate(self.ctx, eng, 0, {r: f for r, f in self.fols.items() if r}, self.keep, rng, None, append_variant,
+                          reply_variant)
         te._propose(eng, 0, [rng.choice((1, 300)) for _ in range(G)], self.stride, self.keep, self.batch, rng)
         self.planes = self.keep[0]
         torch.cuda.synchronize()
@@ -424,14 +430,14 @@ class _PlainRig:
         return _Rig.snapshot(self)
 
 
-def _step_down_raw(eng, fol, buf, fo, fg, fp, store, pad=64):
+def _step_down_raw(eng, fol, buf, fo, fg, fp, store, pad=64, variants=(AE, AER, RV, RVR)):
     """ss_engine_craft_step_down with every output inside canaries (0xA5) that must come back untouched"""
     import torch
     from summerset_b200 import _lib
     n, dev = fo.numel(), "cuda:0"
     mk = lambda cnt, dt: torch.full((cnt + 2 * pad,), 0xA5 if dt == torch.uint8 else -0x5A5A5A5B, dtype=dt, device=dev)
     so, meta, ml, vd, need = mk(n, torch.int64), mk(32 * n, torch.uint8), mk(n, torch.int32), mk(n, torch.int32), mk(1, torch.int64)
-    spec = _lib.StepDownSpec(AE, AER, RV, RVR)
+    spec = _lib.StepDownSpec(*variants)
     at = lambda t: t.data_ptr() + pad * t.element_size()
     rc = eng.lib.ss_engine_craft_step_down(eng.h, fol.h, C.byref(spec), buf.data_ptr(), buf.numel(), fo.data_ptr(), fg.data_ptr(),
                                            fp.data_ptr(), n, store.data_ptr(), store.numel(), at(so), at(meta), at(ml), at(vd), at(need))

@@ -193,12 +193,12 @@ def serve(fg, slots, d, T, shard, variant=5):
     return reconstruct_reply(ents, variant) if ents else None
 
 
-def absorb(lg, frames, d, T):
+def absorb(lg, frames, d, T, variant=5):
     """lg: dict(start, le, dl={s}, held={s}, plane={(s, j): bytes}); frames: the group's frame bytes in frame order ->
     absorbed per frame (None: malformed)"""
     res = []
     for fr in frames:
-        ents = parse_reply(fr, d, T)
+        ents = parse_reply(fr, d, T, variant)
         if ents is None:
             res.append(None)
             continue

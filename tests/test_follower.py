@@ -86,8 +86,9 @@ class Ent:
 class Group:
     """one group's follower state; log[s] = (term, data_len, {shard: bytes}) for s in [start, le)"""
 
-    def __init__(self, n: int, W: int):
+    def __init__(self, n: int, W: int, reply_variant=1, meta_variant=0):
         self.d, self.T, self.W = n // 2 + 1, n, W
+        self.rv, self.mv = reply_variant, meta_variant             # AppendEntriesReply in PeerMsg, Metadata in DurEntry
         self.absorb_room = True                                   # False: absorbs find no room and change nothing
         self.start, self.le, self.ct, self.ldr, self.lc, self.ls = 0, 1, 0, 0xFF, 0, 0
         self.log = {0: (0, 0, {})}
@@ -101,7 +102,7 @@ class Group:
             return o
         if term > self.ct:
             self.ct = term
-            o["meta"] = dur_metadata(term)
+            o["meta"] = dur_metadata(term, self.mv)
             self.ldr = peer
         if term == self.ct:
             self.ldr = peer
@@ -111,7 +112,7 @@ class Group:
             cs = prev
             while ctm > 0 and cs > self.start and self.log[cs - 1][0] == ctm:
                 cs -= 1
-            o.update(verdict=REJECTED, reply=reply(self.ct, prev + n, (ctm, cs)), reply_to="peer")
+            o.update(verdict=REJECTED, reply=reply(self.ct, prev + n, (ctm, cs), self.rv), reply_to="peer")
             self.ls = max(self.ls, snap)
             return o
         appending = False
@@ -136,7 +137,7 @@ class Group:
                 held = sum(1 << j for j in sh)
                 if bin(held & ((1 << self.d) - 1)).count("1") < self.d and dl == e.dl and held != e.held and self.absorb_room:
                     self.log[s] = (t, dl, {**e.shards, **sh})
-        o["reply"] = reply(self.ct, prev + n)
+        o["reply"] = reply(self.ct, prev + n, variant=self.rv)
         o["reply_to"] = "leader" if o["appended"] else "peer"
         if commit > self.lc:
             # entries.len() after the append loop's drain is first_new - prev - 1 (messages.rs:160-203)
@@ -336,7 +337,8 @@ def _bad_frames(rng: random.Random, n: int, me: int, G: int):
 class Harness:
     """one device follower and its restatement, fed batch after batch"""
 
-    def __init__(self, n, G, window=64, sharded=False, seed=0, frames_per_group=6, dls=(1, 10, 250, 251, 3000)):
+    def __init__(self, n, G, window=64, sharded=False, seed=0, frames_per_group=6, dls=(1, 10, 250, 251, 3000), append_variant=0,
+                 reply_variant=1, meta_variant=0, log_variant=1):
         import torch
         from summerset_b200.api import Context
         from summerset_b200.engine import Follower
@@ -344,9 +346,10 @@ class Harness:
         self.rng = random.Random(seed)
         self.n, self.G, self.me, self.d = n, G, n - 1, n // 2 + 1
         self.ctx = Context(0)
-        self.fol = Follower(self.ctx, G, n, self.me, window)
+        self.av, self.lv = append_variant, log_variant
+        self.fol = Follower(self.ctx, G, n, self.me, window, append_variant, reply_variant, meta_variant, log_variant)
         self.W = self.fol.W
-        self.models = [Group(n, self.W) for _ in range(G)]
+        self.models = [Group(n, self.W, reply_variant, meta_variant) for _ in range(G)]
         peers = [q for q in range(n) if q != self.me]
         self.streams = [_leader_stream(self.rng, n, peers, frames_per_group, sharded, self.me, dls) for _ in range(G)]
         self.stores = []                                          # every store a live entry may point into
@@ -380,7 +383,7 @@ class Harness:
         for it in seq:
             if it[0] == "ok":
                 pe, t, prev, pt, es, cm, sn = it[2]
-                w, g = append_entries(t, prev, pt, [e.wire() for e in es], cm, sn), it[1]
+                w, g = append_entries(t, prev, pt, [e.wire() for e in es], cm, sn, self.av), it[1]
             else:
                 _, g, pe, w, _v = it
             buf += bytes(rng.randint(0, 5))                       # odd offsets
@@ -396,7 +399,7 @@ class Harness:
             if es and prev + len(es) >= self.models[g].start + self.W:
                 continue
             so += sum(len(e.shards) * pitch(-(-e.dl // d)) for e in es)
-            wo += sum(r16(len(dur_log_entry(e.to_external()))) for e in es)
+            wo += sum(r16(len(dur_log_entry(e.to_external(), self.lv))) for e in es)
         scap = so - store_short if store_short is not None else None
         wcap = wo - wal_short if wal_short is not None else None
         dev = "cuda:0"
@@ -423,7 +426,7 @@ class Harness:
             if es and prev + len(es) >= self.models[g].start + self.W:
                 continue
             s_run += sum(len(e.shards) * pitch(-(-e.dl // d)) for e in es)
-            w_run += sum(r16(len(dur_log_entry(e.to_external()))) for e in es)
+            w_run += sum(r16(len(dur_log_entry(e.to_external(), self.lv))) for e in es)
             if cut_i is None and ((scap is not None and s_run > scap) or (wcap is not None and w_run > wcap)):
                 cut_i, cut_kind = i, STORE_FULL if scap is not None and s_run > scap else WAL_FULL
         for m in self.models:
@@ -457,7 +460,7 @@ class Harness:
                 continue
             at, sat = int(o["wal_off"][i]), int(o["store_off"][i])
             for e in want["appended"]:
-                rec = dur_log_entry(e.to_external())
+                rec = dur_log_entry(e.to_external(), self.lv)
                 assert wl[at:at + len(rec)].tobytes() == rec
                 at += r16(len(rec))
                 L = -(-e.dl // d)
