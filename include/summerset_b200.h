@@ -1519,6 +1519,62 @@ int ss_follower_tally(ss_follower *follower, const uint8_t *buf, uint64_t buf_le
                       uint8_t *meta, uint32_t *meta_len, uint32_t *verdict, uint32_t *won_group, uint64_t *won_term,
                       uint64_t *n_won);
 
+/* ---- CRaft WAL recovery on the follower ------------------------------------------------------------------------------
+ * recover_from_wal (craft/recovery.rs:11-165) for the records a CRaft replica writes -- DurEntry::Metadata{curr_term,
+ * voted_for} (the 32-byte cells of ss_follower_append, _campaign, _vote, _tally and ss_engine_craft_step_down) and
+ * DurEntry::LogEntry{entry} (ss_follower_append's records, and the leader's own) -- replayed into the term, the vote,
+ * the log ring and the shard store without a record crossing to the host.  A restarted replica is a follower.
+ * Record i is at buf + rec_off[i] (any byte alignment) as the device writes it: an 8-byte big-endian length, then the
+ * bincode DurEntry, whose variant is cfg.meta_variant (Metadata) or cfg.log_variant (LogEntry); the two must differ
+ * (SS_ERR_INVALID_ARG).  Record i belongs to group rec_group[i]; a group's records are replayed in array order, which is
+ * WAL order; groups are independent.  The call imposes no file layout: the host hands the Metadata record over first,
+ * wherever its file keeps it.
+ * Per group with records:
+ *   Metadata (the first record): curr_term, leader = 0xff, vote_term = curr_term, voted_for (0xff = None; any other byte
+ *     is kept as it is).  The election words are taken into use as by ss_follower_vote_view_get; the group is not a
+ *     candidate afterwards, since leader != me.
+ *   LogEntry k (the k-th record after it): slot start_slot + k, with the record's term, data_len and held shards, decoded
+ *     by the rules ss_follower_append applies to an entry (this code, shard_len = ceil(data_len / d), present shards of
+ *     that length, data_copy None, external 0 or 1, non-minimal varints); log_offset is read and ignored.  Its shards go
+ *     into `store`, popcount(held) * SS_CW_SLOT_PITCH(shard_len) bytes in the padded layout ss_follower_append writes,
+ *     and shard_addr names that copy.
+ *   When at least one LogEntry applied: log_end = start_slot + (the LogEntry records applied), and every other ring
+ *     position of the group is zeroed, so the result does not depend on what the follower held before.
+ *   start_slot, last_commit, last_snap and last_exec are not changed: the host installs them from the snapshot through
+ *   the views first, as recover_from_snapshot (craft/snapshot.rs:203-232) does.  A group with no records is not touched.
+ * Regions are placed by an exclusive scan in (group, record) order; *total (device u64, may be NULL) = the store bytes
+ * the batch asked for.  store 16-byte aligned.
+ * verdict[i]:
+ *   SS_FOLLOWER_VERDICT_ACCEPTED       applied;
+ *   SS_FRAME_KIND_MALFORMED            the length runs past buf_len, trailing bytes, a variant that is neither of the two,
+ *                                      an entry that fails the rules above, a Metadata record that is not first or a
+ *                                      second one, or a group >= n_groups.  For a valid group the group's log ends
+ *                                      there: every later record of the group gets SS_RECOVER_VERDICT_AFTER_END;
+ *   SS_FOLLOWER_VERDICT_BEYOND_WINDOW  the group's log holds more than `window` LogEntry records: the whole group is
+ *                                      refused, every record of it gets this verdict, nothing of it changes and
+ *                                      SS_DEV_STATUS_FRAME_OVERFLOW is set; the host needs a follower with a larger
+ *                                      window;
+ *   SS_FOLLOWER_VERDICT_STORE_FULL     the capacity cut is per group: a group whose store region ends past
+ *                                      store_capacity applies nothing, its records that would apply get STORE_FULL and
+ *                                      SS_DEV_STATUS_STORE_FULL is set.  The offsets are monotone, so the placed groups
+ *                                      are a prefix in group order; re-submitting the STORE_FULL records finishes the job.
+ * The file never holds superseded entries: a conflicting append truncates it first (trunc_slot of ss_follower_append).
+ * Absorbed shards and the shards a leader holds only in memory are never written, so they do not come back.
+ * Stated differences from the reference:
+ *   1. the ring: a log longer than `window` refuses the whole group (above).  A shorter log would be unsafe: a follower
+ *      that lost an acknowledged entry can vote for a candidate that lacks it.  A host that discards its WAL prefix
+ *      whenever it advances the follower, as take_new_snapshot does, never meets this case;
+ *   2. a record that does not decode, or a misplaced Metadata record, ends the group's log; the reference aborts the
+ *      replica's recovery;
+ *   3. the per-group capacity cut;
+ *   4. external and log_offset are not kept: the follower has no such fields, and the host keeps the file offsets;
+ *   5. the snapshot state stays with the host.
+ * Cost: the walk and the apply take a thread per group segment, so a batch costs its largest per-group run of records
+ * there (and the apply writes the group's whole ring); the shard copies take a warp per applied LogEntry. */
+int ss_follower_recover(ss_follower *follower, const uint8_t *buf, uint64_t buf_len, const uint64_t *rec_off,
+                        const uint32_t *rec_group, uint64_t n_records, uint8_t *store, uint64_t store_capacity,
+                        uint32_t *verdict, uint64_t *total);
+
 /* ---- CRaft step-down: check_term for the groups a replica leads (SS_PROTO_CRAFT engines) -------------------------------
  * An engine leads the groups whose `led` byte is set.  The bytes are allocated on the first ss_engine_craft_step_down or
  * ss_engine_craft_role_view_get, every one set (until then the engine leads every group, as before); a host whose

@@ -162,6 +162,7 @@ SIGNATURES = {
     "ss_follower_campaign": (_i, [_vp, _vp, _u64, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ss_follower_vote": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ss_follower_tally": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "ss_follower_recover": (_i, [_vp, _vp, _u64, _vp, _vp, _u64, _vp, _u64, _vp, _vp]),
     "ss_rs_set_variant": (_i, [_vp, _i]),
     "ss_rs_last_kernel": (C.c_char_p, [_vp]),
     "ss_rs_jit_status": (C.c_char_p, [_vp]),

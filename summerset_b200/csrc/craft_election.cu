@@ -276,7 +276,7 @@ __global__ void __launch_bounds__(kElThreads) tally_won_kernel(const __grid_cons
 }
 
 // the election arrays, allocated on first use: no vote, no candidacy
-static int el_state(ss_follower *f) {
+int el_state(ss_follower *f) {
     if (f->vote_term != nullptr) return SS_OK;
     ss_ctx *ctx = f->ctx;
     const uint64_t G = f->G;

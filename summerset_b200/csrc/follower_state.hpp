@@ -1,5 +1,5 @@
 // follower_state.hpp -- the CRaft follower handle (ss_follower_*), shared by follower.cu, the reconstruct serve and
-// step-up calls (craft_recon.cu) and the elections (craft_election.cu).
+// step-up calls (craft_recon.cu), the elections (craft_election.cu) and the WAL replay (craft_recover.cu).
 #pragma once
 #include "ss_internal.hpp"
 
@@ -11,6 +11,8 @@ struct ss_follower;
 namespace ssb {
 // grows the per-call scratch to n frames: headers, sort keys, scan partials (follower.cu)
 int fol_scratch(ss_follower *f, uint64_t n);
+// allocates the election arrays on first use (craft_election.cu)
+int el_state(ss_follower *f);
 }  // namespace ssb
 
 struct ss_follower {

@@ -759,6 +759,23 @@ class Follower:
                                                      p(res["reply_len"]), p(res["verdict"]), p(res["total"])))
         return res
 
+    def recover(self, buf: torch.Tensor, rec_off: torch.Tensor, rec_group: torch.Tensor, store: torch.Tensor,
+                store_capacity: Optional[int] = None) -> dict:
+        """Replays WAL records (recover_from_wal): buf uint8 holds DurEntry::Metadata and DurEntry::LogEntry records as the
+        device wrote them (8-byte big-endian length + bincode DurEntry, any alignment), record i at rec_off[i] (int64) of
+        group rec_group[i] (int32), each group's Metadata record first and the rest in WAL order.  The entries' shards go
+        to store (uint8, 16-byte aligned, caller-owned; keep it alive while the log holds it).  Returns device tensors
+        verdict (int32 [n]) and total (int64 [1]: the store bytes the batch asked for)."""
+        assert buf.dtype == torch.uint8 and rec_off.dtype == torch.int64 and rec_group.dtype == torch.int32
+        assert store.dtype == torch.uint8 and rec_group.numel() == rec_off.numel()
+        n, dev = rec_off.numel(), buf.device
+        res = dict(verdict=torch.empty(n, dtype=torch.int32, device=dev), total=torch.empty(1, dtype=torch.int64, device=dev))
+        p = lambda x: x.data_ptr()
+        check(self.lib.ss_follower_recover(self.h, p(buf), buf.numel(), p(rec_off), p(rec_group), n, p(store),
+                                           store.numel() if store_capacity is None else store_capacity, p(res["verdict"]),
+                                           p(res["total"])))
+        return res
+
     # ---- elections: campaigns, RequestVote frames answered, votes tallied ----
     def vote_view(self) -> dict:
         """Takes the election state into use and returns zero-copy views: vote_term int64 [G], voted_for uint8 [G] (0xff =

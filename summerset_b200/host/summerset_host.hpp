@@ -473,6 +473,13 @@ class Follower {
         check(ss_follower_tally(fol_, buf, buf_len, frame_off, frame_group, frame_peer, n_frames, reply_variant, meta, meta_len, verdict,
                                 won_group, won_term, n_won));
     }
+    // recover_from_wal over a group-tagged batch of Metadata (cfg.meta_variant) and LogEntry (cfg.log_variant) records,
+    // each group's Metadata first and the rest in WAL order; the shards go to store.  A group cut by the store is
+    // finished by re-submitting its STORE_FULL records (see ss_follower_recover)
+    void recover(const uint8_t *buf, uint64_t buf_len, const uint64_t *rec_off, const uint32_t *rec_group, uint64_t n_records,
+                 uint8_t *store, uint64_t store_capacity, uint32_t *verdict, uint64_t *total = nullptr) {
+        check(ss_follower_recover(fol_, buf, buf_len, rec_off, rec_group, n_records, store, store_capacity, verdict, total));
+    }
     // the handle, for ss_engine_craft_step_up
     const ss_follower *get() const { return fol_; }
 
