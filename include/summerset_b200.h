@@ -1064,7 +1064,7 @@ typedef struct ss_follower_config {
     uint32_t protocol;          /* SS_PROTO_CRAFT (the field leaves room for plain Raft without an ABI change) */
     uint32_t population;        /* replicas, 1..32 */
     uint32_t me;                /* this replica's id: a frame from `me` is malformed */
-    uint32_t window;            /* ring entries per group, power of two <= 4096 (0 = 64) */
+    uint32_t window;            /* ring entries per group, power of two, 2..4096 (0 = 64) */
     uint32_t append_variant;    /* index of AppendEntries in PeerMsg (0), < 2^16 */
     uint32_t reply_variant;     /* index of AppendEntriesReply in PeerMsg (1), < 251: a reply fills at most 47 bytes of
                                    its 48-byte cell */

@@ -465,8 +465,11 @@ int ss_follower_create(ss_ctx *ctx, const ss_follower_config *cfg, uint64_t G, s
     if (cfg->protocol != SS_PROTO_CRAFT) return set_error(SS_ERR_INVALID_ARG, "the follower serves CRaft, not protocol %u", cfg->protocol);
     if (cfg->population == 0 || cfg->population > 32 || cfg->me >= cfg->population)
         return set_error(SS_ERR_INVALID_ARG, "bad population %u / me %u", cfg->population, cfg->me);
+    // a ring of one entry holds only start_slot, so no entry could ever be appended: the window filter refuses every slot
+    // past start_slot, nothing commits, and start_slot can never move
     const uint32_t W = cfg->window ? cfg->window : 64u;
-    if ((W & (W - 1u)) || W > 4096u) return set_error(SS_ERR_INVALID_ARG, "window must be a power of two <= 4096 (got %u)", cfg->window);
+    if (W < 2u || (W & (W - 1u)) || W > 4096u)
+        return set_error(SS_ERR_INVALID_ARG, "window must be a power of two in 2..4096 (got %u)", cfg->window);
     // a reply is at most 8 + 1 + wv_len(reply_variant) + 9 + 9 + 1 + 9 + 9 bytes: one-byte variants fill at most 47 of its
     // 48-byte cell; a Metadata record at most 8 + 3 + 9 + 1 of its 32
     if (cfg->reply_variant >= 251u || cfg->meta_variant >= 65536u || cfg->append_variant >= 65536u || cfg->log_variant >= 65536u)

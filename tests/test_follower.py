@@ -338,14 +338,14 @@ class Harness:
     """one device follower and its restatement, fed batch after batch"""
 
     def __init__(self, n, G, window=64, sharded=False, seed=0, frames_per_group=6, dls=(1, 10, 250, 251, 3000), append_variant=0,
-                 reply_variant=1, meta_variant=0, log_variant=1):
+                 reply_variant=1, meta_variant=0, log_variant=1, me=None, ctx=None):
         import torch
         from summerset_b200.api import Context
         from summerset_b200.engine import Follower
         self.torch = torch
         self.rng = random.Random(seed)
-        self.n, self.G, self.me, self.d = n, G, n - 1, n // 2 + 1
-        self.ctx = Context(0)
+        self.n, self.G, self.me, self.d = n, G, n - 1 if me is None else me, n // 2 + 1
+        self.ctx = Context(0) if ctx is None else ctx
         self.av, self.lv = append_variant, log_variant
         self.fol = Follower(self.ctx, G, n, self.me, window, append_variant, reply_variant, meta_variant, log_variant)
         self.W = self.fol.W
@@ -353,6 +353,8 @@ class Harness:
         peers = [q for q in range(n) if q != self.me]
         self.streams = [_leader_stream(self.rng, n, peers, frames_per_group, sharded, self.me, dls) for _ in range(G)]
         self.stores = []                                          # every store a live entry may point into
+        self.host_stores = []                                     # (address, host copy) of each store after its call
+        self.absorb_room = 1 << 25                                # store bytes past the frames' regions for absorbed entries
         self.pending = [[] for _ in range(G)]                     # BEYOND frames to re-submit
 
     def take(self, k):
@@ -403,7 +405,7 @@ class Harness:
         scap = so - store_short if store_short is not None else None
         wcap = wo - wal_short if wal_short is not None else None
         dev = "cuda:0"
-        store = torch.full((max(so, 1) + (1 << 25),), 0xA5, dtype=torch.uint8, device=dev)
+        store = torch.full((max(so, 1) + self.absorb_room,), 0xA5, dtype=torch.uint8, device=dev)
         wal = torch.full((max(wo, 1) + 4096,), 0xA5, dtype=torch.uint8, device=dev)
         self.stores.append(store)
         tb = torch.tensor(np.frombuffer(bytes(buf), dtype=np.uint8), device=dev)
@@ -431,6 +433,7 @@ class Harness:
                 cut_i, cut_kind = i, STORE_FULL if scap is not None and s_run > scap else WAL_FULL
         for m in self.models:
             m.absorb_room = scap is None                          # an exact store leaves no room after the regions
+        s_written, w_written = np.zeros(st.size, dtype=bool), np.zeros(wl.size, dtype=bool)
         for i, it in enumerate(seq):
             if it[0] == "bad":
                 assert o["verdict"][i] == it[4], (i, hex(o["verdict"][i]), hex(it[4]))
@@ -462,13 +465,20 @@ class Harness:
             for e in want["appended"]:
                 rec = dur_log_entry(e.to_external(), self.lv)
                 assert wl[at:at + len(rec)].tobytes() == rec
+                w_written[at:at + len(rec)] = True
                 at += r16(len(rec))
                 L = -(-e.dl // d)
                 for j in sorted(e.shards):
                     assert st[sat:sat + L].tobytes() == e.shards[j]
                     assert not st[sat + L:sat + r16(L)].any()
+                    s_written[sat:sat + r16(L)] = True
                     sat += pitch(L)
             assert int(o["wal_len"][i]) == at - int(o["wal_off"][i])
+        # outside the records and the appended shards only the absorbed entries' regions, placed after every frame's
+        # region, may have changed
+        s_written[so:int(o["totals"][0])] = True
+        assert (st[~s_written] == 0xA5).all(), "store bytes outside the written regions changed"
+        assert (wl[~w_written] == 0xA5).all(), "WAL bytes outside the records changed"
         self.check_state(o, seq)
         return o, seq, (so, wo)
 
@@ -477,11 +487,16 @@ class Harness:
         pitch = lambda L: (L + 31) & ~31
         v = {k: getattr(fol, k).cpu().numpy() for k in ("start_slot", "log_end", "curr_term", "last_commit", "last_snap", "leader",
                                                          "term", "held", "data_len", "shard_addr")}
-        stores = [(s.data_ptr(), s.cpu().numpy()) for s in self.stores]
+        # a store is written only by the call it was passed to, so each is copied to the host once, after that call
+        for s in self.stores[len(self.host_stores):]:
+            self.host_stores.append((s.data_ptr(), s.cpu().numpy()))
+        stores = self.host_stores
+        used = {len(stores) - 1} if stores else set()
 
         def read(addr, nb):
-            for b, arr in stores:
+            for k, (b, arr) in enumerate(stores):
                 if b <= addr and addr + nb <= b + arr.size:
+                    used.add(k)
                     return arr[addr - b:addr - b + nb].tobytes()
             raise AssertionError("shard address outside every store")
 
@@ -491,13 +506,17 @@ class Harness:
             for s in range(m.start, m.le):
                 t, dl, sh = m.log[s]
                 pos = s & (self.W - 1)
-                assert v["term"][g][pos] == t and v["data_len"][g][pos] == dl and v["held"][g][pos] == sum(1 << j for j in sh), (g, s)
+                held = int(v["held"][g][pos]) & 0xFFFFFFFF                # shard 31 is the sign bit of the int32 view
+                assert v["term"][g][pos] == t and v["data_len"][g][pos] == dl and held == sum(1 << j for j in sh), (g, s)
                 if not sh:
                     continue
                 L = -(-dl // d)
                 a = int(v["shard_addr"][g][pos])
                 for r, j in enumerate(sorted(sh)):
                     assert read(a + r * pitch(L), L) == sh[j], (g, s, j)
+        # a store no live entry points into is let go: later calls read only the shards of live entries
+        keep = sorted(used)
+        self.stores, self.host_stores = [self.stores[k] for k in keep], [stores[k] for k in keep]
         if o is not None:
             for i, it in enumerate(seq):
                 if it[0] == "ok" and int(o["verdict"][i]) == ACCEPTED and o["wal_len"][i]:
@@ -512,11 +531,17 @@ class Harness:
         self.check_state()
 
 
+# (population, me): me = n - 1 keeps the id the population alone; populations 2 (d = 2, p = 0), 16, 31 and 32 (d = 17,
+# shard 31 held) and me = 0 and n // 2 move the peers around `me`
+POPULATIONS = [pytest.param(n, n - 1, id=str(n)) for n in (2, 3, 5, 7, 9, 16, 31, 32)]
+POPULATIONS += [pytest.param(n, me, id=f"{n}-me{me}") for n in (2, 3, 5, 7, 9, 16, 31, 32) for me in sorted({0, n // 2} - {n - 1})]
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("n", [3, 5, 7, 9])
+@pytest.mark.parametrize("n,me", POPULATIONS)
 @pytest.mark.parametrize("sharded", [True, False])
-def test_follower_matches_restatement(n, sharded):
-    h = Harness(n, 64, sharded=sharded, seed=n * 10 + sharded)
+def test_follower_matches_restatement(n, me, sharded):
+    h = Harness(n, 64, sharded=sharded, seed=n * 10 + sharded + (0 if me == n - 1 else 1000 * (me + 1)), me=me)
     h.batch(h.take(6), bad=_bad_frames(h.rng, n, h.me, h.G) + _bad_frames(h.rng, n, h.me, h.G))
 
 
@@ -531,38 +556,51 @@ def test_follower_capacity_cut(which, short):
     assert cut.any() == bool(short)
 
 
-@pytest.mark.gpu
-def test_follower_window_wrap_after_advance():
-    # a ring of 8: each group's log runs several times around it; leaders back off to the follower's log, rewrite
-    # uncommitted suffixes in new terms, and send past the window; BEYOND frames come back after each advance
-    h = Harness(5, 16, window=8, seed=3, frames_per_group=0)
+def wrap_after_advance(h, rounds, grow=3, send=5, dls=(1, 10, 251, 3000), until=None):
+    """Rounds of frames that run each group's log around its ring: leaders append 1..grow entries a round, back off to
+    the follower's log, rewrite uncommitted suffixes in new terms and send up to `send` entries a frame, past the window
+    too; BEYOND frames come back after each advance.  Stops after `rounds` or once until(h) holds; returns the number of
+    BEYOND verdicts."""
     rng, d, n = h.rng, h.d, h.n
+    peers = [q for q in range(n) if q != h.me]
     logs = [[(0, None)] for _ in range(h.G)]                      # the leader's (term, Ent) per slot
     terms = [1] * h.G
+    safe = [0] * h.G                                              # the highest commit sent: no leader rewrites below it
     beyond = 0
-    for _ in range(14):
+    for _ in range(rounds):
         frames = []
         for g, m in enumerate(h.models):
             log = logs[g]
             if rng.random() < 0.2:                                # a new leader rewrites the uncommitted suffix
                 terms[g] += 1
-                del log[rng.randint(m.lc + 1, len(log)):]
-            for _ in range(rng.randint(1, 3)):
-                dl = rng.choice((1, 10, 251, 3000))
+                del log[rng.randint(safe[g] + 1, len(log)):]
+            safe[g] = len(log) - 1                                # the entries of earlier rounds commit from now on
+            for _ in range(rng.randint(1, grow)):
+                dl = rng.choice(dls)
                 L = -(-dl // d)
                 log.append((terms[g], Ent(terms[g], d, n - d, dl, {j: rng.randbytes(L) for j in range(d)}, True, 0)))
             prev = min(m.le, len(log)) - 1                        # next_slot after the leader's back-off
             while prev > m.start and m.log.get(prev, (None,))[0] != log[prev][0]:
                 prev -= 1
             for _ in range(rng.randint(1, 2)):
-                k = rng.randint(0, 5)
+                k = rng.randint(0, send)
                 es = [e for _, e in log[prev + 1:prev + 1 + k]]
-                frames.append((g, (rng.randrange(n - 1), terms[g], prev, log[prev][0], es, len(log) - 1, 0)))
+                frames.append((g, (peers[rng.randrange(n - 1)], terms[g], prev, log[prev][0], es, safe[g], 0)))
                 prev = min(prev + len(es), len(log) - 1)
         h.pending, pend = [[] for _ in range(h.G)], h.pending
         o, seq, _ = h.batch([(g, f) for g in range(h.G) for f in pend[g]] + frames)
         beyond += int((o["verdict"] == BEYOND).sum())
         h.advance()
+        if until is not None and until(h):
+            break
+    return beyond
+
+
+@pytest.mark.gpu
+def test_follower_window_wrap_after_advance():
+    # a ring of 8: each group's log runs several times around it, frames of up to 8 entries run past its end
+    h = Harness(5, 16, window=8, seed=3, frames_per_group=0)
+    beyond = wrap_after_advance(h, 14, grow=4, send=8)
     assert beyond > 0
     assert max(m.le for m in h.models) > 3 * h.W                  # ring positions were reused
     assert max(m.start for m in h.models) > 2 * h.W
