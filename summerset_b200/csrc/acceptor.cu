@@ -274,8 +274,7 @@ __global__ void __launch_bounds__(kAccThreads) acceptor_copy_kernel(const __grid
         const uint32_t wvl = static_cast<uint32_t>(wv_len(A.wal_variant));
         const uint64_t tail = h.end - h.slot_at;
         if (lane == 0u) {
-            const uint64_t body = wvl + tail;
-            for (int b = 0; b < 8; ++b) rec[b] = static_cast<uint8_t>(body >> (8 * (7 - b)));
+            put_be64(rec, wvl + tail);
             wv_put(rec + 8, A.wal_variant);
         }
         warp_copy_unaligned(rec + 8u + wvl, fr + h.slot_at, tail, lane);
@@ -296,8 +295,7 @@ __global__ void __launch_bounds__(kAccThreads) acceptor_copy_kernel(const __grid
                 m += wv_put(cell + m, size);
                 cell[m++] = 0u;
             }
-            const uint64_t body = m - 8u;
-            for (int b = 0; b < 8; ++b) cell[b] = static_cast<uint8_t>(body >> (8 * (7 - b)));
+            put_be64(cell, m - 8u);
             A.reply_len[i] = m;
             A.reply_dst[i] = A.source[at_s];
         }
@@ -451,28 +449,11 @@ struct RecWarp {
     uint64_t off[64];               // serve: entry offsets in the reply; absorb: new region offsets (~0: unchanged)
 };
 
-#define SS_GETV(dst) do { if (!(c = wv_get(b + n, len - n, (dst)))) return SS_FRAME_KIND_MALFORMED; n += c; } while (0)
-
 // the 8-byte length, PeerMessage::Msg and the PeerMsg variant of frame i; kPending with b / len / n past the entry count
 // (cnt) when it is `variant`
 __device__ __forceinline__ uint32_t rec_head(const RecArgs &A, uint64_t i, const uint8_t *&b, uint64_t &len, uint64_t &n, uint64_t &cnt) {
-    const uint32_t grp = A.frame_group[i];
-    const uint64_t off = A.frame_off[i];
-    if (grp >= A.G || off > A.buf_len || A.buf_len - off < 8u) return SS_FRAME_KIND_MALFORMED;
-    const uint8_t *fr = A.buf + off;
-    len = 0;
-    for (int k = 0; k < 8; ++k) len = (len << 8) | fr[k];
-    if (len > A.buf_len - off - 8u || len > kMaxFrameBody) return SS_FRAME_KIND_MALFORMED;
-    b = fr + 8;
-    n = 0;
-    uint64_t v = 0;
-    uint32_t c;
-    SS_GETV(v);
-    if (v != 0u) return v < kVariantLimit ? 0x80000000u | static_cast<uint32_t>(v) : SS_FRAME_KIND_MALFORMED;
-    SS_GETV(v);
-    if (v != A.variant) return v < kVariantLimit ? static_cast<uint32_t>(v) : SS_FRAME_KIND_MALFORMED;
-    SS_GETV(cnt);
-    return kPending;
+    if (A.frame_group[i] >= A.G) return SS_FRAME_KIND_MALFORMED;
+    return msg_head_count(A.buf, A.buf_len, A.frame_off[i], A.variant, kMaxFrameBody, b, len, n, cnt);
 }
 
 __device__ __forceinline__ uint64_t ring_slot(uint64_t base, uint32_t pos) { return base + ((pos - base) & 63u); }
@@ -490,10 +471,10 @@ __device__ uint32_t serve_walk(const RecArgs &A, uint64_t i, RecWarp &W, uint32_
     const uint32_t g = A.frame_group[i];
     const uint64_t base = A.window_base[g], live = A.accepting[g] | A.committed[g];
     const uint64_t T = A.T;
-    uint32_t err = 0u, c;
+    uint32_t err = 0u;
     for (uint64_t e = 0; e < cnt; ++e) {
         uint64_t slot = 0;
-        SS_GETV(slot);
+        if (!wv_next(b, len, n, slot)) return SS_FRAME_KIND_MALFORMED;
         uint32_t sel = 0xffffffffu;
         bool range_bad = false;
         if (A.crossword) {
@@ -503,11 +484,10 @@ __device__ uint32_t serve_walk(const RecArgs &A, uint64_t i, RecWarp &W, uint32_
             // exclusion leaves clear, and one at index >= T makes subset_copy fail: every bit of [T, size mod 256) must
             // be set.
             uint64_t sz = 0, nb = 0, blk = 0, lo = 0;
-            SS_GETV(sz);
-            SS_GETV(nb);
+            if (!wv_next(b, len, n, sz) || !wv_next(b, len, n, nb)) return SS_FRAME_KIND_MALFORMED;
             const uint64_t walk = sz & 255u;
             for (uint64_t k = 0; k < nb; ++k) {
-                SS_GETV(blk);
+                if (!wv_next(b, len, n, blk)) return SS_FRAME_KIND_MALFORMED;
                 if (k == 0u) lo = blk;
                 const uint64_t b0 = 64u * k, from = T > b0 ? T : b0, to = walk < b0 + 64u ? walk : b0 + 64u;
                 if (from < to) {
@@ -538,17 +518,13 @@ __device__ uint32_t serve_walk(const RecArgs &A, uint64_t i, RecWarp &W, uint32_
     return err != 0u ? err : kPending;
 }
 
-// bytes of a bincode RSCodeword carrying the shards m: d, p, data_len, shard_len, T shard Options, data_copy None
-__device__ __forceinline__ uint64_t codeword_bytes(uint32_t d, uint32_t T, uint64_t dl, uint32_t m) {
-    const uint64_t L = (dl + d - 1u) / d, k = static_cast<uint64_t>(__popc(m));
-    return 2u + wv_len(dl) + wv_len(L) + wv_len(T) + (T - k) + k * (1u + wv_len(L) + L) + 1u;
-}
-
-// that codeword at e (any alignment): lane 0 writes the header, the Option tags and the shard lengths; the warp copies
-// shard j of m from its padded slot in the instance's store region at src, rank popcount(held & below j).  Not inlined:
-// inlined into serve_copy_kernel it made that kernel spill; the call costs one per entry.
+// the codeword of cw_bytes at e (any alignment): lane 0 writes the header, the Option tags and the shard lengths; the
+// warp copies shard j of m from its padded slot in the instance's store region at src, rank popcount(held & below j).
+// Not inlined: inlined into serve_copy_kernel it made that kernel spill; the call costs one per entry.  It keeps its own
+// loop rather than warp_put_cw's, whose lane-0 writes between the shard copies made ss_acceptor_reconstruct_serve 3-5 %
+// slower on an H100.
 __device__ __noinline__ void warp_put_codeword(uint8_t *e, uint32_t d, uint32_t T, uint64_t dl, uint32_t m, uint32_t held, const uint8_t *src,
-                                  uint32_t lane) {
+                                               uint32_t lane) {
     const uint64_t L = (dl + d - 1u) / d, pitch = SS_CW_SLOT_PITCH(L);
     const uint64_t h0 = 2u + wv_len(dl) + wv_len(L) + wv_len(T), some = 1u + wv_len(L);
     if (lane == 0u) {
@@ -580,7 +556,7 @@ __device__ __noinline__ void warp_put_codeword(uint8_t *e, uint32_t d, uint32_t 
 
 // bytes of one (slot, (inst.bal, RSCodeword)) map entry carrying the shards m of instance `at`
 __device__ __forceinline__ uint64_t serve_entry_bytes(const RecArgs &A, uint64_t slot, uint64_t at, uint32_t m) {
-    return wv_len(slot) + wv_len(A.inst_bal[at]) + codeword_bytes(A.d, A.T, A.data_len[at], m);
+    return wv_len(slot) + wv_len(A.inst_bal[at]) + cw_bytes(A.data_len[at], A.d, A.T, __popc(m));
 }
 
 __device__ __forceinline__ uint64_t warp_sum(uint64_t x) {
@@ -665,8 +641,7 @@ __global__ void __launch_bounds__(kAccThreads) serve_copy_kernel(const __grid_co
         __syncwarp();
         uint8_t *dst = A.out + off;
         if (lane == 0u) {
-            const uint64_t body = len - 8u;
-            for (int k = 0; k < 8; ++k) dst[k] = static_cast<uint8_t>(body >> (8 * (7 - k)));
+            put_be64(dst, len - 8u);
             uint32_t m = 8u;
             m += wv_put(dst + m, 0u);                                            // PeerMessage::Msg
             m += wv_put(dst + m, A.reply_variant);
@@ -693,41 +668,11 @@ struct RecEntry {
     uint32_t dlen, L, mask;
 };
 __device__ __forceinline__ bool absorb_entry(const RecArgs &A, const uint8_t *b, uint64_t len, uint64_t &n, RecEntry &E) {
-    uint64_t v = 0, dl = 0, sl = 0;
-    uint32_t c;
-#define SS_GETB(dst) do { if (!(c = wv_get(b + n, len - n, (dst)))) return false; n += c; } while (0)
-    SS_GETB(E.slot);
-    SS_GETB(E.bal);
-    if (len - n < 2u || b[n] != A.d || b[n + 1] != A.T - A.d) return false;
-    n += 2;
-    SS_GETB(dl);
-    SS_GETB(sl);
-    SS_GETB(v);
-    if (dl > 0xffffffffull || v != A.T || sl != (dl + A.d - 1u) / A.d) return false;
-    E.tags_at = n;
-    uint32_t mask = 0;
-    for (uint32_t j = 0; j < A.T; ++j) {
-        if (n >= len) return false;
-        const uint8_t tag = b[n++];
-        if (tag == 0u) continue;
-        if (tag != 1u) return false;
-        SS_GETB(v);
-        if (v != sl || len - n < sl) return false;
-        mask |= 1u << j;
-        n += sl;
-    }
-    if (n >= len) return false;
-    const uint8_t tag = b[n++];                                                  // data_copy
-    if (tag == 1u) {
-        if (len - n < dl) return false;
-        n += dl;
-    } else if (tag != 0u) {
+    uint64_t dl = 0, sl = 0;
+    if (!wv_next(b, len, n, E.slot) || !wv_next(b, len, n, E.bal) || !cw_parse<true>(b, len, n, A.d, A.T, dl, sl, E.tags_at, E.mask))
         return false;
-    }
-#undef SS_GETB
     E.dlen = static_cast<uint32_t>(dl);
     E.L = static_cast<uint32_t>(sl);
-    E.mask = mask;
     return true;
 }
 
@@ -922,7 +867,6 @@ __global__ void __launch_bounds__(kAccThreads) absorb_copy_kernel(const __grid_c
     }
     if (full) atomicOr(A.status, SS_DEV_STATUS_STORE_FULL);
 }
-#undef SS_GETV
 
 // ---- prepare -----------------------------------------------------------------------------------------------------
 struct PrepArgs {
@@ -961,28 +905,11 @@ __device__ __forceinline__ PrepHdr decode_prepare(const PrepArgs &A, uint64_t i)
     h.kind = SS_FRAME_KIND_MALFORMED;
     const uint32_t grp = A.frame_group[i];
     const uint64_t off = A.frame_off[i];
-    if (grp >= A.G || off > A.buf_len || A.buf_len - off < 8u) return h;
-    const uint8_t *fr = A.buf + off;
-    uint64_t len = 0;
-    for (int k = 0; k < 8; ++k) len = (len << 8) | fr[k];
-    if (len > A.buf_len - off - 8u || len > kMaxFrameBody) return h;
-    const uint8_t *b = fr + 8;
-    uint64_t n = 0, v = 0, trig = 0, bal = 0;
-    uint32_t c;
-#define SS_GETP(dst) do { if (!(c = wv_get(b + n, len - n, (dst)))) return h; n += c; } while (0)
-    SS_GETP(v);
-    if (v != 0u) {
-        if (v < kVariantLimit) h.kind = 0x80000000u | static_cast<uint32_t>(v);
-        return h;
-    }
-    SS_GETP(v);
-    if (v != A.variant) {
-        if (v < kVariantLimit) h.kind = static_cast<uint32_t>(v);
-        return h;
-    }
-    SS_GETP(trig);
-    SS_GETP(bal);
-#undef SS_GETP
+    if (grp >= A.G) return h;
+    const uint8_t *b;
+    uint64_t len, n, trig = 0, bal = 0;
+    if (!msg_head(A.buf, A.buf_len, off, A.variant, kMaxFrameBody, true, b, len, n, h.kind)) return h;
+    if (!wv_next(b, len, n, trig) || !wv_next(b, len, n, bal)) return h;
     if (n != len || A.frame_peer[i] == A.me) return h;
     h.trigger = trig;
     h.ballot = bal;
@@ -1172,7 +1099,7 @@ __device__ __forceinline__ uint64_t prep_reply_bytes(const PrepReplyArgs &A, uin
     *at = static_cast<uint64_t>(g) * 64u + p;
     const uint64_t trig = A.prep_trigger[*at], vb = A.voted_bal[*at];
     uint64_t len = 9u + wv_len(A.variant) + wv_len(s) + wv_len(trig) + wv_len(trig + A.prep_span[*at]) + wv_len(A.inst_bal[*at]) + 1u;
-    if (vb > 0u) len += wv_len(vb) + codeword_bytes(A.d, A.T, A.data_len[*at], A.voted_mask[*at]);
+    if (vb > 0u) len += wv_len(vb) + cw_bytes(A.data_len[*at], A.d, A.T, __popc(A.voted_mask[*at]));
     return len;
 }
 
@@ -1211,8 +1138,7 @@ __global__ void __launch_bounds__(kAccThreads) prep_reply_copy_kernel(const __gr
         q += wv_len(0u) + wv_len(A.variant) + wv_len(s) + wv_len(trig) + wv_len(trig + A.prep_span[at]) + wv_len(A.inst_bal[at]) + 1u;
         if (vb > 0u) q += wv_len(vb);
         if (lane == 0u) {
-            const uint64_t body = len - 8u;
-            for (int b = 0; b < 8; ++b) dst[b] = static_cast<uint8_t>(body >> (8 * (7 - b)));
+            put_be64(dst, len - 8u);
             uint64_t m = 8u;
             m += wv_put(dst + m, 0u);                                           // PeerMessage::Msg
             m += wv_put(dst + m, A.variant);
@@ -1444,8 +1370,7 @@ __global__ void __launch_bounds__(kAccThreads) request_write_kernel(const __grid
                     A.frame_off[f] = o;
                     A.frame_len[f] = static_cast<uint32_t>(len);
                     uint8_t *dst = A.out + o;
-                    const uint64_t body = len - 8u;
-                    for (int b = 0; b < 8; ++b) dst[b] = static_cast<uint8_t>(body >> (8 * (7 - b)));
+                    put_be64(dst, len - 8u);
                     uint32_t m = 8u;
                     m += wv_put(dst + m, 0u);                                   // PeerMessage::Msg
                     m += wv_put(dst + m, A.variant);

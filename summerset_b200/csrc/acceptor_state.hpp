@@ -1,6 +1,7 @@
 // acceptor_state.hpp -- the RSPaxos / Crossword acceptor handle (ss_acceptor_*) and the Accept body decoder, shared by
 // acceptor.cu and the WAL replay (acceptor_recover.cu).
 #pragma once
+#include "codeword_wire.cuh"
 #include "ss_internal.hpp"
 #include "wire_common.cuh"
 
@@ -53,9 +54,6 @@ struct ss_acceptor {
 namespace ssb {
 
 constexpr int kAccThreads = 256;
-constexpr uint32_t kPending = 0xfffffffeu;          // in the window, ballot not yet checked
-constexpr uint32_t kVariantLimit = 1u << 16;        // no enum of the protocol has this many variants: malformed
-constexpr uint64_t kMaxFrameBody = 0xffffffffull - 64u;   // longer frames are malformed: every record length fits a u32
 // WAL records in the window that are not AcceptData (ss_acceptor_recover)
 constexpr uint32_t kPendingPrepareBal = 0xfffffffdu;
 constexpr uint32_t kPendingCommitSlot = 0xfffffffcu;
@@ -78,22 +76,16 @@ __device__ __forceinline__ FrameHdr decode_frame(const Args &A, uint64_t i) {
     h.kind = SS_FRAME_KIND_MALFORMED;
     const uint32_t grp = A.frame_group[i];
     const uint64_t off = A.frame_off[i];
-    if (grp >= A.G || off > A.buf_len || A.buf_len - off < 8u) return h;
-    const uint8_t *fr = A.buf + off;
-    uint64_t len = 0;
-    for (int b = 0; b < 8; ++b) len = (len << 8) | fr[b];
-    if (len > A.buf_len - off - 8u || len > kMaxFrameBody) return h;
-    const uint8_t *b = fr + 8;
-    uint64_t n = 0, v = 0;
-    uint32_t c;
-#define SS_GET(dst) do { if (!(c = wv_get(b + n, len - n, (dst)))) return h; n += c; } while (0)
-    SS_GET(v);
+    if (grp >= A.G) return h;
+    const uint8_t *b;
+    uint64_t len, n = 0, v = 0;
     if constexpr (kWal) {
+        if (!frame_body(A.buf, A.buf_len, off, kMaxFrameBody, b, len) || !wv_next(b, len, n, v)) return h;
         if (v != A.wal_variant) {
             if (v != A.prepare_variant && v != A.commit_variant) return h;
             h.slot_at = static_cast<uint32_t>(8u + n);
-            SS_GET(h.slot);
-            if (v == A.prepare_variant) SS_GET(h.ballot);
+            if (!wv_next(b, len, n, h.slot)) return h;
+            if (v == A.prepare_variant && !wv_next(b, len, n, h.ballot)) return h;
             if (n != len) return h;
             h.end = 8u + len;
             const uint64_t base = A.window_base[grp];
@@ -104,54 +96,24 @@ __device__ __forceinline__ FrameHdr decode_frame(const Args &A, uint64_t i) {
             return h;
         }
     } else {
-        if (v != 0u) {                                                      // LeaseMsg / Leave / LeaveReply
-            if (v < kVariantLimit) h.kind = 0x80000000u | static_cast<uint32_t>(v);
-            return h;
-        }
-        SS_GET(v);
-        if (v != A.accept_variant) {                                        // another PeerMsg: the host's business
-            if (v < kVariantLimit) h.kind = static_cast<uint32_t>(v);
-            return h;
-        }
+        if (!msg_head(A.buf, A.buf_len, off, A.accept_variant, kMaxFrameBody, true, b, len, n, h.kind)) return h;
     }
     h.slot_at = static_cast<uint32_t>(8u + n);
-    SS_GET(h.slot);
-    SS_GET(h.ballot);
-    if (len - n < 2u || b[n] != A.d || b[n + 1] != A.T - A.d) return h;   // num_data_shards, num_parity_shards
-    n += 2;
-    uint64_t dl = 0, sl = 0;
-    SS_GET(dl);
-    SS_GET(sl);
-    SS_GET(v);
-    if (dl > 0xffffffffull || v != A.T || sl != (dl + A.d - 1u) / A.d) return h;   // rscoding.rs:177-181
-    h.tags_at = static_cast<uint32_t>(8u + n);
+    if (!wv_next(b, len, n, h.slot) || !wv_next(b, len, n, h.ballot)) return h;
+    uint64_t dl = 0, sl = 0, tags_at = 0;
     uint32_t held = 0;
-    for (uint32_t j = 0; j < A.T; ++j) {
-        if (n >= len) return h;
-        const uint8_t tag = b[n++];
-        if (tag == 0u) continue;
-        if (tag != 1u) return h;
-        SS_GET(v);
-        if (v != sl || len - n < sl) return h;
-        held |= 1u << j;
-        n += sl;
-    }
-    if (n >= len || b[n++] != 0u) return h;                                 // data_copy: None
+    if (!cw_parse<false>(b, len, n, A.d, A.T, dl, sl, tags_at, held)) return h;
+    h.tags_at = static_cast<uint32_t>(8u + tags_at);
     if (A.crossword) {                                                      // assignment: Vec<Bitmap>, one row per replica
-        SS_GET(v);
-        if (v != A.population) return h;
+        if (!wv_next(b, len, n, v) || v != A.population) return h;
         h.asg_at = static_cast<uint32_t>(8u + n);
         for (uint32_t r = 0; r < A.population; ++r) {
             uint64_t sz = 0, nb = 0, blk = 0;
-            SS_GET(sz);
-            SS_GET(nb);
-            if (sz != A.T || nb != 1u) return h;
-            SS_GET(blk);
-            if (blk >> A.T) return h;
+            if (!wv_next(b, len, n, sz) || !wv_next(b, len, n, nb) || sz != A.T || nb != 1u) return h;
+            if (!wv_next(b, len, n, blk) || (blk >> A.T)) return h;
             if (r == A.me) h.asg = static_cast<uint32_t>(blk);
         }
     }
-#undef SS_GET
     if (n != len) return h;
     h.end = 8u + len;
     h.held = held;

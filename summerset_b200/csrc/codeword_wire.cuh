@@ -1,8 +1,7 @@
-// codeword_wire.cuh -- the bincode RSCodeword on the device: the warp copies of its shards into padded store slots, shared
-// by the acceptor (acceptor.cu) and the CRaft follower (follower.cu), and the follower's codeword parser.
+// codeword_wire.cuh -- the bincode RSCodeword on the device, for every call that reads or writes one (the acceptor, the
+// CRaft follower, leader and reconstruct calls, the PrepareReply parser): its parser, its size, its warp writer, and the
+// warp copies of its shards into padded store slots.
 #pragma once
-#include "device_common.cuh"
-#include "ss_internal.hpp"
 #include "wire_common.cuh"
 
 namespace ssb {
@@ -17,6 +16,10 @@ __device__ __forceinline__ void warp_fill_slot(uint8_t *dst, const uint8_t *src,
     }
 }
 
+// A present shard's Some tag plus its length varint, from the varint's tag byte t: a non-minimal varint is as valid as
+// cw_parse found it, so its width comes from its own tag byte
+__device__ __forceinline__ uint64_t some_len(uint8_t t) { return 1u + (t < 251u ? 1u : t == 251u ? 3u : t == 252u ? 5u : 9u); }
+
 // the T shard Options of a bincode RSCodeword starting at tags (Option tag, length varint, bytes): the shards of `take`
 // (a subset of the present ones, `present`) go to their padded slots of the region at dst: one after the other, or with
 // a dst_mask, shard j at its rank among the shards of dst_mask
@@ -27,51 +30,95 @@ __device__ __forceinline__ void warp_fill_shards(uint8_t *dst, const uint8_t *ta
     uint32_t k = 0;
     for (uint32_t j = 0; j < T; ++j) {
         if (!((present >> j) & 1u)) { at += 1u; continue; }
-        // Some tag, then the shard length as the frame spells it: a non-minimal varint is as valid as the header pass
-        // found it, so its width comes from its own tag byte
-        const uint8_t t = tags[at + 1u];
-        const uint64_t some_len = 1u + (t < 251u ? 1u : t == 251u ? 3u : t == 252u ? 5u : 9u);
+        const uint64_t sl = some_len(tags[at + 1u]);
         if ((take >> j) & 1u) {
             const uint64_t slot = dst_mask == ~0ull ? k++ : static_cast<uint64_t>(__popc(static_cast<uint32_t>(dst_mask) & ((1u << j) - 1u)));
-            warp_fill_slot(dst + slot * pitch, tags + at + some_len, L, lane);
+            warp_fill_slot(dst + slot * pitch, tags + at + sl, L, lane);
         }
-        at += some_len + static_cast<uint64_t>(L);
+        at += sl + static_cast<uint64_t>(L);
     }
 }
 
-// An RSCodeword of the code (d, T) in the body b[0..len) from position n on (rscoding.rs:43-72), checked by the rules of
-// the acceptor's decode_frame (which keeps its own inline copy: calling this function from there changes the SASS of
-// acceptor_header_kernel): num_data_shards and
+// An RSCodeword of the code (d, T) in the body b[0..len) from position n on (rscoding.rs:43-72): num_data_shards and
 // num_parity_shards as raw bytes, data_len < 2^32, shard_len = ceil(data_len / d) (rscoding.rs:177-181), exactly T shard
-// Options each present one shard_len bytes, data_copy None.  On success n is past data_copy, tags_at is the position
-// of shard 0's Option tag counted from the frame's start (8 + the body position), held the
-// present shards, v is scratch; false: malformed or truncated (the outputs are then unspecified).
+// Options each present one shard_len bytes, then data_copy: None, or with kSomeCopy also Some(data_len bytes).  On
+// success n is past data_copy, tags_at is the body position of shard 0's Option tag and held the present shards;
+// false: malformed or truncated (the outputs are then unspecified).
+template <bool kSomeCopy>
 __device__ __forceinline__ bool cw_parse(const uint8_t *b, uint64_t len, uint64_t &n, uint32_t d, uint32_t T, uint64_t &dl,
-                                         uint64_t &sl, uint32_t &tags_at, uint32_t &held, uint64_t &v) {
-    uint32_t c;
+                                         uint64_t &sl, uint64_t &tags_at, uint32_t &held) {
+    uint64_t v = 0;
     if (len - n < 2u || b[n] != d || b[n + 1] != T - d) return false;      // num_data_shards, num_parity_shards
     n += 2;
-    if (!(c = wv_get(b + n, len - n, dl))) return false;
-    n += c;
-    if (!(c = wv_get(b + n, len - n, sl))) return false;
-    n += c;
-    if (!(c = wv_get(b + n, len - n, v))) return false;
-    n += c;
+    if (!wv_next(b, len, n, dl) || !wv_next(b, len, n, sl) || !wv_next(b, len, n, v)) return false;
     if (dl > 0xffffffffull || v != T || sl != (dl + d - 1u) / d) return false;
-    tags_at = static_cast<uint32_t>(8u + n);
+    tags_at = n;
     held = 0;
     for (uint32_t j = 0; j < T; ++j) {
         if (n >= len) return false;
         const uint8_t tag = b[n++];
         if (tag == 0u) continue;
-        if (tag != 1u) return false;
-        if (!(c = wv_get(b + n, len - n, v))) return false;
-        n += c;
-        if (v != sl || len - n < sl) return false;
+        if (tag != 1u || !wv_next(b, len, n, v) || v != sl || len - n < sl) return false;
         held |= 1u << j;
         n += sl;
     }
-    return n < len && b[n++] == 0u;                                         // data_copy: None
+    if (n >= len) return false;
+    const uint8_t tag = b[n++];                                             // data_copy
+    if (kSomeCopy && tag == 1u) {
+        if (len - n < dl) return false;
+        n += dl;
+        return true;
+    }
+    return tag == 0u;
+}
+
+// bytes of a bincode RSCodeword of data_len dl under the code (d, T) carrying k shards: d, p, data_len, shard_len, T,
+// T shard Options, data_copy None
+__device__ __forceinline__ uint64_t cw_bytes(uint64_t dl, uint32_t d, uint32_t T, uint32_t k) {
+    const uint64_t L = (dl + d - 1u) / d;
+    return 2u + wv_len(dl) + wv_len(L) + wv_len(T) + T + static_cast<uint64_t>(k) * (wv_len(L) + L) + 1u;
+}
+
+// shard j of a codeword whose shards sit in planes: src + j * plane_stride
+struct Planes {
+    const uint8_t *src;
+    uint64_t stride;
+    __device__ __forceinline__ const uint8_t *operator()(uint32_t j) const { return src + static_cast<uint64_t>(j) * stride; }
+};
+
+// That codeword carrying the shards `mask`, written by a warp at p (any alignment): lane 0 writes the varints and the
+// Option tags, the warp copies shard j from shard(j), a 16-byte aligned address: a store slot by rank (the follower's
+// reconstruct serve passes a lambda) or a plane (Planes).  Returns its bytes.
+template <typename Src>
+__device__ __forceinline__ uint64_t warp_put_cw(uint8_t *p, uint32_t d, uint32_t T, uint64_t dl, uint32_t mask, Src &&shard,
+                                                uint32_t lane) {
+    const uint64_t L = (dl + d - 1u) / d;
+    const uint32_t wl = static_cast<uint32_t>(wv_len(L));
+    if (lane == 0u) {
+        p[0] = static_cast<uint8_t>(d);
+        p[1] = static_cast<uint8_t>(T - d);
+        uint64_t m = 2u;
+        m += wv_put(p + m, dl);
+        m += wv_put(p + m, L);
+        wv_put(p + m, T);
+    }
+    uint64_t m = 2u + wv_len(dl) + wl + wv_len(T);
+    for (uint32_t j = 0; j < T; ++j) {
+        if ((mask >> j) & 1u) {
+            if (lane == 0u) {
+                p[m] = 1u;
+                wv_put(p + m + 1u, L);
+            }
+            m += 1u + wl;
+            warp_copy_bytes(p + m, shard(j), static_cast<uint32_t>(L), lane);
+            m += L;
+        } else {
+            if (lane == 0u) p[m] = 0u;
+            m += 1u;
+        }
+    }
+    if (lane == 0u) p[m] = 0u;                                            // data_copy: None
+    return m + 1u;
 }
 
 }  // namespace ssb

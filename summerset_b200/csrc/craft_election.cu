@@ -109,7 +109,7 @@ __global__ void __launch_bounds__(kElThreads) campaign_kernel(const __grid_const
             m += wv_put(cell + m, nt);
             m += wv_put(cell + m, last);
             m += wv_put(cell + m, A.term[static_cast<uint64_t>(g) * A.W + (last & (A.W - 1u))]);
-            cl_put_be64(cell, m - 8u);
+            put_be64(cell, m - 8u);
             for (uint32_t q = m; q < kVoteCell; ++q) cell[q] = 0u;
             A.frame_len[i] = m;
             A.verdict[i] = SS_CAMPAIGN_VERDICT_DONE;
@@ -130,8 +130,8 @@ __device__ __forceinline__ void el_head(const ElectArgs &A) {
             A.reply_len[i] = 0u;
             A.reply_dst[i] = kNone;
         }
-        if (kind != kElPending) A.verdict[i] = kind;
-        A.key_in[i] = kind == kElPending ? A.frame_group[i] : static_cast<uint32_t>(A.G);
+        if (kind != kPending) A.verdict[i] = kind;
+        A.key_in[i] = kind == kPending ? A.frame_group[i] : static_cast<uint32_t>(A.G);
         A.idx_in[i] = static_cast<uint32_t>(i);
     }
 }
@@ -146,7 +146,7 @@ __device__ __forceinline__ uint32_t el_put_reply(uint8_t *cell, uint32_t variant
     m += wv_put(cell + m, variant);
     m += wv_put(cell + m, term);
     cell[m++] = granted ? 1u : 0u;
-    cl_put_be64(cell, m - 8u);
+    put_be64(cell, m - 8u);
     for (uint32_t q = m; q < kReplyCell; ++q) cell[q] = 0u;
     return m;
 }
@@ -347,7 +347,7 @@ int ss_follower_vote_view_get(ss_follower *f, ss_follower_vote_view *v) {
 int ss_follower_campaign(ss_follower *f, const uint32_t *groups, uint64_t n_listed, const uint8_t *timeout_source,
                          uint32_t request_vote_variant, uint8_t *meta, uint32_t *meta_len, uint8_t *frames, uint32_t *frame_len,
                          uint8_t *frame_dst, uint32_t *verdict) {
-    if (request_vote_variant >= kElVariantLimit) return set_error(SS_ERR_INVALID_ARG, "request_vote_variant must be < 2^16");
+    if (request_vote_variant >= kVariantLimit) return set_error(SS_ERR_INVALID_ARG, "request_vote_variant must be < 2^16");
     if (f == nullptr) return set_error(SS_ERR_INVALID_ARG, "null follower");
     ss_ctx *ctx = f->ctx;
     SS_TRY(ctx_bind(ctx));
@@ -374,7 +374,7 @@ int ss_follower_campaign(ss_follower *f, const uint32_t *groups, uint64_t n_list
 int ss_follower_vote(ss_follower *f, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
                      const uint8_t *frame_peer, uint64_t n, uint32_t request_vote_variant, uint32_t reply_variant, uint8_t *meta,
                      uint32_t *meta_len, uint8_t *replies, uint32_t *reply_len, uint8_t *reply_dst, uint32_t *verdict) {
-    if (request_vote_variant >= kElVariantLimit || reply_variant >= kElVariantLimit)
+    if (request_vote_variant >= kVariantLimit || reply_variant >= kVariantLimit)
         return set_error(SS_ERR_INVALID_ARG, "the variants must be < 2^16");
     if (f == nullptr) return set_error(SS_ERR_INVALID_ARG, "null follower");
     ss_ctx *ctx = f->ctx;
@@ -401,7 +401,7 @@ int ss_follower_vote(ss_follower *f, const uint8_t *buf, uint64_t buf_len, const
 int ss_follower_tally(ss_follower *f, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
                       const uint8_t *frame_peer, uint64_t n, uint32_t reply_variant, uint8_t *meta, uint32_t *meta_len, uint32_t *verdict,
                       uint32_t *won_group, uint64_t *won_term, uint64_t *n_won) {
-    if (reply_variant >= kElVariantLimit) return set_error(SS_ERR_INVALID_ARG, "reply_variant must be < 2^16");
+    if (reply_variant >= kVariantLimit) return set_error(SS_ERR_INVALID_ARG, "reply_variant must be < 2^16");
     if (f == nullptr) return set_error(SS_ERR_INVALID_ARG, "null follower");
     ss_ctx *ctx = f->ctx;
     SS_TRY(ctx_bind(ctx));

@@ -9,34 +9,6 @@
 
 namespace ssb {
 
-// ---- the head every PeerMsg frame starts with (the reconstruct calls' decoder, craft_recon.cu) -----------------------
-constexpr uint32_t kRcVariantLimit = 1u << 16;
-constexpr uint32_t kRcPending = 0xfffffffeu;
-
-// the 8-byte length, PeerMessage::Msg and the PeerMsg variant of the frame at buf + off; kRcPending with b / len / n past
-// the element count (cnt) when it is `variant`
-__device__ __forceinline__ uint32_t rc_head(const uint8_t *buf, uint64_t buf_len, uint64_t off, uint32_t variant, const uint8_t *&b,
-                                            uint64_t &len, uint64_t &n, uint64_t &cnt) {
-    if (off > buf_len || buf_len - off < 8u) return SS_FRAME_KIND_MALFORMED;
-    const uint8_t *fr = buf + off;
-    len = 0;
-    for (int k = 0; k < 8; ++k) len = (len << 8) | fr[k];
-    if (len > buf_len - off - 8u) return SS_FRAME_KIND_MALFORMED;
-    b = fr + 8;
-    n = 0;
-    uint64_t v = 0;
-    uint32_t c;
-    if (!(c = wv_get(b + n, len - n, v))) return SS_FRAME_KIND_MALFORMED;
-    n += c;
-    if (v != 0u) return v < kRcVariantLimit ? 0x80000000u | static_cast<uint32_t>(v) : SS_FRAME_KIND_MALFORMED;
-    if (!(c = wv_get(b + n, len - n, v))) return SS_FRAME_KIND_MALFORMED;
-    n += c;
-    if (v != variant) return v < kRcVariantLimit ? static_cast<uint32_t>(v) : SS_FRAME_KIND_MALFORMED;
-    if (!(c = wv_get(b + n, len - n, cnt))) return SS_FRAME_KIND_MALFORMED;
-    n += c;
-    return kRcPending;
-}
-
 // ---- AppendEntries (the follower's decoder) ------------------------------------------------------------------------
 // one decoded AppendEntries frame
 struct FolHdr {
@@ -52,10 +24,6 @@ struct Ent {
     uint64_t term, dl, sl;
     uint32_t held, tags_at, start, ext_end, next;
 };
-
-constexpr uint32_t kFolPending = 0xfffffffeu;
-constexpr uint32_t kFolVariantLimit = 1u << 16;
-constexpr uint64_t kFolMaxBody = 0xffffffffull - 64u;
 
 struct FolArgs {
     const uint8_t *buf;
@@ -91,17 +59,14 @@ struct FolArgs {
 __device__ __forceinline__ bool ent_parse(const uint8_t *fr, uint64_t end, uint64_t at, uint32_t d, uint32_t T, Ent &e) {
     const uint8_t *b = fr + 8;
     const uint64_t len = end - 8u;
-    uint64_t n = at - 8u, v = 0, term = 0, dl = 0, sl = 0;
-    uint32_t c, tags_at = 0, held = 0;
-    if (!(c = wv_get(b + n, len - n, term))) return false;
-    n += c;
-    if (!cw_parse(b, len, n, d, T, dl, sl, tags_at, held, v)) return false;
+    uint64_t n = at - 8u, v = 0, term = 0, dl = 0, sl = 0, tags_at = 0;
+    uint32_t held = 0;
+    if (!wv_next(b, len, n, term) || !cw_parse<false>(b, len, n, d, T, dl, sl, tags_at, held)) return false;
     if (n >= len || b[n] > 1u) return false;                                // external: bool
     const uint32_t ext_end = static_cast<uint32_t>(8u + n + 1u);
     ++n;
-    if (!(c = wv_get(b + n, len - n, v))) return false;                     // log_offset, dropped
-    n += c;
-    e.term = term; e.dl = dl; e.sl = sl; e.held = held; e.tags_at = tags_at;
+    if (!wv_next(b, len, n, v)) return false;                               // log_offset, dropped
+    e.term = term; e.dl = dl; e.sl = sl; e.held = held; e.tags_at = static_cast<uint32_t>(8u + tags_at);
     e.start = static_cast<uint32_t>(at); e.ext_end = ext_end; e.next = static_cast<uint32_t>(8u + n);
     return true;
 }
@@ -119,30 +84,14 @@ __device__ __forceinline__ FolHdr fol_decode(const FolArgs &A, uint64_t i) {
     h.kind = SS_FRAME_KIND_MALFORMED;
     const uint32_t grp = A.frame_group[i];
     const uint64_t off = A.frame_off[i];
-    if (grp >= A.G || A.frame_peer[i] == A.me || A.frame_peer[i] >= A.population || off > A.buf_len || A.buf_len - off < 8u) return h;
-    const uint8_t *fr = A.buf + off;
-    uint64_t len = 0;
-    for (int b = 0; b < 8; ++b) len = (len << 8) | fr[b];
-    if (len > A.buf_len - off - 8u || len > kFolMaxBody) return h;
-    const uint8_t *b = fr + 8;
-    uint64_t n = 0, v = 0;
-    uint32_t c;
-#define SS_GET(dst) do { if (!(c = wv_get(b + n, len - n, (dst)))) return h; n += c; } while (0)
-    SS_GET(v);
-    if (v != 0u) {                                                          // LeaseMsg / Leave / LeaveReply
-        if (v < kFolVariantLimit) h.kind = 0x80000000u | static_cast<uint32_t>(v);
-        return h;
-    }
-    SS_GET(v);
-    if (v != A.append_variant) {                                            // another PeerMsg: the host's business
-        if (v < kFolVariantLimit) h.kind = static_cast<uint32_t>(v);
-        return h;
-    }
+    if (grp >= A.G || A.frame_peer[i] == A.me || A.frame_peer[i] >= A.population) return h;
+    const uint8_t *b;
+    uint64_t len, n;
+    if (!msg_head(A.buf, A.buf_len, off, A.append_variant, kMaxFrameBody, true, b, len, n, h.kind)) return h;
+    const uint8_t *fr = b - 8;
     uint64_t term = 0, prev = 0, prev_term = 0, n_ent = 0;
-    SS_GET(term);
-    SS_GET(prev);
-    SS_GET(prev_term);
-    SS_GET(n_ent);
+    if (!wv_next(b, len, n, term) || !wv_next(b, len, n, prev) || !wv_next(b, len, n, prev_term) || !wv_next(b, len, n, n_ent))
+        return h;
     const uint64_t ents_at = 8u + n;
     uint64_t sz = 0, wz = 0;
     for (uint64_t k = 0; k < n_ent; ++k) {
@@ -153,10 +102,7 @@ __device__ __forceinline__ FolHdr fol_decode(const FolArgs &A, uint64_t i) {
         n = e.next - 8u;
     }
     uint64_t commit = 0, snap = 0;
-    SS_GET(commit);
-    SS_GET(snap);
-#undef SS_GET
-    if (n != len) return h;
+    if (!wv_next(b, len, n, commit) || !wv_next(b, len, n, snap) || n != len) return h;
     h.term = term; h.prev = prev; h.prev_term = prev_term; h.n_ent = n_ent; h.commit = commit; h.snap = snap;
     h.store_sz = sz; h.wal_sz = wz;
     h.ents_at = static_cast<uint32_t>(ents_at);
@@ -164,7 +110,7 @@ __device__ __forceinline__ FolHdr fol_decode(const FolArgs &A, uint64_t i) {
     // every entry inside [start_slot, start_slot + window): the ring holds them
     const uint64_t start = A.start_slot[grp];
     const bool beyond = n_ent != 0u && (prev + n_ent < prev || prev + n_ent >= start + A.W);
-    h.kind = beyond ? SS_FOLLOWER_VERDICT_BEYOND_WINDOW : kFolPending;
+    h.kind = beyond ? SS_FOLLOWER_VERDICT_BEYOND_WINDOW : kPending;
     return h;
 }
 
@@ -177,31 +123,14 @@ __device__ __forceinline__ uint32_t reply_parse(const uint8_t *buf, uint64_t buf
                                                 uint64_t &c_term, uint64_t &c_slot) {
     uint32_t kind = SS_FRAME_KIND_MALFORMED;
     do {
-        if (grp >= G || off > buf_len || buf_len - off < 8u) break;
-        const uint8_t *fr = buf + off;
-        uint64_t len = 0;
-        for (int b = 0; b < 8; ++b) len = (len << 8) | fr[b];
-        if (len > buf_len - off - 8u) break;
-        const uint8_t *b = fr + 8;
-        uint64_t n = 0, v = 0;
-        uint32_t c;
-        if (!(c = wv_get(b + n, len - n, v))) break;
-        n += c;
-        if (v != 0u) { if (v < kFolVariantLimit) kind = 0x80000000u | static_cast<uint32_t>(v); break; }
-        if (!(c = wv_get(b + n, len - n, v))) break;
-        n += c;
-        if (v != reply_variant) { if (v < kFolVariantLimit) kind = static_cast<uint32_t>(v); break; }
-        if (!(c = wv_get(b + n, len - n, term))) break;
-        n += c;
-        if (!(c = wv_get(b + n, len - n, end))) break;
-        n += c;
+        const uint8_t *b;
+        uint64_t len, n;
+        if (grp >= G || !msg_head(buf, buf_len, off, reply_variant, ~0ull, true, b, len, n, kind)) break;
+        if (!wv_next(b, len, n, term) || !wv_next(b, len, n, end)) break;
         if (n >= len) break;
         const uint8_t tag = b[n++];
         if (tag == 1u) {
-            if (!(c = wv_get(b + n, len - n, c_term))) break;
-            n += c;
-            if (!(c = wv_get(b + n, len - n, c_slot))) break;
-            n += c;
+            if (!wv_next(b, len, n, c_term) || !wv_next(b, len, n, c_slot)) break;
         } else if (tag != 0u) {
             break;
         }
@@ -216,8 +145,6 @@ __device__ __forceinline__ uint32_t reply_parse(const uint8_t *buf, uint64_t buf
 }
 
 // ---- RequestVote and RequestVoteReply (the election decoders) -------------------------------------------------------
-constexpr uint32_t kElVariantLimit = 1u << 16;
-constexpr uint32_t kElPending = 0xfffffffeu;
 constexpr uint8_t kNone = 0xffu;                 // ReplicaId::MAX: voted_for None, leader None
 constexpr uint32_t kMetaCell = 32u;
 
@@ -227,7 +154,7 @@ __device__ __forceinline__ uint32_t el_put_meta(uint8_t *cell, uint32_t variant,
     m += wv_put(cell + m, variant);
     m += wv_put(cell + m, term);
     cell[m++] = voted_for;
-    cl_put_be64(cell, m - 8u);
+    put_be64(cell, m - 8u);
     for (uint32_t q = m; q < kMetaCell; ++q) cell[q] = 0u;
     return m;
 }
@@ -261,37 +188,27 @@ struct ElectArgs {
 };
 
 // Frame i: PeerMessage::Msg{RequestVote{term, last_slot, last_term}} (kReply false) or
-// PeerMessage::Msg{RequestVoteReply{term, granted}} (kReply true: f1 = granted).  kElPending when it is one, else its
+// PeerMessage::Msg{RequestVoteReply{term, granted}} (kReply true: f1 = granted).  kPending when it is one, else its
 // verdict: another message's variant index (0x80000000 | k for PeerMessage variants) or SS_FRAME_KIND_MALFORMED
 template <bool kReply>
 __device__ __forceinline__ uint32_t el_decode(const ElectArgs &A, uint64_t i, uint64_t &f0, uint64_t &f1, uint64_t &f2) {
     const uint32_t g = A.frame_group[i];
     const uint64_t off = A.frame_off[i];
     const uint8_t peer = A.frame_peer[i];
-    if (g >= A.G || peer == A.me || peer >= A.population || off > A.buf_len || A.buf_len - off < 8u) return SS_FRAME_KIND_MALFORMED;
-    const uint8_t *fr = A.buf + off;
-    uint64_t len = 0;
-    for (int k = 0; k < 8; ++k) len = (len << 8) | fr[k];
-    if (len > A.buf_len - off - 8u) return SS_FRAME_KIND_MALFORMED;
-    const uint8_t *b = fr + 8;
-    uint64_t n = 0, v = 0;
-    uint32_t c;
-#define SS_GET(dst) do { if (!(c = wv_get(b + n, len - n, (dst)))) return SS_FRAME_KIND_MALFORMED; n += c; } while (0)
-    SS_GET(v);
-    if (v != 0u) return v < kElVariantLimit ? 0x80000000u | static_cast<uint32_t>(v) : SS_FRAME_KIND_MALFORMED;
-    SS_GET(v);
-    if (v != A.variant) return v < kElVariantLimit ? static_cast<uint32_t>(v) : SS_FRAME_KIND_MALFORMED;
-    SS_GET(f0);
+    if (g >= A.G || peer == A.me || peer >= A.population) return SS_FRAME_KIND_MALFORMED;
+    const uint8_t *b;
+    uint64_t len, n;
+    uint32_t kind;
+    if (!msg_head(A.buf, A.buf_len, off, A.variant, ~0ull, true, b, len, n, kind)) return kind;
+    if (!wv_next(b, len, n, f0)) return SS_FRAME_KIND_MALFORMED;
     if (kReply) {
         if (n >= len || b[n] > 1u) return SS_FRAME_KIND_MALFORMED;  // bool
         f1 = b[n++];
         f2 = 0u;
-    } else {
-        SS_GET(f1);
-        SS_GET(f2);
+    } else if (!wv_next(b, len, n, f1) || !wv_next(b, len, n, f2)) {
+        return SS_FRAME_KIND_MALFORMED;
     }
-#undef SS_GET
-    return n == len ? kElPending : SS_FRAME_KIND_MALFORMED;
+    return n == len ? kPending : SS_FRAME_KIND_MALFORMED;
 }
 
 }  // namespace ssb

@@ -30,6 +30,7 @@
 #include <cstring>
 #include <new>
 
+#include "codeword_wire.cuh"
 #include "device_common.cuh"
 #include "engine_state.hpp"
 #include "exec_walk.cuh"
@@ -41,53 +42,11 @@ namespace ssb {
 
 constexpr int kClThreads = 256;
 constexpr uint32_t kLogEntryVariant = 1u;          // DurEntry::LogEntry (craft/mod.rs:148-159: Metadata 0, LogEntry 1)
-constexpr uint32_t kClVariantLimit = 1u << 16;
 
 // one status write per warp, not one per flagged item
 __device__ __forceinline__ void cl_warp_status(bool flag, uint32_t bit, uint32_t *status) {
     const unsigned any = __ballot_sync(__activemask(), flag);
     if (flag && (threadIdx.x & 31u) == static_cast<unsigned>(__ffs(static_cast<int>(any)) - 1)) atomicOr(status, bit);
-}
-
-// bytes of the bincode RSCodeword of a data_len dl batch under the code (d, T) holding `nsh` shards (rscoding.rs:43-72):
-// num_data_shards and num_parity_shards as raw bytes, data_len, shard_len and the shard count as varints, T Options, and
-// data_copy None
-__device__ __forceinline__ uint64_t cw_bytes(uint64_t dl, uint32_t d, uint32_t T, uint32_t nsh) {
-    const uint64_t L = (dl + d - 1u) / d;
-    return 2u + wv_len(dl) + wv_len(L) + wv_len(T) + T + static_cast<uint64_t>(nsh) * (wv_len(L) + L) + 1u;
-}
-
-// the same codeword written by a warp at p: lane 0 writes the varints and tags, the warp copies shard j of `mask` from
-// src + j*plane_stride (16-byte aligned); returns its bytes
-__device__ __forceinline__ uint64_t warp_put_cw(uint8_t *p, uint64_t dl, uint32_t d, uint32_t T, uint32_t mask, const uint8_t *src,
-                                                uint64_t plane_stride, uint32_t lane) {
-    const uint64_t L = (dl + d - 1u) / d;
-    const uint32_t wl = static_cast<uint32_t>(wv_len(L));
-    if (lane == 0u) {
-        p[0] = static_cast<uint8_t>(d);
-        p[1] = static_cast<uint8_t>(T - d);
-        uint64_t m = 2u;
-        m += wv_put(p + m, dl);
-        m += wv_put(p + m, L);
-        wv_put(p + m, T);
-    }
-    uint64_t m = 2u + wv_len(dl) + wl + wv_len(T);
-    for (uint32_t j = 0; j < T; ++j) {
-        if ((mask >> j) & 1u) {
-            if (lane == 0u) {
-                p[m] = 1u;
-                wv_put(p + m + 1u, L);
-            }
-            m += 1u + wl;
-            warp_copy_bytes(p + m, src + static_cast<uint64_t>(j) * plane_stride, static_cast<uint32_t>(L), lane);
-            m += L;
-        } else {
-            if (lane == 0u) p[m] = 0u;
-            m += 1u;
-        }
-    }
-    if (lane == 0u) p[m] = 0u;                                            // data_copy: None
-    return m + 1u;
 }
 
 // ---- propose -------------------------------------------------------------------------------------------------------
@@ -196,12 +155,12 @@ __global__ void __launch_bounds__(kClThreads) craft_propose_wal_kernel(const __g
         const uint32_t t = A.curr_term[g];
         const uint64_t rl = A.wal_len[g];
         if (lane == 0u) {
-            cl_put_be64(rec, rl - 8u);
+            put_be64(rec, rl - 8u);
             const int m = 8 + wv_put(rec + 8, kLogEntryVariant);
             wv_put(rec + m, t);
         }
         const uint64_t m = 8u + wv_len(kLogEntryVariant) + wv_len(t);
-        const uint64_t c = warp_put_cw(rec + m, len, A.d, A.T, mask, A.shards + A.shard_off[g], A.plane_stride, lane);
+        const uint64_t c = warp_put_cw(rec + m, A.d, A.T, len, mask, Planes{A.shards + A.shard_off[g], A.plane_stride}, lane);
         if (lane == 0u) {
             rec[m + c] = 1u;                                                // external: true
             rec[m + c + 1u] = 0u;                                           // log_offset: 0
@@ -425,7 +384,7 @@ __global__ void __launch_bounds__(kClThreads) append_write_kernel(const __grid_c
         const uint32_t want = peer_want(A, q);
         uint8_t *fr = A.out + A.frame_off[f];
         if (lane == 0u) {
-            cl_put_be64(fr, A.frame_len[f] - 8u);
+            put_be64(fr, A.frame_len[f] - 8u);
             uint64_t m = 8u;
             m += wv_put(fr + m, 0u);                                        // PeerMessage::Msg
             m += wv_put(fr + m, A.variant);
@@ -443,7 +402,8 @@ __global__ void __launch_bounds__(kClThreads) append_write_kernel(const __grid_c
             const uint64_t lof = A.ent_log_offset[pos];
             if (lane == 0u) wv_put(fr + m, et);
             m += wv_len(et);
-            m += warp_put_cw(fr + m, A.ent_len[pos], A.d, A.T, pack_mask<kHeld>(A, pos, want), reinterpret_cast<const uint8_t *>(A.ent_addr[pos]), A.plane_stride, lane);
+            m += warp_put_cw(fr + m, A.d, A.T, A.ent_len[pos], pack_mask<kHeld>(A, pos, want),
+                             Planes{reinterpret_cast<const uint8_t *>(A.ent_addr[pos]), A.plane_stride}, lane);
             if (lane == 0u) {
                 fr[m] = 0u;
                 wv_put(fr + m + 1u, lof);
@@ -458,33 +418,16 @@ __global__ void __launch_bounds__(kClThreads) append_write_kernel(const __grid_c
 }
 
 // ---- conflict back-off ---------------------------------------------------------------------------------------------
-// PeerMessage::Msg{AppendEntriesReply{term, end_slot, conflict: Some((conflict_term, conflict_slot))}}; the leader's parser
-// (follower.cu, append_reply_parse_kernel) keeps its own decode so that its code stays as it is
+// PeerMessage::Msg{AppendEntriesReply{term, end_slot, conflict: Some((conflict_term, conflict_slot))}}
 __device__ __forceinline__ bool conflict_decode(const uint8_t *buf, uint64_t buf_len, uint64_t off, uint32_t variant, uint64_t &end,
                                                 uint64_t &c_term, uint64_t &c_slot) {
-    if (off > buf_len || buf_len - off < 8u) return false;
-    const uint8_t *fr = buf + off;
-    uint64_t len = 0;
-    for (int b = 0; b < 8; ++b) len = (len << 8) | fr[b];
-    if (len > buf_len - off - 8u) return false;
-    const uint8_t *b = fr + 8;
-    uint64_t n = 0, v = 0;
-    uint32_t c;
-    if (!(c = wv_get(b + n, len - n, v)) || v != 0u) return false;
-    n += c;
-    if (!(c = wv_get(b + n, len - n, v)) || v != variant) return false;
-    n += c;
-    if (!(c = wv_get(b + n, len - n, v))) return false;                     // term
-    n += c;
-    if (!(c = wv_get(b + n, len - n, end))) return false;
-    n += c;
-    if (n >= len || b[n] != 1u) return false;
+    const uint8_t *b;
+    uint64_t len, n, term = 0;
+    uint32_t kind;
+    if (!msg_head(buf, buf_len, off, variant, ~0ull, true, b, len, n, kind)) return false;
+    if (!wv_next(b, len, n, term) || !wv_next(b, len, n, end) || n >= len || b[n] != 1u) return false;
     ++n;
-    if (!(c = wv_get(b + n, len - n, c_term))) return false;
-    n += c;
-    if (!(c = wv_get(b + n, len - n, c_slot))) return false;
-    n += c;
-    return n == len;
+    return wv_next(b, len, n, c_term) && wv_next(b, len, n, c_slot) && n == len;
 }
 
 struct BackoffArgs {
@@ -765,7 +708,7 @@ int ss_frame_append_pack_dev(ss_engine *e, const ss_append_pack_spec *spec, cons
                              uint64_t *n_frames, uint32_t *pair_status, uint64_t *total) {
     if (spec == nullptr) return set_error(SS_ERR_INVALID_ARG, "null spec");
     if (spec->msg_chunk_size == 0) return set_error(SS_ERR_INVALID_ARG, "msg_chunk_size must be >= 1");
-    if (spec->append_variant >= kClVariantLimit) return set_error(SS_ERR_INVALID_ARG, "append_variant must be < 2^16");
+    if (spec->append_variant >= kVariantLimit) return set_error(SS_ERR_INVALID_ARG, "append_variant must be < 2^16");
     if (reinterpret_cast<uintptr_t>(out) & 15u) return set_error(SS_ERR_INVALID_ARG, "out must be 16-byte aligned");
     SS_TRY(craft_check(e));
     if (spec->me >= e->n) return set_error(SS_ERR_INVALID_ARG, "me %u >= population %u", spec->me, e->n);
@@ -810,7 +753,7 @@ int ss_frame_append_pack_dev(ss_engine *e, const ss_append_pack_spec *spec, cons
 int ss_engine_craft_backoff(ss_engine *e, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
                             const uint8_t *frame_peer, const uint32_t *rec_kind, uint64_t n_frames, uint32_t reply_variant,
                             uint64_t *want_end) {
-    if (reply_variant >= kClVariantLimit) return set_error(SS_ERR_INVALID_ARG, "reply_variant must be < 2^16");
+    if (reply_variant >= kVariantLimit) return set_error(SS_ERR_INVALID_ARG, "reply_variant must be < 2^16");
     SS_TRY(craft_check(e));
     if (want_end == nullptr) return set_error(SS_ERR_INVALID_ARG, "null want_end");
     const uint64_t PG = uint64_t(e->n_peers) * e->G;

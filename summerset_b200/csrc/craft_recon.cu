@@ -283,7 +283,7 @@ __global__ void __launch_bounds__(kRcThreads) recon_write_kernel(const __grid_co
             ++k;
             last = s;
             if (k % A.chunk == 0u || k == total) {                          // its last entry: the length and the records
-                cl_put_be64(fr, at - 8u);
+                put_be64(fr, at - 8u);
                 A.frame_group[f] = g;
                 A.frame_dst[f] = 0xffu;
                 A.frame_off[f] = o;
@@ -313,34 +313,24 @@ struct ServeArgs {
     uint32_t *verdict, *status;
 };
 
-// bytes of a bincode RSCodeword carrying the shards m: d, p, data_len, shard_len, T shard Options, data_copy None
-__device__ __forceinline__ uint64_t rc_cw_bytes(uint32_t d, uint32_t T, uint64_t dl, uint32_t m) {
-    const uint64_t L = (dl + d - 1u) / d, k = static_cast<uint64_t>(__popc(m));
-    return 2u + wv_len(dl) + wv_len(L) + wv_len(T) + (T - k) + k * (1u + wv_len(L) + L) + 1u;
-}
-
 // The Reconstruct{slots: Vec<(usize, Term)>} of frame i walked as handle_msg_reconstruct walks it: f(slot, ring
 // position) for each entry the reply carries -- inside [start_slot, log_end) with the ring's term, and not an earlier
 // entry's (slot, term) again (the map keeps one entry per slot; entries follow their first occurrence).  Returns
-// kRcPending for a well-formed frame, else its verdict.
+// kPending for a well-formed frame, else its verdict.
 template <typename F>
 __device__ __forceinline__ uint32_t serve_walk(const ServeArgs &A, uint64_t i, F &&f) {
     const uint8_t *b = nullptr;
     uint64_t len = 0, n = 0, cnt = 0;
     const uint32_t g = A.frame_group[i];
     if (g >= A.G) return SS_FRAME_KIND_MALFORMED;
-    const uint32_t kind = rc_head(A.buf, A.buf_len, A.frame_off[i], A.variant, b, len, n, cnt);
-    if (kind != kRcPending) return kind;
+    const uint32_t kind = msg_head_count(A.buf, A.buf_len, A.frame_off[i], A.variant, ~0ull, b, len, n, cnt);
+    if (kind != kPending) return kind;
     const uint64_t st = A.start_slot[g], le = A.log_end[g], row = static_cast<uint64_t>(g) * A.FW;
     const uint64_t n0 = n;
-    uint32_t c;
     bool rising = true;                                                     // slots strictly rising: no entry repeats
     for (uint64_t e = 0, prev = 0; e < cnt; ++e) {
         uint64_t slot = 0, t = 0;
-        if (!(c = wv_get(b + n, len - n, slot))) return SS_FRAME_KIND_MALFORMED;
-        n += c;
-        if (!(c = wv_get(b + n, len - n, t))) return SS_FRAME_KIND_MALFORMED;
-        n += c;
+        if (!wv_next(b, len, n, slot) || !wv_next(b, len, n, t)) return SS_FRAME_KIND_MALFORMED;
         rising &= e == 0u || slot > prev;
         prev = slot;
     }
@@ -362,7 +352,7 @@ __device__ __forceinline__ uint32_t serve_walk(const ServeArgs &A, uint64_t i, F
         }
         if (!seen) f(slot, pos);
     }
-    return kRcPending;
+    return kPending;
 }
 
 __global__ void __launch_bounds__(kRcThreads) serve_size_kernel(const __grid_constant__ ServeArgs A) {
@@ -371,9 +361,9 @@ __global__ void __launch_bounds__(kRcThreads) serve_size_kernel(const __grid_con
         uint64_t cnt = 0, bytes = 0;
         uint32_t kind = serve_walk(A, i, [&](uint64_t slot, uint64_t pos) {
             ++cnt;
-            bytes += wv_len(slot) + rc_cw_bytes(A.d, A.T, A.data_len[pos], A.held[pos]);
+            bytes += wv_len(slot) + cw_bytes(A.data_len[pos], A.d, A.T, __popc(A.held[pos]));
         });
-        if (kind == kRcPending) kind = SS_ACCEPT_VERDICT_ACCEPTED;
+        if (kind == kPending) kind = SS_ACCEPT_VERDICT_ACCEPTED;
         if (kind != SS_ACCEPT_VERDICT_ACCEPTED || cnt == 0u) bytes = 0;
         else bytes += 9u + wv_len(A.reply_variant) + wv_len(cnt);
         A.verdict[i] = kind;
@@ -408,43 +398,21 @@ __global__ void __launch_bounds__(kRcThreads, 1) serve_write_kernel(const __grid
         uint8_t *dst = A.out + off;
         uint64_t at = 8u + 1u + wv_len(A.reply_variant) + wv_len(cnt);
         if (lane == 0u) {
-            cl_put_be64(dst, len - 8u);
+            put_be64(dst, len - 8u);
             uint64_t m = 8u;
             m += wv_put(dst + m, 0u);                                       // PeerMessage::Msg
             m += wv_put(dst + m, A.reply_variant);
             wv_put(dst + m, cnt);
         }
         serve_walk(A, i, [&](uint64_t slot, uint64_t pos) {
-            const uint32_t d = A.d, T = A.T, held = A.held[pos];
-            const uint64_t dl = A.data_len[pos], L = (dl + d - 1u) / d, pitch = SS_CW_SLOT_PITCH(L);
+            const uint32_t held = A.held[pos];
+            const uint64_t dl = A.data_len[pos], pitch = SS_CW_SLOT_PITCH((dl + A.d - 1u) / A.d);
             const uint8_t *src = reinterpret_cast<const uint8_t *>(A.shard_addr[pos]);
-            uint8_t *e = dst + at;
-            if (lane == 0u) {
-                uint64_t q = wv_put(e, slot);
-                e[q++] = static_cast<uint8_t>(d);
-                e[q++] = static_cast<uint8_t>(T - d);
-                q += wv_put(e + q, dl);
-                q += wv_put(e + q, L);
-                wv_put(e + q, T);
-            }
-            uint64_t q = wv_len(slot) + 2u + wv_len(dl) + wv_len(L) + wv_len(T);
-            uint32_t r = 0;
-            for (uint32_t j = 0; j < T; ++j) {
-                if ((held >> j) & 1u) {
-                    if (lane == 0u) {
-                        e[q] = 1u;
-                        wv_put(e + q + 1u, L);
-                    }
-                    q += 1u + wv_len(L);
-                    warp_copy_bytes(e + q, src + static_cast<uint64_t>(r++) * pitch, static_cast<uint32_t>(L), lane);
-                    q += L;
-                } else {
-                    if (lane == 0u) e[q] = 0u;
-                    q += 1u;
-                }
-            }
-            if (lane == 0u) e[q] = 0u;                                      // data_copy: None
-            at += q + 1u;
+            if (lane == 0u) wv_put(dst + at, slot);
+            at += wv_len(slot);
+            at += warp_put_cw(dst + at, A.d, A.T, dl, held, [&](uint32_t j) {
+                return src + static_cast<uint64_t>(__popc(held & ((1u << j) - 1u))) * pitch;
+            }, lane);
         });
         __syncwarp();
     }
@@ -478,41 +446,7 @@ struct AbsEntry {
 };
 
 __device__ __forceinline__ bool abs_entry(const uint8_t *b, uint64_t len, uint64_t &n, uint32_t d, uint32_t T, AbsEntry &E) {
-    uint64_t v = 0;
-    uint32_t c;
-    if (!(c = wv_get(b + n, len - n, E.slot))) return false;
-    n += c;
-    if (len - n < 2u || b[n] != d || b[n + 1] != T - d) return false;
-    n += 2;
-    if (!(c = wv_get(b + n, len - n, E.dl))) return false;
-    n += c;
-    if (!(c = wv_get(b + n, len - n, E.L))) return false;
-    n += c;
-    if (!(c = wv_get(b + n, len - n, v))) return false;
-    n += c;
-    if (E.dl > 0xffffffffull || v != T || E.L != (E.dl + d - 1u) / d) return false;
-    E.tags_at = n;
-    E.mask = 0;
-    for (uint32_t j = 0; j < T; ++j) {
-        if (n >= len) return false;
-        const uint8_t tag = b[n++];
-        if (tag == 0u) continue;
-        if (tag != 1u) return false;
-        if (!(c = wv_get(b + n, len - n, v))) return false;
-        n += c;
-        if (v != E.L || len - n < E.L) return false;
-        E.mask |= 1u << j;
-        n += E.L;
-    }
-    if (n >= len) return false;
-    const uint8_t tag = b[n++];                                             // data_copy
-    if (tag == 1u) {
-        if (len - n < E.dl) return false;
-        n += E.dl;
-    } else if (tag != 0u) {
-        return false;
-    }
-    return true;
+    return wv_next(b, len, n, E.slot) && cw_parse<true>(b, len, n, d, T, E.dl, E.L, E.tags_at, E.mask);
 }
 
 __global__ void __launch_bounds__(kRcThreads) absorb_head_kernel(const __grid_constant__ AbsorbArgs A) {
@@ -521,8 +455,8 @@ __global__ void __launch_bounds__(kRcThreads) absorb_head_kernel(const __grid_co
         const uint8_t *b = nullptr;
         uint64_t len = 0, n = 0, cnt = 0;
         const uint32_t g = A.frame_group[i];
-        uint32_t kind = g >= A.G ? SS_FRAME_KIND_MALFORMED : rc_head(A.buf, A.buf_len, A.frame_off[i], A.variant, b, len, n, cnt);
-        if (kind == kRcPending) {
+        uint32_t kind = g >= A.G ? SS_FRAME_KIND_MALFORMED : msg_head_count(A.buf, A.buf_len, A.frame_off[i], A.variant, ~0ull, b, len, n, cnt);
+        if (kind == kPending) {
             A.fr_at[i] = n;
             A.fr_at[A.n + i] = cnt;
             AbsEntry E;
@@ -557,8 +491,7 @@ __global__ void __launch_bounds__(kRcThreads, 1) absorb_apply_kernel(const __gri
         for (uint64_t k = t; k < A.n && A.key[k] == g; ++k) {
             const uint32_t i = A.idx[k];
             const uint8_t *fr = A.buf + A.frame_off[i];
-            uint64_t len = 0;
-            for (int q = 0; q < 8; ++q) len = (len << 8) | fr[q];
+            const uint64_t len = get_be64(fr);
             const uint8_t *b = fr + 8;
             const uint64_t cnt = A.fr_at[A.n + i];
             const bool may_repeat = A.fr_at[2u * A.n + i] != 0u;
@@ -584,12 +517,9 @@ __global__ void __launch_bounds__(kRcThreads, 1) absorb_apply_kernel(const __gri
                 uint64_t at = 0;
                 for (uint32_t j = 0; j < A.T; ++j) {
                     if (!((E.mask >> j) & 1u)) { at += 1u; continue; }
-                    // Some tag, then the shard length as the frame spells it: a non-minimal varint decodes as well, so
-                    // its width comes from its own tag byte
-                    const uint8_t w = tags[at + 1u];
-                    const uint64_t some_len = 1u + (w < 251u ? 1u : w == 251u ? 3u : w == 252u ? 5u : 9u);
-                    if ((add >> j) & 1u) warp_fill_slot(dst + j * A.plane_stride, tags + at + some_len, E.L, lane);
-                    at += some_len + E.L;
+                    const uint64_t sl = some_len(tags[at + 1u]);
+                    if ((add >> j) & 1u) warp_fill_slot(dst + j * A.plane_stride, tags + at + sl, E.L, lane);
+                    at += sl + E.L;
                 }
                 __syncwarp();
                 if (lane == 0u) A.held[pos] |= add;
@@ -686,7 +616,7 @@ int ss_engine_craft_reconstruct_reads(ss_engine *e, const uint32_t *groups, uint
                                       uint8_t *frame_dst, uint64_t *frame_off, uint32_t *frame_len, uint64_t frame_capacity,
                                       uint64_t *totals) {
     if (chunk_size == 0) return set_error(SS_ERR_INVALID_ARG, "chunk_size must be at least 1");
-    if (reconstruct_variant >= kRcVariantLimit) return set_error(SS_ERR_INVALID_ARG, "reconstruct_variant must be < 2^16");
+    if (reconstruct_variant >= kVariantLimit) return set_error(SS_ERR_INVALID_ARG, "reconstruct_variant must be < 2^16");
     SS_TRY(craft_check(e));
     SS_TRY(craft_log_init(e));
     SS_TRY(craft_held_in_use(e));                                           // it reads held
@@ -725,7 +655,7 @@ int ss_follower_reconstruct_serve(ss_follower *f, const uint8_t *buf, uint64_t b
                                   uint32_t reply_variant, uint8_t *out, uint64_t out_capacity, uint64_t *reply_off,
                                   uint64_t *reply_len, uint32_t *verdict, uint64_t *total) {
     if (f == nullptr) return set_error(SS_ERR_INVALID_ARG, "null follower");
-    if (reconstruct_variant >= kRcVariantLimit || reply_variant >= kRcVariantLimit)
+    if (reconstruct_variant >= kVariantLimit || reply_variant >= kVariantLimit)
         return set_error(SS_ERR_INVALID_ARG, "the variants must be < 2^16");
     ss_ctx *ctx = f->ctx;
     SS_TRY(ctx_bind(ctx));
@@ -754,7 +684,7 @@ int ss_follower_reconstruct_serve(ss_follower *f, const uint8_t *buf, uint64_t b
 
 int ss_engine_craft_absorb(ss_engine *e, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, const uint32_t *frame_group,
                            const uint8_t *frame_peer, uint64_t n, uint32_t reply_variant, uint32_t *absorbed, uint32_t *verdict) {
-    if (reply_variant >= kRcVariantLimit) return set_error(SS_ERR_INVALID_ARG, "reply_variant must be < 2^16");
+    if (reply_variant >= kVariantLimit) return set_error(SS_ERR_INVALID_ARG, "reply_variant must be < 2^16");
     SS_TRY(craft_check(e));
     if (n > 0x7fffffffull) return set_error(SS_ERR_INVALID_ARG, "at most 2^31 - 1 frames per call");
     if (n != 0 && (!buf || !frame_off || !frame_group || !frame_peer || !absorbed || !verdict)) return set_error(SS_ERR_INVALID_ARG, "null buffer");

@@ -72,22 +72,15 @@ __device__ __forceinline__ FrHdr fr_decode(const FrArgs &A, uint64_t i) {
     FrHdr h{};
     h.kind = SS_FRAME_KIND_MALFORMED;
     const uint64_t off = A.rec_off[i];
-    if (off > A.buf_len || A.buf_len - off < 8u) return h;
-    const uint8_t *fr = A.buf + off;
-    uint64_t len = 0;
-    for (int b = 0; b < 8; ++b) len = (len << 8) | fr[b];
-    if (len > A.buf_len - off - 8u || len > kFolMaxBody) return h;
-    uint64_t v = 0, n = 0;
-    uint32_t c;
-    if (!(c = wv_get(fr + 8, len, v))) return h;
-    n = c;
+    const uint8_t *b;
+    uint64_t len, v = 0, n = 0;
+    if (!frame_body(A.buf, A.buf_len, off, kMaxFrameBody, b, len) || !wv_next(b, len, n, v)) return h;
+    const uint8_t *fr = b - 8;
     if (v == A.meta_variant) {
         uint64_t ct = 0;
-        if (!(c = wv_get(fr + 8 + n, len - n, ct))) return h;
-        n += c;
-        if (len - n != 1u) return h;                                        // voted_for, then the end
+        if (!wv_next(b, len, n, ct) || len - n != 1u) return h;            // voted_for, then the end
         h.term = ct;
-        h.voted_for = fr[8 + n];
+        h.voted_for = b[n];
         h.kind = kFrMeta;
     } else if (v == A.log_variant) {
         Ent e;

@@ -25,7 +25,7 @@ namespace ssb {
 
 constexpr int kSdThreads = 256;
 constexpr uint32_t kSdTerm = 0xfffffffdu;         // decoded, carries a term
-constexpr uint32_t kSdNoVariant = 0xffffffffu;    // rc_head's variant that no frame has: it returns the frame's
+constexpr uint32_t kSdNoVariant = 0xffffffffu;    // msg_head_count's variant that no frame has: it returns the frame's
 
 struct StepDownArgs {
     FolArgs fa;                     // the append decoder's view (frames, follower window and start_slot)
@@ -60,13 +60,13 @@ __device__ __forceinline__ uint32_t sd_decode(const StepDownArgs &A, uint64_t i,
     if (A.fa.frame_group[i] >= A.G) return SS_FRAME_KIND_MALFORMED;
     const uint8_t *b = nullptr;
     uint64_t len = 0, n = 0, cnt = 0;
-    const uint32_t v = rc_head(A.fa.buf, A.fa.buf_len, A.fa.frame_off[i], kSdNoVariant, b, len, n, cnt);
+    const uint32_t v = msg_head_count(A.fa.buf, A.fa.buf_len, A.fa.frame_off[i], kSdNoVariant, ~0ull, b, len, n, cnt);
     if (v == SS_FRAME_KIND_MALFORMED || (v & 0x80000000u)) return v;
     uint32_t kind;
     if (v == A.fa.append_variant) {
         const FolHdr h = fol_decode(A.fa, i);
         // a frame past the follower's window still carries its term
-        kind = h.kind == kFolPending || h.kind == SS_FOLLOWER_VERDICT_BEYOND_WINDOW ? kFolPending : h.kind;
+        kind = h.kind == kPending || h.kind == SS_FOLLOWER_VERDICT_BEYOND_WINDOW ? kPending : h.kind;
         term = h.term;
     } else if (v == A.reply_variant) {
         // the reply parser's rules, and a sender that is a peer: it becomes the follower's leader
@@ -75,17 +75,17 @@ __device__ __forceinline__ uint32_t sd_decode(const StepDownArgs &A, uint64_t i,
         uint64_t end = 0, c_term = 0, c_slot = 0;
         const uint32_t r = reply_parse(A.fa.buf, A.fa.buf_len, A.fa.frame_off[i], A.fa.frame_group[i], A.G, A.reply_variant,
                                        A.curr_term, term, end, c_term, c_slot);
-        kind = r >= SS_APPEND_REPLY_INGEST && r <= SS_APPEND_REPLY_END_RANGE ? kFolPending : r;
+        kind = r >= SS_APPEND_REPLY_INGEST && r <= SS_APPEND_REPLY_END_RANGE ? kPending : r;
     } else if (v == A.ev.variant) {
         uint64_t f1 = 0, f2 = 0;
-        kind = el_decode<false>(A.ev, i, term, f1, f2) == kElPending ? kFolPending : SS_FRAME_KIND_MALFORMED;
+        kind = el_decode<false>(A.ev, i, term, f1, f2) == kPending ? kPending : SS_FRAME_KIND_MALFORMED;
     } else if (v == A.er.variant) {
         uint64_t f1 = 0, f2 = 0;
-        kind = el_decode<true>(A.er, i, term, f1, f2) == kElPending ? kFolPending : SS_FRAME_KIND_MALFORMED;
+        kind = el_decode<true>(A.er, i, term, f1, f2) == kPending ? kPending : SS_FRAME_KIND_MALFORMED;
     } else {
         return SS_STEPDOWN_VERDICT_PASS;                                    // Reconstruct, ReconstructReply
     }
-    return kind == kFolPending ? kSdTerm : kind;
+    return kind == kPending ? kSdTerm : kind;
 }
 
 __global__ void __launch_bounds__(kSdThreads) sd_head_kernel(const __grid_constant__ StepDownArgs A) {
@@ -281,7 +281,7 @@ int ss_engine_craft_step_down(ss_engine *e, ss_follower *f, const ss_step_down_s
     if (spec == nullptr) return set_error(SS_ERR_INVALID_ARG, "null spec");
     const uint32_t vs[4] = {spec->append_variant, spec->append_reply_variant, spec->request_vote_variant, spec->vote_reply_variant};
     for (int a = 0; a < 4; ++a) {
-        if (vs[a] >= kRcVariantLimit) return set_error(SS_ERR_INVALID_ARG, "the variants must be < 2^16");
+        if (vs[a] >= kVariantLimit) return set_error(SS_ERR_INVALID_ARG, "the variants must be < 2^16");
         for (int b = 0; b < a; ++b)
             if (vs[a] == vs[b]) return set_error(SS_ERR_INVALID_ARG, "the four variants must differ");
     }

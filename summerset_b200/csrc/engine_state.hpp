@@ -79,8 +79,4 @@ int craft_led_mark(ss_engine *e, const uint32_t *groups, const uint32_t *verdict
 int backoff_scratch(ss_engine *e, uint64_t n, int bits);
 // the recon / step-down scratch (rc_words), grow-only: `words` u64 (craft_recon.cu)
 int rc_scratch(ss_engine *e, uint64_t words);
-
-__device__ __forceinline__ void cl_put_be64(uint8_t *p, uint64_t v) {
-    for (int b = 0; b < 8; ++b) p[b] = static_cast<uint8_t>(v >> (8 * (7 - b)));
-}
 }  // namespace ssb

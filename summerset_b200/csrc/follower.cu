@@ -52,7 +52,7 @@ __global__ void __launch_bounds__(kFolThreads) follower_header_kernel(const __gr
     for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kFolThreads + threadIdx.x; i < A.n; i += stride) {
         const FolHdr h = fol_decode(A, i);
         A.hdr[i] = h;
-        const bool pending = h.kind == kFolPending;
+        const bool pending = h.kind == kPending;
         A.store_off[i] = pending ? h.store_sz : 0ull;
         A.wal_off[i] = pending ? h.wal_sz : 0ull;
         const uint32_t grp = A.frame_group[i];
@@ -67,17 +67,13 @@ __global__ void __launch_bounds__(kFolThreads) follower_cut_kernel(const __grid_
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kFolThreads;
     for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kFolThreads + threadIdx.x; i < A.n; i += stride) {
         const FolHdr &h = A.hdr[i];
-        if (h.kind != kFolPending) continue;
+        if (h.kind != kPending) continue;
         const uint64_t so = A.store_off[i], wo = A.wal_off[i];
         const bool s_over = so > A.store_cap || h.store_sz > A.store_cap - so;
         const bool w_over = wo > A.wal_cap || h.wal_sz > A.wal_cap - wo;
         if (s_over || w_over)
             atomicMin(reinterpret_cast<unsigned long long *>(A.cut), static_cast<unsigned long long>(2u * i + (s_over ? 0u : 1u)));
     }
-}
-
-__device__ __forceinline__ void put_be64(uint8_t *p, uint64_t v) {
-    for (int b = 0; b < 8; ++b) p[b] = static_cast<uint8_t>(v >> (8 * (7 - b)));
 }
 
 // PeerMessage::Msg{AppendEntriesReply{term, end_slot, conflict}} into a 48-byte cell (at most 47 bytes)
@@ -102,10 +98,9 @@ __device__ __forceinline__ const uint8_t *shard_in_frame(const uint8_t *tags, ui
     uint64_t at = 0;
     for (uint32_t q = 0; q <= j; ++q) {
         if (!((present >> q) & 1u)) { at += 1u; continue; }
-        const uint8_t t = tags[at + 1u];
-        const uint64_t some_len = 1u + (t < 251u ? 1u : t == 251u ? 3u : t == 252u ? 5u : 9u);
-        if (q == j) return tags + at + some_len;
-        at += some_len + L;
+        const uint64_t sl = some_len(tags[at + 1u]);
+        if (q == j) return tags + at + sl;
+        at += sl + L;
     }
     return nullptr;
 }
@@ -165,12 +160,12 @@ __global__ void __launch_bounds__(kFolThreads) follower_replay_kernel(const __gr
             A.reply_dst[i] = 0xffu;
             A.trunc_slot[i] = ~0ull;
             A.wal_len[i] = 0u;
-            if (kind == kFolPending && i >= cut_i) {
+            if (kind == kPending && i >= cut_i) {
                 kind = cut_kind;
                 cut_store |= kind == SS_FOLLOWER_VERDICT_STORE_FULL;
                 cut_wal |= kind == SS_FOLLOWER_VERDICT_WAL_FULL;
             }
-            if (kind != kFolPending) {
+            if (kind != kPending) {
                 A.verdict[i] = kind;
                 A.store_off[i] = ~0ull;
                 A.wal_off[i] = ~0ull;
@@ -615,7 +610,7 @@ int ss_append_reply_parse_dev(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len,
                               uint64_t *rec_term, uint64_t *rec_conflict_term, uint64_t *rec_conflict_slot, uint32_t *rec_kind) {
     // a frame's variant >= 2^16 is malformed, so no index from there on can name the reply (ss_engine_craft_backoff, which
     // takes the same reply_variant, refuses it too)
-    if (reply_variant >= kFolVariantLimit) return set_error(SS_ERR_INVALID_ARG, "reply_variant must be < 2^16");
+    if (reply_variant >= kVariantLimit) return set_error(SS_ERR_INVALID_ARG, "reply_variant must be < 2^16");
     if (ctx == nullptr) return set_error(SS_ERR_INVALID_ARG, "null context");
     SS_TRY(ctx_bind(ctx));
     if (n_frames == 0) return SS_OK;

@@ -20,6 +20,7 @@
 //
 // bincode 2 standard config facts are from knowledge of the crate (unpinned against the reference, DESIGN.md section 4);
 // every kernel is tested byte for byte against oracle/ss_wire.c.
+#include "codeword_wire.cuh"
 #include "device_common.cuh"
 #include "ss_internal.hpp"
 #include "wire_common.cuh"
@@ -220,34 +221,16 @@ __global__ void __launch_bounds__(kWireThreads) accept_reply_parse_kernel(const 
         const uint32_t grp = A.frame_group[i];
         const uint64_t off = A.frame_off[i];
         do {
-            if (off > A.buf_len || A.buf_len - off < 8u) break;                       // off + 8 would wrap near 2^64
-            const uint8_t *fr = A.buf + off;
-            uint64_t len = 0;
-            for (int b = 0; b < 8; ++b) len = (len << 8) | fr[b];
-            if (len > A.buf_len - off - 8u) break;
-            const uint8_t *b = fr + 8;
-            uint64_t n = 0, v = 0, slot = 0;
-            uint32_t c;
-            if (!(c = wv_get(b + n, len - n, v))) break;
-            n += c;
-            if (v != 0u) { kind = 0x80000000u | static_cast<uint32_t>(v); break; }   // LeaseMsg / Leave / LeaveReply
-            if (!(c = wv_get(b + n, len - n, v))) break;
-            n += c;
-            if (v != A.reply_variant) { kind = static_cast<uint32_t>(v); break; }    // another PeerMsg: the host's business
-            if (!(c = wv_get(b + n, len - n, slot))) break;
-            n += c;
-            if (!(c = wv_get(b + n, len - n, ballot))) break;
-            n += c;
+            const uint8_t *b;
+            uint64_t len, n, v = 0, slot = 0;
+            // every variant index is reported as such: no cap
+            if (!msg_head(A.buf, A.buf_len, off, A.reply_variant, ~0ull, false, b, len, n, kind)) break;
+            if (!wv_next(b, len, n, slot) || !wv_next(b, len, n, ballot)) break;
             if (A.with_size) {                                                        // crossword: size, reply_ts
-                if (!(c = wv_get(b + n, len - n, v))) break;
-                n += c;
-                if (n >= len) break;
+                if (!wv_next(b, len, n, v) || n >= len) break;
                 const uint8_t tag = b[n++];
                 if (tag == 1) {
-                    if (!(c = wv_get(b + n, len - n, v))) break;
-                    n += c;
-                    if (!(c = wv_get(b + n, len - n, v))) break;
-                    n += c;
+                    if (!wv_next(b, len, n, v) || !wv_next(b, len, n, v)) break;
                 } else if (tag != 0) break;
             }
             if (n != len) break;
@@ -278,7 +261,6 @@ struct PrepParseArgs {
 // a thread per frame: PrepareReply{slot, trigger_slot, endprep_slot, ballot, voted} with the codeword checked as
 // ss_acceptor_absorb checks one; the shards stay where they are (shards_at)
 __global__ void __launch_bounds__(kWireThreads) prepare_reply_parse_kernel(const __grid_constant__ PrepParseArgs A) {
-    constexpr uint64_t kVariantLimit = 1u << 16;
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kWireThreads;
     for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kWireThreads + threadIdx.x; i < A.n_frames; i += stride) {
         ss_prepare_reply_rec r{};
@@ -286,59 +268,22 @@ __global__ void __launch_bounds__(kWireThreads) prepare_reply_parse_kernel(const
         r.shards_at = ~0ull;
         const uint64_t off = A.frame_off[i];
         do {
-            if (off > A.buf_len || A.buf_len - off < 8u) break;
-            const uint8_t *fr = A.buf + off;
-            uint64_t len = 0;
-            for (int b = 0; b < 8; ++b) len = (len << 8) | fr[b];
-            if (len > A.buf_len - off - 8u) break;
-            const uint8_t *b = fr + 8;
-            uint64_t n = 0, v = 0, f[4], vb = 0, dl = 0, sl = 0, at = ~0ull;
-            uint32_t c, mask = 0;
-            bool ok = true;
-#define SS_GETR(dst) if (!(c = wv_get(b + n, len - n, (dst)))) break; n += c
-            SS_GETR(v);
-            if (v != 0u) { if (v < kVariantLimit) r.kind = 0x80000000u | static_cast<uint32_t>(v); break; }
-            SS_GETR(v);
-            if (v != A.reply_variant) { if (v < kVariantLimit) r.kind = static_cast<uint32_t>(v); break; }
-            SS_GETR(f[0]);
-            SS_GETR(f[1]);
-            SS_GETR(f[2]);
-            SS_GETR(f[3]);
-            if (n >= len) break;
+            const uint8_t *b;
+            uint64_t len, n, f0 = 0, f1 = 0, f2 = 0, f3 = 0, vb = 0, dl = 0, sl = 0, at = ~0ull;
+            uint32_t mask = 0;
+            if (!msg_head(A.buf, A.buf_len, off, A.reply_variant, ~0ull, true, b, len, n, r.kind)) break;
+            if (!wv_next(b, len, n, f0) || !wv_next(b, len, n, f1) || !wv_next(b, len, n, f2) || !wv_next(b, len, n, f3) || n >= len)
+                break;
             const uint8_t tag = b[n++];
             if (tag == 1u) {
-                SS_GETR(vb);
-                if (len - n < 2u || b[n] != A.d || b[n + 1] != A.T - A.d) break;
-                n += 2;
-                SS_GETR(dl);
-                SS_GETR(sl);
-                SS_GETR(v);
-                if (dl > 0xffffffffull || v != A.T || sl != (dl + A.d - 1u) / A.d) break;
-                at = off + 8u + n;
-                for (uint32_t j = 0; j < A.T && ok; ++j) {
-                    if (n >= len) { ok = false; break; }
-                    const uint8_t t = b[n++];
-                    if (t == 0u) continue;
-                    if (t != 1u || !(c = wv_get(b + n, len - n, v))) { ok = false; break; }
-                    n += c;
-                    if (v != sl || len - n < sl) { ok = false; break; }
-                    mask |= 1u << j;
-                    n += sl;
-                }
-                if (!ok || n >= len) break;
-                const uint8_t dc = b[n++];                                            // data_copy
-                if (dc == 1u) {
-                    if (len - n < dl) break;
-                    n += dl;
-                } else if (dc != 0u) {
-                    break;
-                }
+                uint64_t tags_at = 0;
+                if (!wv_next(b, len, n, vb) || !cw_parse<true>(b, len, n, A.d, A.T, dl, sl, tags_at, mask)) break;
+                at = off + 8u + tags_at;
             } else if (tag != 0u) {
                 break;
             }
-#undef SS_GETR
             if (n != len) break;
-            r.slot = f[0]; r.trigger_slot = f[1]; r.endprep_slot = f[2]; r.ballot = f[3];
+            r.slot = f0; r.trigger_slot = f1; r.endprep_slot = f2; r.ballot = f3;
             r.vote_bal = vb; r.vote_mask = mask; r.data_len = static_cast<uint32_t>(dl); r.shards_at = at;
             r.kind = A.reply_variant;
         } while (false);
