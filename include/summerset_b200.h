@@ -895,6 +895,9 @@ int ss_acceptor_prepare(ss_acceptor *acceptor, const uint8_t *buf, uint64_t buf_
  * reply_off UINT64_MAX with reply_len kept, reply_dst 0xff, SS_DEV_STATUS_FRAME_OVERFLOW; the offsets are monotone, so
  * the written replies are a prefix and a host drains by calling again with the rest.  *total (device u64, may be NULL)
  * = the bytes the batch asked for.  Acceptor state is not changed.
+ * The records of ss_acceptor_step_up go through this call too: their instances have source = me, so their replies have
+ * reply_dst = me, the new leader's reply from itself (rspaxos/durability.rs:29-48).  Nothing here refuses that; the host
+ * hands those frames to ss_prepare_reply_parse_dev with its peers' replies instead of sending them.
  * Cost: a thread per record sizes, a warp per record writes. */
 int ss_acceptor_prepare_reply(ss_acceptor *acceptor, const uint32_t *rec_group, const uint64_t *rec_slot, uint64_t n_records,
                               uint32_t reply_variant, uint8_t *out, uint64_t out_capacity, uint64_t *reply_off,
@@ -1011,11 +1014,64 @@ int ss_acceptor_gossip(ss_acceptor *acceptor, const uint32_t *groups, uint64_t n
  * d shards (RSPaxos: majority, the acceptor's d) is listed; the list is cut into frames of chunk_size entries,
  * PeerMessage::Msg{Reconstruct{slots}} (RSPaxos) or {slots_excl} with the exclusion = held as a size-T Bitmap
  * (Crossword), each with frame_dst 0xff: the host broadcasts it.  No state changes; the Prepare, PrepareBal and ballot
- * parts of become_a_leader stay with the host. */
+ * parts of become_a_leader are ss_acceptor_step_up, which runs first: the instances it leaves Preparing are not listed. */
 int ss_acceptor_step_up_reads(ss_acceptor *acceptor, const uint32_t *groups, uint64_t n_listed, uint64_t chunk_size,
                               uint32_t reconstruct_variant, uint8_t *out, uint64_t out_capacity, uint32_t *frame_group,
                               uint8_t *frame_dst, uint64_t *frame_off, uint32_t *frame_len, uint64_t frame_capacity,
                               uint64_t *totals);
+/* Step-up (RSPaxos and Crossword): the Prepare half of become_a_leader (rspaxos/leadership.rs:45-185,
+ * crossword/leadership.rs:47-190) on this replica's acceptor, whose window is the new leader's instance log.  groups
+ * (device u32 [n_listed]) lists the groups to step up in; NULL steps up every group in index order.  A listed group >=
+ * n_groups is ignored: verdict SS_FRAME_KIND_MALFORMED, ballot, trigger_slot and endprep_slot 0.  Each group's entries run
+ * in list order as if they came one at a time, so a group listed twice steps up twice: the second entry takes
+ * make_greater_ballot of the first entry's ballot, finds the same trigger, endprep and instances, and defines them.
+ * Per entry of group g, in window terms:
+ *   ballot b = make_greater_ballot(bal_max_seen[g]) = ((bal_max_seen[g] >> 8) + 1) << 8 | (me + 1), in u64
+ *     (rspaxos/mod.rs:446-454); then bal_max_seen[g] = b;
+ *   log_end = window_base + 1 + the last window position that is Preparing, Accepting or Committed (window_base when
+ *     none is), as in ss_acceptor_gossip; a slot is done when it is Committed or below exec_bar (Executed);
+ *   trigger_slot = the first slot of [window_base, log_end) that is not done, log_end when every slot is done (the
+ *     reference pushes a null instance there; here that position is taken into the Prepare); endprep_slot = the last
+ *     slot that is not done, trigger_slot when every slot is done;
+ *   trigger_slot = window_base + 64: SS_ACCEPT_VERDICT_BEYOND_WINDOW and nothing changes; the host advances and lists
+ *     the group again;
+ *   every slot of [max(exec_bar, window_base), endprep_slot] that is not Committed gets inst_bal = b, Status::Preparing
+ *     (Accepting cleared), source = me, trigger_slot and endprep_slot - trigger_slot (replica_bk, read by
+ *     ss_acceptor_prepare_reply).  A slot that was null becomes a fresh null_instance(): voted None, held 0, data_len 0
+ *     (Crossword: an empty assignment row); an accepted instance keeps its vote, held shards and store region.
+ *     Committed instances are not touched: ss_acceptor_step_up_reads lists them afterwards.
+ * Records: one WalEntry::PrepareBal{slot, b} per marked slot, in slot order, numbered by an exclusive scan in list order;
+ * record k is the 32-byte cell wal + 32k that ss_acceptor_prepare writes, with rec_group[k] and rec_slot[k] (absolute).
+ * Frames: one PeerMessage::Msg{Prepare{trigger_slot, ballot: b}} per applied entry, numbered by an exclusive scan in list
+ * order: frame f is the 32-byte cell out + 32f (8-byte big-endian length + body, at most 30 bytes, zero to the end of the
+ * cell), frame_off[f] = 32f, frame_len[f], frame_group[f] and frame_dst[f] = 0xff: the host broadcasts it.
+ * prepare_variant (PeerMsg::Prepare, 0) and wal_variant (WalEntry::PrepareBal, 0) are below 2^16.
+ * Per listed entry i: verdict[i], ballot[i] = b, trigger_slot[i] and endprep_slot[i], the values the entry takes when
+ * the whole list applies.  verdict[i]: SS_ACCEPT_VERDICT_ACCEPTED, SS_ACCEPT_VERDICT_BEYOND_WINDOW, or
+ * SS_ACCEPT_VERDICT_WAL_FULL: its records end past rec_capacity or past wal_capacity / 32 cells, or its frame past
+ * frame_capacity or past out_capacity / 32 cells.  Such an entry changes nothing, and neither does any later entry: the
+ * ends are monotone, so the applied entries are a prefix of the list; SS_DEV_STATUS_FRAME_OVERFLOW is set, its frame
+ * record below frame_capacity gets frame_off UINT64_MAX, frame_len 0 and frame_dst 0xff, and calling again with the
+ * rest of the list finishes the job.  totals (device u64[4], may be NULL): the records, WAL bytes, frames and frame
+ * bytes the call asked for.  wal and out 16-byte aligned.
+ * The leader's own vote: once the PrepareBal records are durable, the host passes rec_group / rec_slot to
+ * ss_acceptor_prepare_reply, which sends a replica's PrepareReply to the instance's source.  Here that is me: the
+ * replies with reply_dst = me are the leader's "reply from myself" (rspaxos/durability.rs:29-48), carrying its voted
+ * shards, and ss_prepare_reply_parse_dev reads them like any peer's.
+ * What stays with the host: disallow_step_up, the timeout_source check, the leader status, the heartbeat broadcast,
+ * peer_exec_bar and the engine's bal_prepared (cleared through ss_engine_set_prepared_ballots); bal_prep_sent is
+ * ballot[i], which the acceptor does not keep.
+ * Stated differences from the reference:
+ *   1. the 64-slot window, not start_slot + insts.len(): the reference also counts trailing null instances that a
+ *      Prepare or an earlier step-up appended to its vector, and a trigger at window_base + 64 is BEYOND_WINDOW;
+ *   2. the capacity cut above (the reference logs and sends everything).
+ * Cost: the walk and the apply pass take a thread per group segment; the records, frames and per-slot writes take a warp
+ * per applied entry. */
+int ss_acceptor_step_up(ss_acceptor *acceptor, const uint32_t *groups, uint64_t n_listed, uint32_t prepare_variant,
+                        uint32_t wal_variant, uint8_t *wal, uint64_t wal_capacity, uint32_t *rec_group, uint64_t *rec_slot,
+                        uint64_t rec_capacity, uint8_t *out, uint64_t out_capacity, uint32_t *frame_group, uint8_t *frame_dst,
+                        uint64_t *frame_off, uint32_t *frame_len, uint64_t frame_capacity, uint32_t *verdict, uint64_t *ballot,
+                        uint64_t *trigger_slot, uint64_t *endprep_slot, uint64_t *totals);
 /* PrepareReply frames -> one record per frame for the new leader (a thread per frame, no copies; the PrepareReply
  * counterpart of ss_accept_reply_parse_dev).  Frame i at buf + frame_off[i] (any alignment) must be
  * PeerMessage::Msg{PrepareReply{slot, trigger_slot, endprep_slot, ballot, voted}} whose codeword, when voted is Some,

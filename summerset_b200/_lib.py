@@ -133,6 +133,8 @@ SIGNATURES = {
     "ss_acceptor_gossip_view_get": (_i, [_vp, _vp]),
     "ss_acceptor_gossip": (_i, [_vp, _vp, _u64, _vp, _u64, _u64, _u32, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp]),
     "ss_acceptor_step_up_reads": (_i, [_vp, _vp, _u64, _u64, _u32, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp]),
+    "ss_acceptor_step_up": (_i, [_vp, _vp, _u64, _u32, _u32, _vp, _u64, _vp, _vp, _u64, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp, _vp, _vp,
+                                 _vp, _vp]),
     "ss_prepare_reply_parse_dev": (_i, [_vp, _vp, _u64, _vp, _u64, _u32, _u32, _u32, _vp]),
     "ss_follower_create": (_i, [_vp, _vp, _u64, C.POINTER(_vp)]),
     "ss_follower_destroy": (_i, [_vp]),

@@ -1039,20 +1039,7 @@ __global__ void __launch_bounds__(kAccThreads) prepare_write_kernel(const __grid
         const uint64_t first = A.cnt[i], count = h.endprep - h.trigger + 1u;
         for (uint64_t q = lane; q < count; q += 32u) {
             const uint64_t k = first + q, slot = h.trigger + q;
-            uint8_t cell[32];
-#pragma unroll
-            for (int b = 0; b < 32; ++b) cell[b] = 0u;
-            uint32_t m = 8u;
-            m += wv_put(cell + m, A.wal_variant);
-            m += wv_put(cell + m, slot);
-            m += wv_put(cell + m, h.ballot);
-            cell[7] = static_cast<uint8_t>(m - 8u);                          // the body is < 256 bytes
-            uint4 lo, hi;
-            memcpy(&lo, cell, 16);
-            memcpy(&hi, cell + 16, 16);
-            uint4 *dst = reinterpret_cast<uint4 *>(A.wal + k * 32u);
-            dst[0] = lo;
-            dst[1] = hi;
+            put_prepare_bal_cell(A.wal + k * 32u, A.wal_variant, slot, h.ballot);
             A.rec_group[k] = g;
             A.rec_slot[k] = slot;
             A.rec_frame[k] = static_cast<uint32_t>(i);

@@ -124,6 +124,26 @@ __device__ __forceinline__ FrameHdr decode_frame(const Args &A, uint64_t i) {
     return h;
 }
 
+// WalEntry::PrepareBal{slot, ballot} as the 32-byte cell at dst (16-byte aligned): 8-byte big-endian length, the bincode
+// body (at most 21 bytes with wal_variant < 2^16), zero to the end of the cell.  Written by ss_acceptor_prepare and
+// ss_acceptor_step_up.
+__device__ __forceinline__ void put_prepare_bal_cell(uint8_t *dst, uint32_t wal_variant, uint64_t slot, uint64_t ballot) {
+    uint8_t cell[32];
+#pragma unroll
+    for (int b = 0; b < 32; ++b) cell[b] = 0u;
+    uint32_t m = 8u;
+    m += wv_put(cell + m, wal_variant);
+    m += wv_put(cell + m, slot);
+    m += wv_put(cell + m, ballot);
+    cell[7] = static_cast<uint8_t>(m - 8u);                                  // the body is < 256 bytes
+    uint4 lo, hi;
+    memcpy(&lo, cell, 16);
+    memcpy(&hi, cell + 16, 16);
+    uint4 *d = reinterpret_cast<uint4 *>(dst);
+    d[0] = lo;
+    d[1] = hi;
+}
+
 // the whole assignment of a frame whose rows decode_frame validated, from rb = the frame + asg_at, lim = end - asg_at
 // bytes on: row r into rows[first + r]
 __device__ __forceinline__ void read_assign_rows(const uint8_t *rb, uint64_t lim, uint32_t population, uint32_t *rows, uint64_t first) {

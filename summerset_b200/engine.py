@@ -638,6 +638,34 @@ class Acceptor:
         no state changes."""
         return self._requests(True, out, frame_capacity, groups, chunk_size, out_capacity, reconstruct_variant)
 
+    def step_up(self, wal: torch.Tensor, rec_capacity: int, out: torch.Tensor, frame_capacity: int,
+                groups: Optional[torch.Tensor] = None, wal_capacity: Optional[int] = None, out_capacity: Optional[int] = None,
+                prepare_variant: int = 0, wal_variant: int = 0) -> dict:
+        """The Prepare half of become_a_leader over the listed groups (int32, None = all): a greater ballot, the
+        in-progress instances Preparing with source = me, one 32-byte PrepareBal cell per marked slot into wal and one
+        32-byte Prepare frame per group into out (uint8, 16-byte aligned), each to be broadcast.  Returns device tensors
+        rec_group (int32), rec_slot (int64), each [rec_capacity]; frame_group (int32), frame_dst (uint8), frame_off (int64,
+        -1 = not written), frame_len (int32), each [frame_capacity]; verdict (int32), ballot, trigger_slot, endprep_slot
+        (int64), each [n]; totals (int64 [4]: records, WAL bytes, frames, frame bytes asked for).  Once the records are
+        durable, prepare_reply(rec_group, rec_slot) gives the leader's own votes (reply_dst = me)."""
+        assert wal.dtype == torch.uint8 and out.dtype == torch.uint8
+        assert groups is None or groups.dtype == torch.int32
+        dev = out.device
+        n = self.G if groups is None else groups.numel()
+        rc, fc, m = max(rec_capacity, 1), max(frame_capacity, 1), max(n, 1)
+        e = lambda k, dt: torch.empty(k, dtype=dt, device=dev)
+        res = dict(rec_group=e(rc, torch.int32), rec_slot=e(rc, torch.int64), frame_group=e(fc, torch.int32),
+                   frame_dst=e(fc, torch.uint8), frame_off=e(fc, torch.int64), frame_len=e(fc, torch.int32), verdict=e(m, torch.int32),
+                   ballot=e(m, torch.int64), trigger_slot=e(m, torch.int64), endprep_slot=e(m, torch.int64), totals=e(4, torch.int64))
+        p = lambda x: None if x is None else x.data_ptr()
+        check(self.lib.ss_acceptor_step_up(self.h, p(groups), 0 if groups is None else n, prepare_variant, wal_variant, p(wal),
+                                           wal.numel() if wal_capacity is None else wal_capacity, p(res["rec_group"]),
+                                           p(res["rec_slot"]), rec_capacity, p(out), out.numel() if out_capacity is None else out_capacity,
+                                           p(res["frame_group"]), p(res["frame_dst"]), p(res["frame_off"]), p(res["frame_len"]),
+                                           frame_capacity, p(res["verdict"]), p(res["ballot"]), p(res["trigger_slot"]),
+                                           p(res["endprep_slot"]), p(res["totals"])))
+        return res
+
     def close(self) -> None:
         if getattr(self, "h", None) is not None and self.h:
             self.lib.ss_acceptor_destroy(self.h)

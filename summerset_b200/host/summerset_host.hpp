@@ -377,6 +377,18 @@ class Acceptor {
         check(ss_acceptor_step_up_reads(acc_, groups, n_listed, chunk_size, reconstruct_variant, out, out_capacity, frame_group, frame_dst,
                                         frame_off, frame_len, frame_capacity, totals));
     }
+    // become_a_leader's Prepare half: a greater ballot, the in-progress instances Preparing with source = me, 32-byte
+    // PrepareBal cells (variant 0) and one 32-byte Prepare frame (variant 0) per group to broadcast; once the records are
+    // durable, prepare_reply() on them gives the leader's own votes (reply_dst = me).  A capacity cut leaves a prefix of
+    // the groups applied (see the header)
+    void step_up(const uint32_t *groups, uint64_t n_listed, uint8_t *wal, uint64_t wal_capacity, uint32_t *rec_group, uint64_t *rec_slot,
+                 uint64_t rec_capacity, uint8_t *out, uint64_t out_capacity, uint32_t *frame_group, uint8_t *frame_dst, uint64_t *frame_off,
+                 uint32_t *frame_len, uint64_t frame_capacity, uint32_t *verdict, uint64_t *ballot, uint64_t *trigger_slot,
+                 uint64_t *endprep_slot, uint64_t *totals, uint32_t prepare_variant = 0, uint32_t wal_variant = 0) {
+        check(ss_acceptor_step_up(acc_, groups, n_listed, prepare_variant, wal_variant, wal, wal_capacity, rec_group, rec_slot,
+                                  rec_capacity, out, out_capacity, frame_group, frame_dst, frame_off, frame_len, frame_capacity, verdict,
+                                  ballot, trigger_slot, endprep_slot, totals));
+    }
     ss_acceptor_gossip_view gossip_view() const {
         ss_acceptor_gossip_view v;
         check(ss_acceptor_gossip_view_get(acc_, &v));
