@@ -1092,6 +1092,87 @@ typedef struct ss_prepare_reply_rec {
 } ss_prepare_reply_rec;
 int ss_prepare_reply_parse_dev(ss_ctx *ctx, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off, uint64_t n_frames,
                                uint32_t data_shards, uint32_t total_shards, uint32_t reply_variant, ss_prepare_reply_rec *rec);
+/* PrepareReply absorb on the new leader (RSPaxos and Crossword engines): handle_msg_prepare_reply (rspaxos/messages.rs:
+ * 88-326, crossword/messages.rs:140-400) for a batch of PrepareReply frames over many groups, after ss_acceptor_step_up
+ * on this replica's acceptor `acceptor`.  The engine and the acceptor must share context, protocol, n_groups, population,
+ * d and T (else SS_ERR_INVALID_ARG, as is any other protocol); a code with d + p > 12 gives SS_ERR_UNSUPPORTED, because
+ * the batched reconstruct does not take it.
+ * Frames are taken as ss_acceptor_prepare takes them: buf at any byte alignment, frame i at frame_off[i], of group
+ * frame_group[i] (>= n_groups: malformed), from replica frame_peer[i] (>= population: malformed); reply_variant is
+ * PeerMsg::PrepareReply (1), wal_variant WalEntry::PrepareBal (0).  The leader's own replies, the frames of
+ * ss_acceptor_prepare_reply with reply_dst = me, go in the same batch as any peer's.  bal_prep_sent (device [G]) is the
+ * ballot ss_acceptor_step_up returned for the group, 0 where this replica is not preparing: is_leader and bal_prep_sent
+ * stay with the host.  policy (Crossword, device [G], may be NULL = 0) is the assignment policy of the re-accepts.
+ * Each group's frames are replayed in frame order as if they arrived one at a time.  Per frame, decoded by the decoder of
+ * ss_prepare_reply_parse_dev, in the reference's order:
+ *   slot < window_base: SS_ACCEPT_VERDICT_STALE_SLOT;
+ *   ballot != bal_prep_sent[g], bal_prep_sent[g] = 0, or a trigger_slot outside the window or whose instance this leader
+ *     did not prepare before the call (source != me: leader_bk is None; a position the call filled lies past the
+ *     leader's endprep_slot, so it is no trigger of this leader): SS_PREP_VERDICT_IGNORED;
+ *   slot >= window_base + 64: SS_ACCEPT_VERDICT_BEYOND_WINDOW, re-submitted after an advance;
+ *   external fill (messages.rs:127-170): every position from the log end (one past the last position that is Preparing,
+ *     Accepting or Committed, counting the positions earlier frames of the call filled) through the slot becomes a fresh
+ *     null instance, Preparing on the acceptor with inst_bal = bal_prep_sent, source = me and the trigger's trigger and
+ *     span, and gets one WalEntry::PrepareBal 32-byte cell as ss_acceptor_prepare writes them;
+ *   the instance is not Preparing (or was decided at this ballot), or ballot < inst_bal: SS_PREP_VERDICT_IGNORED;
+ *   vote merge (ss_prepare_merge_dev's rule): a higher vote ballot replaces prepare_max_bal and the gathered codeword,
+ *     which takes a new store slot sized by its data_len (an empty Some clears the shards); an equal one adds the shards
+ *     not gathered yet; a same-ballot codeword with another data_len is rejected alone, SS_PREP_VERDICT_DATA_LEN, where
+ *     absorb_other errors; SS_ACCEPT_VERDICT_ACCEPTED otherwise;
+ *   slot == endprep_slot: the peer joins prepare_acks; whenever the count is then at least the majority, bal_prepared[g]
+ *     = ballot and every Preparing position from the trigger on that is not decided is decided by ss_prepare_merge_dev's
+ *     rule: USE (at least d shards gathered), NULL (fewer, but acks >= population - f: RSCodeword::from_data(ReqBatch::new(),
+ *     d, p), which is data_len 1 -- bincode 2 standard() writes an empty Vec as the single byte 0x00, from knowledge of the
+ *     crate, unpinned -- shard_len 1 and every shard zero), or not yet: a later decision point decides it.  The first
+ *     quorum of a ballot rebuilds the engine's window of g from the acceptor (window_base, committed, commit_bar = its
+ *     committed prefix, accepting and ack planes cleared); each decided instance enters Accepting as a proposal does,
+ *     with an empty ack set, inst_bal = ballot and (Crossword) policy_idx = policy[g].
+ * The engine keeps the bookkeeping between calls: per group the ballot it belongs to, prepare_acks and the decided
+ * positions, per ring position prepare_max_bal and the gathered codeword; it resets when bal_prep_sent[g] differs from
+ * that ballot, so a second step-up needs no host reset.
+ * Store: CALLER-owned, T planes at shards + j*plane_stride (plane_stride a multiple of 32, shards 16-byte aligned), the
+ * layout ss_engine_propose_ragged writes.  Slots of SS_CW_SLOT_PITCH(shard_len) bytes in every plane are bump-allocated
+ * in group order from *store_used (device u64, in/out, rounded up to 32); an abandoned slot is not reused.  Shard j of
+ * a gathered codeword is at shards + j*plane_stride + its slot, bytes shard_len..round_up(shard_len, 16) zero.
+ * Outputs, the decided list ordered by group, then by the frame that decided the instance, then by slot, as separate
+ * arrays in the order ss_frame_accept_pack_ragged_dev takes them: dec_slot (absolute), dec_ballot, dec_shard_off,
+ * dec_data_len, dec_policy (may be NULL), dec_group.  Every decided codeword holds all T shards: the missing ones of a
+ * USE codeword are regenerated in place by one ss_rs_reconstruct_batch_dev launch over the list's capacity; entries
+ * past the decided count get dec_data_len 0.  The external fill's cells at wal + 32k with rec_group[k], rec_slot[k].
+ * pending[g] (device [G]): the acceptor's Preparing ring positions not yet decided at bal_prep_sent[g] (0 where it is
+ * 0).  verdict[i] per frame.  totals (device u64[3], may be NULL): decided records, PrepareBal records and store bytes
+ * the call asked for.
+ * Capacity is per group, as in ss_acceptor_recover: a group whose store slots end past plane_stride, whose cells end
+ * past min(rec_capacity, wal_capacity / 32) or whose decided records end past dec_capacity applies none of its frames;
+ * its well-formed frames get SS_ACCEPT_VERDICT_STORE_FULL (SS_DEV_STATUS_STORE_FULL) or SS_ACCEPT_VERDICT_WAL_FULL
+ * (SS_DEV_STATUS_FRAME_OVERFLOW).  The ends are monotone in group order, so the applied groups are a prefix and
+ * re-submitting the cut frames finishes the job.
+ * After the call the host packs each peer's Accept, and its own, with ss_frame_accept_pack_ragged_dev over the decided
+ * list (peer = r), and hands its own frame to its own ss_acceptor_accept in the same turn, before any other frame of
+ * those groups: that call leaves Preparing with voted = (ballot, my shards), writes the AcceptData record and emits the
+ * self AcceptReply, which goes through ss_accept_reply_parse_dev to ss_engine_ingest (handle_logged_accept_data);
+ * ss_engine_tick then commits.
+ * Stated differences from the reference:
+ *   1. the 64-slot window, with BEYOND_WINDOW and re-submission;
+ *   2. proposals are fenced by the host: the reference's first_null_slot skips Preparing slots, ss_engine_propose_* do
+ *      not know them, so a host does not propose in a group while pending[g] != 0;
+ *   3. parity is always regenerated: where the reference skips compute_parity (avail_shards >= population, Crossword
+ *      with T > n), its Accepts carry None for the missing parity shards, here the regenerated ones;
+ *   4. the per-group capacity cut;
+ *   5. a same-ballot codeword with another data_len is rejected alone (SS_PREP_VERDICT_DATA_LEN);
+ *   6. `external` and the client replies stay with the host.
+ * Cost: decode a thread per frame; the walk a warp per group segment, twice (count, then apply), so a batch costs its
+ * largest per-group run of frames there; the shard copy a warp per frame; the reconstruct a warp per decided record of
+ * the capacity. */
+#define SS_PREP_VERDICT_IGNORED 0xfffffffau       /* not this leader's Prepare, not Preparing, or ballot < inst_bal */
+#define SS_PREP_VERDICT_DATA_LEN 0xfffffffbu      /* a same-ballot codeword whose data_len differs: rejected alone */
+int ss_engine_prepare_absorb(ss_engine *engine, ss_acceptor *acceptor, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off,
+                             const uint32_t *frame_group, const uint8_t *frame_peer, uint64_t n_frames, uint32_t reply_variant,
+                             uint32_t wal_variant, const uint64_t *bal_prep_sent, const uint8_t *policy, uint8_t *shards,
+                             uint64_t plane_stride, uint64_t *store_used, uint8_t *wal, uint64_t wal_capacity, uint32_t *rec_group,
+                             uint64_t *rec_slot, uint64_t rec_capacity, uint64_t *dec_slot, uint64_t *dec_ballot,
+                             uint64_t *dec_shard_off, uint32_t *dec_data_len, uint8_t *dec_policy, uint32_t *dec_group,
+                             uint64_t dec_capacity, uint64_t *pending, uint32_t *verdict, uint64_t *totals);
 
 /* ---- batched CRaft follower (the Raft-family counterpart of the acceptor) ----------------------------------------
  * For n_groups CRaft groups this replica follows: AppendEntries frames in (handle_msg_append_entries,

@@ -136,6 +136,8 @@ SIGNATURES = {
     "ss_acceptor_step_up": (_i, [_vp, _vp, _u64, _u32, _u32, _vp, _u64, _vp, _vp, _u64, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _vp, _vp, _vp,
                                  _vp, _vp]),
     "ss_prepare_reply_parse_dev": (_i, [_vp, _vp, _u64, _vp, _u64, _u32, _u32, _u32, _vp]),
+    "ss_engine_prepare_absorb": (_i, [_vp, _vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _u32, _vp, _vp, _vp, _u64, _vp, _vp, _u64, _vp,
+                                      _vp, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _u64, _vp, _vp, _vp]),
     "ss_follower_create": (_i, [_vp, _vp, _u64, C.POINTER(_vp)]),
     "ss_follower_destroy": (_i, [_vp]),
     "ss_follower_view_get": (_i, [_vp, _vp]),
@@ -335,6 +337,9 @@ SS_APPEND_REPLY_INGEST = 0xFFFFFFF0
 SS_APPEND_REPLY_CONFLICT = 0xFFFFFFF1
 SS_APPEND_REPLY_HIGHER_TERM = 0xFFFFFFF2
 SS_APPEND_REPLY_END_RANGE = 0xFFFFFFF3
+# verdicts of ss_engine_prepare_absorb, beside the acceptor's
+SS_PREP_VERDICT_IGNORED = 0xFFFFFFFA
+SS_PREP_VERDICT_DATA_LEN = 0xFFFFFFFB
 # verdicts of ss_engine_craft_step_up
 SS_STEPUP_VERDICT_DONE, SS_STEPUP_VERDICT_IGNORED, SS_STEPUP_VERDICT_WINDOW, SS_STEPUP_VERDICT_RANGE, \
     SS_STEPUP_VERDICT_STALE_TERM, SS_STEPUP_VERDICT_STORE_FULL = range(6)

@@ -121,4 +121,35 @@ __device__ __forceinline__ uint64_t warp_put_cw(uint8_t *p, uint32_t d, uint32_t
     return m + 1u;
 }
 
+// PeerMessage::Msg{PrepareReply{slot, trigger_slot, endprep_slot, ballot, voted}} at buf + off, with the codeword checked
+// as ss_acceptor_absorb checks one; the shards stay where they are (shards_at).  Shared by ss_prepare_reply_parse_dev
+// and ss_engine_prepare_absorb.
+__device__ __forceinline__ ss_prepare_reply_rec prepare_reply_decode(const uint8_t *buf, uint64_t buf_len, uint64_t off, uint32_t d,
+                                                                     uint32_t T, uint32_t variant) {
+    ss_prepare_reply_rec r{};
+    r.kind = SS_FRAME_KIND_MALFORMED;
+    r.shards_at = ~0ull;
+    do {
+        const uint8_t *b;
+        uint64_t len, n, f0 = 0, f1 = 0, f2 = 0, f3 = 0, vb = 0, dl = 0, sl = 0, at = ~0ull;
+        uint32_t mask = 0;
+        if (!msg_head(buf, buf_len, off, variant, ~0ull, true, b, len, n, r.kind)) break;
+        if (!wv_next(b, len, n, f0) || !wv_next(b, len, n, f1) || !wv_next(b, len, n, f2) || !wv_next(b, len, n, f3) || n >= len)
+            break;
+        const uint8_t tag = b[n++];
+        if (tag == 1u) {
+            uint64_t tags_at = 0;
+            if (!wv_next(b, len, n, vb) || !cw_parse<true>(b, len, n, d, T, dl, sl, tags_at, mask)) break;
+            at = off + 8u + tags_at;
+        } else if (tag != 0u) {
+            break;
+        }
+        if (n != len) break;
+        r.slot = f0; r.trigger_slot = f1; r.endprep_slot = f2; r.ballot = f3;
+        r.vote_bal = vb; r.vote_mask = mask; r.data_len = static_cast<uint32_t>(dl); r.shards_at = at;
+        r.kind = variant;
+    } while (false);
+    return r;
+}
+
 }  // namespace ssb

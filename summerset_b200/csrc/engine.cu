@@ -53,21 +53,6 @@ __device__ __forceinline__ uint32_t first_null(uint64_t acc, uint64_t cm, uint64
     return dev::commit_prefix(ring_to_window(acc | cm, static_cast<uint32_t>(base & 63u)));
 }
 
-// instance s of group g enters Accepting; acc / cm are the group's accepting / committed words as loaded
-__device__ __forceinline__ void enter_accepting(uint64_t g, uint64_t s, uint64_t acc, uint64_t cm, uint64_t *__restrict__ planes,
-                                                uint32_t R, uint64_t G, const uint64_t *__restrict__ bal_prepared,
-                                                uint64_t *__restrict__ inst_bal, uint64_t *__restrict__ accepting,
-                                                uint64_t *__restrict__ committed, uint8_t *__restrict__ policy_idx,
-                                                const uint8_t *__restrict__ new_policy) {
-    const uint32_t pos = static_cast<uint32_t>(s & 63u);
-    const uint64_t bit = 1ull << pos;
-    accepting[g] = acc | bit;                              // Status::Accepting (request.rs: inst.status = Accepting)
-    committed[g] = cm & ~bit;                              // a re-used window slot starts uncommitted
-    inst_bal[g * 64 + pos] = bal_prepared[g];              // inst.bal = bal_prepared
-    for (uint32_t r = 0; r < R; ++r) planes[static_cast<uint64_t>(r) * G + g] &= ~bit;   // fresh accept_acks
-    if (policy_idx != nullptr) policy_idx[g * 64 + pos] = new_policy != nullptr ? new_policy[g] : 0;
-}
-
 // one status write per warp, not one per flagged group
 __device__ __forceinline__ void warp_status(bool flag, uint32_t bit, uint32_t *status) {
     const unsigned any = __ballot_sync(__activemask(), flag);
@@ -490,6 +475,7 @@ int ss_engine_destroy(ss_engine *e) {
     for (void *b : bufs)
         if (b) cudaFree(b);
     craft_log_free(e);
+    prepare_free(e);
     if (e->coder) ss_rs_coder_destroy(e->coder);
     if (e->ctx) ctx_release(e->ctx);
     delete e;

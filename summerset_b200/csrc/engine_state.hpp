@@ -61,9 +61,37 @@ struct ss_engine {
     uint32_t *bo_keys = nullptr, *bo_idx = nullptr;
     void *bo_sort_tmp = nullptr;
     size_t bo_sort_bytes = 0;
+    // RSPaxos / Crossword Prepare phase (engine_prepare.cu), allocated on the first ss_engine_prepare_absorb: the
+    // bookkeeping of ballot pa_ballot[g] (reset when bal_prep_sent differs): prepare_acks, the decided ring positions,
+    // and per ring position [G*64] prepare_max_bal and the gathered codeword (shards, data_len, slot offset)
+    uint64_t *pa_ballot = nullptr, *pa_done = nullptr, *pa_max_bal = nullptr, *pa_off = nullptr;
+    uint32_t *pa_acks = nullptr, *pa_mask = nullptr, *pa_len = nullptr;
+    uint64_t *pa_words = nullptr;           // [5] applied store bytes and decided records, the totals the caller does not ask for
+    uint64_t pa_cap = 0, pa_dec_cap = 0;    // per-frame and per-decided-record scratch, grow-only
+    ss_prepare_reply_rec *pa_rec = nullptr;
+    uint64_t *pa_cnt = nullptr, *pa_dst = nullptr, *pa_fill = nullptr, *pa_partials = nullptr;
+    uint32_t *pa_take = nullptr, *pa_present = nullptr;
+    int32_t *pa_status = nullptr;
 };
 
 namespace ssb {
+// instance s of group g enters Accepting; acc / cm are the group's accepting / committed words as loaded
+__device__ __forceinline__ void enter_accepting(uint64_t g, uint64_t s, uint64_t acc, uint64_t cm, uint64_t *__restrict__ planes,
+                                                uint32_t R, uint64_t G, const uint64_t *__restrict__ bal_prepared,
+                                                uint64_t *__restrict__ inst_bal, uint64_t *__restrict__ accepting,
+                                                uint64_t *__restrict__ committed, uint8_t *__restrict__ policy_idx,
+                                                const uint8_t *__restrict__ new_policy) {
+    const uint32_t pos = static_cast<uint32_t>(s & 63u);
+    const uint64_t bit = 1ull << pos;
+    accepting[g] = acc | bit;                              // Status::Accepting (request.rs: inst.status = Accepting)
+    committed[g] = cm & ~bit;                              // a re-used window slot starts uncommitted
+    inst_bal[g * 64 + pos] = bal_prepared[g];              // inst.bal = bal_prepared
+    for (uint32_t r = 0; r < R; ++r) planes[static_cast<uint64_t>(r) * G + g] &= ~bit;   // fresh accept_acks
+    if (policy_idx != nullptr) policy_idx[g * 64 + pos] = new_policy != nullptr ? new_policy[g] : 0;
+}
+
+// frees the Prepare-phase state and scratch (engine_prepare.cu)
+void prepare_free(ss_engine *e);
 // frees the CRaft log's state and scratch (craft_leader.cu)
 void craft_log_free(ss_engine *e);
 // the configuration checks every log call makes, and taking the log into use on the first call (craft_leader.cu)

@@ -11,6 +11,7 @@
 // needed except for the Crossword look-up table.
 #include "device_common.cuh"
 #include "gossip_walk.cuh"
+#include "prepare_rule.cuh"
 #include "ss_internal.hpp"
 
 namespace ssb {
@@ -419,18 +420,9 @@ prepare_merge_kernel(const uint64_t *__restrict__ vote_bal, const uint32_t *__re
             if (b > mb) { mb = b; cw = m; }
             else if (b == mb) cw |= m;
         }
-        uint32_t avail = __popc(cw), act = 0;
-        if (avail >= d) {
-            act = 1u;
-            if (static_cast<uint32_t>(__popc(cw & data_mask)) < d) act |= 4u;
-        } else if (acks_cnt[i] >= population - f) {
-            act = 2u;
-            avail = d;
-        }
-        if (act != 0u && avail < population) act |= 8u;
         max_bal[i] = mb;
         merged[i] = cw;
-        action[i] = static_cast<uint8_t>(act);
+        action[i] = static_cast<uint8_t>(prepare_action(cw, [&] { return static_cast<uint32_t>(acks_cnt[i]); }, d, data_mask, population, f));
     }
 }
 

@@ -258,37 +258,11 @@ struct PrepParseArgs {
     ss_prepare_reply_rec *rec;
 };
 
-// a thread per frame: PrepareReply{slot, trigger_slot, endprep_slot, ballot, voted} with the codeword checked as
-// ss_acceptor_absorb checks one; the shards stay where they are (shards_at)
+// a thread per frame: PrepareReply{slot, trigger_slot, endprep_slot, ballot, voted} (prepare_reply_decode)
 __global__ void __launch_bounds__(kWireThreads) prepare_reply_parse_kernel(const __grid_constant__ PrepParseArgs A) {
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kWireThreads;
-    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kWireThreads + threadIdx.x; i < A.n_frames; i += stride) {
-        ss_prepare_reply_rec r{};
-        r.kind = SS_FRAME_KIND_MALFORMED;
-        r.shards_at = ~0ull;
-        const uint64_t off = A.frame_off[i];
-        do {
-            const uint8_t *b;
-            uint64_t len, n, f0 = 0, f1 = 0, f2 = 0, f3 = 0, vb = 0, dl = 0, sl = 0, at = ~0ull;
-            uint32_t mask = 0;
-            if (!msg_head(A.buf, A.buf_len, off, A.reply_variant, ~0ull, true, b, len, n, r.kind)) break;
-            if (!wv_next(b, len, n, f0) || !wv_next(b, len, n, f1) || !wv_next(b, len, n, f2) || !wv_next(b, len, n, f3) || n >= len)
-                break;
-            const uint8_t tag = b[n++];
-            if (tag == 1u) {
-                uint64_t tags_at = 0;
-                if (!wv_next(b, len, n, vb) || !cw_parse<true>(b, len, n, A.d, A.T, dl, sl, tags_at, mask)) break;
-                at = off + 8u + tags_at;
-            } else if (tag != 0u) {
-                break;
-            }
-            if (n != len) break;
-            r.slot = f0; r.trigger_slot = f1; r.endprep_slot = f2; r.ballot = f3;
-            r.vote_bal = vb; r.vote_mask = mask; r.data_len = static_cast<uint32_t>(dl); r.shards_at = at;
-            r.kind = A.reply_variant;
-        } while (false);
-        A.rec[i] = r;
-    }
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kWireThreads + threadIdx.x; i < A.n_frames; i += stride)
+        A.rec[i] = prepare_reply_decode(A.buf, A.buf_len, A.frame_off[i], A.d, A.T, A.reply_variant);
 }
 
 // newly committed instances -> CommitSlot records (24-byte cells: the record is at most 8 + 1 + 9 bytes)

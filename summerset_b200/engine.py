@@ -165,6 +165,40 @@ class LeaderEngine(_EngineBase):
                                          policy.data_ptr() if policy is not None else None, C.byref(base)))
         return self.shards[slot % self.keep] if self.shards is not None else None
 
+    def prepare_absorb(self, acceptor: "Acceptor", buf: torch.Tensor, frame_off: torch.Tensor, frame_group: torch.Tensor,
+                       frame_peer: torch.Tensor, bal_prep_sent: torch.Tensor, store: torch.Tensor, store_used: torch.Tensor,
+                       wal: torch.Tensor, rec_capacity: int, dec_capacity: int, policy: Optional[torch.Tensor] = None,
+                       wal_capacity: Optional[int] = None, reply_variant: int = 1, wal_variant: int = 0) -> dict:
+        """handle_msg_prepare_reply for a batch of PrepareReply frames (buf uint8 at any alignment, frame_off int64, frame_group
+        int32, frame_peer uint8, each [n]; the leader's own replies included) after acceptor.step_up on this replica's
+        acceptor.  bal_prep_sent: int64 [G], the step-up's ballot per group, 0 where not preparing; policy: Crossword uint8
+        [G].  Gathered codewords go to store (uint8 [T, plane_stride], caller-owned, the ragged proposal layout) from
+        store_used (int64 [1], in/out); the external fill's PrepareBal cells to wal (uint8, 16-byte aligned).  Returns device
+        tensors rec_group (int32), rec_slot (int64), each [rec_capacity]; the decided list dec_slot, dec_ballot,
+        dec_shard_off (int64), dec_data_len (int32), dec_policy (uint8), dec_group (int32), each [dec_capacity], ready for
+        ss_frame_accept_pack_ragged_dev; pending (int64 [G]), verdict (int32 [n]) and totals (int64 [3]: decided records,
+        PrepareBal records and store bytes asked for)."""
+        assert buf.dtype == torch.uint8 and frame_off.dtype == torch.int64 and frame_group.dtype == torch.int32
+        assert frame_peer.dtype == torch.uint8 and bal_prep_sent.dtype == torch.int64 and bal_prep_sent.numel() == self.G
+        assert store.dtype == torch.uint8 and store.dim() == 2 and store.is_contiguous() and store_used.dtype == torch.int64
+        assert wal.dtype == torch.uint8 and (policy is None or (policy.dtype == torch.uint8 and policy.numel() == self.G))
+        n, dev = frame_off.numel(), self.dev
+        e = lambda k, dt: torch.empty(max(k, 1), dtype=dt, device=dev)
+        res = dict(rec_group=e(rec_capacity, torch.int32), rec_slot=e(rec_capacity, torch.int64), dec_slot=e(dec_capacity, torch.int64),
+                   dec_ballot=e(dec_capacity, torch.int64), dec_shard_off=e(dec_capacity, torch.int64),
+                   dec_data_len=e(dec_capacity, torch.int32), dec_policy=e(dec_capacity, torch.uint8),
+                   dec_group=e(dec_capacity, torch.int32), pending=e(self.G, torch.int64), verdict=e(n, torch.int32),
+                   totals=e(3, torch.int64))
+        p = lambda x: None if x is None else x.data_ptr()
+        check(self.lib.ss_engine_prepare_absorb(self.h, acceptor.h, p(buf), buf.numel(), p(frame_off), p(frame_group), p(frame_peer), n,
+                                                reply_variant, wal_variant, p(bal_prep_sent), p(policy), p(store), store.shape[1],
+                                                p(store_used), p(wal), wal.numel() if wal_capacity is None else wal_capacity,
+                                                p(res["rec_group"]), p(res["rec_slot"]), rec_capacity, p(res["dec_slot"]),
+                                                p(res["dec_ballot"]), p(res["dec_shard_off"]), p(res["dec_data_len"]),
+                                                p(res["dec_policy"]), p(res["dec_group"]), dec_capacity, p(res["pending"]),
+                                                p(res["verdict"]), p(res["totals"])))
+        return res
+
     def propose_next(self, store: int, payloads: Optional[torch.Tensor],
                      policy: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
         """One new instance per group at its first Null slot; shards into shard store `store` (< keep_slots).

@@ -553,6 +553,21 @@ inline void craft_step_up(ss_engine *e, const Follower &follower, const uint32_t
                           uint8_t *shards, uint64_t plane_stride, uint64_t *shard_off, uint32_t *verdict, uint64_t *need = nullptr) {
     check(ss_engine_craft_step_up(e, follower.get(), groups, n_listed, term, shards, plane_stride, shard_off, need, verdict));
 }
+// RSPaxos / Crossword fail-over on the new leader: PrepareReply frames (its own and its peers') absorbed after
+// Acceptor::step_up; the decided list feeds ss_frame_accept_pack_ragged_dev, and the leader's own frame goes to its own
+// Acceptor::accept in the same turn (see ss_engine_prepare_absorb for the capacity cut and the host's part)
+inline void prepare_absorb(ss_engine *e, Acceptor &acceptor, const uint8_t *buf, uint64_t buf_len, const uint64_t *frame_off,
+                           const uint32_t *frame_group, const uint8_t *frame_peer, uint64_t n_frames, const uint64_t *bal_prep_sent,
+                           const uint8_t *policy, uint8_t *shards, uint64_t plane_stride, uint64_t *store_used, uint8_t *wal,
+                           uint64_t wal_capacity, uint32_t *rec_group, uint64_t *rec_slot, uint64_t rec_capacity, uint64_t *dec_slot,
+                           uint64_t *dec_ballot, uint64_t *dec_shard_off, uint32_t *dec_data_len, uint8_t *dec_policy,
+                           uint32_t *dec_group, uint64_t dec_capacity, uint64_t *pending, uint32_t *verdict,
+                           uint64_t *totals = nullptr, uint32_t reply_variant = 1, uint32_t wal_variant = 0) {
+    check(ss_engine_prepare_absorb(e, acceptor.handle(), buf, buf_len, frame_off, frame_group, frame_peer, n_frames, reply_variant,
+                                   wal_variant, bal_prep_sent, policy, shards, plane_stride, store_used, wal, wal_capacity, rec_group,
+                                   rec_slot, rec_capacity, dec_slot, dec_ballot, dec_shard_off, dec_data_len, dec_policy, dec_group,
+                                   dec_capacity, pending, verdict, totals));
+}
 // step-down: the led bytes, and check_term over a batch of incoming frames (ss_engine_craft_step_down)
 inline ss_engine_craft_role_view craft_role_view(ss_engine *e) {
     ss_engine_craft_role_view v{};
