@@ -1173,6 +1173,57 @@ int ss_engine_prepare_absorb(ss_engine *engine, ss_acceptor *acceptor, const uin
                              uint64_t *rec_slot, uint64_t rec_capacity, uint64_t *dec_slot, uint64_t *dec_ballot,
                              uint64_t *dec_shard_off, uint32_t *dec_data_len, uint8_t *dec_policy, uint32_t *dec_group,
                              uint64_t dec_capacity, uint64_t *pending, uint32_t *verdict, uint64_t *totals);
+/* Soft fallback on a Crossword leader: fallback_redo_accepts (crossword/leadership.rs:389-550), which the reference runs
+ * from bcast_heartbeats when peer_alive loses a member (:247-251), for a list of groups this replica leads.  Other
+ * engines, and a Crossword engine before ss_engine_set_policies, give SS_ERR_INVALID_ARG.
+ * Codeword locations: a Crossword engine records, per ring position, where the full T-shard codeword of the instance
+ * that last entered Accepting there lives (shard 0, plane stride, data_len; 16 bytes per position, 1 KiB per group):
+ * ss_engine_propose / _next its own store, ss_engine_propose_ragged shards + shard_off[g], ss_engine_prepare_absorb the
+ * decided codeword's slot in that call's store (a NULL decision: the zero codeword of data_len 1).  So a Crossword host
+ * that calls the fallback keeps the store of every Accepting instance alive and unmodified until the instance commits or
+ * retires; hosts that never call it are unaffected.  The fallback's own output store is not recorded: the host may reuse
+ * it once the Accepts are packed.  Plane strides on a Crossword engine are below 2^36 (else SS_ERR_INVALID_ARG).
+ * groups (device u32 [n_listed]); peer_alive (device [G] replica masks, NULL = every one of the population alive;
+ * bits past the population are ignored); policy (device u8 [G]): the index of pick_assignment_policy's result for the
+ * group, which the host computes.
+ * Per listed entry, in list order, every window position in slot order that is Accepting and not Committed:
+ *   kept when the engine is balanced, its policy_idx < n_policies and popcount(policies[policy_idx][0]) >= min_spr,
+ *     min_spr = (majority + f + 1 - alive) * (d / majority) in u8 arithmetic (adaptive.rs:98-106), alive the popcount
+ *     of peer_alive[g];
+ *   redone otherwise (every such instance of an unbalanced engine): inst_bal = bal_prepared[g], its bit cleared in every
+ *     ack plane, policy_idx = policy[g], its full codeword copied from the recorded location into a bump-allocated
+ *     SS_CW_SLOT_PITCH(shard_len) slot of every plane of the CALLER-owned store (shards + j*plane_stride, plane_stride a
+ *     multiple of 32, shards 16-byte aligned, from *store_used, device u64 in/out rounded up to 32; bytes
+ *     shard_len..round_up(shard_len, 16) zero), and one record appended to the decided list.
+ * accepting, committed and commit_bar do not change.  A position with no recorded location (state installed through
+ * the view) is kept.  A group listed twice is processed once per entry, as two reference calls would be: the second
+ * entry redoes its instances again only when policy[g] is not responsive either.
+ * Outputs: the decided list in the order and layout of ss_engine_prepare_absorb's (dec_slot absolute, dec_ballot,
+ * dec_shard_off, dec_data_len, dec_policy (may be NULL), dec_group), which ss_frame_accept_pack_ragged_dev takes;
+ * verdict[i]: SS_ACCEPT_VERDICT_ACCEPTED (applied, possibly with nothing to redo), SS_FRAME_KIND_MALFORMED (group >=
+ * n_groups: nothing happens), SS_ACCEPT_VERDICT_STORE_FULL (SS_DEV_STATUS_STORE_FULL) or SS_ACCEPT_VERDICT_WAL_FULL
+ * (SS_DEV_STATUS_FRAME_OVERFLOW) for an entry whose store slots end past plane_stride or whose records end past
+ * dec_capacity: it changes nothing, and neither does any later entry, since the ends are monotone in list order, so
+ * re-submitting the cut entries finishes the job.  totals (device u64[2], may be NULL): the records and store bytes the
+ * whole list asked for.
+ * After the call the host does what it does after ss_engine_prepare_absorb: ss_frame_accept_pack_ragged_dev over the
+ * decided list for every peer (dead ones too, as the reference sends to them) and for itself, its own frame to its own
+ * ss_acceptor_accept in the same turn, then ss_accept_reply_parse_dev, ss_engine_ingest and ss_engine_tick.  The Accepts
+ * go out under bal_prepared, normally the instance's ballot already, so a late AcceptReply of the old round is still
+ * credited, under the new assignment: an AcceptReply carries none.
+ * Stated differences from the reference:
+ *   1. the 64-slot window;
+ *   2. one policy per group, not one per data_len: it differs only under the adaptive or b_to_d_threshold chooser, which
+ *      is the host's;
+ *   3. where (majority + f + 1 - alive) underflows u8 (more replicas alive than majority + f + 1) the threshold is 0 and
+ *      every balanced instance is kept; the reference panics there (u8 overflow, or brr_assignments has no entry);
+ *   4. the per-entry capacity cut;
+ *   5. pending_accepts, the RTT bookkeeping and the heartbeats injected every msg_chunk_size Accepts stay with the host.
+ * Cost: the walk a warp per listed entry, each lane two window positions; the copy a warp per decided record. */
+int ss_engine_fallback_redo(ss_engine *engine, const uint32_t *groups, uint64_t n_listed, const uint32_t *peer_alive,
+                            const uint8_t *policy, uint8_t *shards, uint64_t plane_stride, uint64_t *store_used, uint64_t *dec_slot,
+                            uint64_t *dec_ballot, uint64_t *dec_shard_off, uint32_t *dec_data_len, uint8_t *dec_policy,
+                            uint32_t *dec_group, uint64_t dec_capacity, uint32_t *verdict, uint64_t *totals);
 
 /* ---- batched CRaft follower (the Raft-family counterpart of the acceptor) ----------------------------------------
  * For n_groups CRaft groups this replica follows: AppendEntries frames in (handle_msg_append_entries,

@@ -138,6 +138,7 @@ SIGNATURES = {
     "ss_prepare_reply_parse_dev": (_i, [_vp, _vp, _u64, _vp, _u64, _u32, _u32, _u32, _vp]),
     "ss_engine_prepare_absorb": (_i, [_vp, _vp, _vp, _u64, _vp, _vp, _vp, _u64, _u32, _u32, _vp, _vp, _vp, _u64, _vp, _vp, _u64, _vp,
                                       _vp, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _u64, _vp, _vp, _vp]),
+    "ss_engine_fallback_redo": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u64, _vp, _vp]),
     "ss_follower_create": (_i, [_vp, _vp, _u64, C.POINTER(_vp)]),
     "ss_follower_destroy": (_i, [_vp]),
     "ss_follower_view_get": (_i, [_vp, _vp]),

@@ -13,7 +13,7 @@ from pathlib import Path
 PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 OUT = PKG / "libsummerset_b200.so"
-SOURCES = ["capi.cu", "rs_kernels.cu", "tally_kernels.cu", "engine.cu", "wire_kernels.cu", "acceptor.cu", "acceptor_recover.cu", "acceptor_stepup.cu", "engine_prepare.cu", "follower.cu", "craft_leader.cu", "craft_recon.cu", "craft_election.cu", "craft_stepdown.cu", "craft_recover.cu", "jit.cu"]
+SOURCES = ["capi.cu", "rs_kernels.cu", "tally_kernels.cu", "engine.cu", "wire_kernels.cu", "acceptor.cu", "acceptor_recover.cu", "acceptor_stepup.cu", "engine_prepare.cu", "engine_fallback.cu", "follower.cu", "craft_leader.cu", "craft_recon.cu", "craft_election.cu", "craft_stepdown.cu", "craft_recover.cu", "jit.cu"]
 HEADERS = ["ss_internal.hpp", "device_common.cuh", "gf256.hpp", "static_codes.hpp", "rs32_decode.cuh", "horner_row_kernels.cuh",
            "wire_common.cuh", "window_ring.cuh", "gossip_walk.cuh", "codeword_wire.cuh", "engine_state.hpp", "prepare_rule.cuh", "acceptor_state.hpp", "follower_state.hpp", "exec_walk.cuh", "craft_frames.cuh",
            "../../include/summerset_b200.h"]

@@ -66,7 +66,8 @@ __global__ void __launch_bounds__(kEngThreads)
 engine_propose_kernel(uint64_t *__restrict__ planes, uint32_t R, uint64_t G, uint32_t slot, const uint64_t *__restrict__ window_base,
                       const uint64_t *__restrict__ bal_prepared, uint64_t *__restrict__ inst_bal, uint64_t *__restrict__ accepting,
                       uint64_t *__restrict__ committed, uint8_t *__restrict__ policy_idx, const uint8_t *__restrict__ new_policy,
-                      uint64_t *__restrict__ slot_out, uint32_t *status) {
+                      ss_cw_loc *__restrict__ cw_loc, const uint8_t *store, uint64_t shard_stride, uint64_t plane_stride,
+                      uint32_t data_len, uint64_t *__restrict__ slot_out, uint32_t *status) {
     bool full = false;
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kEngThreads;
     for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kEngThreads + threadIdx.x; g < G; g += stride) {
@@ -82,7 +83,8 @@ engine_propose_kernel(uint64_t *__restrict__ planes, uint32_t R, uint64_t G, uin
             }
         }
         const uint64_t s = base + rel;
-        enter_accepting(g, s, acc, cm, planes, R, G, bal_prepared, inst_bal, accepting, committed, policy_idx, new_policy);
+        enter_accepting(g, s, acc, cm, planes, R, G, bal_prepared, inst_bal, accepting, committed, policy_idx, new_policy, cw_loc,
+                        store + g * shard_stride, plane_stride, data_len);
         if (slot_out != nullptr) slot_out[g] = s;
     }
     warp_status(full, SS_DEV_STATUS_WINDOW_FULL, status);
@@ -118,7 +120,8 @@ engine_ragged_commit_kernel(uint32_t *__restrict__ eff_len, uint64_t *__restrict
                             uint64_t *__restrict__ planes, uint32_t R, uint64_t G, const uint64_t *__restrict__ window_base,
                             const uint64_t *__restrict__ bal_prepared, uint64_t *__restrict__ inst_bal,
                             uint64_t *__restrict__ accepting, uint64_t *__restrict__ committed, uint8_t *__restrict__ policy_idx,
-                            const uint8_t *__restrict__ new_policy, uint64_t *__restrict__ slot_out, uint32_t *status) {
+                            const uint8_t *__restrict__ new_policy, ss_cw_loc *__restrict__ cw_loc, const uint8_t *shards,
+                            uint64_t *__restrict__ slot_out, uint32_t *status) {
     bool over = false;
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kEngThreads;
     for (uint64_t g = static_cast<uint64_t>(blockIdx.x) * kEngThreads + threadIdx.x; g < G; g += stride) {
@@ -137,7 +140,8 @@ engine_ragged_commit_kernel(uint32_t *__restrict__ eff_len, uint64_t *__restrict
         const uint64_t base = window_base[g];
         const uint64_t acc = accepting[g], cm = committed[g];
         const uint64_t s = base + first_null(acc, cm, base);   // not full: the prepare kernel checked the same words
-        enter_accepting(g, s, acc, cm, planes, R, G, bal_prepared, inst_bal, accepting, committed, policy_idx, new_policy);
+        enter_accepting(g, s, acc, cm, planes, R, G, bal_prepared, inst_bal, accepting, committed, policy_idx, new_policy, cw_loc,
+                        shards + off, capacity, len);
         slot_out[g] = s;
     }
     warp_status(over, SS_DEV_STATUS_STORE_FULL, status);
@@ -471,11 +475,12 @@ int ss_engine_destroy(ss_engine *e) {
     }
     void *bufs[] = {e->planes, e->bal_prepared, e->inst_bal, e->accepting, e->committed, e->window_base, e->commit_bar, e->shards, e->policy_idx,
                     e->policies, e->lut_bits, e->match, e->next_slot, e->last_commit, e->log_end, e->curr_term, e->terms,
-                    e->last_snap, e->touched, e->rg_len, e->rg_partials, e->rg_need};
+                    e->last_snap, e->touched, e->rg_len, e->rg_partials, e->rg_need, e->cw_loc};
     for (void *b : bufs)
         if (b) cudaFree(b);
     craft_log_free(e);
     prepare_free(e);
+    fallback_free(e);
     if (e->coder) ss_rs_coder_destroy(e->coder);
     if (e->ctx) ctx_release(e->ctx);
     delete e;
@@ -549,7 +554,9 @@ int ss_engine_create(ss_ctx *ctx, const ss_engine_config *cfg, uint64_t G, ss_en
         if ((rc = dalloc(ctx, &e->shards, size_t(keep) * e->T * G * e->ds))) return fail(rc);
     }
     if (cfg->protocol == SS_PROTO_CROSSWORD) {
-        if ((rc = dalloc(ctx, &e->policy_idx, G * 64))) return fail(rc);
+        if (G * e->ds >= kCwLocStrideLimit)
+            return fail(set_error(SS_ERR_INVALID_ARG, "a Crossword engine's shard plane (n_groups * shard_stride) must be below 2^36 bytes"));
+        if ((rc = dalloc(ctx, &e->policy_idx, G * 64)) || (rc = dalloc(ctx, &e->cw_loc, G * 64))) return fail(rc);
     }
     *out = e;
     return SS_OK;
@@ -617,7 +624,8 @@ static int engine_propose(ss_engine *e, uint32_t store, uint32_t slot, const uin
     }
     engine_propose_kernel<<<eng_grid(ctx, e->G), kEngThreads, 0, ctx->stream>>>(e->planes, e->n, e->G, slot, e->window_base,
                                                                              e->bal_prepared, e->inst_bal, e->accepting, e->committed,
-                                                                             e->policy_idx, policy, slot_out, ctx->dev_status);
+                                                                             e->policy_idx, policy, e->cw_loc, e->shards + uint64_t(store) * e->T * e->G * e->ds,
+                                                                             e->ds, e->G * e->ds, e->cfg.data_len, slot_out, ctx->dev_status);
     return launched(ctx);
 }
 
@@ -649,6 +657,8 @@ int ss_engine_propose_ragged(ss_engine *e, const uint8_t *arena, const uint64_t 
     if (reinterpret_cast<uintptr_t>(shards) & 15u) return set_error(SS_ERR_INVALID_ARG, "the shard store must be 16-byte aligned");
     if (e->cfg.protocol == SS_PROTO_CROSSWORD && e->lut_bits == nullptr)
         return set_error(SS_ERR_INVALID_ARG, "ss_engine_set_policies must be called before proposing");
+    if (e->cw_loc != nullptr && plane_stride >= kCwLocStrideLimit)
+        return set_error(SS_ERR_INVALID_ARG, "a Crossword engine's plane_stride must be below 2^36");
     ss_ctx *ctx = e->ctx;
     SS_TRY(ctx_bind(ctx));
     if (e->rg_len == nullptr) SS_TRY(dalloc(ctx, &e->rg_len, e->G, false));
@@ -661,7 +671,8 @@ int ss_engine_propose_ragged(ss_engine *e, const uint8_t *arena, const uint64_t 
     SS_TRY(launch_exclusive_scan_u64(ctx, shard_off, e->G, e->rg_partials, need != nullptr ? need : e->rg_need));
     engine_ragged_commit_kernel<<<grid, kEngThreads, 0, ctx->stream>>>(e->rg_len, shard_off, plane_stride, e->d, e->planes, e->n, e->G,
                                                                      e->window_base, e->bal_prepared, e->inst_bal, e->accepting,
-                                                                     e->committed, e->policy_idx, policy, slot_out, ctx->dev_status);
+                                                                     e->committed, e->policy_idx, policy, e->cw_loc, shards, slot_out,
+                                                                     ctx->dev_status);
     SS_TRY(launched(ctx));
     // from_data + compute_parity + subset_copy's per-peer buffers for every proposing group, one launch: data shards into
     // planes 0..d-1, parity into planes d..T-1, each at the group's slot (rspaxos/request.rs:72-77,127-142,

@@ -54,6 +54,7 @@ struct PaArgs {
     uint64_t *planes, *bal_prepared, *inst_bal, *accepting, *committed, *window_base;
     uint32_t *commit_bar;
     uint8_t *policy_idx;
+    ss_cw_loc *cw_loc;              // Crossword [G*64], else nullptr
     uint64_t *pa_ballot, *pa_done, *pa_max_bal, *pa_off;
     uint32_t *pa_acks, *pa_mask, *pa_len;
     // scratch
@@ -284,13 +285,15 @@ __global__ void __launch_bounds__(kPaThreads, 1) pa_walk_kernel(const __grid_con
                                     A.dec_group[kd] = g;
                                     if (A.dec_policy != nullptr) A.dec_policy[kd] = A.policy != nullptr ? A.policy[g] : 0u;
                                     A.present[kd] = pres;
+                                    if (A.cw_loc != nullptr) put_cw_loc(A.cw_loc, row + q, A.shards + off, A.plane_stride, len);
                                 }
                                 if (lane == 0u && dec != 0u) {
                                     uint64_t acc = A.accepting[g], cm = A.committed[g];
                                     for (uint64_t m = dec; m != 0u; m &= m - 1u) {
                                         const uint32_t q = static_cast<uint32_t>(__ffsll(static_cast<long long>(m)) - 1);
                                         enter_accepting(g, base + ((q - r) & 63u), acc, cm, A.planes, A.population, A.G, A.bal_prepared,
-                                                        A.inst_bal, A.accepting, A.committed, A.policy_idx, A.policy);
+                                                        A.inst_bal, A.accepting, A.committed, A.policy_idx, A.policy, nullptr, nullptr, 0u,
+                                                        0u);   // the owning lanes recorded the locations above
                                         acc |= 1ull << q;
                                         cm &= ~(1ull << q);
                                     }
@@ -471,6 +474,8 @@ extern "C" int ss_engine_prepare_absorb(ss_engine *e, ss_acceptor *a, const uint
     if ((reinterpret_cast<uintptr_t>(shards) | reinterpret_cast<uintptr_t>(wal)) & 15u)
         return set_error(SS_ERR_INVALID_ARG, "the shard store and wal must be 16-byte aligned");
     if (n_frames > 0x7fffffffull) return set_error(SS_ERR_INVALID_ARG, "at most 2^31 - 1 frames per call");
+    if (e->cw_loc != nullptr && plane_stride >= kCwLocStrideLimit)
+        return set_error(SS_ERR_INVALID_ARG, "a Crossword engine's plane_stride must be below 2^36");
     ss_ctx *ctx = e->ctx;
     SS_TRY(ctx_bind(ctx));
     SS_TRY(prepare_scratch(e, n_frames, dec_capacity));
@@ -487,6 +492,7 @@ extern "C" int ss_engine_prepare_absorb(ss_engine *e, ss_acceptor *a, const uint
     A.a_source = a->source; A.a_prep_span = a->prep_span;
     A.planes = e->planes; A.bal_prepared = e->bal_prepared; A.inst_bal = e->inst_bal; A.accepting = e->accepting;
     A.committed = e->committed; A.window_base = e->window_base; A.commit_bar = e->commit_bar; A.policy_idx = e->policy_idx;
+    A.cw_loc = e->cw_loc;
     A.pa_ballot = e->pa_ballot; A.pa_done = e->pa_done; A.pa_max_bal = e->pa_max_bal; A.pa_off = e->pa_off; A.pa_acks = e->pa_acks;
     A.pa_mask = e->pa_mask; A.pa_len = e->pa_len;
     A.rec = e->pa_rec;

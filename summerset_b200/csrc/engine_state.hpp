@@ -2,6 +2,16 @@
 #pragma once
 #include "ss_internal.hpp"
 
+// Where an Accepting Crossword instance's full T-shard codeword lives, so ss_engine_fallback_redo can send it again:
+// shard j at addr + j * (stride16 << 4), data_len bytes of payload.  16 bytes per ring position, 1 KiB per group (1 GiB
+// at 2^20 groups); plane strides are multiples of 16 below 2^36, so stride16 fits 32 bits.  addr 0: no location recorded.
+struct alignas(16) ss_cw_loc {
+    uint64_t addr;
+    uint32_t stride16;
+    uint32_t data_len;
+};
+constexpr uint64_t kCwLocStrideLimit = 1ull << 36;
+
 struct ss_engine {
     ss_ctx *ctx = nullptr;
     ss_rs_coder *coder = nullptr;
@@ -24,6 +34,13 @@ struct ss_engine {
     uint32_t *policies = nullptr, *lut_bits = nullptr;
     uint32_t n_policies = 0, lut_words = 0;
     int balanced = 1;
+    ss_cw_loc *cw_loc = nullptr;            // [G*64] written by every path into Accepting (enter_accepting)
+    // soft fallback (engine_fallback.cu), allocated on the first ss_engine_fallback_redo: fb_first [G] the first list
+    // entry of each group (UINT32_MAX between calls); per listed entry the redone ring positions and the records and
+    // store bytes they add, then their scans
+    uint32_t *fb_first = nullptr;
+    uint64_t *fb_mask = nullptr, *fb_cnt = nullptr, *fb_partials = nullptr, *fb_words = nullptr;
+    uint64_t fb_cap = 0;
     // Raft
     uint32_t *match = nullptr, *next_slot = nullptr, *last_commit = nullptr, *log_end = nullptr, *curr_term = nullptr,
              *terms = nullptr, *last_snap = nullptr;
@@ -75,12 +92,24 @@ struct ss_engine {
 };
 
 namespace ssb {
-// instance s of group g enters Accepting; acc / cm are the group's accepting / committed words as loaded
+__device__ __forceinline__ void put_cw_loc(ss_cw_loc *__restrict__ cw_loc, uint64_t at, const uint8_t *shard0, uint64_t plane_stride,
+                                           uint32_t data_len) {
+    ss_cw_loc v;
+    v.addr = reinterpret_cast<uint64_t>(shard0);
+    v.stride16 = static_cast<uint32_t>(plane_stride >> 4);
+    v.data_len = data_len;
+    cw_loc[at] = v;
+}
+
+// instance s of group g enters Accepting; acc / cm are the group's accepting / committed words as loaded.  cw_loc
+// (Crossword engines; nullptr otherwise or when the caller records the location itself) receives where the instance's
+// full codeword lives: shard 0 at shard0, plane_stride apart, data_len bytes.
 __device__ __forceinline__ void enter_accepting(uint64_t g, uint64_t s, uint64_t acc, uint64_t cm, uint64_t *__restrict__ planes,
                                                 uint32_t R, uint64_t G, const uint64_t *__restrict__ bal_prepared,
                                                 uint64_t *__restrict__ inst_bal, uint64_t *__restrict__ accepting,
                                                 uint64_t *__restrict__ committed, uint8_t *__restrict__ policy_idx,
-                                                const uint8_t *__restrict__ new_policy) {
+                                                const uint8_t *__restrict__ new_policy, ss_cw_loc *__restrict__ cw_loc,
+                                                const uint8_t *shard0, uint64_t plane_stride, uint32_t data_len) {
     const uint32_t pos = static_cast<uint32_t>(s & 63u);
     const uint64_t bit = 1ull << pos;
     accepting[g] = acc | bit;                              // Status::Accepting (request.rs: inst.status = Accepting)
@@ -88,10 +117,13 @@ __device__ __forceinline__ void enter_accepting(uint64_t g, uint64_t s, uint64_t
     inst_bal[g * 64 + pos] = bal_prepared[g];              // inst.bal = bal_prepared
     for (uint32_t r = 0; r < R; ++r) planes[static_cast<uint64_t>(r) * G + g] &= ~bit;   // fresh accept_acks
     if (policy_idx != nullptr) policy_idx[g * 64 + pos] = new_policy != nullptr ? new_policy[g] : 0;
+    if (cw_loc != nullptr) put_cw_loc(cw_loc, g * 64 + pos, shard0, plane_stride, data_len);
 }
 
 // frees the Prepare-phase state and scratch (engine_prepare.cu)
 void prepare_free(ss_engine *e);
+// frees the soft fallback's scratch (engine_fallback.cu)
+void fallback_free(ss_engine *e);
 // frees the CRaft log's state and scratch (craft_leader.cu)
 void craft_log_free(ss_engine *e);
 // the configuration checks every log call makes, and taking the log into use on the first call (craft_leader.cu)

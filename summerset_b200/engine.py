@@ -9,6 +9,8 @@ torch tensors (zero-copy views) so tests can read results and install state; it 
         propose(slot, payloads[, policy])   multipaxos/request.rs:112-221, rspaxos/request.rs:72-142, crossword/request.rs:82-185
         propose_next(store, payloads[, policy])   the same at each group's first Null slot (rspaxos/mod.rs:434-442)
         propose_ragged(arena, data_off, data_len, store[, policy])   variable-length batches into a caller-owned store
+        fallback_redo(groups, policy, store, store_used, dec_capacity[, peer_alive])   Crossword's soft fallback
+                                            (crossword/leadership.rs:389-550): unresponsive Accepting instances re-assigned
         on_accept_replies(records)          handle_msg_accept_reply filters (multipaxos/messages.rs:377-409, ...)
         tick()                              commit decision + commit_bar, one kernel
         advance([upto])                     retire committed prefixes: window_base moves on (multipaxos/snapshot.rs:121-171)
@@ -197,6 +199,30 @@ class LeaderEngine(_EngineBase):
                                                 p(res["dec_ballot"]), p(res["dec_shard_off"]), p(res["dec_data_len"]),
                                                 p(res["dec_policy"]), p(res["dec_group"]), dec_capacity, p(res["pending"]),
                                                 p(res["verdict"]), p(res["totals"])))
+        return res
+
+    def fallback_redo(self, groups: torch.Tensor, policy: torch.Tensor, store: torch.Tensor, store_used: torch.Tensor,
+                      dec_capacity: int, peer_alive: Optional[torch.Tensor] = None) -> dict:
+        """Crossword's fallback_redo_accepts for the listed groups (int32 [n]): every Accepting instance whose policy is not
+        responsive for peer_alive (int32 [G] replica masks, None = all alive) takes policy (uint8 [G]), loses its acks and
+        has its codeword copied from where it was proposed into store (uint8 [T, plane_stride], caller-owned) from
+        store_used (int64 [1], in/out).  Returns device tensors dec_slot, dec_ballot, dec_shard_off (int64), dec_data_len
+        (int32), dec_policy (uint8), dec_group (int32), each [dec_capacity], ready for ss_frame_accept_pack_ragged_dev;
+        verdict (int32 [n]) and totals (int64 [2]: records and store bytes asked for)."""
+        assert groups.dtype == torch.int32 and policy.dtype == torch.uint8 and policy.numel() == self.G
+        assert store.dtype == torch.uint8 and store.dim() == 2 and store.is_contiguous() and store_used.dtype == torch.int64
+        assert peer_alive is None or (peer_alive.dtype == torch.int32 and peer_alive.numel() == self.G)
+        n, dev = groups.numel(), self.dev
+        e = lambda k, dt: torch.empty(max(k, 1), dtype=dt, device=dev)
+        res = dict(dec_slot=e(dec_capacity, torch.int64), dec_ballot=e(dec_capacity, torch.int64), dec_shard_off=e(dec_capacity, torch.int64),
+                   dec_data_len=e(dec_capacity, torch.int32), dec_policy=e(dec_capacity, torch.uint8),
+                   dec_group=e(dec_capacity, torch.int32), verdict=torch.empty(n, dtype=torch.int32, device=dev),
+                   totals=e(2, torch.int64))
+        p = lambda x: None if x is None else x.data_ptr() or None
+        check(self.lib.ss_engine_fallback_redo(self.h, p(groups), n, p(peer_alive), p(policy), p(store), store.shape[1], p(store_used),
+                                               p(res["dec_slot"]), p(res["dec_ballot"]), p(res["dec_shard_off"]),
+                                               p(res["dec_data_len"]), p(res["dec_policy"]), p(res["dec_group"]), dec_capacity,
+                                               p(res["verdict"]), p(res["totals"])))
         return res
 
     def propose_next(self, store: int, payloads: Optional[torch.Tensor],

@@ -568,6 +568,15 @@ inline void prepare_absorb(ss_engine *e, Acceptor &acceptor, const uint8_t *buf,
                                    rec_slot, rec_capacity, dec_slot, dec_ballot, dec_shard_off, dec_data_len, dec_policy, dec_group,
                                    dec_capacity, pending, verdict, totals));
 }
+// Crossword soft fallback when a peer dies: unresponsive Accepting instances re-assigned `policy` and their codewords
+// copied out for ss_frame_accept_pack_ragged_dev (see ss_engine_fallback_redo for the host contract and the cut)
+inline void fallback_redo(ss_engine *e, const uint32_t *groups, uint64_t n_listed, const uint32_t *peer_alive, const uint8_t *policy,
+                          uint8_t *shards, uint64_t plane_stride, uint64_t *store_used, uint64_t *dec_slot, uint64_t *dec_ballot,
+                          uint64_t *dec_shard_off, uint32_t *dec_data_len, uint8_t *dec_policy, uint32_t *dec_group,
+                          uint64_t dec_capacity, uint32_t *verdict, uint64_t *totals = nullptr) {
+    check(ss_engine_fallback_redo(e, groups, n_listed, peer_alive, policy, shards, plane_stride, store_used, dec_slot, dec_ballot,
+                                  dec_shard_off, dec_data_len, dec_policy, dec_group, dec_capacity, verdict, totals));
+}
 // step-down: the led bytes, and check_term over a batch of incoming frames (ss_engine_craft_step_down)
 inline ss_engine_craft_role_view craft_role_view(ss_engine *e) {
     ss_engine_craft_role_view v{};
